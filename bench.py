@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """bench.py — cells / second / Harmony-iteration on synthetic embeddings (BASELINE.json metric).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl b200|reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl b200|reference] [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 \
         --master-port P bench.py --gpus N --steps K --warmup W
 
@@ -16,6 +16,11 @@ ranks), `e2e` (the same metric through the public API with HOST buffers: setup H
 getZcorr D2H), `roofline` (dominant kernel, algorithmic bytes / measured launch time, against
 MEASURED_PEAKS.json) and `cpu_baseline` (the CPU oracle = restatement of the reference, timed on this
 box's host cores on a bounded sample).
+
+--dump-outputs DIR writes what the timed loop computed in its last step, as a caller of harmony() would read it
+back: Z_corr.npy (cells x d), R.npy (cells x K) and Y.npy (K x d), float32, for a fixed seeded sample of at most
+DUMP_CELLS cells (rank 0's shard); sample_cells.npy lists the sampled cells.  The inputs depend on the arguments
+only, so two builds can be compared output for output.
 """
 import argparse
 import json
@@ -32,6 +37,7 @@ sys.path.insert(0, ROOT)
 
 T = 4
 N_TYPES = 30
+DUMP_CELLS = 65536   # cells sampled by --dump-outputs (c5: 65536 x (100 + 200) x 4 B = 79 MB would be too many)
 # BASELINE.json configs 3 / 4 / 5 as PER-GPU shards (config 4: 10M cells over 8 GPUs, config 5: 50M over 8);
 # the headline metric is quoted on config 3.  Level counts beyond config 3's are SURVEY.md 8(d)'s stated choice.
 WORKLOADS = {
@@ -118,7 +124,7 @@ def setup_kwargs(lv):
 
 
 class ClockSampler(threading.Thread):
-    """SM clock / throttle reasons during the timed region (B200_PROFILING.md recipe).  NVML is polled every
+    """SM clock / throttle reasons during the timed region.  NVML is polled every
     few milliseconds (the timed region lasts tens of ms); nvidia-smi is the fallback."""
 
     REASONS = {0x8: "hw_slowdown", 0x40: "hw_thermal_slowdown", 0x20: "sw_thermal_slowdown", 0x4: "sw_power_cap"}
@@ -199,18 +205,26 @@ def measured_peaks():
             return json.load(open(p)), "measured"
         except Exception:
             pass
-    return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0}, "fallback"
+    return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0}, "fallback"   # H100 SXM data sheet (700 W), dense
 
 
-def measured_traffic(kernel, config, n_local):
-    """DRAM bytes per launch (dram__bytes_read.sum + dram__bytes_write.sum) of the dominant kernel from the committed
-    ncu --set full capture of this workload (profiles/traffic.json: {config: {kernel: {"cells": n, "bytes": b}}});
-    None when no capture of this kernel at this shard size has been committed."""
-    try:
-        t = json.load(open(os.path.join(ROOT, "profiles", "traffic.json")))[config][kernel]
-        return float(t["bytes"]) if int(t["cells"]) == int(n_local) else None
-    except Exception:
-        return None
+def dump_outputs(g, out_dir):
+    """Z_corr, R and Y after the last timed step, float32; cells: a fixed seeded sample (sorted) of the shard."""
+    Zc = g.getZcorr()   # d x n
+    R = g.getR()        # K x n
+    Y = g.getCentroids()  # d x K
+    n = Zc.shape[1]
+    cells = np.arange(n) if n <= DUMP_CELLS else np.sort(np.random.default_rng(7).choice(n, DUMP_CELLS, replace=False))
+    # the largest sample within the 64 MB bound (wider shapes than c3 / c4 need fewer cells)
+    per_cell = 4 * (Zc.shape[0] + R.shape[0]) + 8
+    if cells.size * per_cell + 4 * Y.size > 64 << 20:
+        cells = cells[np.sort(np.random.default_rng(8).choice(cells.size, ((64 << 20) - 4 * Y.size) // per_cell, replace=False))]
+    os.makedirs(out_dir, exist_ok=True)
+    np.save(os.path.join(out_dir, "Z_corr.npy"), np.ascontiguousarray(Zc[:, cells].T, dtype=np.float32))
+    np.save(os.path.join(out_dir, "R.npy"), np.ascontiguousarray(R[:, cells].T, dtype=np.float32))
+    np.save(os.path.join(out_dir, "Y.npy"), np.ascontiguousarray(Y.T, dtype=np.float32))
+    np.save(os.path.join(out_dir, "sample_cells.npy"), cells.astype(np.float64))
+    log(f"dump-outputs: {cells.size} of {n} cells -> {out_dir}")
 
 
 def cpu_sample_cells():
@@ -331,6 +345,8 @@ def main():
     ap.add_argument("--clock-period", type=float, default=0.003, help="seconds between NVML clock samples during the timed region")
     ap.add_argument("--kernel-set", type=int, default=0, help="HB_KERNEL_SET test hook of the library (A/B runs only)")
     ap.add_argument("--ref-cells", type=int, default=0, help="cells of the bounded CPU sample (--impl reference); 0 = by workload")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write Z_corr, R and Y of the last timed step (seeded cell sample) as DIR/<name>.npy")
     args = ap.parse_args()
     W.clear()
     W.update(WORKLOADS[args.config])
@@ -407,8 +423,8 @@ def main():
     for _ in range(max(3, args.warmup)):
         step(g)
     g.synchronize()
-    # Clocks under load.  NVML queries perturb sharded runs badly (measured on 2 x B200: a query every 3 ms inside the
-    # timed loop turns 2.9 ms per iteration into 5.0 — the ranks run in lockstep, every stall of one GPU is a stall of
+    # Clocks under load.  NVML queries perturb sharded runs badly (a query every few ms inside the
+    # timed loop stalls every rank — the ranks run in lockstep, every stall of one GPU is a stall of
     # all; a single GPU does not notice).  So the same steps run untimed once more under dense sampling (the load and
     # therefore the clocks are those of the timed region), and inside the timed region the sampler only looks a couple
     # of times (period = a third of the region's expected length).
@@ -444,6 +460,8 @@ def main():
         ms = float(tm.item())
     clocks = sampler.stop() if sampler else None
     ms_per_step = ms / args.steps
+    if args.dump_outputs and rank == 0:
+        dump_outputs(g, args.dump_outputs)
     value = N_global / (ms_per_step * 1e-3)
 
     # ---- per-kernel timing pass (region timers: CUDA events on the library stream, extra syncs) -> roofline
@@ -489,10 +507,7 @@ def main():
     roofline = None
     if kernels:
         top = max(kernels, key=lambda r: kernels[r]["share_of_step"])
-        # DRAM bytes of one launch of the dominant kernel from the ncu --set full capture of this exact
-        # workload (profiles/r01_final_kernels.md: dram__bytes_read.sum + dram__bytes_write.sum); null otherwise
-        traffic = measured_traffic(top, args.config, n_local)
-        roofline = dict(kernel=top, traffic=traffic, peak_kind=peak_kind, **kernels[top])
+        roofline = dict(kernel=top, peak_kind=peak_kind, **kernels[top])
     step_ach = ALGO_BYTES_PER_CELL_ITER * n_local / (ms_per_step * 1e-3) / 1e9
 
     # ---- e2e: public API with host buffers (pinned), H2D of inputs and D2H of the result in the timed region
@@ -547,7 +562,8 @@ def main():
                            "config_id": args.config,
                            "cells_per_gpu": n_local, "parallelism": f"cells sharded x{world}",
                            "switches": sorted(k for k in os.environ if k.startswith("HB_")) + ([f"kernel_set={args.kernel_set}"] if args.kernel_set else []),
-                           "l2": f"state (U,R,Z = {n_local * (2 * KS + 2 * DS) * 4 / 1e9:.1f} GB per GPU) is far larger than the 126 MB L2"},
+                           "l2": f"state (U,R,Z = {n_local * (2 * KS + 2 * DS) * 4 / 1e9:.1f} GB per GPU) against the "
+                                 f"{torch.cuda.get_device_properties(local_rank).L2_cache_size / 2**20:.0f} MB L2"},
                 "clocks": clocks, "e2e": e2e, "gpu_launches": int(launches),
                 "roofline": roofline,
                 "roofline_kernels": {r: {k2: (round(v2, 4) if isinstance(v2, float) else v2) for k2, v2 in kv.items()}

@@ -1,4 +1,4 @@
-"""harmony_b200 — B200-native (sm_100a) implementation of the Harmony hot loop.
+"""harmony_b200 — H100-native (sm_90a) implementation of the Harmony hot loop.
 
 Host side mirrors the reference's R surface (RunHarmony / harmonize / the ``harmony`` module
 class); all arithmetic on cell matrices runs in hand-written CUDA behind include/harmony_b200.h.

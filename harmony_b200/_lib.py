@@ -2,7 +2,7 @@
 
 There is no CPU fallback: if the shared library is missing or no CUDA device is present the
 constructors raise.  The library is built IN-TREE (harmony_b200/libharmony_b200.so) with
-``nvcc -gencode arch=compute_100a,code=sm_100a`` by ``build()`` / ``__graft_entry__.build()``.
+``nvcc -gencode arch=compute_90a,code=sm_90a`` (H100) by ``build()`` / ``__graft_entry__.build()``.
 """
 import ctypes
 import os
@@ -14,7 +14,7 @@ SO_PATH = os.path.join(_HERE, "libharmony_b200.so")
 SOURCES = [os.path.join(_HERE, "csrc", f) for f in ("harmony_b200.cu", "kernels.cuh", "common.cuh", "update_kernel.cuh", "update_kernel4.cuh", "update_kernel5.cuh",
                                                      "umma.cuh", "assign_tc3.cuh", "logits_tc.cuh", "stats_tc3.cuh", "apply_tc3.cuh")]
 HEADER = os.path.join(ROOT, "include", "harmony_b200.h")
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17", "-shared",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17", "-shared",
               "-Xcompiler", "-fPIC"]
 
 _LIB = None
@@ -28,7 +28,7 @@ def needs_build():
 
 
 def build(force=False, verbose=False):
-    """Compile the CUDA library for sm_100a (cross-compiles without a GPU)."""
+    """Compile the CUDA library for sm_90a (cross-compiles without a GPU)."""
     if not force and not needs_build():
         return SO_PATH
     nvcc = os.environ.get("NVCC", "nvcc")

@@ -1,33 +1,29 @@
 // apply_tc3.cuh — K5 on the tensor cores: the correction of harmony.cpp:347 + :615 for all clusters at once,
 //   Zc_i = Zo_i - sum_k R_ik V_q[k][:]        (q = covariate tuple of cell i, V_q from k_ridge_solve)
 // computed transposed so that the per-tile operand is the small one:
-//   D'[c][cell] = sum_k A[c][k] * B[cell][k],   A = V_q^T (static while the tuple does not change, M = 128 rows of
-//   which d are used),  B = a 64-cell tile of R (N = 64),  3xTF32, fp32 accumulators in TMEM.
-// Second generation.  The first one (bulk-copied raw tiles -> converter warps -> ONE converted operand stage)
-// spent 5.4 us per tile on a chain load -> convert -> MMA -> convert ... with a single tile in flight.  Here, as in
-// assign_tc3.cuh:
+//   D'[c][cell] = sum_k A[c][k] * B[cell][k],   A = V_q^T (static while the tuple does not change, M = 64 rows per
+//   wgmma, one or two halves for d <= 64 / d <= 128),  B = a 64-cell tile of R (N = 64),  3xTF32, fp32 accumulators
+//   in registers.
 //   * a loader thread owns half a row of the tile: it copies its 16-byte pieces with cp.async straight into the
 //     canonical K-major operand layout (the raw fp32 tile IS the `hi` operand: the tensor core reads the upper 19
 //     bits), waits for its OWN copies (cp.async.wait_group, no mbarrier between loading and converting), and writes
-//     the `lo` pieces; two operand stages, so the rows of tile t + 1 land while tile t is multiplied and stored;
-//   * A = V_q^T is rebuilt by the same threads when the tuple changes (after the previous tile's MMAs);
-//   * epilogue as before: TMEM lane = embedding column c, Zc[cell][c] = Zo[cell][c] - D'[c][cell], coalesced
-//     across the warp; one warp pair per accumulator, tile records fetched one tile ahead.
-// Warp roles (576 threads): 0 MMA issuer; 2, 3, 6, 7 loaders / converters; epilogue warps serve TMEM lane quarter
-// warp % 4 (= 32 embedding columns) of one accumulator, for d <= 64 split further into two cell halves (eight warps).  Limits per launch: d <= 128 and
-// <= 112 clusters (shared memory); more clusters run as several launches over cluster ranges, each subtracting its
-// share from the partial result (the first from Zo).
+//     the `lo` pieces; two or three operand stages, so the rows of tile t + 1 land while tile t is multiplied;
+//   * A = V_q^T is rebuilt by the same threads when the tuple changes (after the MMAs of the previous tiles);
+//   * two MMA warpgroups take alternate tiles and subtract their accumulators straight from registers
+//     (Zc[cell][c] = minuend[cell][c] - D'[c][cell], 32-byte pieces of a row per quad of lanes): the MMAs of one
+//     tile overlap the stores of the other.
+// Warp roles (384 threads): 0-3 loaders / converters; 4-7 MMA warpgroup of the even tiles, 8-11 of the odd tiles.
+// Limits per launch: d <= 128 and <= 112 clusters (shared memory); more clusters run as several launches over
+// cluster ranges, each subtracting its share from the partial result (the first from Zo).
 #pragma once
-#include <type_traits>
-
 #include "common.cuh"
 #include "umma.cuh"
 
 namespace hb {
 
-constexpr int AP_TN = 64;         // cells per tile (= UMMA N), equals the static tile size TM
-constexpr int AP_THREADS = 576;   // 18 warps
-constexpr int AP_LOAD = 128;      // loader / converter threads (warps 2, 3, 6, 7)
+constexpr int AP_TN = 64;         // cells per tile (= wgmma N), equals the static tile size TM
+constexpr int AP_THREADS = 384;   // 12 warps
+constexpr int AP_LOAD = 128;      // loader / converter threads (warps 0-3)
 constexpr int AP_MAXK = 112;      // clusters per launch: (2 x 128 + 4 x 64) x KD floats of operands must fit 227 KB
 
 struct ApplyTcArgs {
@@ -45,9 +41,8 @@ struct ApplyTcArgs {
   long long* dbg;
 };
 
-// A = V_q^T is stored with AROWS = 64 rows per 16-byte K chunk when d <= 64 (descriptor LBO = 64 x 16 bytes): the MMA
-// still reads M = 128 rows, rows 64-127 alias the next chunk and land in accumulator lanes nobody reads.  The freed
-// 53 KB buy a third operand stage.
+// A = V_q^T is stored with AROWS = 64 rows per 16-byte K chunk when d <= 64 (one wgmma M = 64 half; descriptor
+// LBO = 64 x 16 bytes), 128 rows (two halves) otherwise.  The freed 53 KB buy a third operand stage.
 __host__ __device__ inline int apply_tc_arows(int d) { return d <= 64 ? 64 : 128; }
 __host__ __device__ inline size_t apply_tc_smem_bytes_n(int KD, int d, int nst) {
   // A hi/lo: 2 x AROWS x KD (+ one chunk plane of slack for the aliased rows of the last chunk); B hi/lo: nst x 2 x 64 x KD
@@ -58,10 +53,12 @@ __host__ __device__ inline int apply_tc_stages(int KD, int d) {
 }
 __host__ __device__ inline size_t apply_tc_smem_bytes(int KD, int d) { return apply_tc_smem_bytes_n(KD, d, apply_tc_stages(KD, d)); }
 
+// NH: 64-row halves of A = embedding columns (1: d <= 64, 2: d <= 128), fixed at compile time so that the
+// accumulators and minuends stay in registers
+template <int NH>
 __global__ void __launch_bounds__(AP_THREADS, 1) k_apply_tc(ApplyTcArgs a) {
   extern __shared__ __align__(128) unsigned char smem_raw[];
   const int KD = a.KD, K = a.K, d = a.d, KS = a.KS, DS = a.DS, Kp = a.Kp;
-  const int nq = (d + 31) >> 5;  // TMEM lane quarters in use (embedding columns / 32)
   const int AR = apply_tc_arows(d);       // rows of A per K chunk
   const int NST = apply_tc_stages(KD, d);  // operand stages of B
   const int BST = AP_TN * KD;              // floats per B tile
@@ -71,10 +68,7 @@ __global__ void __launch_bounds__(AP_THREADS, 1) k_apply_tc(ApplyTcArgs a) {
   float* Blo = Bhi + (size_t)NST * BST;              // [NST][KD/4][64][4]
   uint64_t* bars = reinterpret_cast<uint64_t*>(Blo + (size_t)NST * BST);
   uint64_t* lo_full = bars + 0;    // [3]  loaders (128): operands of the stage complete
-  uint64_t* st_empty = bars + 3;   // [3]  tcgen05.commit: operands consumed
-  uint64_t* t_full = bars + 6;     // [2]  tcgen05.commit: accumulator ready
-  uint64_t* t_empty = bars + 8;    // [2]  epilogue warps (32 per lane quarter in use): accumulator drained
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 10);
+  uint64_t* st_empty = bars + 3;   // [3]  MMA warpgroup (128): operands consumed
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int R4 = ((KS - a.k_off < KD ? KS - a.k_off : KD)) >> 2;   // 16-byte chunks of this launch's cluster range in a row of R
 
@@ -83,20 +77,11 @@ __global__ void __launch_bounds__(AP_THREADS, 1) k_apply_tc(ApplyTcArgs a) {
   if (tid == 0) {
     for (int i = 0; i < 3; ++i) {
       umma::mbar_init(lo_full + i, AP_LOAD);
-      umma::mbar_init(st_empty + i, 1);
-    }
-    for (int i = 0; i < 2; ++i) {
-      umma::mbar_init(t_full + i, 1);
-      umma::mbar_init(t_empty + i, 32 * nq * (nq <= 2 ? 2 : 1));
+      umma::mbar_init(st_empty + i, 128);
     }
     umma::fence_barrier_init();
   }
-  if (warp == 0) umma::tmem_alloc(tmem_slot, 128);  // two 64-column accumulators
-  umma::fence_proxy_async();
-  umma::fence_before_sync();
   __syncthreads();
-  umma::fence_after_sync();
-  const uint32_t tmem = *tmem_slot;
 
   const int t_begin = blockIdx.x * a.tiles_per_cta;
   const int t_end = (t_begin + a.tiles_per_cta < a.ntiles) ? t_begin + a.tiles_per_cta : a.ntiles;
@@ -108,41 +93,9 @@ __global__ void __launch_bounds__(AP_THREADS, 1) k_apply_tc(ApplyTcArgs a) {
     }
   };
 
-  if (warp == 0) {
-    // =============================== MMA issuer (one thread) ===============================
-    if (lane == 0) {
-      const uint32_t idesc = umma::make_idesc_tf32(128, AP_TN, 0, 0);
-      const uint32_t lboA = (uint32_t)AR * 16, lboB = AP_TN * 16, sbo = 128;
-      const uint32_t aH = umma::smem_u32(Ahi), aL = umma::smem_u32(Alo);
-      int it = 0;
-      for (int tile = t_begin; tile < t_end; ++tile, ++it) {
-        const int s = it % NST, acc = it & 1;
-        umma::mbar_wait(lo_full + s, (it / NST) & 1);
-        stamp(it, 5);
-        if (it >= 2) umma::mbar_wait(t_empty + acc, ((it >> 1) - 1) & 1);
-        stamp(it, 6);
-        umma::fence_after_sync();
-        const uint32_t bH = umma::smem_u32(Bhi + (size_t)s * BST), bL = umma::smem_u32(Blo + (size_t)s * BST);
-        const uint32_t dt = tmem + acc * AP_TN;
-        uint32_t accum = 0;
-        for (int ks = 0; ks < KD / 8; ++ks) {
-          const uint64_t ah = umma::make_desc(aH + ks * 2 * lboA, lboA, sbo);
-          const uint64_t al = umma::make_desc(aL + ks * 2 * lboA, lboA, sbo);
-          const uint64_t bh = umma::make_desc(bH + ks * 2 * lboB, lboB, sbo);
-          const uint64_t bl = umma::make_desc(bL + ks * 2 * lboB, lboB, sbo);
-          umma::mma_tf32(dt, al, bh, idesc, accum);
-          umma::mma_tf32(dt, ah, bl, idesc, 1);
-          umma::mma_tf32(dt, ah, bh, idesc, 1);
-          accum = 1;
-        }
-        umma::mma_commit(st_empty + s);
-        umma::mma_commit(t_full + acc);
-        stamp(it, 7);
-      }
-    }
-  } else if (warp == 2 || warp == 3 || warp == 6 || warp == 7) {
+  if (warp < 4) {
     // =============================== loaders / converters ===============================
-    const int lt = (warp < 4 ? warp - 2 : warp - 4) * 32 + lane;   // 0..127
+    const int lt = tid;                  // 0..127
     const int cell = lt & (AP_TN - 1);   // row of the tile
     const int half = lt >> 6;            // which half of the row's 16-byte pieces
     const int hsplit = (R4 + 1) >> 1;
@@ -167,6 +120,7 @@ __global__ void __launch_bounds__(AP_THREADS, 1) k_apply_tc(ApplyTcArgs a) {
       }
       asm volatile("cp.async.commit_group;" ::: "memory");
     };
+    auto wait_mma = [&](int t) { umma::mbar_wait(st_empty + (t % NST), (t / NST) & 1); };  // MMAs of tile t are done
     // tile records run NST tiles ahead of the conversion: m[j] = record of tile it + j
     int mc[4], ml[4], mq[4];
 #pragma unroll
@@ -184,8 +138,10 @@ __global__ void __launch_bounds__(AP_THREADS, 1) k_apply_tc(ApplyTcArgs a) {
         asm volatile("cp.async.wait_group 0;" ::: "memory");
       if (lt == 0) stamp(it, 1);
       if (mq[0] != cur_q) {
-        // new tuple: A = V_q^T (k contiguous per embedding column c), tf32 hi/lo — after the previous tile's MMAs
-        if (it >= 1) umma::mbar_wait(st_empty + ((it - 1) % NST), ((it - 1) / NST) & 1);
+        // new tuple: A = V_q^T (k contiguous per embedding column c), tf32 hi/lo — after the MMAs of the previous
+        // tiles (the two warpgroups finish theirs in either order)
+        if (it >= 1) wait_mma(it - 1);
+        if (it >= 2) wait_mma(it - 2);
         const float* Vq = a.V + ((size_t)mq[0] * K + a.k_off) * d;
         for (int idx = lt; idx < AR * KD; idx += AP_LOAD) {
           const int k = idx / AR, c = idx - k * AR;
@@ -220,7 +176,7 @@ __global__ void __launch_bounds__(AP_THREADS, 1) k_apply_tc(ApplyTcArgs a) {
       umma::mbar_arrive(lo_full + s);
       if (lt == 0) stamp(it, 2);
       // tile it + NST - 1 goes into the stage tile it - 1 used: after that tile's MMAs
-      if (tile + NST - 1 < t_end && it >= 1) umma::mbar_wait(st_empty + ((it - 1) % NST), ((it - 1) / NST) & 1);
+      if (tile + NST - 1 < t_end && it >= 1) wait_mma(it - 1);
       issue_row(it + NST - 1, NST == 3 ? mc[2] : mc[1], NST == 3 ? ml[2] : ml[1]);
       if (lt == 0) stamp(it, 3);
 #pragma unroll
@@ -233,89 +189,57 @@ __global__ void __launch_bounds__(AP_THREADS, 1) k_apply_tc(ApplyTcArgs a) {
     }
     asm volatile("cp.async.wait_all;" ::: "memory");
   } else {
-    // =============================== epilogue ===============================
-    // A warp may only touch TMEM lane quarter warp % 4 (= 32 embedding columns).  d <= 64: four warps per accumulator,
-    // lane quarter x cell half (warps 4,5 / 12,13 -> accumulator 0, warps 8,9 / 16,17 -> accumulator 1); d > 64: one
-    // warp per accumulator and lane quarter (4,5,10,11 / 8,9,14,15), all 64 cells.
-    const int wq = warp & 3;  // TMEM lane quarter (hardware: warp % 4)
-    const bool split = nq <= 2;
-    int es = -1, half = 0;
-    if (split) {
-      if (warp == 4 || warp == 5) es = 0, half = 0;
-      else if (warp == 12 || warp == 13) es = 0, half = 1;
-      else if (warp == 8 || warp == 9) es = 1, half = 0;
-      else if (warp == 16 || warp == 17) es = 1, half = 1;
-    } else {
-      if (warp == 4 || warp == 5 || warp == 10 || warp == 11) es = 0;
-      else if (warp == 8 || warp == 9 || warp == 14 || warp == 15) es = 1;
-    }
-    if (es >= 0 && wq < nq) {
-      const int c = wq * 32 + lane;  // embedding column = TMEM lane
-      auto run = [&](auto nc_tag) {
-        constexpr int NC = decltype(nc_tag)::value;  // cells per warp and tile
-        const int j0 = half * NC;
-        int use = 0;
-        int cell0_n = 0, len_n = 0;
-        if (t_begin + es < t_end) {
-          cell0_n = __ldg(a.tile_cell0 + t_begin + es);
-          len_n = __ldg(a.tile_len + t_begin + es);
+    // =============================== MMA warpgroups + epilogue ===============================
+    const int e = (warp >> 2) - 1;   // tiles t_begin + e, + e + 2, ..
+    const int w = warp & 3;          // warp of the warpgroup
+    const uint32_t lboA = (uint32_t)AR * 16, lboB = AP_TN * 16, sbo = 128;
+    const uint32_t aH = umma::smem_u32(Ahi), aL = umma::smem_u32(Alo);
+    for (int tile = t_begin + e; tile < t_end; tile += 2) {
+      const int it = tile - t_begin, s = it % NST;
+      const int cell0 = __ldg(a.tile_cell0 + tile), len = __ldg(a.tile_len + tile);
+      // the minuend of this thread's accumulator elements travels while the operands are prepared and multiplied
+      float zo[NH][32];
+#pragma unroll
+      for (int g = 0; g < NH; ++g)
+#pragma unroll
+        for (int i = 0; i < 32; ++i) {
+          const int c = 64 * g + umma::frag_row(i, w, lane), j = umma::frag_col(i, lane);
+          zo[g][i] = (c < d && j < len) ? ld_stream(a.minuend + (size_t)(cell0 + j) * DS + c) : 0.f;
         }
-        for (int tile = t_begin + es; tile < t_end; tile += 2, ++use) {
-          const int cell0 = cell0_n, len = len_n;
-          if (tile + 2 < t_end) {
-            cell0_n = __ldg(a.tile_cell0 + tile + 2);
-            len_n = __ldg(a.tile_len + tile + 2);
+      umma::mbar_wait(lo_full + s, (it / NST) & 1);
+      if (lane == 0 && w == 0) stamp(it, 5);
+      float acc[NH][32];  // overwritten by the first MMA of each half (accumulate = 0)
+      const uint32_t bH = umma::smem_u32(Bhi + (size_t)s * BST), bL = umma::smem_u32(Blo + (size_t)s * BST);
+      umma::fence();
+#pragma unroll
+      for (int g = 0; g < NH; ++g) {
+        {
+          for (int ks = 0; ks < KD / 8; ++ks) {
+            const uint32_t ao = ks * 2 * lboA + g * 64 * 16, bo = ks * 2 * lboB;
+            const uint64_t ah = umma::make_desc(aH + ao, lboA, sbo);
+            const uint64_t al = umma::make_desc(aL + ao, lboA, sbo);
+            const uint64_t bh = umma::make_desc(bH + bo, lboB, sbo);
+            const uint64_t bl = umma::make_desc(bL + bo, lboB, sbo);
+            umma::mma_n64(acc[g], al, bh, ks > 0);
+            umma::mma_n64(acc[g], ah, bl, 1);
+            umma::mma_n64(acc[g], ah, bh, 1);
           }
-          // NC = 32: the tile's minuend values are fetched while the MMAs run and both TMEM loads of the warp's cells
-          // are in flight together; NC = 64 (d > 64): 16 cells at a time (registers)
-          constexpr int CH = (NC == 32) ? 32 : 16;
-          float zo[CH];
-          auto fetch = [&](int j) {
-            if (c < d) {
-#pragma unroll
-              for (int i = 0; i < CH; ++i)
-                zo[i] = (j0 + j + i < len) ? ld_stream(a.minuend + (size_t)(cell0 + j0 + j + i) * DS + c) : 0.f;
-            }
-          };
-          if (NC == CH) fetch(0);
-          umma::mbar_wait(t_full + es, use & 1);
-          umma::fence_after_sync();
-          if (lane == 0 && wq == 0 && half == 0) stamp(2 * use + es, 8);
-          const uint32_t trow = tmem + es * AP_TN + j0 + ((uint32_t)(wq * 32) << 16);
-#pragma unroll
-          for (int j = 0; j < NC; j += CH) {
-            if (NC != CH) fetch(j);
-            float tv[CH];
-#pragma unroll
-            for (int u = 0; u < CH; u += 16) {
-              float t16[16];
-              umma::tmem_ld16(trow + j + u, t16);
-#pragma unroll
-              for (int i = 0; i < 16; ++i) tv[u + i] = t16[i];
-            }
-            umma::tmem_ld_wait();
-            if (j + CH == NC) {  // this warp's part of the accumulator is read -> the issuer may overwrite it
-              umma::fence_before_sync();
-              umma::mbar_arrive(t_empty + es);
-            }
-            if (c < d) {
-#pragma unroll
-              for (int i = 0; i < CH; ++i)
-                if (j0 + j + i < len) a.Zc[(size_t)(cell0 + j0 + j + i) * DS + c] = zo[i] - tv[i];
-            }
-          }
-          if (lane == 0 && wq == 0 && half == 0) stamp(2 * use + es, 9);
         }
-      };
-      if (split)
-        run(std::integral_constant<int, 32>());
-      else
-        run(std::integral_constant<int, 64>());
+      }
+      umma::commit();
+      umma::wait0();
+      umma::mbar_arrive(st_empty + s);  // operands consumed -> the loaders may refill the stage
+      if (lane == 0 && w == 0) stamp(it, 7);
+#pragma unroll
+      for (int g = 0; g < NH; ++g)
+#pragma unroll
+        for (int i = 0; i < 32; ++i) {
+          const int c = 64 * g + umma::frag_row(i, w, lane), j = umma::frag_col(i, lane);
+          if (c < d && j < len) a.Zc[(size_t)(cell0 + j) * DS + c] = zo[g][i] - acc[g][i];
+        }
+      if (lane == 0 && w == 0) stamp(it, 9);
     }
   }
-  umma::fence_before_sync();
-  __syncthreads();
-  if (warp == 0) umma::tmem_dealloc(tmem, 128);
 }
 
 }  // namespace hb

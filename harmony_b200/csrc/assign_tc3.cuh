@@ -1,10 +1,10 @@
 // assign_tc3.cuh — K1, the assignment step of harmony.cpp:141-150 (init) / :220-227 (cold start), third generation:
 //   cos = z . y_k / |z|,  dist = 2 (1 - cos),  U = -dist / sigma,  R = softmax_k(U),  column sums of R per level
-// for tiles of 128 cells, the K x d contraction as tcgen05.mma.kind::tf32 in 3xTF32 form, fp32 accumulators in TMEM.
+// for tiles of 128 cells, the K x d contraction as wgmma (tf32) in 3xTF32 form, fp32 accumulators in registers.
 //
 // What changed against k_assign_tc / k_assign_tc2 (both deleted):
 //   * the rows of a tile are GATHERED (an index per row) with 16-byte cp.async straight into the canonical K-major
-//     UMMA operand layout: the raw fp32 tile IS the `hi` operand (the tensor core reads the upper 19 bits of every
+//     wgmma operand layout: the raw fp32 tile IS the `hi` operand (the tensor core reads the upper 19 bits of every
 //     word), CUDA cores only produce the `lo` tile (z - trunc_tf32(z), rounded to tf32) and the row norms; the
 //     L2 normalisation moves behind the contraction (cos = (z . y) / |z|), so nothing is normalised, split or
 //     written back before the MMAs can start.
@@ -16,8 +16,11 @@
 //   * U rows leave through a shared-memory stage and coalesced row stores (a thread-per-row store of 16-byte pieces
 //     costs 32 LSU wavefronts per instruction: 3200 per tile and matrix); exp() is evaluated once per element,
 //     the column sums come out of registers through a shuffle butterfly.
-// Warp roles (448 threads): 0 gather producer, 1 MMA issuer, 2-5 `lo` converters (row per thread), 6-13 epilogue
-// (TMEM lane quarter x column half).  Two operand stages, two TMEM accumulators.
+// Warp roles (384 threads): 0-3 row gather + `lo` converters (row per thread), then the MMA warpgroup (two 64-row
+// halves, m64n32k8 per 32 clusters + m64n16k8 for a 16-cluster tail), which leaves the accumulator columns < KS in
+// the U stage (padding clusters have zero centroids: their dot products are 0); 4-11 epilogue (row quarter x
+// column half).  Two operand stages: the rows of tile t + 1 land while tile t is multiplied; the epilogue of tile t
+// overlaps the conversion and the MMAs of tile t + 1.
 // Limits: K <= 128 (NP), d <= 64 (KD); other shapes run the FFMA kernel k_assign.
 #pragma once
 #include "common.cuh"
@@ -25,8 +28,8 @@
 
 namespace hb {
 
-constexpr int TC_TM = 128;        // cells per tile (= UMMA M)
-constexpr int A3_THREADS = 448;
+constexpr int TC_TM = 128;        // cells per tile (two wgmma M = 64 halves)
+constexpr int A3_THREADS = 384;
 constexpr int A3_NS = 2;          // operand stages (1 when two do not fit shared memory)
 constexpr int A3_RING_N = 4;      // row-norm ring (tiles): written by the converters, read at the start of the epilogue
 constexpr int A3_RING_C = 8;      // row -> cell ring (tiles): written by the producer, read until the rows have left
@@ -76,7 +79,7 @@ __global__ void __launch_bounds__(A3_THREADS, 1) k_assign_tc3(Assign3Args a) {
   float* Alo = Ahi + (size_t)NS * TC_TM * KD;                    // [NS][KD/4][128][4]
   float* Bhi = Alo + (size_t)NS * TC_TM * KD;                    // [KD/4][NP][4]
   float* Blo = Bhi + (size_t)NP * KD;
-  float* Ust = Blo + (size_t)NP * KD;                            // [128][SS]
+  float* Ust = Blo + (size_t)NP * KD;                            // [128][SS]  accumulator, then U
   float* ca = Ust + (size_t)TC_TM * SS;                          // [NP]  2 / sigma          (1e30 in padding columns)
   float* ca2 = ca + NP;                                          // [NP]  2 log2(e) / sigma
   float* sig = ca2 + NP;                                         // [NP]
@@ -85,12 +88,8 @@ __global__ void __launch_bounds__(A3_THREADS, 1) k_assign_tc3(Assign3Args a) {
   float* rs_part = reinterpret_cast<float*>(rowcell + (size_t)A3_RING_C * TC_TM);  // [2][128]
   float* cs_part = rs_part + 2 * TC_TM;                          // [4][NP]
   uint64_t* bars = reinterpret_cast<uint64_t*>(cs_part + 4 * (size_t)NP);
-  uint64_t* raw_full = bars;                      // [2]  gather landed (32 cp.async arrivals + 1)
-  uint64_t* lo_full = raw_full + 2;               // [2]  converters (128)
-  uint64_t* st_empty = lo_full + 2;               // [2]  tcgen05.commit: operands consumed
-  uint64_t* t_full = st_empty + 2;                // [2]  tcgen05.commit: accumulator ready
-  uint64_t* t_empty = t_full + 2;                 // [2]   epilogue (256): accumulator drained
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(t_empty + 2);
+  uint64_t* t_full = bars;                        // MMA warpgroup (128): accumulator in the U stage
+  uint64_t* t_empty = bars + 1;                   // epilogue (256): U stage drained
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   constexpr float L2E = 1.4426950408889634f;
@@ -114,23 +113,11 @@ __global__ void __launch_bounds__(A3_THREADS, 1) k_assign_tc3(Assign3Args a) {
   // the hi stages: padding chunks (columns >= DS) and rows beyond short tiles must hold finite values
   for (int i = tid; i < NS * TC_TM * KD; i += A3_THREADS) Ahi[i] = 0.f;
   if (tid == 0) {
-    for (int i = 0; i < 2; ++i) {
-      umma::mbar_init(raw_full + i, 1);  // (unused)
-      umma::mbar_init(lo_full + i, 128);
-      umma::mbar_init(st_empty + i, 1);
-    }
-    for (int i = 0; i < 2; ++i) {
-      umma::mbar_init(t_full + i, 1);
-      umma::mbar_init(t_empty + i, 256);
-    }
+    umma::mbar_init(t_full, 128);
+    umma::mbar_init(t_empty, 256);
     umma::fence_barrier_init();
   }
-  if (warp == 1) umma::tmem_alloc(tmem_slot, 256);  // two 128-column accumulators
-  umma::fence_proxy_async();
-  umma::fence_before_sync();
   __syncthreads();
-  umma::fence_after_sync();
-  const uint32_t tmem = *tmem_slot;
 
   const int my_first = blockIdx.x, stride = gridDim.x;
   if (a.ntiles_ptr) a.ntiles = __ldg(a.ntiles_ptr);
@@ -142,49 +129,19 @@ __global__ void __launch_bounds__(A3_THREADS, 1) k_assign_tc3(Assign3Args a) {
     }
   };
 
-  if (warp == 0) {
-    // (spare warp: the row gather is done by the converter threads, one row each)
-  } else if (warp == 1) {
-    // =============================== MMA issuer ===============================
-    if (lane == 0) {
-      const uint32_t idesc = umma::make_idesc_tf32(TC_TM, NP, 0, 0);
-      const uint32_t lboA = TC_TM * 16, lboB = NP * 16, sbo = 128;
-      const uint32_t bH = umma::smem_u32(Bhi), bL = umma::smem_u32(Blo);
-      int it = 0;
-      for (int tile = my_first; tile < a.ntiles; tile += stride, ++it) {
-        const int s = it % NS, acc = it & 1;
-        umma::mbar_wait(lo_full + s, (it / NS) & 1);
-        stamp(it, 5);
-        if (it >= 2) umma::mbar_wait(t_empty + acc, ((it >> 1) - 1) & 1);
-        stamp(it, 6);
-        umma::fence_after_sync();
-        const uint32_t aH = umma::smem_u32(Ahi + (size_t)s * TC_TM * KD);
-        const uint32_t aL = umma::smem_u32(Alo + (size_t)s * TC_TM * KD);
-        const uint32_t dt = tmem + acc * 128;
-        uint32_t accum = 0;
-        for (int ks = 0; ks < KD / 8; ++ks) {
-          const uint64_t ah = umma::make_desc(aH + ks * 2 * lboA, lboA, sbo);
-          const uint64_t al = umma::make_desc(aL + ks * 2 * lboA, lboA, sbo);
-          const uint64_t bh = umma::make_desc(bH + ks * 2 * lboB, lboB, sbo);
-          const uint64_t bl = umma::make_desc(bL + ks * 2 * lboB, lboB, sbo);
-          umma::mma_tf32(dt, al, bh, idesc, accum);
-          umma::mma_tf32(dt, ah, bl, idesc, 1);
-          umma::mma_tf32(dt, ah, bh, idesc, 1);
-          accum = 1;
-        }
-        umma::mma_commit(st_empty + s);   // operands consumed -> the producer may refill the stage
-        umma::mma_commit(t_full + acc);   // accumulator ready
-        stamp(it, 7);
-      }
-    }
-  } else if (warp < 6) {
-    // =============================== row loaders + converters (one row of the tile per thread) ===============================
+  if (warp < 4) {
+    // ============== row loaders + converters (one row of the tile per thread), then the MMA warpgroup ==============
     // Thread r copies ITS row of the next tile with 16-byte cp.async straight into the canonical K-major operand
     // layout (consecutive lanes -> consecutive 16-byte slots of a chunk plane: conflict-free; one warp-wide gather
     // instruction with scattered destinations costs ~290 cycles of a single producer warp, measured), waits for its
     // own copies of the current tile (cp.async.wait_group: no mbarrier between loading and converting), produces the
-    // `lo` operand and the row norm, and hands the stage to the MMA issuer.  Plan entries run two tiles ahead.
-    const int r = tid - 64;  // row of the tile
+    // `lo` operand and the row norm; after a warpgroup barrier the same threads multiply the stage.  Plan entries run
+    // two tiles ahead.
+    const int r = tid;  // row of the tile
+    const int nfull = NP >> 5;          // 32-cluster chunks (wgmma N = 32)
+    const bool tail = (NP & 16) != 0;   // one 16-cluster chunk after them (wgmma N = 16)
+    const uint32_t lboA = TC_TM * 16, lboB = NP * 16, sbo = 128;
+    const uint32_t bH = umma::smem_u32(Bhi), bL = umma::smem_u32(Blo);
     auto tile_of = [&](int it) { return my_first + it * stride; };
     auto ld_meta = [&](int it, int& p0, int& len) {
       const int tile = tile_of(it);
@@ -216,9 +173,9 @@ __global__ void __launch_bounds__(A3_THREADS, 1) k_assign_tc3(Assign3Args a) {
     for (int tile = my_first; tile < a.ntiles; tile += stride, ++it) {
       const int s = it % NS;
       if (r == 0) stamp(it, 0);
-      // next tile -> the other stage (with one stage: after this tile's MMAs, below)
+      // next tile -> the other stage (with one stage: after this tile's MMAs, below); the MMAs of tile it - 1, which
+      // used that stage, are complete (this warpgroup waited for them)
       if (NS == 2) {
-        if (it >= 1 && tile + stride < a.ntiles) umma::mbar_wait(st_empty + ((it + 1) & 1), ((it - 1) >> 1) & 1);  // MMAs of tile it - 1
         if (r == 0) stamp(it, 1);
         issue_row(it + 1, cell1);
         if (r == 0) stamp(it, 2);
@@ -268,12 +225,65 @@ __global__ void __launch_bounds__(A3_THREADS, 1) k_assign_tc3(Assign3Args a) {
         }
       }
       umma::fence_proxy_async();  // this thread's cp.async rows (observed above) and `lo` writes -> tensor core
-      umma::mbar_arrive(lo_full + s);
+      umma::named_sync(2, 128);
       if (r == 0) stamp(it, 4);
-      if (NS == 1) {  // single stage: the next tile's rows can only land once this tile's MMAs are done
-        if (tile + stride < a.ntiles) umma::mbar_wait(st_empty, it & 1);
-        issue_row(it + 1, cell1);
+      {
+        const uint32_t aH = umma::smem_u32(Ahi + (size_t)s * TC_TM * KD);
+        const uint32_t aL = umma::smem_u32(Alo + (size_t)s * TC_TM * KD);
+        for (int g = 0; g < 2; ++g) {  // rows 64 g .. 64 g + 63 of the tile
+          float acc[4][16], tl[8];  // overwritten by the first MMA of each chunk (accumulate = 0)
+          umma::fence();
+          for (int ks = 0; ks < KD / 8; ++ks) {
+            const uint32_t ao = ks * 2 * lboA + g * 64 * 16;
+            const uint64_t ah = umma::make_desc(aH + ao, lboA, sbo);
+            const uint64_t al = umma::make_desc(aL + ao, lboA, sbo);
+#pragma unroll
+            for (int j = 0; j < 4; ++j) {
+              if (j < nfull) {
+                const uint32_t bo = ks * 2 * lboB + j * 32 * 16;
+                const uint64_t bh = umma::make_desc(bH + bo, lboB, sbo);
+                const uint64_t bl = umma::make_desc(bL + bo, lboB, sbo);
+                umma::mma_n32(acc[j], al, bh, ks > 0);
+                umma::mma_n32(acc[j], ah, bl, 1);
+                umma::mma_n32(acc[j], ah, bh, 1);
+              }
+            }
+            if (tail) {
+              const uint32_t bo = ks * 2 * lboB + nfull * 32 * 16;
+              const uint64_t bh = umma::make_desc(bH + bo, lboB, sbo);
+              const uint64_t bl = umma::make_desc(bL + bo, lboB, sbo);
+              umma::mma_n16(tl, al, bh, ks > 0);
+              umma::mma_n16(tl, ah, bl, 1);
+              umma::mma_n16(tl, ah, bh, 1);
+            }
+          }
+          umma::commit();
+          umma::wait0();
+          if (r == 0 && g == 0) stamp(it, 5);
+          if (g == 0 && it >= 1) umma::mbar_wait(t_empty, (it - 1) & 1);  // the epilogue is done with the previous tile
+          if (r == 0 && g == 0) stamp(it, 6);
+#pragma unroll
+          for (int j = 0; j < 4; ++j) {
+            if (j < nfull) {
+#pragma unroll
+              for (int i = 0; i < 16; i += 2) {
+                const int row = 64 * g + umma::frag_row(i, warp, lane), col = 32 * j + umma::frag_col(i, lane);
+                if (col < KS) *reinterpret_cast<float2*>(Ust + (size_t)row * SS + col) = make_float2(acc[j][i], acc[j][i + 1]);
+              }
+            }
+          }
+          if (tail) {
+#pragma unroll
+            for (int i = 0; i < 8; i += 2) {
+              const int row = 64 * g + umma::frag_row(i, warp, lane), col = 32 * nfull + umma::frag_col(i, lane);
+              if (col < KS) *reinterpret_cast<float2*>(Ust + (size_t)row * SS + col) = make_float2(tl[i], tl[i + 1]);
+            }
+          }
+        }
       }
+      umma::mbar_arrive(t_full);
+      if (r == 0) stamp(it, 7);
+      if (NS == 1) issue_row(it + 1, cell1);  // single stage: the next tile's rows land once this tile's MMAs are done
       cell0 = cell1;
       cell1 = cell2;
       p0_2 = p0_3;
@@ -282,13 +292,13 @@ __global__ void __launch_bounds__(A3_THREADS, 1) k_assign_tc3(Assign3Args a) {
     asm volatile("cp.async.wait_all;" ::: "memory");
   } else {
     // =============================== epilogue ===============================
-    const int ew = warp - 6;           // 0..7
-    const int q = warp & 3;            // TMEM lane quarter this warp may access (hardware: warp % 4)
+    const int ew = warp - 4;           // 0..7
+    const int q = warp & 3;            // row quarter
     const int h = ew >> 2;             // column half
-    const int r = q * 32 + lane;       // row of the tile = TMEM lane
+    const int r = q * 32 + lane;       // row of the tile
     const int et = ew * 32 + lane;     // 0..255
     const int C0 = NP > 64 ? 64 : NP;
-    const int cb = h ? C0 : 0, ce = h ? NP : C0;  // this thread's columns (multiples of 16)
+    const int cb = h ? C0 : 0, ce = h ? NP : C0;  // this thread's columns (multiples of 16, at most 64)
     // column owned by this lane after the butterfly (bit i of the column = bit i + 1 of the lane)
     const int bcol = ((lane >> 4) & 1) * 8 + ((lane >> 3) & 1) * 4 + ((lane >> 2) & 1) * 2 + ((lane >> 1) & 1);
     float okd = 0.f, oent = 0.f;
@@ -301,7 +311,6 @@ __global__ void __launch_bounds__(A3_THREADS, 1) k_assign_tc3(Assign3Args a) {
       blk_n = a.tile_blk ? __ldg(a.tile_blk + my_first) : 0;
     }
     for (int tile = my_first; tile < a.ntiles; tile += stride, ++it) {
-      const int acc = it & 1;
       const int len = len_n, tq = tq_n, tblk = blk_n;
       if (tile + stride < a.ntiles) {
         len_n = __ldg(a.tile_len + tile + stride);
@@ -309,11 +318,9 @@ __global__ void __launch_bounds__(A3_THREADS, 1) k_assign_tc3(Assign3Args a) {
         blk_n = a.tile_blk ? __ldg(a.tile_blk + tile + stride) : 0;
       }
       const bool live = r < len;
-      umma::mbar_wait(t_full + acc, (it >> 1) & 1);
-      umma::fence_after_sync();
+      umma::mbar_wait(t_full, it & 1);
       if (et == 0) stamp(it, 8);
       const float rn = rnorm[(size_t)(it % A3_RING_N) * TC_TM + r];
-      const uint32_t trow = tmem + acc * 128 + ((uint32_t)(q * 32) << 16);
       float ev[64];                        // exp(u) of this thread's columns
       float ssum = 0.f, A1 = 0.f, S1 = 0.f;  // sum e, sum e*dist, sum sigma*e*u, sum sigma*e
       float* urow = Ust + (size_t)r * SS;
@@ -321,9 +328,15 @@ __global__ void __launch_bounds__(A3_THREADS, 1) k_assign_tc3(Assign3Args a) {
       for (int ci = 0; ci < 4; ++ci) {
         const int c = cb + ci * 16;
         if (c < ce) {
-          float v[16];
-          umma::tmem_ld16(trow + c, v);
-          umma::tmem_ld_wait();
+          float v[16];  // accumulator columns c .. c + 15 of this row (0 beyond KS); U overwrites them in place
+#pragma unroll
+          for (int i = 0; i < 16; i += 4) {
+            const float4 v4 = (c + i < KS) ? *reinterpret_cast<const float4*>(urow + c + i) : make_float4(0.f, 0.f, 0.f, 0.f);
+            v[i] = v4.x;
+            v[i + 1] = v4.y;
+            v[i + 2] = v4.z;
+            v[i + 3] = v4.w;
+          }
           float uu[16];
 #pragma unroll
           for (int i = 0; i < 16; ++i) {
@@ -347,9 +360,6 @@ __global__ void __launch_bounds__(A3_THREADS, 1) k_assign_tc3(Assign3Args a) {
         }
       }
       rs_part[h * TC_TM + r] = ssum;
-      // TMEM accumulator fully read -> the issuer may overwrite it
-      umma::fence_before_sync();
-      umma::mbar_arrive(t_empty + acc);
       if (et == 0) stamp(it, 9);
       umma::named_sync(1, 256);
       if (et == 0) stamp(it, 10);
@@ -465,6 +475,7 @@ __global__ void __launch_bounds__(A3_THREADS, 1) k_assign_tc3(Assign3Args a) {
         }
       }
       if (et == 0) stamp(it, 12);
+      umma::mbar_arrive(t_empty);  // U stage drained -> the MMA warpgroup may leave the next accumulator there
       umma::named_sync(1, 256);
       if (et == 0) stamp(it, 13);
       // column sums of the tile -> the block's removal sums (plan mode) or O / row sums (natural mode)
@@ -494,10 +505,6 @@ __global__ void __launch_bounds__(A3_THREADS, 1) k_assign_tc3(Assign3Args a) {
       }
     }
   }
-  // ---- teardown ----
-  umma::fence_before_sync();
-  __syncthreads();
-  if (warp == 1) umma::tmem_dealloc(tmem, 256);
 }
 
 }  // namespace hb

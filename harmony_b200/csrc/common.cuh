@@ -1,4 +1,4 @@
-// common.cuh — shared device helpers for libharmony_b200 (sm_100a only).
+// common.cuh — shared device helpers for libharmony_b200 (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>

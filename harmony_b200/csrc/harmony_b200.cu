@@ -1,6 +1,6 @@
 // harmony_b200.cu — host side of libharmony_b200.so: the C ABI of include/harmony_b200.h on top of the
 // kernels in kernels.cuh.  One hb_handle == one instance of the reference's `harmony` class
-// (/root/reference/src/harmony.h:20-70).  sm_100a only; there is no CPU path.
+// (/root/reference/src/harmony.h:20-70).  sm_90a (H100) only; there is no CPU path.
 #include "../../include/harmony_b200.h"
 
 #include <cuda_runtime.h>
@@ -260,7 +260,7 @@ void keep_pool_memory(int device) {
 
 struct hb_handle {
   int device = 0;
-  int num_sms = 148;
+  int num_sms = 132;
   cudaStream_t stream = nullptr;
   std::string err;
   std::deque<std::string> warnings;
@@ -1393,8 +1393,13 @@ int run_correct(hb_handle* h) {
         a.KD = (a.Kp + 7) & ~7;
         a.minuend = (k_off == 0) ? h->Zo.p : h->Zc.p;
         const size_t smem = apply_tc_smem_bytes(a.KD, d);
-        CK(cudaFuncSetAttribute(k_apply_tc, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        k_apply_tc<<<grid, AP_THREADS, smem, h->stream>>>(a);
+        if (d <= 64) {
+          CK(cudaFuncSetAttribute(k_apply_tc<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+          k_apply_tc<1><<<grid, AP_THREADS, smem, h->stream>>>(a);
+        } else {
+          CK(cudaFuncSetAttribute(k_apply_tc<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+          k_apply_tc<2><<<grid, AP_THREADS, smem, h->stream>>>(a);
+        }
         CKL();
         a.dbg = nullptr;
       }

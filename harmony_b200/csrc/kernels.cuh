@@ -1,6 +1,6 @@
-// kernels.cuh — CUDA kernels of the Harmony hot loop (sm_100a).  FFMA generation ("v1"): every
+// kernels.cuh — CUDA kernels of the Harmony hot loop (sm_90a).  FFMA generation ("v1"): every
 // contraction is a shared-memory-tiled fp32 kernel; they double as the in-repo correctness anchor
-// for the tcgen05 versions.
+// for the wgmma versions.
 //
 // Device data layout (all fp32, row-major, one row per cell; cells are stored sorted by their joint
 // covariate tuple so that a tile of consecutive cells shares its levels):

@@ -1,26 +1,27 @@
 // logits_tc.cuh — the cold-start logits of harmony.cpp:220-223 for shapes the fused assignment kernel
 // (assign_tc3.cuh) cannot hold in shared memory (d > 64 or K > 128; BASELINE.json config 5: K = 200, d = 100):
 //   U[i][k] = -dist_ik / sigma_k = (2 / sigma_k) (z_i . y_k / |z_i| - 1)        for clusters k in [n_off, n_off + 64)
-// as one tcgen05 contraction per 128-cell tile and cluster range (3xTF32, fp32 accumulator in TMEM).  The softmax and
-// the per-block column sums need the whole row, so they are NOT fused here: k_softmax_block_sums (below) makes one
+// as one wgmma contraction per 128-cell tile and cluster range (3xTF32, fp32 accumulators in registers).  The softmax
+// and the per-block column sums need the whole row, so they are NOT fused here: k_softmax_block_sums (below) makes one
 // gather pass over U in the update plan's order — the update kernel recomputes R from U anyway.  The tf32 operand pair
 // of all of Y (160 KB at K = 200, d = 100) does not fit beside a cell tile; 64 clusters per launch do (53 KB), at the
 // price of re-reading Z once per range: 4 x 400 + 800 B per cell at config 5 against ~40 kflop of FFMA work.
 // Same operand pipeline as assign_tc3.cuh: a loader thread copies ITS row with 16-byte cp.async into the canonical
 // K-major layout (the raw fp32 tile is the `hi` operand), waits for its own copies, writes the `lo` pieces and the
-// row norm.  One operand stage (a second one does not fit at d = 100), two TMEM accumulators: the epilogue of tile t
-// overlaps the load of tile t + 1.
-// Warp roles (448 threads): 1 MMA issuer, 2-5 loaders / converters (row per thread), 6-13 epilogue (TMEM lane
-// quarter x column half).  Limits: d <= 128.
+// row norm; then the four loader warps, one warpgroup, multiply the tile (two 64-row halves, m64n64k8) and leave the
+// accumulator in the U stage.  One operand stage (a second one does not fit at d = 100): the epilogue of tile t
+// overlaps the load and the MMAs of tile t + 1.
+// Warp roles (384 threads): 0-3 loaders / converters / MMA warpgroup (row per thread), 4-11 epilogue (row quarter x
+// column half).  Limits: d <= 128.
 #pragma once
 #include "common.cuh"
 #include "umma.cuh"
 
 namespace hb {
 
-constexpr int LG_TM = 128;      // cells per tile (= UMMA M)
-constexpr int LG_NP = 64;       // clusters per launch (= UMMA N)
-constexpr int LG_THREADS = 448;
+constexpr int LG_TM = 128;      // cells per tile (two wgmma M = 64 halves)
+constexpr int LG_NP = 64;       // clusters per launch (= wgmma N)
+constexpr int LG_THREADS = 384;
 constexpr int LG_SS = 68;       // row stride of the U stage in floats ((SS / 4) odd: conflict-free row-per-thread stores)
 
 struct LogitsArgs {
@@ -47,15 +48,12 @@ __global__ void __launch_bounds__(LG_THREADS, 1) k_logits_tc(LogitsArgs a) {
   float* Alo = Ahi + (size_t)LG_TM * KD;
   float* Bhi = Alo + (size_t)LG_TM * KD;             // [KD/4][64][4]
   float* Blo = Bhi + (size_t)LG_NP * KD;
-  float* Ust = Blo + (size_t)LG_NP * KD;             // [128][SS]
+  float* Ust = Blo + (size_t)LG_NP * KD;             // [128][SS]  accumulator, then U
   float* ca = Ust + (size_t)LG_TM * LG_SS;           // [64]  2 / sigma (1e30 in padding columns)
   float* rnorm = ca + LG_NP;                         // [4][128]  1 / |z|
   uint64_t* bars = reinterpret_cast<uint64_t*>(rnorm + 4 * LG_TM);
-  uint64_t* lo_full = bars;        // converters (128)
-  uint64_t* st_empty = bars + 1;   // tcgen05.commit: operands consumed
-  uint64_t* t_full = bars + 2;     // [2] tcgen05.commit: accumulator ready
-  uint64_t* t_empty = bars + 4;    // [2] epilogue (256): accumulator drained (and the U stage free)
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 6);
+  uint64_t* t_full = bars;         // MMA warpgroup (128): accumulator in the U stage
+  uint64_t* t_empty = bars + 1;    // epilogue (256): U stage drained
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
 
   for (int i = tid; i < LG_NP * KD; i += LG_THREADS) {
@@ -70,60 +68,25 @@ __global__ void __launch_bounds__(LG_THREADS, 1) k_logits_tc(LogitsArgs a) {
   for (int k = tid; k < LG_NP; k += LG_THREADS) ca[k] = (a.n_off + k < K) ? 2.f / a.sigma[a.n_off + k] : 1.0e30f;  // padding: u = -1e30 = U_PAD
   for (int i = tid; i < LG_TM * KD; i += LG_THREADS) Ahi[i] = 0.f;  // padding chunks / rows beyond short tiles: finite
   if (tid == 0) {
-    umma::mbar_init(lo_full, 128);
-    umma::mbar_init(st_empty, 1);
-    for (int i = 0; i < 2; ++i) {
-      umma::mbar_init(t_full + i, 1);
-      umma::mbar_init(t_empty + i, 256);
-    }
+    umma::mbar_init(t_full, 128);
+    umma::mbar_init(t_empty, 256);
     umma::fence_barrier_init();
   }
-  if (warp == 1) umma::tmem_alloc(tmem_slot, 128);  // two 64-column accumulators
-  umma::fence_proxy_async();
-  umma::fence_before_sync();
   __syncthreads();
-  umma::fence_after_sync();
-  const uint32_t tmem = *tmem_slot;
 
   const int64_t ntiles = (a.n + LG_TM - 1) / LG_TM;
   const int64_t my_first = blockIdx.x, stride = gridDim.x;
 
-  if (warp == 1) {
-    // =============================== MMA issuer ===============================
-    if (lane == 0) {
-      const uint32_t idesc = umma::make_idesc_tf32(LG_TM, LG_NP, 0, 0);
-      const uint32_t lboA = LG_TM * 16, lboB = LG_NP * 16, sbo = 128;
-      const uint32_t aH = umma::smem_u32(Ahi), aL = umma::smem_u32(Alo), bH = umma::smem_u32(Bhi), bL = umma::smem_u32(Blo);
-      int it = 0;
-      for (int64_t tile = my_first; tile < ntiles; tile += stride, ++it) {
-        const int acc = it & 1;
-        umma::mbar_wait(lo_full, it & 1);
-        if (it >= 2) umma::mbar_wait(t_empty + acc, ((it >> 1) - 1) & 1);
-        umma::fence_after_sync();
-        const uint32_t dt = tmem + acc * LG_NP;
-        uint32_t accum = 0;
-        for (int ks = 0; ks < KD / 8; ++ks) {
-          const uint64_t ah = umma::make_desc(aH + ks * 2 * lboA, lboA, sbo);
-          const uint64_t al = umma::make_desc(aL + ks * 2 * lboA, lboA, sbo);
-          const uint64_t bh = umma::make_desc(bH + ks * 2 * lboB, lboB, sbo);
-          const uint64_t bl = umma::make_desc(bL + ks * 2 * lboB, lboB, sbo);
-          umma::mma_tf32(dt, al, bh, idesc, accum);
-          umma::mma_tf32(dt, ah, bl, idesc, 1);
-          umma::mma_tf32(dt, ah, bh, idesc, 1);
-          accum = 1;
-        }
-        umma::mma_commit(st_empty);
-        umma::mma_commit(t_full + acc);
-      }
-    }
-  } else if (warp >= 2 && warp < 6) {
-    // =============================== row loaders + converters (one row of the tile per thread) ===============================
-    const int r = tid - 64;
+  if (warp < 4) {
+    // ================= row loaders + converters (one row of the tile per thread), then the MMA warpgroup =================
+    const int r = tid;
+    const uint32_t lboA = LG_TM * 16, lboB = LG_NP * 16, sbo = 128;
+    const uint32_t aH = umma::smem_u32(Ahi), aL = umma::smem_u32(Alo), bH = umma::smem_u32(Bhi), bL = umma::smem_u32(Blo);
     int it = 0;
     for (int64_t tile = my_first; tile < ntiles; tile += stride, ++it) {
       const int64_t cell = tile * LG_TM + r;
       const bool live = cell < a.n;
-      if (it >= 1) umma::mbar_wait(st_empty, (it - 1) & 1);  // the previous tile's MMAs are done with the stage
+      // the stage is free: this warpgroup waited for the previous tile's MMAs
       if (live) {
         const float* src = a.Zc + (size_t)cell * DS;
         const unsigned dst = umma::smem_u32(Ahi + (size_t)r * 4);
@@ -153,42 +116,57 @@ __global__ void __launch_bounds__(LG_THREADS, 1) k_logits_tc(LogitsArgs a) {
         rn = 1.f / nrm;
       }
       rnorm[(size_t)(it & 3) * LG_TM + r] = live ? rn : 0.f;
-      umma::fence_proxy_async();
-      umma::mbar_arrive(lo_full);
+      umma::fence_proxy_async();  // this thread's cp.async rows (observed above) and `lo` writes -> tensor core
+      umma::named_sync(2, 128);
+      for (int g = 0; g < 2; ++g) {  // rows 64 g .. 64 g + 63 of the tile
+        float acc[32];  // overwritten by the first MMA (accumulate = 0)
+        umma::fence();
+        for (int ks = 0; ks < KD / 8; ++ks) {
+          const uint32_t ao = ks * 2 * lboA + g * 64 * 16, bo = ks * 2 * lboB;
+          const uint64_t ah = umma::make_desc(aH + ao, lboA, sbo);
+          const uint64_t al = umma::make_desc(aL + ao, lboA, sbo);
+          const uint64_t bh = umma::make_desc(bH + bo, lboB, sbo);
+          const uint64_t bl = umma::make_desc(bL + bo, lboB, sbo);
+          umma::mma_n64(acc, al, bh, ks > 0);
+          umma::mma_n64(acc, ah, bl, 1);
+          umma::mma_n64(acc, ah, bh, 1);
+        }
+        umma::commit();
+        umma::wait0();
+        if (g == 0 && it >= 1) umma::mbar_wait(t_empty, (it - 1) & 1);  // the epilogue is done with the previous tile
+#pragma unroll
+        for (int i = 0; i < 32; i += 2) {
+          const int row = 64 * g + umma::frag_row(i, warp, lane), col = umma::frag_col(i, lane);
+          *reinterpret_cast<float2*>(Ust + (size_t)row * LG_SS + col) = make_float2(acc[i], acc[i + 1]);
+        }
+      }
+      umma::mbar_arrive(t_full);
     }
     asm volatile("cp.async.wait_all;" ::: "memory");
-  } else if (warp >= 6) {
+  } else {
     // =============================== epilogue ===============================
-    const int ew = warp - 6;           // 0..7
-    const int q = warp & 3;            // TMEM lane quarter this warp may access (hardware: warp % 4)
+    const int ew = warp - 4;           // 0..7
+    const int q = warp & 3;            // row quarter
     const int h = ew >> 2;             // column half: clusters [32 h, 32 h + 32) of the range
-    const int r = q * 32 + lane;       // row of the tile = TMEM lane
+    const int r = q * 32 + lane;       // row of the tile
     const int ncol4 = ((KS - a.n_off < LG_NP ? KS - a.n_off : LG_NP) + 3) >> 2;  // 16-byte pieces of the range inside a U row
     int it = 0;
     for (int64_t tile = my_first; tile < ntiles; tile += stride, ++it) {
-      const int acc = it & 1;
       const int64_t cell0 = tile * LG_TM;
       const int len = (int)(a.n - cell0 < LG_TM ? a.n - cell0 : LG_TM);
-      umma::mbar_wait(t_full + acc, (it >> 1) & 1);
-      umma::fence_after_sync();
+      umma::mbar_wait(t_full, it & 1);
       const float rn = rnorm[(size_t)(it & 3) * LG_TM + r];
-      const uint32_t trow = tmem + acc * LG_NP + 32 * h + ((uint32_t)(q * 32) << 16);
       float* urow = Ust + (size_t)r * LG_SS + 32 * h;
 #pragma unroll
-      for (int ci = 0; ci < 2; ++ci) {
-        float v[16];
-        umma::tmem_ld16(trow + 16 * ci, v);
-        umma::tmem_ld_wait();
-#pragma unroll
-        for (int i = 0; i < 16; i += 4) {
-          float4 u4;
-          const float* cc = ca + 32 * h + 16 * ci + i;
-          u4.x = fmaf(v[i + 0] * rn, cc[0], -cc[0]);  // -dist / sigma
-          u4.y = fmaf(v[i + 1] * rn, cc[1], -cc[1]);
-          u4.z = fmaf(v[i + 2] * rn, cc[2], -cc[2]);
-          u4.w = fmaf(v[i + 3] * rn, cc[3], -cc[3]);
-          *reinterpret_cast<float4*>(urow + 16 * ci + i) = u4;
-        }
+      for (int i = 0; i < 32; i += 4) {  // in place: accumulator -> U
+        const float4 v = *reinterpret_cast<const float4*>(urow + i);
+        const float* cc = ca + 32 * h + i;
+        float4 u4;
+        u4.x = fmaf(v.x * rn, cc[0], -cc[0]);  // -dist / sigma
+        u4.y = fmaf(v.y * rn, cc[1], -cc[1]);
+        u4.z = fmaf(v.z * rn, cc[2], -cc[2]);
+        u4.w = fmaf(v.w * rn, cc[3], -cc[3]);
+        *reinterpret_cast<float4*>(urow + i) = u4;
       }
       umma::named_sync(1, 256);  // the staged tile is complete
       // rows out: 16 lanes per row (64 clusters = 16 pieces of 16 bytes), two rows per warp instruction
@@ -201,15 +179,9 @@ __global__ void __launch_bounds__(LG_THREADS, 1) k_logits_tc(LogitsArgs a) {
           }
         }
       }
-      // accumulator read and stage drained -> the issuer may overwrite the accumulator, the next tile the stage
-      umma::fence_before_sync();
-      umma::mbar_arrive(t_empty + acc);
-      umma::named_sync(1, 256);  // nobody overwrites the stage while a slower warp still reads it
+      umma::mbar_arrive(t_empty);  // stage drained -> the MMA warpgroup may leave the next accumulator there
     }
   }
-  umma::fence_before_sync();
-  __syncthreads();
-  if (warp == 1) umma::tmem_dealloc(tmem, 128);
 }
 
 // Softmax of the stored logits + column sums per block of an update round (harmony.cpp:224-227 and the removal sums

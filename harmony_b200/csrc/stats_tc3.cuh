@@ -2,25 +2,25 @@
 // all clusters at once,
 //   S[q][k][c] = sum_{cells i of tuple q} R[i][k] * Z1[i][c],   Z1 = [Zo | 1]   (column d carries sum_i R_ik)
 // as D[128 clusters x 64 columns] += A * B^T with the CELLS as the reduction dimension.  The operands are K-major
-// with K = cells, i.e. the TRANSPOSE of the row-major tiles in memory (the no-swizzle MN-major form needs 16-byte
-// steps between consecutive reduction indices, which rows of K or d floats do not have), so the converter threads
-// transpose while they split into tf32 hi / lo.
+// with K = cells (wgmma takes tf32 operands K-major only), i.e. the TRANSPOSE of the row-major tiles in memory, so
+// the converter threads transpose while they split into tf32 hi / lo.
 // Second generation.  The first one staged raw tiles in shared memory (bulk copies) and converted them into ONE
 // operand stage: 2.9 us per 64-cell tile in a chain load -> convert -> MMA -> convert.  Here the converter threads
 // read their values straight from global memory (lanes along the cluster / column index: 128-byte segments of a
 // row), one tile AHEAD in registers, and the freed shared memory holds TWO operand stages: the conversion of tile
 // t + 1 overlaps the MMAs of tile t.  Persistent CTA per SM over a contiguous range of 64-cell tiles; the
-// accumulator stays in TMEM across the tiles of one covariate tuple and is flushed with atomics when the tuple changes.
-//   warp 1     issuer   : 3 x 8 tcgen05.mma (M=128, N=64, K=8 cells) per tile
-//   warps 4-11 convert  : global -> registers (next tile) -> K-major tf32 hi/lo stages; warps 4-7 also flush TMEM
+// accumulator stays in the registers of the MMA warpgroup across the tiles of one covariate tuple and is flushed
+// with atomics when the tuple changes.
+//   warps 0-3  MMA warpgroup : 2 halves x 3 x 8 wgmma (M=64, N=64, K=8 cells) per tile, 64 accumulators per thread
+//   warps 4-11 convert       : global -> registers (next tile) -> K-major tf32 hi/lo stages
 #pragma once
 #include "common.cuh"
 #include "umma.cuh"
 
 namespace hb {
 
-constexpr int ST_TN = 64;        // cells per tile = reduction length per stage (8 UMMA K-steps)
-constexpr int ST_THREADS = 384;  // warp 1 issuer, warps 4-11 converters (warps 0, 2, 3 idle)
+constexpr int ST_TN = 64;        // cells per tile = reduction length per stage (8 wgmma K-steps)
+constexpr int ST_THREADS = 384;  // warps 0-3 MMA warpgroup, warps 4-11 converters
 constexpr int ST_CONV = 256;     // converter threads
 
 struct StatsTcArgs {
@@ -50,69 +50,65 @@ __global__ void __launch_bounds__(ST_THREADS, 1) k_stats_tc(StatsTcArgs a) {
   float* Bhi = Alo + 2 * A_ST;                              // [2][16][64 columns][4]
   float* Blo = Bhi + 2 * B_ST;
   uint64_t* bars = reinterpret_cast<uint64_t*>(Blo + 2 * B_ST);
-  uint64_t* ab_full = bars + 0;     // [2]
-  uint64_t* ab_empty = bars + 2;    // [2]
-  uint64_t* acc_full = bars + 4;
-  uint64_t* acc_empty = bars + 5;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 6);
+  uint64_t* ab_full = bars + 0;     // [2]  converters (256): stage written
+  uint64_t* ab_empty = bars + 2;    // [2]  MMA warpgroup (128): stage consumed
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
 
   if (tid == 0) {
     for (int i = 0; i < 2; ++i) {
       umma::mbar_init(ab_full + i, ST_CONV);
-      umma::mbar_init(ab_empty + i, 1);
+      umma::mbar_init(ab_empty + i, 128);
     }
-    umma::mbar_init(acc_full, 1);
-    umma::mbar_init(acc_empty, 128);
     umma::fence_barrier_init();
   }
-  if (warp == 1) umma::tmem_alloc(tmem_slot, 64);
-  umma::fence_before_sync();
   __syncthreads();
-  umma::fence_after_sync();
-  const uint32_t tmem = *tmem_slot;
 
   const int t_begin = blockIdx.x * a.tiles_per_cta;
   const int t_end = (t_begin + a.tiles_per_cta < a.ntiles) ? t_begin + a.tiles_per_cta : a.ntiles;
 
-  if (warp == 1) {
-    // =============================== MMA issuer ===============================
-    const uint32_t idesc = umma::make_idesc_tf32(128, 64, 0, 0);
+  if (warp < 4) {
+    // =============================== MMA warpgroup ===============================
     const uint32_t lboA = 128 * 16, lboB = 64 * 16, sbo = 128;
-    int it = 0, runs = 0;
-    uint32_t accum = 0;
+    float acc[2][32];  // clusters 64 g + frag_row, columns frag_col
+    int run_acc = 0;   // 0: the first MMA of the tile starts the tuple's sums (overwrites the accumulator)
+    int it = 0;
     for (int tile = t_begin; tile < t_end; ++tile, ++it) {
       const int s = it & 1;
       const int q = a.tile_tuple[tile];
       const bool last_of_run = (tile + 1 == t_end) || (a.tile_tuple[tile + 1] != q);
       umma::mbar_wait(ab_full + s, (it >> 1) & 1);
-      if (accum == 0 && runs >= 1) umma::mbar_wait(acc_empty, (runs - 1) & 1);  // previous run flushed
-      umma::fence_after_sync();
-      if (lane == 0) {
-        const uint32_t aH = umma::smem_u32(Ahi + s * A_ST), aL = umma::smem_u32(Alo + s * A_ST);
-        const uint32_t bH = umma::smem_u32(Bhi + s * B_ST), bL = umma::smem_u32(Blo + s * B_ST);
+      const uint32_t aH = umma::smem_u32(Ahi + s * A_ST), aL = umma::smem_u32(Alo + s * A_ST);
+      const uint32_t bH = umma::smem_u32(Bhi + s * B_ST), bL = umma::smem_u32(Blo + s * B_ST);
+      umma::fence();
+#pragma unroll
+      for (int g = 0; g < 2; ++g)
         for (int ks = 0; ks < ST_TN / 8; ++ks) {
-          const uint64_t ah = umma::make_desc(aH + ks * 2 * lboA, lboA, sbo);
-          const uint64_t al = umma::make_desc(aL + ks * 2 * lboA, lboA, sbo);
-          const uint64_t bh = umma::make_desc(bH + ks * 2 * lboB, lboB, sbo);
-          const uint64_t bl = umma::make_desc(bL + ks * 2 * lboB, lboB, sbo);
-          umma::mma_tf32(tmem, al, bh, idesc, accum);
-          umma::mma_tf32(tmem, ah, bl, idesc, 1);
-          umma::mma_tf32(tmem, ah, bh, idesc, 1);
-          accum = 1;
+          const uint32_t ao = ks * 2 * lboA + g * 64 * 16, bo = ks * 2 * lboB;
+          const uint64_t ah = umma::make_desc(aH + ao, lboA, sbo);
+          const uint64_t al = umma::make_desc(aL + ao, lboA, sbo);
+          const uint64_t bh = umma::make_desc(bH + bo, lboB, sbo);
+          const uint64_t bl = umma::make_desc(bL + bo, lboB, sbo);
+          umma::mma_n64(acc[g], al, bh, run_acc | (ks > 0));
+          umma::mma_n64(acc[g], ah, bl, 1);
+          umma::mma_n64(acc[g], ah, bh, 1);
         }
-        umma::mma_commit(ab_empty + s);
-        if (last_of_run) umma::mma_commit(acc_full);
-      }
-      accum = 1;
-      __syncwarp();
+      umma::commit();
+      umma::wait0();
+      umma::mbar_arrive(ab_empty + s);
+      run_acc = last_of_run ? 0 : 1;
       if (last_of_run) {
-        accum = 0;
-        ++runs;
+        // flush the accumulator of this tuple
+#pragma unroll
+        for (int g = 0; g < 2; ++g)
+#pragma unroll
+          for (int i = 0; i < 32; ++i) {
+            const int k = a.k_off + 64 * g + umma::frag_row(i, warp, lane), c = a.c_off + umma::frag_col(i, lane);
+            if (k < K && c < D1) atomicAdd(a.S + ((size_t)q * K + k) * D1 + c, acc[g][i]);
+          }
       }
     }
   } else if (warp >= 4) {
-    // =============================== converters (+ TMEM flush) ===============================
+    // =============================== converters ===============================
     const int ct = tid - 128;          // 0..255
     const int kA = ct & 127, ccA = ct >> 7;   // A: cluster kA, cell chunks ccA + 2 i (i < 8)
     const int cB = ct & 63, ccB = ct >> 6;    // B: column cB,  cell chunks ccB + 4 i (i < 4)
@@ -160,10 +156,8 @@ __global__ void __launch_bounds__(ST_THREADS, 1) k_stats_tc(StatsTcArgs a) {
     meta(t_begin + 1, c0_1, len1, q1);
     meta(t_begin + 2, c0_2, len2, q2);
     fetch(c0_0, len0);
-    int it = 0, runs = 0;
+    int it = 0;
     for (int tile = t_begin; tile < t_end; ++tile, ++it) {
-      const int q = q0;
-      const bool last_of_run = q1 != q;  // q1 = -1 beyond the CTA's last tile
       const int s = it & 1;
       if (it >= 2) umma::mbar_wait(ab_empty + s, ((it >> 1) - 1) & 1);  // MMAs of tile it - 2 are done with the stage
       float* ah = Ahi + s * A_ST;
@@ -198,31 +192,8 @@ __global__ void __launch_bounds__(ST_THREADS, 1) k_stats_tc(StatsTcArgs a) {
       c0_0 = c0_1, len0 = len1, q0 = q1;
       c0_1 = c0_2, len1 = len2, q1 = q2;
       meta(tile + 3, c0_2, len2, q2);
-      if (last_of_run && warp < 8) {
-        // flush the accumulator of this tuple: thread = cluster row (TMEM lane), 64 columns
-        umma::mbar_wait(acc_full, runs & 1);
-        umma::fence_after_sync();
-        const int wq = warp & 3, k = a.k_off + wq * 32 + lane;
-        const uint32_t trow = tmem + ((uint32_t)(wq * 32) << 16);
-        for (int c0 = 0; c0 < 64; c0 += 16) {
-          float v[16];
-          umma::tmem_ld16(trow + c0, v);
-          umma::tmem_ld_wait();
-          if (k < K) {
-#pragma unroll
-            for (int i = 0; i < 16; ++i)
-              if (a.c_off + c0 + i < D1) atomicAdd(a.S + ((size_t)q * K + k) * D1 + a.c_off + c0 + i, v[i]);
-          }
-        }
-        umma::fence_before_sync();
-        umma::mbar_arrive(acc_empty);
-      }
-      if (last_of_run) ++runs;
     }
   }
-  umma::fence_before_sync();
-  __syncthreads();
-  if (warp == 1) umma::tmem_dealloc(tmem, 64);
 }
 
 }  // namespace hb

@@ -1,7 +1,6 @@
-// umma.cuh — thin inline-PTX wrappers for the sm_100a tensor-core path: tcgen05.mma (kind::tf32) with
-// shared-memory operand descriptors, TMEM allocation / loads, mbarriers.  Layout facts follow the PTX ISA
-// "tcgen05" chapter; the field positions were cross-checked against the CUTLASS headers shipped in this
-// image (cute/arch/mma_sm100_desc.hpp).
+// umma.cuh — thin inline-PTX wrappers for the sm_90a tensor-core path: wgmma.mma_async (tf32 operands from
+// shared memory, fp32 accumulators in the registers of a warpgroup) with shared-memory operand descriptors
+// and mbarriers.  Layout facts follow the PTX ISA "Asynchronous Warpgroup Level Matrix" chapter.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -33,74 +32,60 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
   }
 }
 __device__ __forceinline__ void fence_barrier_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
-// generic-proxy smem writes -> visible to the async proxy (tcgen05.mma / TMA reads)
+// generic-proxy smem writes -> visible to the async proxy (wgmma operand reads)
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-
-// ---- TMEM ---------------------------------------------------------------------------------------
-// One full warp allocates `ncols` (power of two >= 32) columns; the base address lands in *dst (shared).
-__device__ __forceinline__ void tmem_alloc(uint32_t* dst_smem, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)), "r"(ncols) : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void fence_before_sync() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void fence_after_sync() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-// 32 lanes x 16 consecutive 32-bit columns: thread i of the warp gets lane (base_lane + i), columns c..c+15
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, float (&v)[16]) {
-  uint32_t r[16];
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-#pragma unroll
-  for (int i = 0; i < 16; ++i) v[i] = __uint_as_float(r[i]);
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void named_sync(int id, int nthreads) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory"); }
 
 // ---- descriptors --------------------------------------------------------------------------------
 // Shared-memory operand descriptor, no swizzle.  Canonical K-major layout (units of 16 bytes):
 //   ((8, m), 2) : ((1, SBO), LBO)   -> 8 rows x 16 B form a contiguous 128-byte core matrix; the next 8-row
-// group is SBO bytes further, the next 16-byte chunk along K is LBO bytes further.  For MN-major operands
-// the roles are: ((1, n), (8, k)) : ((X, SBO), (1, LBO)) (see make_desc_mn below).
+// group is SBO bytes further, the next 16-byte chunk along K is LBO bytes further.  tf32 operands must be K-major.
 __device__ __forceinline__ uint64_t make_desc(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
   uint64_t d = 0;
   d |= (uint64_t)((smem_addr >> 4) & 0x3FFF);
   d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;
   d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32;
-  d |= (uint64_t)1 << 46;  // descriptor version (Blackwell)
-  return d;                // base_offset = 0, lbo_mode = 0, layout_type = SWIZZLE_NONE (0)
+  return d;  // base_offset = 0, layout_type (bits 62-63) = no swizzle
 }
-// Same, 128-byte swizzled layouts (layout_type = SWIZZLE_128B); the tile base must be 1024-byte aligned.
-__device__ __forceinline__ uint64_t make_desc_sw128(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
-  return make_desc(smem_addr, lbo_bytes, sbo_bytes) | ((uint64_t)2 << 61);
-}
-// Instruction descriptor of tcgen05.mma.kind::tf32, fp32 accumulate, dense.
-__host__ __device__ constexpr uint32_t make_idesc_tf32(int M, int N, int a_mn_major, int b_mn_major) {
-  return (1u << 4)                      // c_format  = F32
-         | (2u << 7)                    // a_format  = TF32
-         | (2u << 10)                   // b_format  = TF32
-         | ((uint32_t)a_mn_major << 15) // 0 = K-major
-         | ((uint32_t)b_mn_major << 16)
-         | ((uint32_t)(N >> 3) << 17)
-         | ((uint32_t)(M >> 4) << 24);
-}
-// D[tmem] (+)= A[smem] * B[smem]; issued by ONE thread.  accumulate = 0 overwrites D.
-__device__ __forceinline__ void mma_tf32(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
+
+// ---- wgmma --------------------------------------------------------------------------------------
+// All 128 threads of a warpgroup (warps 4w .. 4w + 3) execute these together.  fence() orders earlier register and
+// shared-memory accesses before the first MMA of a batch; commit() closes the batch; wait0() returns when every
+// committed batch is complete (accumulators readable, operand stages free).
+__device__ __forceinline__ void fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wait0() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+// D[64 x N] (+)= A[64 x 8] * B[N x 8]^T, tf32 operands (the tensor core reads the upper 19 bits of every word),
+// fp32 accumulate; accumulate = 0 overwrites D.  Accumulator fragment of thread t (warp w = t / 32 of the
+// warpgroup, lane l): d[i] = D[row][col] with row = 16 w + l / 4 + 8 ((i >> 1) & 1), col = 8 (i >> 2) + 2 (l % 4) + (i & 1).
+__device__ __forceinline__ int frag_row(int i, int w, int lane) { return 16 * w + (lane >> 2) + 8 * ((i >> 1) & 1); }
+__device__ __forceinline__ int frag_col(int i, int lane) { return 8 * (i >> 2) + 2 * (lane & 3) + (i & 1); }
+__device__ __forceinline__ void mma_n16(float (&d)[8], uint64_t adesc, uint64_t bdesc, int accumulate) {
   asm volatile(
       "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(d_tmem), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
+      "setp.ne.b32 p, %10, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n16k8.f32.tf32.tf32 "
+      "{%0,%1,%2,%3,%4,%5,%6,%7}, %8, %9, p, 1, 1;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+      : "l"(adesc), "l"(bdesc), "r"(accumulate));
 }
-// All previously issued MMAs of this thread arrive on the mbarrier when they complete.
-__device__ __forceinline__ void mma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
+__device__ __forceinline__ void mma_n32(float (&d)[16], uint64_t adesc, uint64_t bdesc, int accumulate) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\t"
+      "setp.ne.b32 p, %18, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n32k8.f32.tf32.tf32 "
+      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, %16, %17, p, 1, 1;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+      : "l"(adesc), "l"(bdesc), "r"(accumulate));
+}
+__device__ __forceinline__ void mma_n64(float (&d)[32], uint64_t adesc, uint64_t bdesc, int accumulate) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\t"
+      "setp.ne.b32 p, %34, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 "
+      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, %32, %33, p, 1, 1;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(adesc), "l"(bdesc), "r"(accumulate));
 }
 
 // tf32 split for 3xTF32 (error-compensated fp32-grade products): x ~= hi + lo, both exactly representable
@@ -114,43 +99,5 @@ __device__ __forceinline__ void split_tf32(float x, float& hi, float& lo) {
   hi = round_tf32(x);          // nearest tf32: |x - hi| <= 2^-12 |x|
   lo = round_tf32(x - hi);     // the remainder (exact in fp32) at tf32 precision
 }
-
-// mbarrier transaction accounting + 1-D bulk (TMA) copy global -> shared: the copy engine completes `bytes`
-// on the barrier; the issuing thread first arms it with arrive.expect_tx.
-__device__ __forceinline__ void mbar_arrive_expect_tx(uint64_t* bar, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void bulk_load(void* sdst, const void* gsrc, uint32_t bytes, uint64_t* bar) {
-  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(smem_u32(sdst)),
-               "l"(gsrc), "r"(bytes), "r"(smem_u32(bar))
-               : "memory");
-}
-// L2 eviction-priority policies for bulk copies: rows that will be read again soon (evict_last) / never (evict_first)
-__device__ __forceinline__ uint64_t l2_policy_evict_last() {
-  uint64_t p;
-  asm volatile("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(p));
-  return p;
-}
-__device__ __forceinline__ uint64_t l2_policy_evict_first() {
-  uint64_t p;
-  asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(p));
-  return p;
-}
-__device__ __forceinline__ void bulk_load_hint(void* sdst, const void* gsrc, uint32_t bytes, uint64_t* bar, uint64_t policy) {
-  asm volatile(
-      "cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1], %2, [%3], %4;" ::"r"(
-          smem_u32(sdst)),
-      "l"(gsrc), "r"(bytes), "r"(smem_u32(bar)), "l"(policy)
-      : "memory");
-}
-// 1-D bulk (TMA) copy shared -> global, completion tracked by the bulk async-group of the issuing thread
-__device__ __forceinline__ void bulk_store(void* gdst, const void* ssrc, uint32_t bytes) {
-  asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], %2;" ::"l"(gdst), "r"(smem_u32(ssrc)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
-// waits until the sources of all committed bulk groups have been read (smem may be overwritten)
-__device__ __forceinline__ void bulk_wait_read() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
-__device__ __forceinline__ void bulk_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
-__device__ __forceinline__ void named_sync(int id, int nthreads) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory"); }
 
 }  // namespace umma

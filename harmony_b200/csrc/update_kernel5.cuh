@@ -2,9 +2,8 @@
 //
 // Same algorithm, global tables and step protocol as update_kernel4.cuh (every U row read from HBM once per
 // clustering round; accumulator slots, remT filing, in-kernel fold, optional peer-memory exchange) — what
-// changes is how the rows reach the arithmetic.  Measured on B200 (profiles/r02_update_pipeline.md): dedicated
-// producer warps cap the 400-byte row gather at ~0.65 TB/s per producer warp and SM, and an in-order shared ring
-// stalls on the slowest consumer; k_update_steps4 spent 19.5 us per block step where the arithmetic needs 6.
+// changes is how the rows reach the arithmetic: dedicated producer warps limit the 400-byte row gather, and an
+// in-order shared ring stalls on the slowest consumer.
 // Here EVERY warp is a consumer that prefetches its own rows:
 //   * a warp owns a contiguous run of its CTA's rows of every step and a private ring of DG row groups in shared
 //     memory; lane l copies exactly the 16-byte pieces it will later read (cp.async.cg, one commit group per row

@@ -113,7 +113,7 @@ def prepare_inputs(data_mat, meta_data, vars_use=None, theta=None, sigma=0.1, la
 def RunHarmony(data_mat, meta_data, vars_use=None, theta=None, sigma=0.1, lambda_=None, nclust=None, max_iter=10,
                early_stop=True, ncores=1, plot_convergence=False, return_object=False, verbose=True,
                options=None, seed=None, device=None, **kwargs):
-    """RunHarmony.default (R/ui.R:91-309) on B200.
+    """RunHarmony.default (R/ui.R:91-309) on the GPU.
 
     ``ncores`` (CPU BLAS threads, R/ui.R:101,123-128) is accepted and ignored; ``seed`` replaces R's
     ``set.seed`` for the k-means initialisation and the per-round update orders.  Returns the

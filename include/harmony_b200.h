@@ -1,4 +1,4 @@
-/* harmony_b200.h — C ABI of libharmony_b200.so: the B200 (sm_100a) implementation of the Harmony
+/* harmony_b200.h — C ABI of libharmony_b200.so: the H100 (sm_90a) implementation of the Harmony
  * hot loop.  One opaque handle == one instance of the reference's C++ class `harmony`
  * (/root/reference/src/harmony.h:20-70); every entry point below replaces the like-named method /
  * field that the reference exposes to R through its Rcpp module (`RCPP_MODULE(harmony_module)`,
@@ -120,7 +120,7 @@ enum hb_scalar { HB_N = 0, HB_B = 1, HB_K = 2, HB_D = 3, HB_C = 4, HB_ALPHA = 5,
 /* HB_KERNEL_SET (test hook, default 0, read by the next hb_setup): the library picks its kernels from the problem's
  * shape alone; these bits force the kernels that serve shapes outside the default ones' limits onto ANY shape so that
  * the parity suite can hold them to the same bar (tests/test_gpu_parity.py::test_fallback_kernels_match_oracle). */
-enum hb_kernel_set { HB_KS_FFMA_CONTRACTIONS = 1, /* fp32 FFMA assignment / statistics / apply instead of tcgen05 */
+enum hb_kernel_set { HB_KS_FFMA_CONTRACTIONS = 1, /* fp32 FFMA assignment / statistics / apply instead of wgmma */
                      HB_KS_UPDATE_PER_STEP = 2,   /* three launches per block step (first-generation update_R) */
                      HB_KS_UPDATE_TWO_PASS = 4,   /* first persistent update_R generation (look-ahead + update groups) */
                      HB_KS_NO_PEER_EXCHANGE = 8,  /* sharded cells: one NCCL all-reduce per block step */

@@ -331,7 +331,7 @@ def test_field_writes_and_resume():
 
 
 @pytest.mark.parametrize("kernel_set", [
-    1,    # HB_KS_FFMA_CONTRACTIONS: fp32 FFMA assignment / statistics / apply instead of tcgen05
+    1,    # HB_KS_FFMA_CONTRACTIONS: fp32 FFMA assignment / statistics / apply instead of wgmma
     2,    # HB_KS_UPDATE_PER_STEP: three launches per block step
     4,    # HB_KS_UPDATE_TWO_PASS: first persistent update_R generation
     16,   # HB_KS_NO_PLAN_OVERLAP

@@ -231,8 +231,10 @@ def test_c_host_builds_against_the_header_and_fails_loudly_without_a_device(tmp_
            "-Wl,-rpath," + _lib._HERE, "-lm", "-o", exe]
     r = subprocess.run(cmd, capture_output=True, text=True)
     assert r.returncode == 0, r.stderr
-    if torch.cuda.is_available():
-        return   # running it is the GPU box's business (scripts/check_gpu.sh)
+    if torch.cuda.is_available():   # with a device it runs the whole loop
+        r = subprocess.run([exe, "20000"], capture_output=True, text=True, timeout=300)
+        assert r.returncode == 0 and "kernel launches" in r.stdout, (r.returncode, r.stderr[-2000:])
+        return
     r = subprocess.run([exe, "1000"], capture_output=True, text=True, timeout=120)
     assert r.returncode == 3, (r.returncode, r.stderr)
     assert "no usable CUDA device" in r.stderr
