@@ -28,7 +28,6 @@
 
 namespace hb {
 
-constexpr int TC_TM = 128;        // cells per tile (two wgmma M = 64 halves)
 constexpr int A3_THREADS = 384;
 constexpr int A3_NS = 2;          // operand stages (1 when two do not fit shared memory)
 constexpr int A3_RING_N = 4;      // row-norm ring (tiles): written by the converters, read at the start of the epilogue
@@ -59,7 +58,6 @@ struct Assign3Args {
   int ns;         // operand stages (1 or 2)
   int normalise;  // divide by the row norm (cold start; init runs on rows that setup normalised)
   int want_obj;   // objective partial sums (init)
-  long long* dbg; // optional [32 tiles][16] globaltimer stamps of CTA 0 (null = off)
 };
 
 __host__ __device__ inline int assign3_stage_stride(int KS) { return ((KS >> 2) | 1) << 2; }
@@ -121,13 +119,6 @@ __global__ void __launch_bounds__(A3_THREADS, 1) k_assign_tc3(Assign3Args a) {
 
   const int my_first = blockIdx.x, stride = gridDim.x;
   if (a.ntiles_ptr) a.ntiles = __ldg(a.ntiles_ptr);
-  auto stamp = [&](int it, int slot) {
-    if (a.dbg && blockIdx.x == 0 && it < 32) {
-      long long tns;
-      asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(tns));
-      a.dbg[it * 16 + slot] = tns;
-    }
-  };
 
   if (warp < 4) {
     // ============== row loaders + converters (one row of the tile per thread), then the MMA warpgroup ==============
@@ -172,13 +163,10 @@ __global__ void __launch_bounds__(A3_THREADS, 1) k_assign_tc3(Assign3Args a) {
     int it = 0;
     for (int tile = my_first; tile < a.ntiles; tile += stride, ++it) {
       const int s = it % NS;
-      if (r == 0) stamp(it, 0);
       // next tile -> the other stage (with one stage: after this tile's MMAs, below); the MMAs of tile it - 1, which
       // used that stage, are complete (this warpgroup waited for them)
       if (NS == 2) {
-        if (r == 0) stamp(it, 1);
         issue_row(it + 1, cell1);
-        if (r == 0) stamp(it, 2);
         asm volatile("cp.async.wait_group 1;" ::: "memory");
       } else {
         asm volatile("cp.async.wait_group 0;" ::: "memory");
@@ -188,7 +176,6 @@ __global__ void __launch_bounds__(A3_THREADS, 1) k_assign_tc3(Assign3Args a) {
       const int cell2 = ld_cell(p0_2, len2);
       int p0_3, len3;
       ld_meta(it + 3, p0_3, len3);
-      if (r == 0) stamp(it, 3);
       const float* hi = Ahi + (size_t)s * TC_TM * KD;
       float* lo = Alo + (size_t)s * TC_TM * KD;
       float ss = 0.f;
@@ -226,7 +213,6 @@ __global__ void __launch_bounds__(A3_THREADS, 1) k_assign_tc3(Assign3Args a) {
       }
       umma::fence_proxy_async();  // this thread's cp.async rows (observed above) and `lo` writes -> tensor core
       umma::named_sync(2, 128);
-      if (r == 0) stamp(it, 4);
       {
         const uint32_t aH = umma::smem_u32(Ahi + (size_t)s * TC_TM * KD);
         const uint32_t aL = umma::smem_u32(Alo + (size_t)s * TC_TM * KD);
@@ -259,9 +245,7 @@ __global__ void __launch_bounds__(A3_THREADS, 1) k_assign_tc3(Assign3Args a) {
           }
           umma::commit();
           umma::wait0();
-          if (r == 0 && g == 0) stamp(it, 5);
           if (g == 0 && it >= 1) umma::mbar_wait(t_empty, (it - 1) & 1);  // the epilogue is done with the previous tile
-          if (r == 0 && g == 0) stamp(it, 6);
 #pragma unroll
           for (int j = 0; j < 4; ++j) {
             if (j < nfull) {
@@ -282,7 +266,6 @@ __global__ void __launch_bounds__(A3_THREADS, 1) k_assign_tc3(Assign3Args a) {
         }
       }
       umma::mbar_arrive(t_full);
-      if (r == 0) stamp(it, 7);
       if (NS == 1) issue_row(it + 1, cell1);  // single stage: the next tile's rows land once this tile's MMAs are done
       cell0 = cell1;
       cell1 = cell2;
@@ -319,7 +302,6 @@ __global__ void __launch_bounds__(A3_THREADS, 1) k_assign_tc3(Assign3Args a) {
       }
       const bool live = r < len;
       umma::mbar_wait(t_full, it & 1);
-      if (et == 0) stamp(it, 8);
       const float rn = rnorm[(size_t)(it % A3_RING_N) * TC_TM + r];
       float ev[64];                        // exp(u) of this thread's columns
       float ssum = 0.f, A1 = 0.f, S1 = 0.f;  // sum e, sum e*dist, sum sigma*e*u, sum sigma*e
@@ -360,9 +342,7 @@ __global__ void __launch_bounds__(A3_THREADS, 1) k_assign_tc3(Assign3Args a) {
         }
       }
       rs_part[h * TC_TM + r] = ssum;
-      if (et == 0) stamp(it, 9);
       umma::named_sync(1, 256);
-      if (et == 0) stamp(it, 10);
       // R.each_row() /= sum(R, 0) (no zero guard in the reference); rows beyond the tile weigh 0
       const float tot = rs_part[r] + rs_part[TC_TM + r];
       const float inv = live ? 1.f / tot : 0.f;
@@ -418,7 +398,6 @@ __global__ void __launch_bounds__(A3_THREADS, 1) k_assign_tc3(Assign3Args a) {
           if ((lane & 1) == 0) cs_part[q * NP + c + bcol] = w1;
         }
       }
-      if (et == 0) stamp(it, 11);
       // rows out: the staged U tile (and, natural mode, R = exp(U) / row sum) with coalesced row stores
       {
         const int* rc = rowcell + (size_t)(it % A3_RING_C) * TC_TM;
@@ -474,10 +453,8 @@ __global__ void __launch_bounds__(A3_THREADS, 1) k_assign_tc3(Assign3Args a) {
           }
         }
       }
-      if (et == 0) stamp(it, 12);
       umma::mbar_arrive(t_empty);  // U stage drained -> the MMA warpgroup may leave the next accumulator there
       umma::named_sync(1, 256);
-      if (et == 0) stamp(it, 13);
       // column sums of the tile -> the block's removal sums (plan mode) or O / row sums (natural mode)
       if (et < K) {
         const float t = (cs_part[et] + cs_part[NP + et]) + (cs_part[2 * NP + et] + cs_part[3 * NP + et]);

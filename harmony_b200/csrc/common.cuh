@@ -7,6 +7,9 @@
 
 namespace hb {
 constexpr float U_PAD = -1.0e30f;  // logit stored in the padding columns of U (exp -> 0)
+constexpr int TC_TM = 128;         // cells per tile of the tensor-core kernels (two wgmma M = 64 halves)
+// dynamic shared memory a kernel may request: the 227 KB opt-in limit of sm_90 less room for static shared memory
+constexpr size_t SMEM_LIMIT = (size_t)227 * 1024 - 256;
 }
 
 __device__ __forceinline__ float warp_sum(float v) {

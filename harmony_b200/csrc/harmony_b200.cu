@@ -27,9 +27,9 @@
 #include <vector>
 
 #include "kernels.cuh"
-#include "update_kernel.cuh"
-#include "update_kernel4.cuh"
-#include "update_kernel5.cuh"
+#include "update_per_step.cuh"
+#include "update_two_pass.cuh"
+#include "update_single_pass.cuh"
 #include "assign_tc3.cuh"
 #include "logits_tc.cuh"
 #include "apply_tc3.cuh"
@@ -204,12 +204,83 @@ int my_ceil(float num) {
   return inum + 1;
 }
 
+// ---- kernel selection --------------------------------------------------------------------------------------
+// update_R runs the single-pass persistent kernel (update_single_pass.cuh) when every CTA's slice of a block can lie
+// inside one covariate tuple (2 J <= #SMs), its ring fits shared memory and n KS < 2^32; else the two-pass
+// persistent kernel (update_two_pass.cuh) when KS <= 256, J <= 8192 and its buffers fit shared memory; else three
+// launches per block step (update_per_step.cuh).
+enum class UpdatePath { PerStep, TwoPass, SinglePass };
+
+// Contractions that run on the tensor cores (wgmma); the others run the FFMA kernels of kernels.cuh.
+struct Contractions {
+  int k1_stages = 0;    // operand stages (1, 2) of the fused assignment kernel (assign_tc3.cuh); 0: not fused
+  bool logits = false;  // plan-order assignment of shapes the fused kernel cannot hold: logits_tc.cuh + softmax pass
+  bool apply = false;   // ridge apply (apply_tc3.cuh)
+  bool kmeans = false;  // native k-means initialisation from logits with sigma = 1 (logits_tc.cuh)
+};
+
+struct KernelPaths {
+  UpdatePath update = UpdatePath::PerStep;
+  bool tuple_ranges = false;  // 2 J <= #SMs: the plan gives every CTA a slice of a block inside one tuple
+  Contractions mm;
+};
+
+int two_pass_nv(int KS) {
+  int nv = 1;
+  while (4 * UPD_LPR * nv < KS) nv <<= 1;
+  return nv;
+}
+size_t two_pass_smem_bytes(int KS, int nb, int J) {
+  const size_t tabn = (size_t)std::max(2, nb) * KS;
+  const int nv = two_pass_nv(KS);
+  const size_t rowbuf = (size_t)UPD_GWARPS * (upd_depth_upd(nv) + upd_depth_look(nv)) * UPD_RPW * KS;
+  return sizeof(float) * ((size_t)KS + 2 * (tabn + (size_t)UPD_GWARPS * KS + 2 * (size_t)UPD_STAGE + (size_t)((J + 8) & ~3)) + rowbuf);
+}
+
+// The kernels of a shape (n: local cells, nb: update blocks); kernel_set: the HB_KS_* bits of the test hook.
+KernelPaths select_kernels(int K, int d, int J, int64_t n, int nb, int num_sms, int kernel_set) {
+  const int KS = (K + 3) & ~3, KD = (d + 7) & ~7, NP = (K + 15) & ~15;
+  KernelPaths p;
+  p.tuple_ranges = 2 * J <= num_sms;
+  if (kernel_set & HB_KS_UPDATE_PER_STEP)
+    p.update = UpdatePath::PerStep;
+  else if (!(kernel_set & HB_KS_UPDATE_TWO_PASS) && p.tuple_ranges && sp_ring_rows(KS, SMEM_LIMIT) > 0 &&
+           (uint64_t)n * (uint64_t)KS < (1ull << 32))
+    p.update = UpdatePath::SinglePass;
+  else if (KS <= 256 && J <= 8192 && two_pass_smem_bytes(KS, nb, J) <= SMEM_LIMIT)
+    p.update = UpdatePath::TwoPass;
+  if (!(kernel_set & HB_KS_FFMA_CONTRACTIONS)) {
+    const int ns = assign3_smem_bytes(2, KD, NP, KS) <= SMEM_LIMIT ? 2 : 1;
+    if (d <= 64 && K <= 128 && assign3_smem_bytes(ns, KD, NP, KS) <= SMEM_LIMIT) p.mm.k1_stages = ns;
+    const bool logits_fit = d <= 128 && logits_smem_bytes(KD) <= SMEM_LIMIT;
+    p.mm.logits = p.mm.k1_stages == 0 && logits_fit;
+    p.mm.apply = d <= 128;  // cluster ranges of <= AP_MAXK per launch
+    p.mm.kmeans = logits_fit && KS <= 256;
+  }
+  return p;
+}
+
+// The update_R path of a cluster_cpp call of T rounds, and whether a cold-start assignment runs in the order of round
+// 0 of the plan (and hands that round's removal sums to the single-pass kernel) instead of in natural order.  The
+// two-pass kernel keeps its R-store rounds in a 32-bit mask: longer calls run per step, like every call with the
+// legacy centroid step.
+struct CallPath {
+  UpdatePath update;
+  bool plan_order_assign;
+};
+CallPath call_path(const KernelPaths& p, unsigned T, bool legacy_centroid) {
+  CallPath c{p.update, false};
+  if (legacy_centroid || (p.update == UpdatePath::TwoPass && T > 31)) c.update = UpdatePath::PerStep;
+  c.plan_order_assign = c.update == UpdatePath::SinglePass && (p.mm.k1_stages > 0 || p.mm.logits) && T > 0;
+  return c;
+}
+
 // exchange area of the persistent update kernel for sharded cells (see setup_peer_exchange)
 struct XchArea {
   int device = 0, world = 0, rank = 0;
   size_t slots = 0, XH = 0, remT_floats = 0;
   float* base = nullptr;     // [inbox: slots * world * XH floats | flags: slots * world words | remT: remT_floats]
-  void* peer[U4_MAXWORLD] = {};
+  void* peer[XCH_MAXWORLD] = {};
   unsigned epoch = 0;
   bool leased = false;
 };
@@ -288,15 +359,12 @@ struct hb_handle {
   DevBuf<double> obj2;
   DevBuf<unsigned> bar;
   DevBuf<unsigned long long> scan_state;  // chained scan of the plan's histograms: [plan_batch][1 + tiles]
-  DevBuf<long long> dbg;  // optional step-phase timestamps (HB_TRACE_STEPS=<cta>)
-  int dbg_cta = -1;
   int plan_rounds = 0;   // rounds each plan buffer set holds (two sets: current call / prebuilt next call)
   int plan_set = 0;      // set used by the running cluster_cpp call
   bool next_ready = false;  // the other set holds a prebuilt native plan for the next call ...
   int next_T = 0;           // ... covering this many rounds
   cudaStream_t plan_stream = nullptr;
   cudaEvent_t plan_done = nullptr;
-  bool use_v2 = true;
   bool sigma_uniform = false;
   float sigma0 = 0.f;
   bool R_user_set = false;  // R was written through hb_set_field since the last assignment step
@@ -306,23 +374,19 @@ struct hb_handle {
       tuple_chunk0, blk_of, order, prev_at, H, seg_start, tile_base, iscratch, skipped, err_flag;
   DevBuf<int64_t> perms_d;
   DevBuf<int4> ranges;  // [T][nb][coop_grid] tuple-aligned CTA ranges (when 2 J <= grid)
-  bool aligned_ranges = false;
   DevBuf<int> tc_cell0, tc_len, tc_tuple;  // 128-cell tiles of the tensor-core kernels
   int tc_ntiles = 0;
-  bool use_tc_assign = false, use_tc_apply = false, use_tc_stats = false;
-  bool use_tc_logits = false;  // cold start of shapes outside the fused assignment kernel: logits_tc.cuh
+  KernelPaths paths;             // kernels picked by hb_setup (select_kernels)
   int kernel_set = 0;            // HB_KERNEL_SET test hook (bits HB_KS_*), read by hb_setup
   bool legacy_centroid = false;  // HB_LEGACY_CENTROID_STEP: centroid update at the top of every clustering round
   DevBuf<float> Rkeep, OEkeep;   // R / O,E saved around the distance-only assignment of that step
   DevBuf<double> objkeep;
-  bool use_v4 = false;   // single-pass persistent update kernel (update_kernel4.cuh): the default
-  int u5_ring_rows = 0;  // rows of a warp's private ring (update_kernel5.cuh); 0: that kernel cannot run this row width
+  int ring_rows = 0;     // rows of a warp's private ring in the single-pass update kernel
   int plan_batch = 1;    // rounds sorted per launch (size of the histogram scratch)
   int plan_nsub = 1;     // third sort key of the plan: block in the next round (nb values) or off (1)
   bool use_xch = false;  // sharded cells: block steps exchanged through peer memory (one cooperative launch per call)
-  Upd4Xch xch{};
+  PeerXch xch{};
   XchArea* xarea = nullptr;  // leased exchange area (process-wide pool, see setup_peer_exchange)
-  int assign_ns = 2;     // operand stages of the tensor-core assignment kernel
   bool zc_pending_norm = false;  // Zc holds the un-normalised corrected embedding although cluster_cpp has run
   DevBuf<int> pt_p0, pt_len, pt_tuple, pt_blk, pt_count, pt_base;  // [2 sets] 128-row tiles of round 0 in plan order
   size_t pt_cap = 0;
@@ -507,7 +571,7 @@ int run_assign(hb_handle* h, bool normalise, bool plan_mode = false, bool want_o
   a.DS = h->DS;
   a.KS = KS;
   a.normalise = normalise ? 1 : 0;
-  if (h->use_tc_assign) {
+  if (h->paths.mm.k1_stages) {
     Assign3Args t{};
     t.Zc = a.Zc;
     t.Y = a.Y;
@@ -524,7 +588,7 @@ int run_assign(hb_handle* h, bool normalise, bool plan_mode = false, bool want_o
     t.KD = (d + 7) & ~7;
     t.NP = (K + 15) & ~15;
     t.SS = assign3_stage_stride(KS);
-    t.ns = h->assign_ns;
+    t.ns = h->paths.mm.k1_stages;
     t.normalise = a.normalise;
     t.want_obj = want_obj ? 1 : 0;
     int grid_tc;
@@ -559,14 +623,6 @@ int run_assign(hb_handle* h, bool normalise, bool plan_mode = false, bool want_o
       grid_tc = std::max(1, std::min(h->tc_ntiles, h->num_sms));
     }
     const size_t smem_tc = assign3_smem_bytes(t.ns, t.KD, t.NP, KS);
-    t.dbg = nullptr;
-    static int as_calls = 0;
-    const bool tracing = getenv("HB_TRACE_ASSIGN") != nullptr && plan_mode && (++as_calls == 4);
-    if (tracing) {
-      if (h->dbg.n < 32 * 16) CK(h->dbg.alloc(32 * 16));
-      CK(cudaMemsetAsync(h->dbg.p, 0, sizeof(long long) * 32 * 16, h->stream));
-      t.dbg = h->dbg.p;
-    }
     if (want_obj) {
       CK(cudaFuncSetAttribute(k_assign_tc3<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_tc));
       k_assign_tc3<true><<<grid_tc, A3_THREADS, smem_tc, h->stream>>>(t);
@@ -575,19 +631,6 @@ int run_assign(hb_handle* h, bool normalise, bool plan_mode = false, bool want_o
       k_assign_tc3<false><<<grid_tc, A3_THREADS, smem_tc, h->stream>>>(t);
     }
     CKL();
-    if (tracing) {
-      std::vector<long long> st(32 * 16);
-      CK(cudaMemcpyAsync(st.data(), h->dbg.p, sizeof(long long) * st.size(), cudaMemcpyDeviceToHost, h->stream));
-      CK(cudaStreamSynchronize(h->stream));
-      if (FILE* f = fopen("gpurun_out/assign_trace.txt", "w")) {
-        for (int i = 0; i < 32; ++i) {
-          fprintf(f, "%d", i);
-          for (int k = 0; k < 16; ++k) fprintf(f, " %lld", st[(size_t)i * 16 + k] ? st[(size_t)i * 16 + k] - st[0] : -1);
-          fprintf(f, "\n");
-        }
-        fclose(f);
-      }
-    }
     h->R_user_set = false;
     if (plan_mode) {
       // O, E of the assignment = the sums of the blocks' removal terms (harmony.cpp:226-227)
@@ -605,12 +648,12 @@ int run_assign(hb_handle* h, bool normalise, bool plan_mode = false, bool want_o
     CKL();
     return 0;
   }
-  if (plan_mode && h->use_tc_logits) {
+  if (plan_mode && h->paths.mm.logits) {
     // shapes the fused kernel cannot hold (d > 64 or K > 128): logits per 64-cluster range on the tensor cores, then
     // one gather pass over U in the order of round 0 for the softmax + the blocks' removal sums (harmony.cpp:312-313)
     TRY(launch_logits(h, h->sigma.p, normalise));
     const size_t R0 = (size_t)h->plan_set * h->plan_rounds;
-    const int nv = upd4_nv(KS);
+    const int nv = sp_nv(KS);
     const size_t smem_sm = sizeof(float) * 8 * 128 * (size_t)nv;
     if (nv == 1)
       k_softmax_block_sums<1><<<dim3(h->coop_grid, h->nb), 256, smem_sm, h->stream>>>(
@@ -771,18 +814,19 @@ int plan_sort(hb_handle* h, int t, int nt, bool last_has_next, int set, cudaStre
   }
   k_plan_scatter<<<dim3((nc + wpb - 1) / wpb, nt), wpb * 32, sm, st>>>(
       blk_of, nullptr, h->chunk_start.p, h->chunk_q0.p, h->chunk_nq.p, nc, nb, nsub, h->H.p, order, nullptr,
-      (h->use_v2 && !h->use_v4) ? h->prev_at.p + (R0 + t) * n : nullptr, h->use_v4 ? h->next_at.p + (R0 + t) * n : nullptr, n,
+      h->paths.update == UpdatePath::TwoPass ? h->prev_at.p + (R0 + t) * n : nullptr,
+      h->paths.update == UpdatePath::SinglePass ? h->next_at.p + (R0 + t) * n : nullptr, n,
       with_next, t > 0 ? 1 : 0);
   CKL();
   k_plan_segments<<<dim3(grid_for(S + 1, 256, 64), nt), 256, 0, st>>>(h->H.p, h->tuple_chunk0.p, nc, nb, nsub, J, (int)n,
                                                                        seg_start, tile_base);
   CKL();
-  if (h->use_v2 && h->aligned_ranges) {
+  if (h->paths.update != UpdatePath::PerStep && h->paths.tuple_ranges) {
     k_plan_ranges<<<dim3(nb, nt), 256, 0, st>>>(seg_start, nb, J, h->coop_grid,
                                                                             h->ranges.p + (R0 + t) * nb * h->coop_grid);
     CKL();
   }
-  if (tiles) {  // tile offsets of the first-generation update kernels (single round)
+  if (tiles) {  // tile offsets of the per-step update kernels (single round)
     k_plan_tilecount<<<grid_for(S + 1, 256, 64), 256, 0, st>>>(seg_start, S, tile_base);
     CKL();
     k_scan_exclusive<<<1, 1024, 0, st>>>(tile_base, (int64_t)S + 1, nullptr);
@@ -797,7 +841,7 @@ int build_plans(hb_handle* h, int T, const int64_t* orders_d, int set, cudaStrea
     const int nt = std::min(h->plan_batch, T - t);
     TRY(plan_sort(h, t, nt, t + nt < T, set, st));
   }
-  if (T > 0 && h->use_tc_assign && h->use_v4) {
+  if (T > 0 && h->paths.mm.k1_stages && h->paths.update == UpdatePath::SinglePass) {
     // 128-row tiles of round 0, one (block, tuple) segment at a time: the assignment step of the call runs in this order
     RegionScope rs(h, "plan");
     const int S = h->nb * h->J;
@@ -814,14 +858,37 @@ int build_plans(hb_handle* h, int T, const int64_t* orders_d, int set, cudaStrea
   }
   return 0;
 }
-// one round into slot 0 of set 0 (per-round paths: first-generation kernels, legacy centroid step)
+// Buffers of T rounds of update plans, two sets (the running call's, and the next call's prebuilt on the side stream),
+// and the persistent update kernels' per-step accumulators of a T-round call.
+int alloc_plan_rounds(hb_handle* h, int T) {
+  const size_t n = (size_t)h->n, BK = (size_t)h->B * h->KS;
+  const size_t S1 = (size_t)h->nb * h->J + 1;
+  CK(h->blk_of.alloc(2 * (size_t)T * n));
+  CK(h->order.alloc(2 * (size_t)T * n));
+  if (h->paths.update == UpdatePath::SinglePass)
+    CK(h->next_at.alloc(2 * (size_t)T * n));
+  else
+    CK(h->prev_at.alloc(2 * (size_t)T * n));
+  CK(h->seg_start.alloc(2 * (size_t)T * S1));
+  CK(h->tile_base.alloc(2 * (size_t)T * S1));
+  if (h->paths.update != UpdatePath::PerStep) {
+    CK(h->acc2.alloc(2 * (BK + h->KS) * ((size_t)T * h->nb + 2)));
+    CK(h->OEend.alloc((size_t)T * 2 * BK));
+    CK(h->obj2.alloc(2 * (size_t)T));
+    CK(h->bar.alloc(2 * ((size_t)T * h->nb + 2)));
+    if (h->paths.tuple_ranges) CK(h->ranges.alloc(2 * (size_t)T * h->nb * h->coop_grid));
+  }
+  h->plan_rounds = T;
+  return 0;
+}
+// one round into slot 0 of set 0 (the per-step update path)
 int build_plan_single(hb_handle* h, const int64_t* perm_d, cudaStream_t st) {
   TRY(plan_blocks(h, 0, 1, perm_d, 0, st));
   return plan_sort(h, 0, 1, false, 0, st, true);
 }
 
-// ---- v1: one update_R sweep (harmony.cpp:269-342), three launches per block step ------------------
-int run_update_R_v1(hb_handle* h, int t) {
+// ---- per-step path: one update_R sweep (harmony.cpp:269-342), three launches per block step ---------------
+int run_update_per_step(hb_handle* h, int t) {
   RegionScope rs(h, "update_R");
   const int K = h->K, B = h->B, nb = h->nb, KS = h->KS;
   const int KP = (K + 63) & ~63;
@@ -831,7 +898,7 @@ int run_update_R_v1(hb_handle* h, int t) {
   StepArgs a;
   a.U = h->U.p;
   a.R = h->R.p;
-  a.order = h->order.p + (size_t)t * h->n;  // v1 always plans into set 0
+  a.order = h->order.p + (size_t)t * h->n;  // the per-step path always plans into set 0
   a.seg_start = h->seg_start.p + (size_t)t * (S + 1);
   a.tile_base = h->tile_base.p + (size_t)t * (S + 1);
   a.tuple_levels = h->tuple_levels.p;
@@ -981,7 +1048,7 @@ int setup_peer_exchange(hb_handle* h, int Tplan) {
   }
   area->leased = true;
   h->xarea = area;
-  Upd4Xch& x = h->xch;
+  PeerXch& x = h->xch;
   x.world = W;
   x.rank = h->rank;
   x.epoch = area->epoch;
@@ -998,35 +1065,24 @@ int setup_peer_exchange(hb_handle* h, int Tplan) {
 float* remT_ptr(hb_handle* h) { return h->use_xch ? h->xch.peer_remT[h->rank] : h->remT.p; }
 
 // ---- persistent update kernels over rounds [t0, t1) of this cluster_cpp call ---------------------------
-int nv_for(int KS) {
-  int nv = 1;
-  while (4 * UPD_LPR * nv < KS) nv <<= 1;
-  return nv;
-}
 template <typename F>
-int dispatch_nv(hb_handle* h, int KS, F&& f) {
-  switch (nv_for(KS)) {
+int dispatch_two_pass_nv(hb_handle* h, int KS, F&& f) {
+  switch (two_pass_nv(KS)) {
     case 1: return f(std::integral_constant<int, 1>());
     case 2: return f(std::integral_constant<int, 2>());
     case 4: return f(std::integral_constant<int, 4>());
   }
   return fail(h, 2, "K = %d is not supported by the persistent update kernel", h->K);
 }
-size_t upd_smem_bytes(const hb_handle* h) {
-  const size_t tabn = (size_t)std::max(2, h->nb) * h->KS;
-  const int nv = nv_for(h->KS);
-  const size_t rowbuf = (size_t)UPD_GWARPS * (upd_depth_upd(nv) + upd_depth_look(nv)) * UPD_RPW * h->KS;
-  return sizeof(float) * ((size_t)h->KS + 2 * (tabn + (size_t)UPD_GWARPS * h->KS + 2 * (size_t)UPD_STAGE + (size_t)((h->J + 8) & ~3)) + rowbuf);
-}
-UpdArgs make_upd_args(hb_handle* h, int T) {
-  UpdArgs a;
+TwoPassArgs make_two_pass_args(hb_handle* h, int T) {
+  TwoPassArgs a;
   a.U = h->U.p;
   a.R = h->R.p;
   const size_t R0 = (size_t)h->plan_set * h->plan_rounds;
   a.order = h->order.p + R0 * h->n;
   a.seg_start = h->seg_start.p + R0 * ((size_t)h->nb * h->J + 1);
   a.prev_at = h->prev_at.p + R0 * h->n;
-  a.ranges = h->aligned_ranges ? h->ranges.p + R0 * h->nb * h->coop_grid : nullptr;
+  a.ranges = h->paths.tuple_ranges ? h->ranges.p + R0 * h->nb * h->coop_grid : nullptr;
   a.tuple_levels = h->tuple_levels.p;
   a.sigma = h->sigma.p;
   a.theta = h->theta.p;
@@ -1048,12 +1104,10 @@ UpdArgs make_upd_args(hb_handle* h, int T) {
   a.first_round_from_R = h->R_user_set ? 1 : 0;
   a.sigma_uniform = h->sigma_uniform ? 1 : 0;
   a.sigma0 = h->sigma0;
-  a.dbg = (h->dbg_cta >= 0) ? h->dbg.p : nullptr;
-  a.dbg_cta = h->dbg_cta;
   return a;
 }
-Upd4Args make_upd4_args(hb_handle* h, int T) {
-  Upd4Args a;
+SinglePassArgs make_single_pass_args(hb_handle* h, int T) {
+  SinglePassArgs a;
   a.U = h->U.p;
   a.R = h->R.p;
   const size_t R0 = (size_t)h->plan_set * h->plan_rounds;
@@ -1087,86 +1141,68 @@ Upd4Args make_upd4_args(hb_handle* h, int T) {
   a.has_next_from = T - 1;
   a.sigma_uniform = h->sigma_uniform ? 1 : 0;
   a.sigma0 = h->sigma0;
-  a.ring_rows = h->u5_ring_rows;
-  a.dbg_flags = 0;
+  a.ring_rows = h->ring_rows;
   a.coop = 1;
-  a.dbg = (h->dbg_cta >= 0) ? h->dbg.p : nullptr;
-  a.dbg_cta = h->dbg_cta;
   return a;
 }
 // zero the per-step accumulators of a cluster_cpp call ...
-int upd_begin_zero(hb_handle* h, int T) {
+int update_begin_zero(hb_handle* h, int T) {
   const size_t BK = (size_t)h->B * h->KS, SL = 2 * (BK + h->KS);
   CK(cudaMemsetAsync(h->acc2.p, 0, sizeof(float) * SL * ((size_t)T * h->nb + 2), h->stream));
   CK(cudaMemsetAsync(h->obj2.p, 0, sizeof(double) * 2 * (size_t)T, h->stream));
   CK(cudaMemsetAsync(h->bar.p, 0, sizeof(unsigned) * 2 * ((size_t)T * h->nb + 2), h->stream));
-  if (h->use_v4) CK(cudaMemsetAsync(remT_ptr(h), 0, sizeof(float) * 2 * (size_t)h->nb * h->J * h->KS, h->stream));
+  if (h->paths.update == UpdatePath::SinglePass) CK(cudaMemsetAsync(remT_ptr(h), 0, sizeof(float) * 2 * (size_t)h->nb * h->J * h->KS, h->stream));
   if (h->use_xch) h->xch.epoch++;  // flags of earlier calls no longer match
   return 0;
 }
 // ... and seed ring[1] (= "O_{-1}") with the tables the call starts from
-int upd_begin_seed(hb_handle* h) {
+int update_begin_seed(hb_handle* h) {
   const size_t BK = (size_t)h->B * h->KS;
   CK(cudaMemcpyAsync(h->ring.p + 2 * BK, h->O.p, sizeof(float) * BK, cudaMemcpyDeviceToDevice, h->stream));
   CK(cudaMemcpyAsync(h->ring.p + 3 * BK, h->E.p, sizeof(float) * BK, cudaMemcpyDeviceToDevice, h->stream));
   return 0;
 }
-int upd_launch(hb_handle* h, UpdArgs a, bool cooperative) {
-  const size_t smem = upd_smem_bytes(h);
-  return dispatch_nv(h, h->KS, [&](auto nvc) -> int {
+int launch_two_pass(hb_handle* h, TwoPassArgs a, bool cooperative) {
+  const size_t smem = two_pass_smem_bytes(h->KS, h->nb, h->J);
+  return dispatch_two_pass_nv(h, h->KS, [&](auto nvc) -> int {
     constexpr int NV = decltype(nvc)::value;
-    CK(cudaFuncSetAttribute(k_update_steps<NV>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    CK(cudaFuncSetAttribute(k_update_two_pass<NV>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     a.use_barrier = cooperative ? 1 : 0;
     if (cooperative) {
       void* args[] = {&a};
-      CK(cudaLaunchCooperativeKernel((void*)k_update_steps<NV>, dim3(h->coop_grid), dim3(UPD_THREADS), args, smem, h->stream));
+      CK(cudaLaunchCooperativeKernel((void*)k_update_two_pass<NV>, dim3(h->coop_grid), dim3(UPD_THREADS), args, smem, h->stream));
     } else {
-      k_update_steps<NV><<<h->coop_grid, UPD_THREADS, smem, h->stream>>>(a);
+      k_update_two_pass<NV><<<h->coop_grid, UPD_THREADS, smem, h->stream>>>(a);
     }
     CKL();
     return 0;
   });
 }
 template <int NV, bool SIGU>
-int upd5_launch_nv(hb_handle* h, Upd4Args& a, bool cooperative) {
-  const size_t smem = upd5_smem_bytes(NV, a.ring_rows, a.KS);
-  CK(cudaFuncSetAttribute(k_update_steps5<NV, SIGU>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+int launch_single_pass_nv(hb_handle* h, SinglePassArgs& a, bool cooperative) {
+  const size_t smem = sp_smem_bytes(NV, a.ring_rows, a.KS);
+  CK(cudaFuncSetAttribute(k_update_single_pass<NV, SIGU>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   a.coop = cooperative ? 1 : 0;
-  Upd4Launch lp;
+  SinglePassLaunch lp;
   lp.a = a;
   if (h->use_xch) lp.x = h->xch;
   if (cooperative) {
     void* args[] = {&lp};
-    CK(cudaLaunchCooperativeKernel((void*)k_update_steps5<NV, SIGU>, dim3(h->coop_grid), dim3(U5_THREADS), args, smem,
+    CK(cudaLaunchCooperativeKernel((void*)k_update_single_pass<NV, SIGU>, dim3(h->coop_grid), dim3(SP_THREADS), args, smem,
                                    h->stream));
   } else {
-    k_update_steps5<NV, SIGU><<<h->coop_grid, U5_THREADS, smem, h->stream>>>(lp);
+    k_update_single_pass<NV, SIGU><<<h->coop_grid, SP_THREADS, smem, h->stream>>>(lp);
   }
   CKL();
   return 0;
 }
-int upd4_launch(hb_handle* h, Upd4Args a, bool cooperative) {
+int launch_single_pass(hb_handle* h, SinglePassArgs a, bool cooperative) {
   const bool su = h->sigma_uniform;  // the default: scalar sigma (objective terms simplify)
-  switch (upd4_nv(h->KS)) {
-    case 1: return su ? upd5_launch_nv<1, true>(h, a, cooperative) : upd5_launch_nv<1, false>(h, a, cooperative);
-    case 2: return su ? upd5_launch_nv<2, true>(h, a, cooperative) : upd5_launch_nv<2, false>(h, a, cooperative);
+  switch (sp_nv(h->KS)) {
+    case 1: return su ? launch_single_pass_nv<1, true>(h, a, cooperative) : launch_single_pass_nv<1, false>(h, a, cooperative);
+    case 2: return su ? launch_single_pass_nv<2, true>(h, a, cooperative) : launch_single_pass_nv<2, false>(h, a, cooperative);
   }
   return fail(h, 2, "K = %d is not supported by the persistent update kernel", h->K);
-}
-void dump_step_trace(hb_handle* h, int ns, int per_step) {
-  std::vector<long long> st((size_t)(ns + 1) * per_step);
-  if (cudaMemcpyAsync(st.data(), h->dbg.p, sizeof(long long) * st.size(), cudaMemcpyDeviceToHost, h->stream) != cudaSuccess) return;
-  cudaStreamSynchronize(h->stream);
-  static int dumped = 0;
-  if (dumped++ != 3) return;
-  FILE* f = fopen("gpurun_out/step_trace.txt", "w");
-  if (!f) return;
-  for (int s = 0; s <= ns; ++s) {
-    fprintf(f, "%d", s);
-    for (int k = 0; k < per_step; ++k) fprintf(f, " %lld", st[(size_t)s * per_step + k]);
-    fprintf(f, "\n");
-  }
-  fclose(f);
 }
 // compute_objective() of every round in [t0, t1) (harmony.cpp:248) from the kernels' per-round sums and tables
 int push_round_objectives(hb_handle* h, int t0, int t1) {
@@ -1178,12 +1214,12 @@ int push_round_objectives(hb_handle* h, int t0, int t1) {
   }
   return 0;
 }
-// single-pass kernel (update_kernel4.cuh), rounds [t0, t1)
-int run_update_v4(hb_handle* h, int T, int t0, int t1, bool rem_ready) {
+// single-pass kernel (update_single_pass.cuh), rounds [t0, t1)
+int run_update_single_pass(hb_handle* h, int T, int t0, int t1, bool rem_ready) {
   RegionScope rs(h, "update_R");
   const int nb = h->nb;
   const size_t BK = (size_t)h->B * h->KS, XH = BK + h->KS, SL = 2 * XH;
-  Upd4Args a = make_upd4_args(h, T);
+  SinglePassArgs a = make_single_pass_args(h, T);
   if (t0 == 0 && !rem_ready) {
     // removal sums of round 0 from the R in memory (assignment step / user), harmony.cpp:312-313
     RegionScope r0(h, "k_rem_sums");
@@ -1196,7 +1232,7 @@ int run_update_v4(hb_handle* h, int T, int t0, int t1, bool rem_ready) {
     a.s_begin = t0 * nb;
     a.s_end = t1 * nb;
     RegionScope r3(h, "k_update_steps");
-    TRY(upd4_launch(h, a, true));
+    TRY(launch_single_pass(h, a, true));
   } else {
     // sharded cells without peer memory: one launch per block step, the step's add half all-reduced in between; the next round's
     // removal sums (remT) are all-reduced and folded once per round
@@ -1211,55 +1247,53 @@ int run_update_v4(hb_handle* h, int T, int t0, int t1, bool rem_ready) {
         if (s > t0 * nb) TRY(allreduce_f(h, h->acc2.p + (size_t)(s + 1) * SL, XH));  // add_{s-1}
         a.s_begin = s;
         a.s_end = s + 1;
-        TRY(upd4_launch(h, a, false));
+        TRY(launch_single_pass(h, a, false));
       }
     }
     TRY(allreduce_f(h, h->acc2.p + (size_t)(t1 * nb + 1) * SL, XH));  // add_{S-1}
   }
-  if (h->dbg_cta >= 0 && h->rank == 0) dump_step_trace(h, (t1 - t0) * nb, 8);
   {
     RegionScope r4(h, "k_update_finalize");
-    k_update_finalize4<<<grid_for(BK, 256, 64), 256, 0, h->stream>>>(a, h->use_xch ? h->xch : Upd4Xch{}, t1 * nb, h->O.p, h->E.p);
+    k_single_pass_finalize<<<grid_for(BK, 256, 64), 256, 0, h->stream>>>(a, h->use_xch ? h->xch : PeerXch{}, t1 * nb, h->O.p, h->E.p);
     CKL();
   }
   return push_round_objectives(h, t0, t1);
 }
-// first persistent generation (update_kernel.cuh): look-ahead + update warp groups; serves plans whose CTA
-// ranges are not tuple-aligned.  rounds [t0, t1): t0 == 0 runs the prologue look-ahead.  write_mask: rounds that store R.
-int run_update_v2(hb_handle* h, int T, int t0, int t1, unsigned write_mask) {
+// two-pass kernel (update_two_pass.cuh): look-ahead + update warp groups.  rounds [t0, t1): t0 == 0 runs the
+// prologue look-ahead.  write_mask: rounds that store R.
+int run_update_two_pass(hb_handle* h, int T, int t0, int t1, unsigned write_mask) {
   RegionScope rs(h, "update_R");
   const int nb = h->nb;
   const size_t BK = (size_t)h->B * h->KS, SL = 2 * (BK + h->KS);
-  UpdArgs a = make_upd_args(h, T);
+  TwoPassArgs a = make_two_pass_args(h, T);
   a.write_R_mask = write_mask;
   if (h->world <= 1) {
     a.s_begin = t0 * nb;
     a.s_end = t1 * nb;
     a.prologue = (t0 == 0) ? 1 : 0;
     RegionScope r3(h, "k_update_steps");
-    TRY(upd_launch(h, a, true));
+    TRY(launch_two_pass(h, a, true));
   } else {
     // sharded cells: one launch per step, the step's slot [add_{s-1} | rem_s] all-reduced in between
     RegionScope r3(h, "k_update_steps");
     if (t0 == 0) {
       a.s_begin = a.s_end = 0;
       a.prologue = 1;
-      TRY(upd_launch(h, a, false));
+      TRY(launch_two_pass(h, a, false));
     }
     a.prologue = 0;
     for (int s = t0 * nb; s < t1 * nb; ++s) {
       TRY(allreduce_f(h, h->acc2.p + (size_t)(s + 1) * SL, SL));
       a.s_begin = s;
       a.s_end = s + 1;
-      TRY(upd_launch(h, a, false));
+      TRY(launch_two_pass(h, a, false));
     }
     TRY(allreduce_f(h, h->acc2.p + (size_t)(t1 * nb + 1) * SL, SL));  // slot(S): add_{S-1} (+ look-ahead rem_S)
   }
-  if (h->dbg_cta >= 0 && h->world <= 1) dump_step_trace(h, (t1 - t0) * nb, 16);
   // tables at the end of round t1-1 -> O, E (the chain itself continues from the ring)
   {
     RegionScope r4(h, "k_update_finalize");
-    k_update_finalize<<<grid_for(BK, 256, 64), 256, 0, h->stream>>>(a, t1 * nb, h->O.p, h->E.p);
+    k_two_pass_finalize<<<grid_for(BK, 256, 64), 256, 0, h->stream>>>(a, t1 * nb, h->O.p, h->E.p);
     CKL();
   }
   return push_round_objectives(h, t0, t1);
@@ -1301,32 +1335,7 @@ int run_correct(hb_handle* h) {
   {
     RegionScope rs(h, "ridge_stats");
     CK(cudaMemsetAsync(h->S.p, 0, sizeof(float) * (size_t)J * K * D1, h->stream));
-    if (h->use_tc_stats) {
-      TRY(run_stats_tc(h, h->Zo.p));
-    } else {
-    StatsArgs a;
-      a.R = h->R.p;
-      a.Zo = h->Zo.p;
-      a.tile_cell0 = h->tile_cell0.p;
-      a.tile_len = h->tile_len.p;
-      a.tile_tuple = h->tile_tuple.p;
-      a.S = h->S.p;
-      a.ntiles = h->ntiles;
-      a.d = d;
-      a.K = K;
-      a.KS = (K <= 128) ? K : 128;
-      a.ldR = h->KS;
-      a.ldZ = h->DS;
-      const int KSP = (a.KS + 7) & ~7, DP = (D1 + 3) & ~3;
-      dim3 block(DP / 4, KSP / 8);
-      if (block.x * block.y > 1024) return fail(h, 2, "d = %d is too large for the statistics kernel", d);
-      a.tiles_per_cta = std::max(1, (h->ntiles + h->num_sms * 4 - 1) / (h->num_sms * 4));
-      dim3 grid((h->ntiles + a.tiles_per_cta - 1) / a.tiles_per_cta, (K + a.KS - 1) / a.KS);
-      size_t smem = sizeof(float) * (size_t)TM * (KSP + DP);
-      CK(cudaFuncSetAttribute(k_ridge_stats, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-      k_ridge_stats<<<grid, block, smem, h->stream>>>(a);
-      CKL();
-    }
+    TRY(run_stats_tc(h, h->Zo.p));
     TRY(allreduce_f(h, h->S.p, (size_t)J * K * D1));
   }
   {
@@ -1357,7 +1366,7 @@ int run_correct(hb_handle* h) {
     k_ridge_solve<<<K, 256, sizeof(int) * (size_t)(B + C), h->stream>>>(a);
     CKL();
   }
-  if (h->use_tc_apply) {
+  if (h->paths.mm.apply) {
     RegionScope rs(h, "ridge_apply");
     ApplyTcArgs a;
     a.R = h->R.p;
@@ -1374,13 +1383,6 @@ int run_correct(hb_handle* h) {
     a.DS = h->DS;
     a.tiles_per_cta = std::max(1, (h->ntiles + h->num_sms - 1) / h->num_sms);
     a.dbg = nullptr;
-    static int ap_calls = 0;
-    const bool tracing = getenv("HB_TRACE_APPLY") != nullptr && (++ap_calls == 4);
-    if (tracing) {
-      if (h->dbg.n < 64 * 12) CK(h->dbg.alloc(64 * 12));
-      CK(cudaMemsetAsync(h->dbg.p, 0, sizeof(long long) * 64 * 12, h->stream));
-      a.dbg = h->dbg.p;
-    }
     const int grid = (h->ntiles + a.tiles_per_cta - 1) / a.tiles_per_cta;
     {
       // cluster ranges of at most AP_MAXK clusters (shared memory), equal sizes, multiples of 8: the first launch
@@ -1401,20 +1403,6 @@ int run_correct(hb_handle* h) {
           k_apply_tc<2><<<grid, AP_THREADS, smem, h->stream>>>(a);
         }
         CKL();
-        a.dbg = nullptr;
-      }
-    }
-    if (tracing) {
-      std::vector<long long> st(32 * 16);
-      CK(cudaMemcpyAsync(st.data(), h->dbg.p, sizeof(long long) * st.size(), cudaMemcpyDeviceToHost, h->stream));
-      CK(cudaStreamSynchronize(h->stream));
-      if (FILE* f = fopen("gpurun_out/apply_trace.txt", "w")) {
-        for (int i = 0; i < 32; ++i) {
-          fprintf(f, "%d", i);
-          for (int k = 0; k < 16; ++k) fprintf(f, " %lld", st[(size_t)i * 16 + k] ? st[(size_t)i * 16 + k] - st[0] : -1);
-          fprintf(f, "\n");
-        }
-        fclose(f);
       }
     }
     return 0;
@@ -1922,18 +1910,11 @@ int hb_setup(hb_handle* h, const double* Z, int d, int64_t N, const int32_t* phi
   const int KS = h->KS, DS = h->DS;
   const size_t nK = (size_t)N * KS, nd = (size_t)N * DS, BK = (size_t)B * KS;
   const int Tplan = std::max(1, (int)h->max_iter_kmeans);
-  // update_R kernels: the single-pass persistent kernel when every CTA's slice of a block can lie inside one
-  // covariate tuple (2 J <= #SMs) and its ring fits shared memory; else the first persistent generation (K <= 256,
-  // <= 8192 tuples, checked against the shared-memory limit); else one launch triple per block step.
-  const size_t smem_limit = (size_t)227 * 1024 - 256;
-  const bool force_v1 = (h->kernel_set & HB_KS_UPDATE_PER_STEP) != 0, force_v2 = (h->kernel_set & HB_KS_UPDATE_TWO_PASS) != 0;
   h->coop_grid = h->num_sms;  // one persistent CTA per SM
-  h->aligned_ranges = (2 * J <= h->coop_grid);
-  h->u5_ring_rows = upd5_ring_rows(KS, smem_limit);
-  h->use_v4 = !force_v1 && !force_v2 && h->aligned_ranges && h->u5_ring_rows > 0 && (uint64_t)N * (uint64_t)KS < (1ull << 32);
-  h->use_v2 = h->use_v4 || (!force_v1 && (KS <= 256) && (J <= 8192) && upd_smem_bytes(h) <= smem_limit);
-  h->plan_nsub = (h->use_v4 && h->nb <= 64) ? h->nb : 1;
-  h->plan_rounds = Tplan;
+  h->paths = select_kernels(K, d, J, N, h->nb, h->coop_grid, h->kernel_set);
+  h->ring_rows = sp_ring_rows(KS, SMEM_LIMIT);
+  const bool single_pass = h->paths.update == UpdatePath::SinglePass;
+  h->plan_nsub = (single_pass && h->nb <= 64) ? h->nb : 1;
   CK(h->Zo.alloc(nd));
   CK(h->Zc.alloc(nd));
   CK(h->U.alloc(nK));
@@ -1969,15 +1950,8 @@ int hb_setup(hb_handle* h, const double* Z, int d, int64_t N, const int32_t* phi
   CK(h->tc_cell0.alloc(h->tc_ntiles));
   CK(h->tc_len.alloc(h->tc_ntiles));
   CK(h->tc_tuple.alloc(h->tc_ntiles));
-  h->use_tc_apply = (d <= 128) && !(h->kernel_set & HB_KS_FFMA_CONTRACTIONS);   // cluster ranges of <= AP_MAXK per launch
-  h->use_tc_stats = !(h->kernel_set & HB_KS_FFMA_CONTRACTIONS);                  // 128 clusters x 64 columns per launch
-  h->assign_ns = assign3_smem_bytes(2, (d + 7) & ~7, (K + 15) & ~15, KS) <= smem_limit ? 2 : 1;
-  h->use_tc_assign = (d <= 64) && (K <= 128) && assign3_smem_bytes(h->assign_ns, (d + 7) & ~7, (K + 15) & ~15, KS) <= smem_limit &&
-                     !(h->kernel_set & HB_KS_FFMA_CONTRACTIONS);
-  h->use_tc_logits = !h->use_tc_assign && (d <= 128) && logits_smem_bytes((d + 7) & ~7) <= smem_limit &&
-                     !(h->kernel_set & HB_KS_FFMA_CONTRACTIONS);
   h->pt_cap = (size_t)N / TC_TM + (size_t)h->nb * J + 2;
-  if (h->use_tc_assign && h->use_v4) {
+  if (h->paths.mm.k1_stages && single_pass) {
     CK(h->pt_p0.alloc(2 * h->pt_cap));
     CK(h->pt_len.alloc(2 * h->pt_cap));
     CK(h->pt_tuple.alloc(2 * h->pt_cap));
@@ -1987,12 +1961,7 @@ int hb_setup(hb_handle* h, const double* Z, int d, int64_t N, const int32_t* phi
   }
   CK(h->chunk_start.alloc(h->nchunks + 1));
   CK(h->tuple_chunk0.alloc(J));
-  CK(h->blk_of.alloc(2 * (size_t)Tplan * N));
-  CK(h->order.alloc(2 * (size_t)Tplan * N));
-  if (h->use_v4)
-    CK(h->next_at.alloc(2 * (size_t)Tplan * N));
-  else
-    CK(h->prev_at.alloc(2 * (size_t)Tplan * N));
+  TRY(alloc_plan_rounds(h, Tplan));
   {  // histogram scratch of the plan's counting sort: as many rounds per launch as fit 64 MB (at most 8)
     const size_t per_round = (size_t)h->nb * h->plan_nsub * h->nchunks;
     h->plan_batch = (int)std::max<size_t>(1, std::min<size_t>({(size_t)8, (size_t)Tplan, ((size_t)16 << 20) / std::max<size_t>(1, per_round)}));
@@ -2001,26 +1970,14 @@ int hb_setup(hb_handle* h, const double* Z, int d, int64_t N, const int32_t* phi
   }
   CK(h->chunk_q0.alloc(h->nchunks));
   CK(h->chunk_nq.alloc(h->nchunks));
-  CK(h->seg_start.alloc(2 * (size_t)Tplan * ((size_t)h->nb * J + 1)));
-  CK(h->tile_base.alloc(2 * (size_t)Tplan * ((size_t)h->nb * J + 1)));
-  if (h->use_v2) {
+  if (h->paths.update != UpdatePath::PerStep) {
     CK(h->ring.alloc(4 * BK));
-    CK(h->acc2.alloc(2 * (BK + KS) * ((size_t)Tplan * h->nb + 2)));
-    CK(h->Psave.alloc(h->use_v4 ? 1 : 2 * (size_t)h->nb * BK));
-    if (h->use_v4) CK(h->remT.alloc(2 * (size_t)h->nb * J * KS));
-    if (h->use_v4 && h->world > 1) CK(h->remS.alloc((size_t)h->nb * J * KS));
-    CK(h->OEend.alloc((size_t)Tplan * 2 * BK));
-    CK(h->obj2.alloc(2 * (size_t)Tplan));
-    CK(h->bar.alloc(2 * ((size_t)Tplan * h->nb + 2)));
-    if (h->aligned_ranges) CK(h->ranges.alloc(2 * (size_t)Tplan * h->nb * h->coop_grid));
+    CK(h->Psave.alloc(single_pass ? 1 : 2 * (size_t)h->nb * BK));
+    if (single_pass) CK(h->remT.alloc(2 * (size_t)h->nb * J * KS));
+    if (single_pass && h->world > 1) CK(h->remS.alloc((size_t)h->nb * J * KS));
     release_peer_exchange(h);
-    if (h->use_v4 && h->world > 1 && h->world <= U4_MAXWORLD && !(h->kernel_set & HB_KS_NO_PEER_EXCHANGE))
+    if (single_pass && h->world > 1 && h->world <= XCH_MAXWORLD && !(h->kernel_set & HB_KS_NO_PEER_EXCHANGE))
       TRY(setup_peer_exchange(h, Tplan));
-    if (const char* e = getenv("HB_TRACE_STEPS")) {
-      h->dbg_cta = atoi(e);
-      CK(h->dbg.alloc((size_t)(32 * h->nb + 2) * 16));
-      CK(cudaMemsetAsync(h->dbg.p, 0, sizeof(long long) * (size_t)(32 * h->nb + 2) * 16, h->stream));
-    }
     CK(cudaMemsetAsync(h->Psave.p, 0, sizeof(float) * h->Psave.n, h->stream));
     CK(cudaMemsetAsync(h->ring.p, 0, sizeof(float) * 4 * BK, h->stream));
   }
@@ -2141,17 +2098,15 @@ int hb_init_cluster(hb_handle* h, const double* Y0) {
     // (2) the races of all centroids in one pass over the cells (a centroid's race only looks at its own start cell)
     // both steps run from tensor-core logits U = 2 (z . y - 1) (k_logits_tc, sigma = 1) when that kernel takes the
     // shape; else from the FFMA kernels (thread per cell)
-    const bool tc_init = (d <= 128) && logits_smem_bytes((d + 7) & ~7) <= (size_t)227 * 1024 - 256 && h->KS <= 256 &&
-                         !(h->kernel_set & HB_KS_FFMA_CONTRACTIONS);
     DevBuf<float> ones, yy;
-    if (tc_init) {
+    if (h->paths.mm.kmeans) {
       CK(ones.alloc(K));
       CK(yy.alloc(K));
       k_fill_f<<<1, 256, 0, h->stream>>>(ones.p, (int64_t)K, 1.0f);
       CKL();
     }
     const size_t smem_pp = sizeof(float) * Kd;
-    if (!tc_init) {
+    if (!h->paths.mm.kmeans) {
       if (smem_pp > 200 * 1024) return fail(h, 2, "K*d too large for the native k-means initialisation; pass Y0");
       CK(cudaFuncSetAttribute(k_kmeans_race, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_pp));
     }
@@ -2164,13 +2119,13 @@ int hb_init_cluster(hb_handle* h, const double* Y0) {
         CK(cudaMemcpyAsync(taken_d.p, taken.data(), sizeof(int64_t) * taken.size(), cudaMemcpyHostToDevice, h->stream));
       }
       CK(cudaMemsetAsync(best_d.p + i0, 0xff, sizeof(unsigned long long) * (i1 - i0), h->stream));
-      if (tc_init) {
+      if (h->paths.mm.kmeans) {
         if (!logits_of_start) {
           TRY(launch_logits(h, ones.p, false));
           logits_of_start = true;
         }
         const int grid_r = grid_for(h->n * 32, 256, h->num_sms * 8);
-        if (upd4_nv(h->KS) == 1)
+        if (sp_nv(h->KS) == 1)
           k_kmeans_race_u<1><<<grid_r, 256, 0, h->stream>>>(h->U.p, h->sort_perm.p, best_d.p, taken.empty() ? nullptr : taken_d.p,
                                                           (int)taken.size(), h->n, K, h->KS, h->cell_offset, seed, i0, i1);
         else
@@ -2206,15 +2161,15 @@ int hb_init_cluster(hb_handle* h, const double* Y0) {
     h->kmeans_cells = cells;
     TRY(gather(-1));
     const size_t smem = sizeof(float) * Kd;
-    if (!tc_init) CK(cudaFuncSetAttribute(k_kmeans_assign, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    if (!h->paths.mm.kmeans) CK(cudaFuncSetAttribute(k_kmeans_assign, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     for (int iter = 0; iter < 10; ++iter) {
-      if (tc_init) {
+      if (h->paths.mm.kmeans) {
         // Lloyd iteration on the tensor cores: logits -> one-hot rows of R -> members' sums and counts (K3) -> means
         TRY(launch_logits(h, ones.p, false));
         k_kmeans_norms<<<(K + 127) / 128, 128, 0, h->stream>>>(h->Y.p, yy.p, K, d);
         CKL();
         const int grid_p = grid_for(h->n * 32, 256, h->num_sms * 8);
-        if (upd4_nv(h->KS) == 1)
+        if (sp_nv(h->KS) == 1)
           k_kmeans_pick<1><<<grid_p, 256, 0, h->stream>>>(h->U.p, yy.p, h->R.p, h->n, K, h->KS);
         else
           k_kmeans_pick<2><<<grid_p, 256, 0, h->stream>>>(h->U.p, yy.p, h->R.p, h->n, K, h->KS);
@@ -2259,32 +2214,7 @@ int legacy_centroid_step(hb_handle* h) {
   const int D1 = d + 1;
   const size_t nK = (size_t)h->n * KS, BK = (size_t)B * KS;
   CK(cudaMemsetAsync(h->S.p, 0, sizeof(float) * (size_t)J * K * D1, h->stream));
-  if (h->use_tc_stats) {
-    TRY(run_stats_tc(h, h->Zc.p));  // the statistics of the corrected, normalised embedding
-  } else {
-    StatsArgs a;
-    a.R = h->R.p;
-    a.Zo = h->Zc.p;
-    a.tile_cell0 = h->tile_cell0.p;
-    a.tile_len = h->tile_len.p;
-    a.tile_tuple = h->tile_tuple.p;
-    a.S = h->S.p;
-    a.ntiles = h->ntiles;
-    a.d = d;
-    a.K = K;
-    a.KS = (K <= 128) ? K : 128;
-    a.ldR = KS;
-    a.ldZ = h->DS;
-    const int KSP = (a.KS + 7) & ~7, DP = (D1 + 3) & ~3;
-    dim3 block(DP / 4, KSP / 8);
-    if (block.x * block.y > 1024) return fail(h, 2, "d = %d is too large for the statistics kernel", d);
-    a.tiles_per_cta = std::max(1, (h->ntiles + h->num_sms * 4 - 1) / (h->num_sms * 4));
-    dim3 grid((h->ntiles + a.tiles_per_cta - 1) / a.tiles_per_cta, (K + a.KS - 1) / a.KS);
-    size_t smem = sizeof(float) * (size_t)TM * (KSP + DP);
-    CK(cudaFuncSetAttribute(k_ridge_stats, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    k_ridge_stats<<<grid, block, smem, h->stream>>>(a);
-    CKL();
-  }
+  TRY(run_stats_tc(h, h->Zc.p));  // the statistics of the corrected, normalised embedding
   TRY(allreduce_f(h, h->S.p, (size_t)J * K * D1));
   k_centroids_from_stats<<<K, 64, sizeof(float) * (size_t)d, h->stream>>>(h->S.p, h->Y.p, J, K, d);
   CKL();
@@ -2310,25 +2240,8 @@ int ensure_plan_rounds(hb_handle* h, int T) {
   CK(cudaStreamSynchronize(h->stream));
   h->next_ready = false;
   h->plan_set = 0;
-  const size_t BK = (size_t)h->B * h->KS;
-  const size_t S1 = (size_t)h->nb * h->J + 1;
-  CK(h->blk_of.alloc(2 * (size_t)T * h->n));
-  CK(h->order.alloc(2 * (size_t)T * h->n));
-  if (h->use_v4)
-    CK(h->next_at.alloc(2 * (size_t)T * h->n));
-  else
-    CK(h->prev_at.alloc(2 * (size_t)T * h->n));
-  CK(h->seg_start.alloc(2 * (size_t)T * S1));
-  CK(h->tile_base.alloc(2 * (size_t)T * S1));
-  if (h->use_v2) {
-    CK(h->acc2.alloc(2 * (BK + h->KS) * ((size_t)T * h->nb + 2)));
-    CK(h->OEend.alloc((size_t)T * 2 * BK));
-    CK(h->obj2.alloc(2 * (size_t)T));
-    CK(h->bar.alloc(2 * ((size_t)T * h->nb + 2)));
-    if (h->aligned_ranges) CK(h->ranges.alloc(2 * (size_t)T * h->nb * h->coop_grid));
-    if (h->use_xch) TRY(setup_peer_exchange(h, T));  // collective: every rank grows its plan in the same call
-  }
-  h->plan_rounds = T;
+  TRY(alloc_plan_rounds(h, T));
+  if (h->use_xch) TRY(setup_peer_exchange(h, T));  // collective: every rank grows its plan in the same call
   return 0;
 }
 
@@ -2339,11 +2252,8 @@ int hb_cluster(hb_handle* h, const int64_t* update_orders) {
   const unsigned T = h->max_iter_kmeans;
   const bool cold = h->harmony_slots.size() != 1;  // harmony.cpp:214-228 cold start
   TRY(ensure_plan_rounds(h, (int)std::max(1u, T)));
-  // the first persistent generation keeps its R-store rounds in a 32-bit mask: longer calls run the per-round path
-  const bool persistent = h->use_v2 && !h->legacy_centroid && (h->use_v4 || T <= 31);
-  // The single-pass update kernel takes round 0's removal sums from the assignment step itself when that step
-  // runs in plan order (tensor-core kernel); every other combination runs the assignment in natural order first.
-  const bool plan_assign = cold && persistent && h->use_v4 && (h->use_tc_assign || h->use_tc_logits) && T > 0;
+  const CallPath call = call_path(h->paths, T, h->legacy_centroid);
+  const bool plan_assign = cold && call.plan_order_assign;
   if (cold && !plan_assign) {
     TRY(run_assign(h, true, false, false));  // the cold start does not evaluate the objective
     CK(cudaMemsetAsync(h->obj_acc.p, 0, 2 * sizeof(double), h->stream));
@@ -2355,8 +2265,7 @@ int hb_cluster(hb_handle* h, const int64_t* update_orders) {
   }
   if (h->abort_cb && h->abort_cb(h->abort_user)) return -1;  // Progress::check_abort (:233)
   unsigned iter = 0;
-  if (h->legacy_centroid) {
-    // compatibility path: centroid step + one first-generation update_R per round
+  if (call.update == UpdatePath::PerStep) {
     if (h->next_ready) {  // a plan prebuilt by an earlier call on the side stream is not used here
       CK(cudaStreamWaitEvent(h->stream, h->plan_done, 0));
       h->round_counter -= (uint64_t)h->next_T;
@@ -2364,10 +2273,10 @@ int hb_cluster(hb_handle* h, const int64_t* update_orders) {
     }
     for (iter = 0; iter < T; iter++) {
       if (iter > 0 && h->abort_cb && h->abort_cb(h->abort_user)) return -1;
-      TRY(legacy_centroid_step(h));  // :235-238
+      if (h->legacy_centroid) TRY(legacy_centroid_step(h));  // :235-238
       TRY(build_plan_single(h, update_orders ? h->perms_d.p + (size_t)iter * (size_t)h->N_global : nullptr, h->stream));
-      TRY(run_update_R_v1(h, 0));  // :241
-      TRY(push_objective(h));      // :248
+      TRY(run_update_per_step(h, 0));  // :241
+      TRY(push_objective(h));          // :248
       if (iter > h->window_size) {  // :250-256
         int conv = 0;
         TRY(check_convergence_host(h, 0, &conv));
@@ -2377,7 +2286,7 @@ int hb_cluster(hb_handle* h, const int64_t* update_orders) {
         }
       }
     }
-  } else if (persistent) {
+  } else {
     // all T update orders are drawn up front (they do not depend on the data), then the rounds run in
     // chunks: [0, window_size + 2) in one launch, afterwards one round per launch (convergence checks)
     // The native orders of a call depend only on (seed, round counter), so the plan of the NEXT call is
@@ -2394,12 +2303,12 @@ int hb_cluster(hb_handle* h, const int64_t* update_orders) {
     } else {
       TRY(build_plans(h, (int)T, update_orders ? h->perms_d.p : nullptr, h->plan_set, h->stream));
     }
-    if (T > 0) TRY(upd_begin_zero(h, (int)T));
+    if (T > 0) TRY(update_begin_zero(h, (int)T));
     if (plan_assign) {
       TRY(run_assign(h, true, true, false));
       CK(cudaMemsetAsync(h->obj_acc.p, 0, 2 * sizeof(double), h->stream));
     }
-    if (T > 0) TRY(upd_begin_seed(h));
+    if (T > 0) TRY(update_begin_seed(h));
     unsigned t0 = 0;
     while (t0 < T) {
       unsigned t1 = (t0 == 0) ? std::min(T, h->window_size + 2) : t0 + 1;
@@ -2407,10 +2316,10 @@ int hb_cluster(hb_handle* h, const int64_t* update_orders) {
       for (unsigned t = t0; t < t1; ++t)
         if (t < 32 && (t == T - 1 || t > h->window_size)) mask |= 1u << t;  // rounds after which cluster_cpp may stop
       if (t0 > 0 && h->abort_cb && h->abort_cb(h->abort_user)) return -1;
-      if (h->use_v4)
-        TRY(run_update_v4(h, (int)T, (int)t0, (int)t1, plan_assign));
+      if (call.update == UpdatePath::SinglePass)
+        TRY(run_update_single_pass(h, (int)T, (int)t0, (int)t1, plan_assign));
       else
-        TRY(run_update_v2(h, (int)T, (int)t0, (int)t1, mask));
+        TRY(run_update_two_pass(h, (int)T, (int)t0, (int)t1, mask));
       iter = t1;
       if (t1 - 1 > h->window_size) {  // :250-256
         int conv = 0;
@@ -2419,28 +2328,8 @@ int hb_cluster(hb_handle* h, const int64_t* update_orders) {
       }
       t0 = t1;
     }
-  } else {
-    if (h->next_ready) {  // a plan prebuilt by an earlier call on the side stream is not used here
-      CK(cudaStreamWaitEvent(h->stream, h->plan_done, 0));
-      h->round_counter -= (uint64_t)h->next_T;
-      h->next_ready = false;
-    }
-    for (iter = 0; iter < T; iter++) {
-      if (iter > 0 && h->abort_cb && h->abort_cb(h->abort_user)) return -1;
-      TRY(build_plan_single(h, update_orders ? h->perms_d.p + (size_t)iter * (size_t)h->N_global : nullptr, h->stream));
-      TRY(run_update_R_v1(h, 0));  // :241
-      TRY(push_objective(h));      // :248
-      if (iter > h->window_size) {  // :250-256
-        int conv = 0;
-        TRY(check_convergence_host(h, 0, &conv));
-        if (conv) {
-          iter++;
-          break;
-        }
-      }
-    }
   }
-  if (persistent && !update_orders && T > 0 && !h->timing && !(h->kernel_set & HB_KS_NO_PLAN_OVERLAP)) {
+  if (call.update != UpdatePath::PerStep && !update_orders && T > 0 && !h->timing) {
     // prebuild the next call's plan into the other buffer set on the side stream; it starts once this
     // call's own (main-stream) plan build and update kernel are done with the shared scan scratch
     CK(cudaEventRecord(h->ev0, h->stream));
@@ -2699,12 +2588,22 @@ int hb_debug_widen(double* out, const float* in, int64_t n, int threads) {
 int hb_debug_update_geometry(int KS, int nb, int64_t out[9]) {
   (void)nb;
   if (KS <= 0 || (KS & 3)) return 0;
-  const int D = upd5_ring_rows(KS, (size_t)227 * 1024 - 256);
+  const int D = sp_ring_rows(KS, SMEM_LIMIT);
   if (D <= 0) return 0;
-  const int nv = upd4_nv(KS), ru = upd5_ru(nv);
-  const int64_t v[9] = {nv, D / ru, ru, (int64_t)upd5_smem_bytes(nv, D, KS), U5_NW, 0, 0, 0, 0};
+  const int nv = sp_nv(KS), ru = sp_ru(nv);
+  const int64_t v[9] = {nv, D / ru, ru, (int64_t)sp_smem_bytes(nv, D, KS), SP_NW, 0, 0, 0, 0};
   for (int i = 0; i < 9; ++i) out[i] = v[i];
   return 1;
+}
+
+// Kernels hb_setup picks for a shape, and the update path of a cluster_cpp call (test hook, host only).
+int hb_debug_kernel_paths(int K, int d, int J, int64_t n, int nb, int num_sms, int kernel_set, int64_t out[8]) {
+  const KernelPaths p = select_kernels(K, d, J, n, nb, num_sms, kernel_set);
+  const int64_t v[8] = {(int64_t)p.update, p.mm.k1_stages, p.mm.logits, p.mm.apply, p.mm.kmeans,
+                        call_path(p, 20, false).plan_order_assign, (int64_t)call_path(p, 40, false).update,
+                        (int64_t)call_path(p, 20, true).update};
+  for (int i = 0; i < 8; ++i) out[i] = v[i];
+  return 0;
 }
 
 // Test hooks of the native kmeans_centers: the uniform of (centroid i, global cell g) under the handle's seed, and

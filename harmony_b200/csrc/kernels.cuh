@@ -1,4 +1,4 @@
-// kernels.cuh — CUDA kernels of the Harmony hot loop (sm_90a).  FFMA generation ("v1"): every
+// kernels.cuh — CUDA kernels of the Harmony hot loop (sm_90a).  FFMA kernels: every
 // contraction is a shared-memory-tiled fp32 kernel; they double as the in-repo correctness anchor
 // for the wgmma versions.
 //
@@ -890,200 +890,6 @@ __global__ void k_plan_tilecount(const int* __restrict__ seg_start, int S, int* 
   }
 }
 
-// ------------------------------------------------------------------------------------------------
-// update_R block step (harmony.cpp:293-332)
-// ------------------------------------------------------------------------------------------------
-struct StepArgs {
-  const float* U;
-  float* R;
-  const int* order;         // [n] cells sorted by (block, tuple, cell)
-  const int* seg_start;     // [nb*J + 1]
-  const int* tile_base;     // [nb*J + 1] exclusive scan of tiles per segment
-  const int* tuple_levels;  // [J][C]
-  const float* sigma;
-  const float* P;           // [B][K] penalty table of this step
-  float* acc_O;             // [B][K] column sums per level (rem_j or add_j)
-  float* acc_rs;            // [K]
-  double* obj_acc;          // [2]
-  int blk, J, K, C, KP, KS;
-};
-
-// tile -> (segment, first position, length)
-__device__ __forceinline__ bool locate_tile(const StepArgs& a, int t, int* sh_info) {
-  // sh_info: [0] seg, [1] p0, [2] len, [3] valid
-  if (threadIdx.x == 0) {
-    int s_lo = a.blk * a.J, s_hi = (a.blk + 1) * a.J;
-    int t0 = a.tile_base[s_lo], t1 = a.tile_base[s_hi];
-    int tt = t0 + t;
-    if (tt >= t1) {
-      sh_info[3] = 0;
-    } else {
-      int lo = s_lo, hi = s_hi;  // find the last seg with tile_base[seg] <= tt
-      while (hi - lo > 1) {
-        int mid = (lo + hi) >> 1;
-        if (a.tile_base[mid] <= tt) lo = mid; else hi = mid;
-      }
-      int p0 = a.seg_start[lo] + (tt - a.tile_base[lo]) * TM;
-      int len = a.seg_start[lo + 1] - p0;
-      sh_info[0] = lo;
-      sh_info[1] = p0;
-      sh_info[2] = len < TM ? len : TM;
-      sh_info[3] = 1;
-    }
-  }
-  __syncthreads();
-  return sh_info[3] != 0;
-}
-
-// Step 1 (:312-313): column sums of the block's current R, per level  ->  acc_O / acc_rs
-template <int KQ>
-__global__ void __launch_bounds__(ROW_THREADS) k_block_colsum(StepArgs a) {
-  extern __shared__ __align__(16) float smem[];
-  __shared__ int info[4];
-  const int K = a.K, KP = a.KP;
-  float* part = smem;  // [NWARP][KP]
-  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  for (int t = blockIdx.x;; t += gridDim.x) {
-    __syncthreads();
-    if (!locate_tile(a, t, info)) break;
-    const int seg = info[0], p0 = info[1], len = info[2];
-    const int q = seg - a.blk * a.J;
-    float cs[KQ];
-#pragma unroll
-    for (int qq = 0; qq < KQ; ++qq) cs[qq] = 0.f;
-    for (int r = warp; r < len; r += NWARP) {
-      const size_t row = (size_t)a.order[p0 + r];
-#pragma unroll
-      for (int qq = 0; qq < KQ; ++qq) {
-        int k = lane + 32 * qq;
-        if (k < K) cs[qq] += a.R[row * a.KS + k];
-      }
-    }
-#pragma unroll
-    for (int qq = 0; qq < KQ; ++qq) {
-      int k = lane + 32 * qq;
-      if (k < KP) part[warp * KP + k] = cs[qq];
-    }
-    __syncthreads();
-    for (int k = tid; k < K; k += ROW_THREADS) {
-      float s = 0.f;
-#pragma unroll
-      for (int w = 0; w < NWARP; ++w) s += part[w * KP + k];
-      atomicAdd(a.acc_rs + k, s);
-      for (int c = 0; c < a.C; ++c) atomicAdd(a.acc_O + (size_t)a.tuple_levels[q * a.C + c] * a.KS + k, s);
-    }
-  }
-}
-
-// Finish step j-1 and start step j on the K x B tables:
-//   O += add_prev; E += rs_add_prev*Pr_b        (:329-330 of the previous block)
-//   O -= rem;      E -= rs_rem*Pr_b             (:312-313 of this block)
-//   P = ((2E+1)/(O+E+1))^theta                  (:322, harmony_pow utils.cpp:84-90)
-// add_prev / rem may be null (first step of a round / finalisation after the last step).
-__global__ void k_step_prepare(float* __restrict__ O, float* __restrict__ E, const float* __restrict__ add_O,
-                               const float* __restrict__ add_rs, const float* __restrict__ rem_O,
-                               const float* __restrict__ rem_rs, const float* __restrict__ Pr_b,
-                               const float* __restrict__ theta, float* __restrict__ P, int B, int K, int KS) {
-  int idx = blockIdx.x * blockDim.x + threadIdx.x;
-  if (idx >= B * KS) return;
-  int b = idx / KS, k = idx - b * KS;
-  if (k >= K) return;
-  float o = O[idx], e = E[idx];
-  if (add_O) {
-    e += add_rs[k] * Pr_b[b];
-    o += add_O[idx];
-  }
-  if (rem_O) {
-    e -= rem_rs[k] * Pr_b[b];
-    o -= rem_O[idx];
-  }
-  O[idx] = o;
-  E[idx] = e;
-  if (P) P[idx] = powf(((2.f * e) + 1.f) / (o + e + 1.f), theta[b]);
-}
-
-// Step 2+3 (:318-330): R = L1norm(exp(U) * sum_c P[level_c]), column sums of the new R -> acc_O/acc_rs,
-// objective partials of the new R.
-template <int KQ>
-__global__ void __launch_bounds__(ROW_THREADS) k_block_update(StepArgs a) {
-  extern __shared__ __align__(16) float smem[];
-  __shared__ int info[4];
-  const int K = a.K, KP = a.KP;
-  float* part = smem;             // [NWARP][KP]
-  float* Psum = part + NWARP * KP;  // [KP]
-  float* lP = Psum + KP;          // [KP]
-  float* sig = lP + KP;           // [KP]
-  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  for (int k = tid; k < KP; k += ROW_THREADS) sig[k] = (k < K) ? a.sigma[k] : 1.f;
-  float okd = 0.f, oent = 0.f;
-  for (int t = blockIdx.x;; t += gridDim.x) {
-    __syncthreads();
-    if (!locate_tile(a, t, info)) break;
-    const int seg = info[0], p0 = info[1], len = info[2];
-    const int q = seg - a.blk * a.J;
-    for (int k = tid; k < K; k += ROW_THREADS) {
-      float s = 0.f;
-      for (int c = 0; c < a.C; ++c) s += a.P[(size_t)a.tuple_levels[q * a.C + c] * a.KS + k];
-      Psum[k] = s;
-      lP[k] = logf(s);
-    }
-    __syncthreads();
-    float cs[KQ];
-#pragma unroll
-    for (int qq = 0; qq < KQ; ++qq) cs[qq] = 0.f;
-    for (int r = warp; r < len; r += NWARP) {
-      const size_t row = (size_t)a.order[p0 + r];
-      float u[KQ], e[KQ];
-      float s = 0.f;
-#pragma unroll
-      for (int qq = 0; qq < KQ; ++qq) {
-        int k = lane + 32 * qq;
-        if (k < K) {
-          u[qq] = ld_stream(a.U + row * a.KS + k);
-          e[qq] = expf(u[qq]) * Psum[k];
-        } else {
-          u[qq] = 0.f;
-          e[qq] = 0.f;
-        }
-        s += fabsf(e[qq]);
-      }
-      s = warp_sum(s);
-      const float sdiv = (s == 0.f) ? 1.f : s;  // arma::normalise(.., 1, 0): zero norm divides by 1
-      const float ls = logf(sdiv);
-#pragma unroll
-      for (int qq = 0; qq < KQ; ++qq) {
-        int k = lane + 32 * qq;
-        if (k < K) {
-          float rv = e[qq] / sdiv;
-          st_stream(a.R + row * a.KS + k, rv);
-          cs[qq] += rv;
-          okd += rv * (-sig[k] * u[qq]);
-          if (rv > 0.f) oent += sig[k] * rv * (u[qq] + lP[k] - ls);
-        }
-      }
-    }
-#pragma unroll
-    for (int qq = 0; qq < KQ; ++qq) {
-      int k = lane + 32 * qq;
-      if (k < KP) part[warp * KP + k] = cs[qq];
-    }
-    __syncthreads();
-    for (int k = tid; k < K; k += ROW_THREADS) {
-      float s = 0.f;
-#pragma unroll
-      for (int w = 0; w < NWARP; ++w) s += part[w * KP + k];
-      atomicAdd(a.acc_rs + k, s);
-      for (int c = 0; c < a.C; ++c) atomicAdd(a.acc_O + (size_t)a.tuple_levels[q * a.C + c] * a.KS + k, s);
-    }
-  }
-  okd = warp_sum(okd);
-  oent = warp_sum(oent);
-  if (lane == 0) {
-    atomicAdd(a.obj_acc + 0, (double)okd);
-    atomicAdd(a.obj_acc + 1, (double)oent);
-  }
-}
-
 // compute_objective (harmony.cpp:158-170) once the per-cell sums are known:
 //   cross = sum_kb sigma_k theta_b log((O+E+1)/(2E+1)) O_kb   (== the reference's N-pass, SURVEY §8a')
 // Appends (total, dist, entropy, cross) * 2000/N to the device trace at slot `slot` and clears obj_acc.
@@ -1140,96 +946,6 @@ __global__ void __launch_bounds__(ROW_THREADS) k_objective_cells(const float* __
     atomicAdd(obj_acc + 0, (double)okd);
     atomicAdd(obj_acc + 1, (double)oent);
   }
-}
-
-// ------------------------------------------------------------------------------------------------
-// K3: ridge sufficient statistics (harmony.cpp:561-567, 592-609 for all clusters at once)
-//   S[q][k][0..d-1] = sum_{i in tuple q} R_ik * Zo_i      S[q][k][d] = sum_{i in tuple q} R_ik
-// Output-stationary fp32 register tiling: thread (ty, tx) owns clusters ty*8..+7 x columns tx*4..+3.
-// ------------------------------------------------------------------------------------------------
-struct StatsArgs {
-  const float* R;
-  const float* Zo;
-  const int* tile_cell0;
-  const int* tile_len;
-  const int* tile_tuple;
-  float* S;  // [J][K][d+1]
-  int ntiles, d, K, KS;  // KS = clusters per K-slice (blockIdx.y)
-  int tiles_per_cta;
-  int ldR, ldZ;          // row strides of R and Zo
-};
-
-__global__ void k_ridge_stats(StatsArgs a) {
-  extern __shared__ __align__(16) float smem[];
-  const int d = a.d, K = a.K, D1 = d + 1;
-  const int k0 = blockIdx.y * a.KS;
-  const int ks = (K - k0 < a.KS) ? K - k0 : a.KS;  // clusters in this slice
-  const int KSP = (a.KS + 7) & ~7;                   // padded slice width (multiple of 8)
-  const int DP = (D1 + 3) & ~3;
-  float* Rs = smem;                      // [TM][KSP]
-  float* Zs = Rs + (size_t)TM * KSP;     // [TM][DP]
-  const int tx = threadIdx.x, ty = threadIdx.y;
-  const int tid = ty * blockDim.x + tx, nthr = blockDim.x * blockDim.y;
-  float acc[8][4];
-#pragma unroll
-  for (int i = 0; i < 8; ++i)
-#pragma unroll
-    for (int j = 0; j < 4; ++j) acc[i][j] = 0.f;
-  int cur_q = -1;
-  const int t_begin = blockIdx.x * a.tiles_per_cta;
-  const int t_end = (t_begin + a.tiles_per_cta < a.ntiles) ? t_begin + a.tiles_per_cta : a.ntiles;
-
-  auto flush = [&](int q) {
-    if (q < 0) return;
-#pragma unroll
-    for (int i = 0; i < 8; ++i) {
-      int k = ty * 8 + i;
-      if (k < ks) {
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-          int c = tx * 4 + j;
-          if (c < D1) atomicAdd(a.S + ((size_t)q * K + k0 + k) * D1 + c, acc[i][j]);
-          acc[i][j] = 0.f;
-        }
-      } else {
-#pragma unroll
-        for (int j = 0; j < 4; ++j) acc[i][j] = 0.f;
-      }
-    }
-  };
-
-  for (int tile = t_begin; tile < t_end; ++tile) {
-    const int cell0 = a.tile_cell0[tile], len = a.tile_len[tile], q = a.tile_tuple[tile];
-    if (q != cur_q) {
-      flush(cur_q);
-      cur_q = q;
-    }
-    __syncthreads();
-    for (int idx = tid; idx < TM * KSP; idx += nthr) {
-      int r = idx / KSP, k = idx - r * KSP;
-      Rs[idx] = (r < len && k < ks) ? ld_stream(a.R + (size_t)(cell0 + r) * a.ldR + k0 + k) : 0.f;
-    }
-    for (int idx = tid; idx < TM * DP; idx += nthr) {
-      int r = idx / DP, c = idx - r * DP;
-      float v = 0.f;
-      if (r < len) v = (c < d) ? ld_stream(a.Zo + (size_t)(cell0 + r) * a.ldZ + c) : ((c == d) ? 1.f : 0.f);
-      Zs[idx] = v;
-    }
-    __syncthreads();
-#pragma unroll 2
-    for (int r = 0; r < TM; ++r) {
-      float4 r0 = *reinterpret_cast<const float4*>(Rs + (size_t)r * KSP + ty * 8);
-      float4 r1 = *reinterpret_cast<const float4*>(Rs + (size_t)r * KSP + ty * 8 + 4);
-      float4 z = *reinterpret_cast<const float4*>(Zs + (size_t)r * DP + tx * 4);
-      float rr[8] = {r0.x, r0.y, r0.z, r0.w, r1.x, r1.y, r1.z, r1.w};
-      float zz[4] = {z.x, z.y, z.z, z.w};
-#pragma unroll
-      for (int i = 0; i < 8; ++i)
-#pragma unroll
-        for (int j = 0; j < 4; ++j) acc[i][j] = fmaf(rr[i], zz[j], acc[i][j]);
-    }
-  }
-  flush(cur_q);
 }
 
 // ------------------------------------------------------------------------------------------------

@@ -120,17 +120,16 @@ enum hb_scalar { HB_N = 0, HB_B = 1, HB_K = 2, HB_D = 3, HB_C = 4, HB_ALPHA = 5,
 /* HB_KERNEL_SET (test hook, default 0, read by the next hb_setup): the library picks its kernels from the problem's
  * shape alone; these bits force the kernels that serve shapes outside the default ones' limits onto ANY shape so that
  * the parity suite can hold them to the same bar (tests/test_gpu_parity.py::test_fallback_kernels_match_oracle). */
-enum hb_kernel_set { HB_KS_FFMA_CONTRACTIONS = 1, /* fp32 FFMA assignment / statistics / apply instead of wgmma */
-                     HB_KS_UPDATE_PER_STEP = 2,   /* three launches per block step (first-generation update_R) */
-                     HB_KS_UPDATE_TWO_PASS = 4,   /* first persistent update_R generation (look-ahead + update groups) */
-                     HB_KS_NO_PEER_EXCHANGE = 8,  /* sharded cells: one NCCL all-reduce per block step */
-                     HB_KS_NO_PLAN_OVERLAP = 16   /* build every call's update plan on the main stream */ };
+enum hb_kernel_set { HB_KS_FFMA_CONTRACTIONS = 1, /* fp32 FFMA assignment / apply / k-means initialisation instead of wgmma */
+                     HB_KS_UPDATE_PER_STEP = 2,   /* update_R in three launches per block step */
+                     HB_KS_UPDATE_TWO_PASS = 4,   /* update_R in the two-pass persistent kernel (look-ahead + update groups) */
+                     HB_KS_NO_PEER_EXCHANGE = 8   /* sharded cells: one NCCL all-reduce per block step */ };
 int hb_get_scalar(const hb_handle* h, int which, double* out);
 /* Settable: HB_ALPHA, HB_MAX_ITER_KMEANS (vignettes/detailedWalkthrough.Rmd:364), HB_EPSILON_*, HB_KERNEL_SET and
  * HB_LEGACY_CENTROID_STEP (0/1): run STEP 1 of harmony::cluster_cpp — Y = normalise(Z_corr * R.t()),
  * dist_mat = 2 (1 - Y.t() Z_corr), harmony.cpp:235-238, commented out in 2.0.4 — at the top of every clustering
  * round, as the package version that rendered the reference's vignette did.  Compatibility path: one
- * statistics + assignment pass per round on top of the first-generation update kernels. */
+ * statistics + assignment pass per round on top of the per-step update kernels. */
 int hb_set_scalar(hb_handle* h, int which, double value);
 /* B_vec field (harmony.cpp:683): writes C ints. */
 int hb_get_B_vec(const hb_handle* h, int32_t* out);
@@ -168,6 +167,13 @@ int hb_debug_kmeans_cells(const hb_handle* h, int64_t* out);
  * out = {float4 per lane, row groups per warp ring (a power of two), rows per group, shared-memory bytes, warps per
  * CTA, 0, 0, 0, 0}.  Returns 1 if the shape is supported, 0 if the library would use the other update kernels. */
 int hb_debug_update_geometry(int KS, int nb, int64_t out[9]);
+/* Test hook (host only): the kernels hb_setup picks for K clusters, d dimensions, J covariate tuples, n local cells,
+ * nb update blocks on num_sms SMs under the HB_KERNEL_SET bits kernel_set:
+ * out = {update_R path (0 per step, 1 two-pass, 2 single-pass), operand stages of the fused tensor-core assignment
+ * (0: not fused), tensor-core logits for the plan-order assignment, tensor-core ridge apply, tensor-core k-means
+ * initialisation, cold-start assignment of a 20-round cluster_cpp call in the plan's order, update_R path of a
+ * 40-round call, update_R path of a call with HB_LEGACY_CENTROID_STEP}.  Returns 0. */
+int hb_debug_kernel_paths(int K, int d, int J, int64_t n, int nb, int num_sms, int kernel_set, int64_t out[8]);
 
 #ifdef __cplusplus
 }

@@ -331,10 +331,9 @@ def test_field_writes_and_resume():
 
 
 @pytest.mark.parametrize("kernel_set", [
-    1,    # HB_KS_FFMA_CONTRACTIONS: fp32 FFMA assignment / statistics / apply instead of wgmma
+    1,    # HB_KS_FFMA_CONTRACTIONS: fp32 FFMA assignment / apply / k-means initialisation instead of wgmma
     2,    # HB_KS_UPDATE_PER_STEP: three launches per block step
-    4,    # HB_KS_UPDATE_TWO_PASS: first persistent update_R generation
-    16,   # HB_KS_NO_PLAN_OVERLAP
+    4,    # HB_KS_UPDATE_TWO_PASS: two-pass persistent update_R kernel
 ])
 def test_fallback_kernels_match_oracle(kernel_set):
     """The FFMA / per-step / two-pass kernels that serve shapes outside the default kernels' limits (d > 64, K > 128,

@@ -168,6 +168,34 @@ def test_update_kernel_ring_geometry():
     assert supported >= 50
 
 
+PER_STEP, TWO_PASS, SINGLE_PASS = 0, 1, 2
+C3 = dict(K=100, d=50, J=20, n=1_000_000)
+
+
+# shape -> (update path, fused K1 operand stages (0: FFMA or logits), wgmma logits, wgmma apply, tensor-core k-means
+#           init, cold start in plan order, path of a 40-round call, path of a call with the legacy centroid step)
+@pytest.mark.parametrize("shape, kernel_set, expected", [
+    (C3, 0, (SINGLE_PASS, 2, 0, 1, 1, 1, SINGLE_PASS, PER_STEP)),
+    (dict(K=100, d=50, J=40, n=1_250_000), 0, (SINGLE_PASS, 2, 0, 1, 1, 1, SINGLE_PASS, PER_STEP)),    # c4
+    (dict(K=200, d=100, J=40, n=6_250_000), 0, (SINGLE_PASS, 0, 1, 1, 1, 1, SINGLE_PASS, PER_STEP)),   # c5
+    (dict(K=100, d=50, J=100, n=1_000_000), 0, (TWO_PASS, 2, 0, 1, 1, 0, PER_STEP, PER_STEP)),
+    (dict(K=300, d=50, J=20, n=1_000_000), 0, (PER_STEP, 0, 1, 1, 0, 0, PER_STEP, PER_STEP)),
+    (dict(K=50, d=150, J=20, n=1_000_000), 0, (SINGLE_PASS, 0, 0, 0, 0, 0, SINGLE_PASS, PER_STEP)),
+    (C3, 1, (SINGLE_PASS, 0, 0, 0, 0, 0, SINGLE_PASS, PER_STEP)),    # HB_KS_FFMA_CONTRACTIONS
+    (C3, 2, (PER_STEP, 2, 0, 1, 1, 0, PER_STEP, PER_STEP)),          # HB_KS_UPDATE_PER_STEP
+    (C3, 4, (TWO_PASS, 2, 0, 1, 1, 0, PER_STEP, PER_STEP)),          # HB_KS_UPDATE_TWO_PASS
+    (dict(K=100, d=50, J=20, n=50_000_000), 0, (TWO_PASS, 2, 0, 1, 1, 0, PER_STEP, PER_STEP)),   # n KS >= 2^32
+])
+def test_kernel_paths_per_shape(shape, kernel_set, expected):
+    """The kernels hb_setup picks for a shape on a 132-SM H100 with 20 update blocks (the benchmark's c3 / c4 / c5 and
+    one shape past each limit), and the per-call rule of cluster_cpp: the two-pass kernel keeps R-store rounds in a
+    32-bit mask, so a 40-round call runs the per-step path, as does every call with the legacy centroid step."""
+    L = _lib.lib()
+    out = (ctypes.c_int64 * 8)()
+    L.hb_debug_kernel_paths(shape["K"], shape["d"], shape["J"], shape["n"], 20, 132, kernel_set, out)
+    assert tuple(out) == expected
+
+
 def test_host_widen_pool_matches_numpy():
     """The worker pool of the download path widens float32 to float64 exactly, for
     sizes around its slice boundaries and repeatedly (the pool is persistent)."""
