@@ -1300,8 +1300,8 @@ int run_update_two_pass(hb_handle* h, int T, int t0, int t1, unsigned write_mask
 }
 
 
-// S[q][k][:] += R_q^T [Z_q | 1] on the tensor cores (stats_tc3.cuh): one launch per 128 clusters x 64 columns of [Z | 1]
-// (K = 100, d = 50: one launch).  The caller zeroes S.
+// S[q][k][:] += R_q^T [Z_q | 1] on the tensor cores (stats_tc3.cuh): one launch per 128 clusters x 64 or 128 columns
+// of [Z | 1] (K = 100, d = 50: one launch).  The caller zeroes S.
 int run_stats_tc(hb_handle* h, const float* Zsrc) {
   const int K = h->K, D1 = h->d + 1;
   StatsTcArgs t;
@@ -1318,11 +1318,17 @@ int run_stats_tc(hb_handle* h, const float* Zsrc) {
   t.DS = h->DS;
   t.tiles_per_cta = std::max(1, (h->ntiles + h->num_sms - 1) / h->num_sms);
   const int grid_tc = (h->ntiles + t.tiles_per_cta - 1) / t.tiles_per_cta;
-  const size_t smem_tc = stats_tc_smem_bytes(h->KS, h->DS);
-  CK(cudaFuncSetAttribute(k_stats_tc, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_tc));
+  const int nb = D1 > 64 ? 128 : 64;
   for (t.k_off = 0; t.k_off < K; t.k_off += 128)
-    for (t.c_off = 0; t.c_off < D1; t.c_off += 64) {
-      k_stats_tc<<<grid_tc, ST_THREADS, smem_tc, h->stream>>>(t);
+    for (t.c_off = 0; t.c_off < D1; t.c_off += nb) {
+      const size_t smem = stats_tc_smem_bytes(stats_tc_rk(h->KS, t.k_off), stats_tc_rc(h->DS, t.c_off, nb), nb);
+      if (nb == 64) {
+        CK(cudaFuncSetAttribute(k_stats_tc<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        k_stats_tc<1><<<grid_tc, ST_THREADS, smem, h->stream>>>(t);
+      } else {
+        CK(cudaFuncSetAttribute(k_stats_tc<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        k_stats_tc<2><<<grid_tc, ST_THREADS, smem, h->stream>>>(t);
+      }
       CKL();
     }
   return 0;
@@ -1370,7 +1376,6 @@ int run_correct(hb_handle* h) {
     RegionScope rs(h, "ridge_apply");
     ApplyTcArgs a;
     a.R = h->R.p;
-    a.Zo = h->Zo.p;
     a.V = h->V.p;
     a.Zc = h->Zc.p;
     a.tile_cell0 = h->tile_cell0.p;
@@ -1382,19 +1387,22 @@ int run_correct(hb_handle* h) {
     a.KS = h->KS;
     a.DS = h->DS;
     a.tiles_per_cta = std::max(1, (h->ntiles + h->num_sms - 1) / h->num_sms);
-    a.dbg = nullptr;
     const int grid = (h->ntiles + a.tiles_per_cta - 1) / a.tiles_per_cta;
     {
-      // cluster ranges of at most AP_MAXK clusters (shared memory), equal sizes, multiples of 8: the first launch
-      // subtracts its share from Zo, the following ones from the partial result in Zc
-      const int npass = (K + AP_MAXK - 1) / AP_MAXK;
-      const int Kpass = (((K + npass - 1) / npass) + 7) & ~7;
+      // cluster ranges of at most AP_MAXK clusters, equal sizes, multiples of 8, and small enough for two raw stages
+      // of shared memory: the first launch subtracts its share from Zo, the following ones from the partial result
+      // in Zc
+      int npass = (K + AP_MAXK - 1) / AP_MAXK, Kpass = 0;
+      for (;; ++npass) {
+        Kpass = (((K + npass - 1) / npass) + 7) & ~7;
+        if (apply_tc_stages(apply_tc_rs(Kpass, h->KS, 0), d, h->DS) >= 2) break;
+      }
       for (int k_off = 0; k_off < K; k_off += Kpass) {
         a.k_off = k_off;
         a.Kp = std::min(Kpass, K - k_off);
         a.KD = (a.Kp + 7) & ~7;
         a.minuend = (k_off == 0) ? h->Zo.p : h->Zc.p;
-        const size_t smem = apply_tc_smem_bytes(a.KD, d);
+        const size_t smem = apply_tc_smem_bytes(apply_tc_rs(a.KD, h->KS, k_off), d, h->DS);
         if (d <= 64) {
           CK(cudaFuncSetAttribute(k_apply_tc<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
           k_apply_tc<1><<<grid, AP_THREADS, smem, h->stream>>>(a);

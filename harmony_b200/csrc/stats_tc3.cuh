@@ -1,27 +1,33 @@
 // stats_tc3.cuh — K3 on the tensor cores: the ridge sufficient statistics of harmony.cpp:561-567 / 592-609 for
 // all clusters at once,
 //   S[q][k][c] = sum_{cells i of tuple q} R[i][k] * Z1[i][c],   Z1 = [Zo | 1]   (column d carries sum_i R_ik)
-// as D[128 clusters x 64 columns] += A * B^T with the CELLS as the reduction dimension.  The operands are K-major
-// with K = cells (wgmma takes tf32 operands K-major only), i.e. the TRANSPOSE of the row-major tiles in memory, so
-// the converter threads transpose while they split into tf32 hi / lo.
-// Second generation.  The first one staged raw tiles in shared memory (bulk copies) and converted them into ONE
-// operand stage: 2.9 us per 64-cell tile in a chain load -> convert -> MMA -> convert.  Here the converter threads
-// read their values straight from global memory (lanes along the cluster / column index: 128-byte segments of a
-// row), one tile AHEAD in registers, and the freed shared memory holds TWO operand stages: the conversion of tile
-// t + 1 overlaps the MMAs of tile t.  Persistent CTA per SM over a contiguous range of 64-cell tiles; the
-// accumulator stays in the registers of the MMA warpgroup across the tiles of one covariate tuple and is flushed
-// with atomics when the tuple changes.
-//   warps 0-3  MMA warpgroup : 2 halves x 3 x 8 wgmma (M=64, N=64, K=8 cells) per tile, 64 accumulators per thread
-//   warps 4-11 convert       : global -> registers (next tile) -> K-major tf32 hi/lo stages
+// as D[clusters x columns] += A * B^T with the CELLS as the reduction dimension, per launch 128 clusters x NB = 64 NH
+// columns of [Zo | 1].  A = R^T comes from registers, B = Z1^T from shared memory, 3xTF32, fp32 accumulators in
+// registers across the tiles of one covariate tuple, flushed with atomics when the tuple changes.
+//   * each tile's rows of R (this launch's clusters) and of Zo (this launch's columns) go into a ring of NST raw
+//     stages with bulk asynchronous copies, issued by one warp, whose bytes complete on the stage's "full" mbarrier.
+//     A tile never crosses a tuple and cells are sorted by tuple, so when a launch covers whole rows the tile is one
+//     contiguous span of each array (one copy each; narrower ranges copy row by row).  The copies of the next
+//     NST - 1 tiles stay in flight while a tile is converted and multiplied: at K = 100, d = 50 a stage holds
+//     64 x (100 + 52) x 4 B = 38.9 KB and four fit, up to 117-156 KB per SM in flight.
+//   * all 256 threads turn the tile's Zo rows into the K-major B operand (cells contiguous per column: the
+//     transpose), tf32 hi / lo, with the ones column and zeros beyond the tile; then each MMA warpgroup loads its
+//     A fragments (64 clusters x 8 cells per K step, zero beyond the tile and beyond the launch's clusters)
+//     straight from the raw R rows, splits them in registers and issues 3 x 8 wgmma, and completes them only after
+//     the next tile's B is written (two B buffers for NB = 64; NB = 128 has room for one and waits first).  When
+//     both warpgroups have read the stage, warp 0 refills it with tile it + NST.
+// Warp roles (256 threads): warpgroup e = 0, 1 owns clusters k_off + 64 e .. + 63 of every tile.
+// Shared memory: NBB B buffers of hi/lo 2 x NB x 64 floats ([16][NB][4]), then NST raw stages of 64 x (RK + RC)
+// floats (RK, RC = floats of R and of Zo per row in this launch), then the barriers.
 #pragma once
 #include "common.cuh"
 #include "umma.cuh"
 
 namespace hb {
 
-constexpr int ST_TN = 64;        // cells per tile = reduction length per stage (8 wgmma K-steps)
-constexpr int ST_THREADS = 384;  // warps 0-3 MMA warpgroup, warps 4-11 converters
-constexpr int ST_CONV = 256;     // converter threads
+constexpr int ST_TN = 64;        // cells per tile = reduction length per tile (8 wgmma K-steps)
+constexpr int ST_THREADS = 256;  // two MMA warpgroups
+constexpr int ST_MAXST = 4;      // raw stages
 
 struct StatsTcArgs {
   const float* R;   // [n][KS]
@@ -31,169 +37,171 @@ struct StatsTcArgs {
   const int* tile_tuple;
   float* S;         // [J][K][d+1]
   int ntiles, d, K, KS, DS, tiles_per_cta;
-  int k_off, c_off;  // this launch: clusters [k_off, k_off + 128) x columns [c_off, c_off + 64) of [Zo | 1] (wider shapes: several launches)
+  int k_off, c_off;  // this launch: clusters [k_off, k_off + 128) x columns [c_off, c_off + NB) of [Zo | 1]
 };
 
-__host__ __device__ inline size_t stats_tc_smem_bytes(int KS, int DS) {
-  // two operand stages: A hi/lo 2 x 128 x 64, B hi/lo 2 x 64 x 64 floats each
-  (void)KS;
-  (void)DS;
-  return sizeof(float) * 2 * (2 * 128 * ST_TN + 2 * 64 * ST_TN) + 1024;
+// floats per row of a raw stage: this launch's clusters of R, and its columns of Zo (none when it covers only the
+// ones column)
+__host__ __device__ inline int stats_tc_rk(int KS, int k_off) { return KS - k_off < 128 ? KS - k_off : 128; }
+__host__ __device__ inline int stats_tc_rc(int DS, int c_off, int nb) {
+  return DS - c_off < nb ? (DS - c_off > 0 ? DS - c_off : 0) : nb;
+}
+// B hi/lo buffers: two (the conversion of a tile overlaps the MMAs of the previous one) where shared memory allows
+__host__ __device__ constexpr int stats_tc_bbufs(int nb) { return nb == 64 ? 2 : 1; }
+__host__ __device__ inline size_t stats_tc_fixed_bytes(int nb) {
+  return sizeof(float) * 2 * stats_tc_bbufs(nb) * (size_t)nb * ST_TN + ST_MAXST * sizeof(uint64_t);
+}
+__host__ __device__ inline int stats_tc_stages(int RK, int RC, int nb) {
+  const size_t fixed = stats_tc_fixed_bytes(nb);
+  const int n = (int)((SMEM_LIMIT - fixed) / (sizeof(float) * (size_t)ST_TN * (RK + RC)));  // >= 2: RK, RC <= 128
+  return n < ST_MAXST ? n : ST_MAXST;
+}
+__host__ __device__ inline size_t stats_tc_smem_bytes(int RK, int RC, int nb) {
+  return stats_tc_fixed_bytes(nb) + stats_tc_stages(RK, RC, nb) * sizeof(float) * (size_t)ST_TN * (RK + RC);
 }
 
+// NH: 64-column halves of B (1: launches of 64 columns, 2: of 128), fixed at compile time so that the accumulators
+// stay in registers
+template <int NH>
 __global__ void __launch_bounds__(ST_THREADS, 1) k_stats_tc(StatsTcArgs a) {
   extern __shared__ __align__(128) unsigned char smem_raw[];
+  constexpr int NB = 64 * NH, NBB = stats_tc_bbufs(NB);
   const int K = a.K, d = a.d, KS = a.KS, DS = a.DS, D1 = d + 1;
-  constexpr int A_ST = 128 * ST_TN, B_ST = 64 * ST_TN;      // floats per operand tile
-  float* Ahi = reinterpret_cast<float*>(smem_raw);          // [2][16 cell chunks][128 clusters][4 cells]
-  float* Alo = Ahi + 2 * A_ST;
-  float* Bhi = Alo + 2 * A_ST;                              // [2][16][64 columns][4]
-  float* Blo = Bhi + 2 * B_ST;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(Blo + 2 * B_ST);
-  uint64_t* ab_full = bars + 0;     // [2]  converters (256): stage written
-  uint64_t* ab_empty = bars + 2;    // [2]  MMA warpgroup (128): stage consumed
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-
-  if (tid == 0) {
-    for (int i = 0; i < 2; ++i) {
-      umma::mbar_init(ab_full + i, ST_CONV);
-      umma::mbar_init(ab_empty + i, 128);
-    }
-    umma::fence_barrier_init();
-  }
-  __syncthreads();
+  const int RK = stats_tc_rk(KS, a.k_off), RC = stats_tc_rc(DS, a.c_off, NB);
+  const int Kp = K - a.k_off;                        // clusters of this launch (>= 128: all 128 rows of A)
+  const int NST = stats_tc_stages(RK, RC, NB);
+  const int SST = ST_TN * (RK + RC);                 // floats per raw stage: R rows [64][RK], then Zo rows [64][RC]
+  float* Bhi = reinterpret_cast<float*>(smem_raw);   // [NBB][hi, lo][16 cell chunks][NB columns][4 cells]
+  float* raw = Bhi + NBB * 2 * NB * ST_TN;
+  uint64_t* full = reinterpret_cast<uint64_t*>(raw + (size_t)NST * SST);  // [NST]  the stage's bytes have landed
+  // the warp index through a shuffle: ptxas sees the role branches as warp-uniform and does not serialise the wgmma
+  const int tid = threadIdx.x, warp = __shfl_sync(0xffffffffu, tid >> 5, 0), lane = tid & 31;
 
   const int t_begin = blockIdx.x * a.tiles_per_cta;
   const int t_end = (t_begin + a.tiles_per_cta < a.ntiles) ? t_begin + a.tiles_per_cta : a.ntiles;
+  // tile `it` of the range -> stage it % NST; called by one whole warp
+  auto load = [&](int it) {
+    const int tile = t_begin + it, s = it % NST;
+    const int cell0 = __ldg(a.tile_cell0 + tile), len = __ldg(a.tile_len + tile);
+    float* rR = raw + (size_t)s * SST;
+    float* rZ = rR + ST_TN * RK;
+    if (lane == 0) {
+      umma::mbar_arrive_expect_tx(full + s, (uint32_t)(sizeof(float) * len * (RK + RC)));
+      if (RK == KS) umma::bulk_g2s(rR, a.R + (size_t)cell0 * KS, (uint32_t)(sizeof(float) * len * KS), full + s);
+      if (RC == DS) umma::bulk_g2s(rZ, a.Zo + (size_t)cell0 * DS, (uint32_t)(sizeof(float) * len * DS), full + s);
+    }
+    if (RK != KS || (RC != DS && RC > 0)) {  // ranges narrower than the rows: row by row
+      __syncwarp();  // the expected bytes are registered before any row completes
+      for (int j = lane; j < len; j += 32) {
+        if (RK != KS)
+          umma::bulk_g2s(rR + (size_t)j * RK, a.R + (size_t)(cell0 + j) * KS + a.k_off, (uint32_t)(sizeof(float) * RK), full + s);
+        if (RC != DS && RC > 0)
+          umma::bulk_g2s(rZ + (size_t)j * RC, a.Zo + (size_t)(cell0 + j) * DS + a.c_off, (uint32_t)(sizeof(float) * RC), full + s);
+      }
+    }
+  };
 
-  if (warp < 4) {
-    // =============================== MMA warpgroup ===============================
-    const uint32_t lboA = 128 * 16, lboB = 64 * 16, sbo = 128;
-    float acc[2][32];  // clusters 64 g + frag_row, columns frag_col
-    int run_acc = 0;   // 0: the first MMA of the tile starts the tuple's sums (overwrites the accumulator)
-    int it = 0;
-    for (int tile = t_begin; tile < t_end; ++tile, ++it) {
-      const int s = it & 1;
-      const int q = a.tile_tuple[tile];
-      const bool last_of_run = (tile + 1 == t_end) || (a.tile_tuple[tile + 1] != q);
-      umma::mbar_wait(ab_full + s, (it >> 1) & 1);
-      const uint32_t aH = umma::smem_u32(Ahi + s * A_ST), aL = umma::smem_u32(Alo + s * A_ST);
-      const uint32_t bH = umma::smem_u32(Bhi + s * B_ST), bL = umma::smem_u32(Blo + s * B_ST);
-      umma::fence();
-#pragma unroll
-      for (int g = 0; g < 2; ++g)
-        for (int ks = 0; ks < ST_TN / 8; ++ks) {
-          const uint32_t ao = ks * 2 * lboA + g * 64 * 16, bo = ks * 2 * lboB;
-          const uint64_t ah = umma::make_desc(aH + ao, lboA, sbo);
-          const uint64_t al = umma::make_desc(aL + ao, lboA, sbo);
-          const uint64_t bh = umma::make_desc(bH + bo, lboB, sbo);
-          const uint64_t bl = umma::make_desc(bL + bo, lboB, sbo);
-          umma::mma_n64(acc[g], al, bh, run_acc | (ks > 0));
-          umma::mma_n64(acc[g], ah, bl, 1);
-          umma::mma_n64(acc[g], ah, bh, 1);
-        }
-      umma::commit();
-      umma::wait0();
-      umma::mbar_arrive(ab_empty + s);
-      run_acc = last_of_run ? 0 : 1;
-      if (last_of_run) {
-        // flush the accumulator of this tuple
-#pragma unroll
-        for (int g = 0; g < 2; ++g)
-#pragma unroll
-          for (int i = 0; i < 32; ++i) {
-            const int k = a.k_off + 64 * g + umma::frag_row(i, warp, lane), c = a.c_off + umma::frag_col(i, lane);
-            if (k < K && c < D1) atomicAdd(a.S + ((size_t)q * K + k) * D1 + c, acc[g][i]);
-          }
-      }
-    }
-  } else if (warp >= 4) {
-    // =============================== converters ===============================
-    const int ct = tid - 128;          // 0..255
-    const int kA = ct & 127, ccA = ct >> 7;   // A: cluster kA, cell chunks ccA + 2 i (i < 8)
-    const int cB = ct & 63, ccB = ct >> 6;    // B: column cB,  cell chunks ccB + 4 i (i < 4)
-    float vA[8][4], vB[4][4];
-    // operand pair of a value: hi = the value itself (the tensor core reads its upper 19 bits), lo = the remainder
-    // v - trunc_tf32(v), exact in fp32 and truncated by the tensor core in turn (relative error of the pair <= 2^-20)
-    auto split = [](float v, float& hi, float& lo) {
-      hi = v;
-      lo = v - __uint_as_float(__float_as_uint(v) & 0xffffe000u);
-    };
-    // tile records (first cell, cells, tuple) run two tiles ahead of the value loads, the value loads one tile ahead of
-    // the conversion: no load that feeds an address or a branch is waited for
-    auto meta = [&](int tile, int& cell0, int& len, int& q) {
-      cell0 = 0;
-      len = 0;
-      q = -1;
-      if (tile < t_end) {
-        cell0 = __ldg(a.tile_cell0 + tile);
-        len = __ldg(a.tile_len + tile);
-        q = __ldg(a.tile_tuple + tile);
-      }
-    };
-    auto fetch = [&](int cell0, int len) {  // this thread's values of a tile, straight from global memory
-      const float* rR = a.R + (size_t)cell0 * KS + a.k_off + kA;
-      const float* rZ = a.Zo + (size_t)cell0 * DS + a.c_off + cB;
-#pragma unroll
-      for (int i = 0; i < 8; ++i)
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-          const int cell = 4 * (ccA + 2 * i) + j;
-          vA[i][j] = (cell < len && a.k_off + kA < K) ? ld_stream(rR + (size_t)cell * KS) : 0.f;
-        }
-#pragma unroll
-      for (int i = 0; i < 4; ++i)
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-          const int cell = 4 * (ccB + 4 * i) + j;
-          float v = 0.f;
-          if (cell < len) v = (a.c_off + cB < d) ? ld_stream(rZ + (size_t)cell * DS) : (a.c_off + cB == d ? 1.f : 0.f);  // column d: the ones column
-          vB[i][j] = v;
-        }
-    };
-    int c0_0, len0, q0, c0_1, len1, q1, c0_2, len2, q2;
-    meta(t_begin, c0_0, len0, q0);
-    meta(t_begin + 1, c0_1, len1, q1);
-    meta(t_begin + 2, c0_2, len2, q2);
-    fetch(c0_0, len0);
-    int it = 0;
-    for (int tile = t_begin; tile < t_end; ++tile, ++it) {
-      const int s = it & 1;
-      if (it >= 2) umma::mbar_wait(ab_empty + s, ((it >> 1) - 1) & 1);  // MMAs of tile it - 2 are done with the stage
-      float* ah = Ahi + s * A_ST;
-      float* al = Alo + s * A_ST;
-      float* bh = Bhi + s * B_ST;
-      float* bl = Blo + s * B_ST;
-#pragma unroll
-      for (int i = 0; i < 8; ++i) {
-        float4 hi, lo;
-        split(vA[i][0], hi.x, lo.x);
-        split(vA[i][1], hi.y, lo.y);
-        split(vA[i][2], hi.z, lo.z);
-        split(vA[i][3], hi.w, lo.w);
-        const int off = ((ccA + 2 * i) * 128 + kA) * 4;
-        *reinterpret_cast<float4*>(ah + off) = hi;
-        *reinterpret_cast<float4*>(al + off) = lo;
-      }
-#pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        float4 hi, lo;
-        split(vB[i][0], hi.x, lo.x);
-        split(vB[i][1], hi.y, lo.y);
-        split(vB[i][2], hi.z, lo.z);
-        split(vB[i][3], hi.w, lo.w);
-        const int off = ((ccB + 4 * i) * 64 + cB) * 4;
-        *reinterpret_cast<float4*>(bh + off) = hi;
-        *reinterpret_cast<float4*>(bl + off) = lo;
-      }
-      umma::fence_proxy_async();
-      umma::mbar_arrive(ab_full + s);
-      fetch(c0_1, len1);  // the next tile's values travel while this one is multiplied
-      c0_0 = c0_1, len0 = len1, q0 = q1;
-      c0_1 = c0_2, len1 = len2, q1 = q2;
-      meta(tile + 3, c0_2, len2, q2);
-    }
+  if (tid == 0) {
+    for (int i = 0; i < NST; ++i) umma::mbar_init(full + i, 1);
+    umma::fence_barrier_init();
   }
+  __syncthreads();
+  if (warp == 0)
+    for (int it = 0; it < NST && t_begin + it < t_end; ++it) load(it);
+
+  const int e = warp >> 2;   // clusters k_off + 64 e ..
+  const int w = warp & 3;    // warp of the warpgroup
+  const uint32_t lboB = NB * 16, sbo = 128;
+  float acc[NB / 2];  // clusters 64 e + frag_row, columns frag_col
+  int run_acc = 0;    // 0: the first MMA of the tile starts the tuple's sums (overwrites the accumulator)
+  int q_prev = -1;
+  // completes the MMAs of the previous tile and flushes the accumulator when that tile ended its tuple's run
+  auto retire = [&](bool last_of_run) {
+    umma::wait0();
+    if (last_of_run) {
+#pragma unroll
+      for (int i = 0; i < NB / 2; ++i) {
+        const int k = a.k_off + 64 * e + umma::frag_row(i, w, lane), c = a.c_off + umma::frag_col(i, lane);
+        if (k < K && c < D1) atomicAdd(a.S + ((size_t)q_prev * K + k) * D1 + c, acc[i]);
+      }
+    }
+  };
+  for (int tile = t_begin, it = 0; tile < t_end; ++tile, ++it) {
+    const int s = it % NST;
+    const int len = __ldg(a.tile_len + tile), q = __ldg(a.tile_tuple + tile);
+    const float* rR = raw + (size_t)s * SST;
+    const float* rZ = rR + ST_TN * RK;
+    float* bh_t = Bhi + (NBB == 2 ? (it & 1) * 2 * NB * ST_TN : 0);
+    float* bl_t = bh_t + NB * ST_TN;
+    if (NBB == 1 && it > 0) {  // one B buffer: both warpgroups finish the previous tile's MMAs before it is rewritten
+      retire(q != q_prev);
+      umma::named_sync(1, ST_THREADS);
+    }
+    umma::mbar_wait(full + s, (it / NST) & 1);
+
+    // B = Z1^T of the tile: column c of [Zo | 1] for 4 cells per float4; zero beyond the tile (stale rows) and
+    // beyond column d.  hi = the value itself (the tensor core reads its upper 19 bits), lo = the remainder
+    // v - trunc_tf32(v), exact in fp32 and truncated by the tensor core in turn (relative error of the pair
+    // <= 2^-20).  With two B buffers this overlaps the previous tile's MMAs.
+    for (int idx = tid; idx < NB * (ST_TN / 4); idx += ST_THREADS) {
+      const int c = idx % NB, ch = idx / NB, cg = a.c_off + c;
+      float v[4];
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        const int cell = 4 * ch + j;
+        v[j] = cell < len ? (cg < d ? rZ[cell * RC + c] : (cg == d ? 1.f : 0.f)) : 0.f;
+      }
+      float4 hi, lo;
+      hi = make_float4(v[0], v[1], v[2], v[3]);
+      lo.x = v[0] - __uint_as_float(__float_as_uint(v[0]) & 0xffffe000u);
+      lo.y = v[1] - __uint_as_float(__float_as_uint(v[1]) & 0xffffe000u);
+      lo.z = v[2] - __uint_as_float(__float_as_uint(v[2]) & 0xffffe000u);
+      lo.w = v[3] - __uint_as_float(__float_as_uint(v[3]) & 0xffffe000u);
+      *reinterpret_cast<float4*>(bh_t + (ch * NB + c) * 4) = hi;
+      *reinterpret_cast<float4*>(bl_t + (ch * NB + c) * 4) = lo;
+    }
+    // two B buffers: the previous tile's MMAs end before the barrier, so the buffer written at tile it + 1 is free
+    if (NBB == 2 && it > 0) retire(q != q_prev);
+    umma::fence_proxy_async();
+    umma::named_sync(1, ST_THREADS);  // B is written; the stage of the previous tile has been read by everyone
+    if (warp == 0 && it > 0 && tile - 1 + NST < t_end) load(it - 1 + NST);
+    run_acc = (it > 0 && q == q_prev) ? 1 : 0;
+    q_prev = q;
+
+    // A fragments: A[m][kk] = R[cell 8 ks + kk][cluster 64 e + m], split like B
+    uint32_t ah[ST_TN / 8][4], al[ST_TN / 8][4];
+    {
+      const int m0 = 64 * e + 16 * w + (lane >> 2), kk0 = lane & 3;
+#pragma unroll
+      for (int ks = 0; ks < ST_TN / 8; ++ks)
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+          const int m = m0 + 8 * (j & 1), cell = 8 * ks + kk0 + 4 * (j >> 1);
+          const float z = (cell < len && m < Kp) ? rR[cell * RK + m] : 0.f;
+          ah[ks][j] = __float_as_uint(z);
+          al[ks][j] = __float_as_uint(z - __uint_as_float(__float_as_uint(z) & 0xffffe000u));
+        }
+    }
+    const uint32_t bH = umma::smem_u32(bh_t), bL = umma::smem_u32(bl_t);
+    umma::fence();
+#pragma unroll
+    for (int ks = 0; ks < ST_TN / 8; ++ks) {
+      const uint32_t bo = ks * 2 * lboB;
+      const uint64_t bh = umma::make_desc(bH + bo, lboB, sbo);
+      const uint64_t bl = umma::make_desc(bL + bo, lboB, sbo);
+      if constexpr (NH == 1) {
+        umma::mma_rs_n64(acc, al[ks], bh, run_acc | (ks > 0));
+        umma::mma_rs_n64(acc, ah[ks], bl, 1);
+        umma::mma_rs_n64(acc, ah[ks], bh, 1);
+      } else {
+        umma::mma_rs_n128(acc, al[ks], bh, run_acc | (ks > 0));
+        umma::mma_rs_n128(acc, ah[ks], bl, 1);
+        umma::mma_rs_n128(acc, ah[ks], bh, 1);
+      }
+    }
+    umma::commit();
+  }
+  retire(t_begin < t_end);  // unconditional wait: a conditional one makes ptxas add its own at the loop exit
 }
 
 }  // namespace hb
