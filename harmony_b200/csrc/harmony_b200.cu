@@ -20,6 +20,7 @@
 #include <cstring>
 #include <deque>
 #include <map>
+#include <memory>
 #include <numeric>
 #include <string>
 #include <tuple>
@@ -327,6 +328,8 @@ void keep_pool_memory(int device) {
   cudaGetLastError();
 }
 
+struct Plan;  // plan.cuh
+
 }  // namespace
 
 struct hb_handle {
@@ -346,7 +349,7 @@ struct hb_handle {
   unsigned max_iter_kmeans = 0, window_size = 3;
   bool lambda_estimation = false, ran_setup = false, ran_init = false;
   int verbose = 0;
-  uint64_t seed = 0x5eedULL, round_counter = 0;
+  uint64_t seed = 0x5eedULL;
   int nb = 0;
   uint32_t cpb = 0;
   int half_bits = 1;
@@ -358,22 +361,14 @@ struct hb_handle {
   DevBuf<float> ring, acc2, Psave, OEend, tmpT;  // persistent update kernel state
   DevBuf<double> obj2;
   DevBuf<unsigned> bar;
-  DevBuf<unsigned long long> scan_state;  // chained scan of the plan's histograms: [plan_batch][1 + tiles]
-  int plan_rounds = 0;   // rounds each plan buffer set holds (two sets: current call / prebuilt next call)
-  int plan_set = 0;      // set used by the running cluster_cpp call
-  bool next_ready = false;  // the other set holds a prebuilt native plan for the next call ...
-  int next_T = 0;           // ... covering this many rounds
-  cudaStream_t plan_stream = nullptr;
-  cudaEvent_t plan_done = nullptr;
+  std::unique_ptr<Plan> plan;  // update-order plan (plan.cuh)
   bool sigma_uniform = false;
   float sigma0 = 0.f;
   bool R_user_set = false;  // R was written through hb_set_field since the last assignment step
   int coop_grid = 0;
   DevBuf<double> obj_acc, stage;
-  DevBuf<int> sort_perm, inv_sort, tuple_levels, cov_of_d, tile_cell0, tile_len, tile_tuple, chunk_start,
-      tuple_chunk0, blk_of, order, prev_at, H, seg_start, tile_base, iscratch, skipped, err_flag;
+  DevBuf<int> sort_perm, inv_sort, tuple_levels, cov_of_d, tile_cell0, tile_len, tile_tuple, iscratch, skipped, err_flag;
   DevBuf<int64_t> perms_d;
-  DevBuf<int4> ranges;  // [T][nb][coop_grid] tuple-aligned CTA ranges (when 2 J <= grid)
   DevBuf<int> tc_cell0, tc_len, tc_tuple;  // 128-cell tiles of the tensor-core kernels
   int tc_ntiles = 0;
   KernelPaths paths;             // kernels picked by hb_setup (select_kernels)
@@ -382,19 +377,14 @@ struct hb_handle {
   DevBuf<float> Rkeep, OEkeep;   // R / O,E saved around the distance-only assignment of that step
   DevBuf<double> objkeep;
   int ring_rows = 0;     // rows of a warp's private ring in the single-pass update kernel
-  int plan_batch = 1;    // rounds sorted per launch (size of the histogram scratch)
-  int plan_nsub = 1;     // third sort key of the plan: block in the next round (nb values) or off (1)
   bool use_xch = false;  // sharded cells: block steps exchanged through peer memory (one cooperative launch per call)
   PeerXch xch{};
   XchArea* xarea = nullptr;  // leased exchange area (process-wide pool, see setup_peer_exchange)
   bool zc_pending_norm = false;  // Zc holds the un-normalised corrected embedding although cluster_cpp has run
-  DevBuf<int> pt_p0, pt_len, pt_tuple, pt_blk, pt_count, pt_base;  // [2 sets] 128-row tiles of round 0 in plan order
-  size_t pt_cap = 0;
   DevBuf<float> remT;    // [2][nb][J][KS] next round's removal sums per (block, tuple)
   DevBuf<float> remS;    // [nb][J][KS] sharded cells: the ranks' remT of one round, summed
-  DevBuf<int> next_at, chunk_q0, chunk_nq;
   DevBuf<int> lvl_ptr, lvl_tup;  // CSR level -> tuples (+ one trailing word: B_vec[0])
-  int ntiles = 0, nchunks = 0;  // nchunks includes the trailing empty chunk
+  int ntiles = 0;
   int trace_cap = 0;
   std::vector<int> tuple_levels_h;  // [J][C]
   std::vector<int> sort_perm_h;
@@ -415,7 +405,6 @@ struct hb_handle {
   int64_t launches = 0;
   bool timing = false;
   std::map<std::string, Region> regions;
-  cudaEvent_t ev0 = nullptr;  // orders the side-stream plan build after the main stream
 };
 
 namespace {
@@ -543,6 +532,12 @@ int launch_logits(hb_handle* h, const float* sigma, bool normalise) {
   return 0;
 }
 
+}  // namespace
+
+#include "plan.cuh"
+
+namespace {
+
 // ---- K1 launcher: assignment from centroids (init + cold start) -------------------------------
 // plan_mode: tiles follow round 0 of the current plan set (tensor-core kernel only); want_obj: objective sums (init)
 int run_assign(hb_handle* h, bool normalise, bool plan_mode = false, bool want_obj = true) {
@@ -595,15 +590,14 @@ int run_assign(hb_handle* h, bool normalise, bool plan_mode = false, bool want_o
     if (plan_mode) {
       // rows in the order of round 0 of the coming cluster_cpp call: a tile's column sums are a share of its block's
       // removal sums and go to the update kernel's accumulator slots; R is not stored
-      const size_t R0 = (size_t)h->plan_set * h->plan_rounds;
-      const size_t cap = h->pt_cap;
+      const PlanRound0 r = plan_round0(h, h->plan->set);
       t.R = nullptr;
-      t.row_index = h->order.p + R0 * h->n;
-      t.tile_p0 = h->pt_p0.p + (size_t)h->plan_set * cap;
-      t.tile_len = h->pt_len.p + (size_t)h->plan_set * cap;
-      t.tile_tuple = h->pt_tuple.p + (size_t)h->plan_set * cap;
-      t.tile_blk = h->pt_blk.p + (size_t)h->plan_set * cap;
-      t.ntiles_ptr = h->pt_count.p + h->plan_set;
+      t.row_index = r.order;
+      t.tile_p0 = r.tile_p0;
+      t.tile_len = r.tile_len;
+      t.tile_tuple = r.tile_tuple;
+      t.tile_blk = r.tile_blk;
+      t.ntiles_ptr = r.tile_count;
       t.ntiles = 0;
       t.acc = h->acc2.p;
       t.Zc_out = nullptr;
@@ -652,17 +646,15 @@ int run_assign(hb_handle* h, bool normalise, bool plan_mode = false, bool want_o
     // shapes the fused kernel cannot hold (d > 64 or K > 128): logits per 64-cluster range on the tensor cores, then
     // one gather pass over U in the order of round 0 for the softmax + the blocks' removal sums (harmony.cpp:312-313)
     TRY(launch_logits(h, h->sigma.p, normalise));
-    const size_t R0 = (size_t)h->plan_set * h->plan_rounds;
+    const PlanRound0 r = plan_round0(h, h->plan->set);
     const int nv = sp_nv(KS);
     const size_t smem_sm = sizeof(float) * 8 * 128 * (size_t)nv;
     if (nv == 1)
       k_softmax_block_sums<1><<<dim3(h->coop_grid, h->nb), 256, smem_sm, h->stream>>>(
-          h->U.p, h->order.p + R0 * h->n, h->ranges.p + R0 * h->nb * h->coop_grid, h->tuple_levels.p, h->acc2.p, h->coop_grid, K, KS,
-          h->C, B);
+          h->U.p, r.order, r.ranges, h->tuple_levels.p, h->acc2.p, h->coop_grid, K, KS, h->C, B);
     else
       k_softmax_block_sums<2><<<dim3(h->coop_grid, h->nb), 256, smem_sm, h->stream>>>(
-          h->U.p, h->order.p + R0 * h->n, h->ranges.p + R0 * h->nb * h->coop_grid, h->tuple_levels.p, h->acc2.p, h->coop_grid, K, KS,
-          h->C, B);
+          h->U.p, r.order, r.ranges, h->tuple_levels.p, h->acc2.p, h->coop_grid, K, KS, h->C, B);
     CKL();
     h->R_user_set = false;
     const size_t XH = (size_t)B * KS + KS;
@@ -763,144 +755,20 @@ int check_convergence_host(hb_handle* h, int type, int* out) {
   return 0;
 }
 
-// ---- update-order plan (buffers hold plan_rounds rounds, two sets) ----------------------------------
-// Phase A: the block of every local cell in round t (harmony.cpp:272-291: position in the shuffled order / cells
-// per block).  Phase B: the round's rows sorted by (block, tuple, block in the next round) + the derived tables.
-// rounds [t, t + nt) of a buffer set in one launch (blockIdx.y = round)
-int plan_blocks(hb_handle* h, int t, int nt, const int64_t* perm_d /* device, nt x N_global, or null */, int set, cudaStream_t st) {
-  RegionScope rs(h, "plan");
-  const int64_t n = h->n;
-  const size_t R0 = (size_t)set * h->plan_rounds;  // first round slot of this buffer set
-  int* blk_of = h->blk_of.p + (R0 + t) * n;
-  if (perm_d) {
-    CK(cudaMemsetAsync(blk_of, 0xff, sizeof(int) * (size_t)n * nt, st));
-    k_plan_block_injected<<<dim3(grid_for(h->N_global, 256, h->num_sms * 8), nt), 256, 0, st>>>(
-        perm_d, h->N_global, h->cell_offset, n, h->inv_sort.p, h->cpb, h->nb, blk_of, h->err_flag.p);
-    CKL();
-  } else {
-    k_plan_block_native<<<dim3(grid_for(n, 256, h->num_sms * 8), nt), 256, 0, st>>>(
-        h->N_global, h->cell_offset, n, h->sort_perm.p, h->cpb, h->nb, h->half_bits, h->seed, h->round_counter, blk_of);
-    CKL();
-  }
-  h->round_counter += (uint64_t)nt;
-  return 0;
-}
-// counting sort of rounds [t, t + nt) (nt <= plan_batch: the histogram scratch holds that many rounds); round
-// t + nt - 1 has a next round iff last_has_next
-int plan_sort(hb_handle* h, int t, int nt, bool last_has_next, int set, cudaStream_t st, bool tiles = false) {
-  RegionScope rs(h, "plan");
-  const int nb = h->nb, J = h->J, nc = h->nchunks, nsub = h->plan_nsub;
-  const int64_t n = h->n;
-  const int S = nb * J;
-  const size_t R0 = (size_t)set * h->plan_rounds;
-  const int* blk_of = h->blk_of.p + (R0 + t) * n;
-  int* order = h->order.p + (R0 + t) * n;
-  int* seg_start = h->seg_start.p + (R0 + t) * (S + 1);
-  int* tile_base = h->tile_base.p + (R0 + t) * (S + 1);
-  const size_t per_warp = sizeof(int) * (size_t)nb * nsub;
-  const int wpb = (int)std::max<size_t>(1, std::min<size_t>(8, (48 * 1024) / per_warp));  // warps per block
-  const size_t sm = per_warp * wpb;
-  const int with_next = last_has_next ? nt : nt - 1;
-  k_plan_hist<<<dim3((nc + wpb - 1) / wpb, nt), wpb * 32, sm, st>>>(blk_of, nullptr, h->chunk_start.p, h->chunk_q0.p,
-                                                                   h->chunk_nq.p, nc, nb, nsub, h->H.p, h->err_flag.p, n,
-                                                                   with_next);
-  CKL();
-  {  // offsets of the counting sort: chained multi-CTA scan of the nt histograms (a single CTA per round took ~145 us)
-    const int64_t hn = (int64_t)nb * nsub * nc;
-    const int tiles = (int)((hn + SCAN_TILE - 1) / SCAN_TILE);
-    CK(cudaMemsetAsync(h->scan_state.p, 0, sizeof(unsigned long long) * (size_t)nt * (tiles + 1), st));
-    k_scan_chained<<<dim3(tiles, nt), 1024, 0, st>>>(h->H.p, hn, h->scan_state.p, tiles);
-    CKL();
-  }
-  k_plan_scatter<<<dim3((nc + wpb - 1) / wpb, nt), wpb * 32, sm, st>>>(
-      blk_of, nullptr, h->chunk_start.p, h->chunk_q0.p, h->chunk_nq.p, nc, nb, nsub, h->H.p, order, nullptr,
-      h->paths.update == UpdatePath::TwoPass ? h->prev_at.p + (R0 + t) * n : nullptr,
-      h->paths.update == UpdatePath::SinglePass ? h->next_at.p + (R0 + t) * n : nullptr, n,
-      with_next, t > 0 ? 1 : 0);
-  CKL();
-  k_plan_segments<<<dim3(grid_for(S + 1, 256, 64), nt), 256, 0, st>>>(h->H.p, h->tuple_chunk0.p, nc, nb, nsub, J, (int)n,
-                                                                       seg_start, tile_base);
-  CKL();
-  if (h->paths.update != UpdatePath::PerStep && h->paths.tuple_ranges) {
-    k_plan_ranges<<<dim3(nb, nt), 256, 0, st>>>(seg_start, nb, J, h->coop_grid,
-                                                                            h->ranges.p + (R0 + t) * nb * h->coop_grid);
-    CKL();
-  }
-  if (tiles) {  // tile offsets of the per-step update kernels (single round)
-    k_plan_tilecount<<<grid_for(S + 1, 256, 64), 256, 0, st>>>(seg_start, S, tile_base);
-    CKL();
-    k_scan_exclusive<<<1, 1024, 0, st>>>(tile_base, (int64_t)S + 1, nullptr);
-    CKL();
-  }
-  return 0;
-}
-// all T rounds of a cluster_cpp call (orders: device, T x N_global, or null for the native keyed orders)
-int build_plans(hb_handle* h, int T, const int64_t* orders_d, int set, cudaStream_t st) {
-  if (T > 0) TRY(plan_blocks(h, 0, T, orders_d, set, st));
-  for (int t = 0; t < T; t += h->plan_batch) {
-    const int nt = std::min(h->plan_batch, T - t);
-    TRY(plan_sort(h, t, nt, t + nt < T, set, st));
-  }
-  if (T > 0 && h->paths.mm.k1_stages && h->paths.update == UpdatePath::SinglePass) {
-    // 128-row tiles of round 0, one (block, tuple) segment at a time: the assignment step of the call runs in this order
-    RegionScope rs(h, "plan");
-    const int S = h->nb * h->J;
-    const int* seg_start = h->seg_start.p + (size_t)set * h->plan_rounds * (S + 1);
-    k_plan_tilecount128<<<grid_for(S + 1, 256, 64), 256, 0, st>>>(seg_start, S, h->pt_base.p);
-    CKL();
-    k_scan_exclusive<<<1, 1024, 0, st>>>(h->pt_base.p, (int64_t)S + 1, h->pt_count.p + set);
-    CKL();
-    k_plan_tilefill128<<<grid_for(S, 128, 64), 128, 0, st>>>(seg_start, h->pt_base.p, S, h->J, h->pt_p0.p + (size_t)set * h->pt_cap,
-                                                          h->pt_len.p + (size_t)set * h->pt_cap,
-                                                          h->pt_tuple.p + (size_t)set * h->pt_cap,
-                                                          h->pt_blk.p + (size_t)set * h->pt_cap);
-    CKL();
-  }
-  return 0;
-}
-// Buffers of T rounds of update plans, two sets (the running call's, and the next call's prebuilt on the side stream),
-// and the persistent update kernels' per-step accumulators of a T-round call.
-int alloc_plan_rounds(hb_handle* h, int T) {
-  const size_t n = (size_t)h->n, BK = (size_t)h->B * h->KS;
-  const size_t S1 = (size_t)h->nb * h->J + 1;
-  CK(h->blk_of.alloc(2 * (size_t)T * n));
-  CK(h->order.alloc(2 * (size_t)T * n));
-  if (h->paths.update == UpdatePath::SinglePass)
-    CK(h->next_at.alloc(2 * (size_t)T * n));
-  else
-    CK(h->prev_at.alloc(2 * (size_t)T * n));
-  CK(h->seg_start.alloc(2 * (size_t)T * S1));
-  CK(h->tile_base.alloc(2 * (size_t)T * S1));
-  if (h->paths.update != UpdatePath::PerStep) {
-    CK(h->acc2.alloc(2 * (BK + h->KS) * ((size_t)T * h->nb + 2)));
-    CK(h->OEend.alloc((size_t)T * 2 * BK));
-    CK(h->obj2.alloc(2 * (size_t)T));
-    CK(h->bar.alloc(2 * ((size_t)T * h->nb + 2)));
-    if (h->paths.tuple_ranges) CK(h->ranges.alloc(2 * (size_t)T * h->nb * h->coop_grid));
-  }
-  h->plan_rounds = T;
-  return 0;
-}
-// one round into slot 0 of set 0 (the per-step update path)
-int build_plan_single(hb_handle* h, const int64_t* perm_d, cudaStream_t st) {
-  TRY(plan_blocks(h, 0, 1, perm_d, 0, st));
-  return plan_sort(h, 0, 1, false, 0, st, true);
-}
-
 // ---- per-step path: one update_R sweep (harmony.cpp:269-342), three launches per block step ---------------
-int run_update_per_step(hb_handle* h, int t) {
+int run_update_per_step(hb_handle* h) {
   RegionScope rs(h, "update_R");
   const int K = h->K, B = h->B, nb = h->nb, KS = h->KS;
   const int KP = (K + 63) & ~63;
   const size_t slot = 2 * ((size_t)B * KS + KS);  // [add_O | add_rs | rem_O | rem_rs]
-  const int S = nb * h->J;
   CK(cudaMemsetAsync(h->acc.p, 0, sizeof(float) * 2 * slot, h->stream));
+  const PlanRound0 r = plan_round0(h, 0);  // the one round the per-step path plans
   StepArgs a;
   a.U = h->U.p;
   a.R = h->R.p;
-  a.order = h->order.p + (size_t)t * h->n;  // the per-step path always plans into set 0
-  a.seg_start = h->seg_start.p + (size_t)t * (S + 1);
-  a.tile_base = h->tile_base.p + (size_t)t * (S + 1);
+  a.order = r.order;
+  a.seg_start = r.seg_start;
+  a.tile_base = r.tile_base;
   a.tuple_levels = h->tuple_levels.p;
   a.sigma = h->sigma.p;
   a.P = h->P.p;
@@ -1078,11 +946,11 @@ TwoPassArgs make_two_pass_args(hb_handle* h, int T) {
   TwoPassArgs a;
   a.U = h->U.p;
   a.R = h->R.p;
-  const size_t R0 = (size_t)h->plan_set * h->plan_rounds;
-  a.order = h->order.p + R0 * h->n;
-  a.seg_start = h->seg_start.p + R0 * ((size_t)h->nb * h->J + 1);
-  a.prev_at = h->prev_at.p + R0 * h->n;
-  a.ranges = h->paths.tuple_ranges ? h->ranges.p + R0 * h->nb * h->coop_grid : nullptr;
+  const PlanRound0 r = plan_round0(h, h->plan->set);
+  a.order = r.order;
+  a.seg_start = r.seg_start;
+  a.prev_at = r.prev_at;
+  a.ranges = r.ranges;
   a.tuple_levels = h->tuple_levels.p;
   a.sigma = h->sigma.p;
   a.theta = h->theta.p;
@@ -1110,10 +978,10 @@ SinglePassArgs make_single_pass_args(hb_handle* h, int T) {
   SinglePassArgs a;
   a.U = h->U.p;
   a.R = h->R.p;
-  const size_t R0 = (size_t)h->plan_set * h->plan_rounds;
-  a.order = h->order.p + R0 * h->n;
-  a.next_at = h->next_at.p + R0 * h->n;
-  a.ranges = h->ranges.p + R0 * h->nb * h->coop_grid;
+  const PlanRound0 r = plan_round0(h, h->plan->set);
+  a.order = r.order;
+  a.next_at = r.next_at;
+  a.ranges = r.ranges;
   a.tuple_levels = h->tuple_levels.p;
   a.lvl_ptr = h->lvl_ptr.p;
   a.lvl_tup = h->lvl_tup.p;
@@ -1144,6 +1012,27 @@ SinglePassArgs make_single_pass_args(hb_handle* h, int T) {
   a.ring_rows = h->ring_rows;
   a.coop = 1;
   return a;
+}
+// per-call state of the persistent update kernels for calls of up to T rounds: accumulator slots, the tables after
+// every round, the objective sums and the step counters
+int alloc_update_rounds(hb_handle* h, int T) {
+  if (h->paths.update == UpdatePath::PerStep) return 0;
+  const size_t BK = (size_t)h->B * h->KS;
+  CK(h->acc2.alloc(2 * (BK + h->KS) * ((size_t)T * h->nb + 2)));
+  CK(h->OEend.alloc((size_t)T * 2 * BK));
+  CK(h->obj2.alloc(2 * (size_t)T));
+  CK(h->bar.alloc(2 * ((size_t)T * h->nb + 2)));
+  return 0;
+}
+// grows the buffers sized by the rounds of a call (a prebuilt plan is dropped: its buffers go)
+int ensure_plan_rounds(hb_handle* h, int T) {
+  if (T <= h->plan->rounds) return 0;
+  TRY(plan_discard(h));
+  CK(cudaStreamSynchronize(h->stream));
+  TRY(plan_alloc_rounds(h, T));
+  TRY(alloc_update_rounds(h, T));
+  if (h->use_xch) TRY(setup_peer_exchange(h, T));  // collective: every rank grows its plan in the same call
+  return 0;
 }
 // zero the per-step accumulators of a cluster_cpp call ...
 int update_begin_zero(hb_handle* h, int T) {
@@ -1611,9 +1500,7 @@ int hb_create(hb_handle** out, int device) {
   cudaDeviceProp prop;
   if (cudaGetDeviceProperties(&prop, device) == cudaSuccess) h->num_sms = prop.multiProcessorCount;
   cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking);
-  cudaStreamCreateWithFlags(&h->plan_stream, cudaStreamNonBlocking);
-  cudaEventCreateWithFlags(&h->plan_done, cudaEventDisableTiming);
-  cudaEventCreateWithFlags(&h->ev0, cudaEventDisableTiming);
+  h->plan.reset(new Plan());
   ensure_pinned_staging();  // process-wide; the first handle pays for it, not the first download
   keep_pool_memory(device);
   widen_pool();
@@ -1624,11 +1511,7 @@ int hb_create(hb_handle** out, int device) {
 void hb_destroy(hb_handle* h) {
   if (!h) return;
   cudaSetDevice(h->device);
-  if (h->plan_stream) cudaStreamSynchronize(h->plan_stream);
   if (h->stream) cudaStreamSynchronize(h->stream);
-  if (h->plan_done) cudaEventDestroy(h->plan_done);
-  if (h->plan_stream) cudaStreamDestroy(h->plan_stream);
-  if (h->ev0) cudaEventDestroy(h->ev0);
   release_peer_exchange(h);
   cudaStream_t s = h->stream;
   delete h;  // frees device buffers
@@ -1693,10 +1576,9 @@ int hb_set_shard(hb_handle* h, int64_t N_global, int64_t cell_offset) {
 
 int hb_set_seed(hb_handle* h, uint64_t seed) {
   if (!h) return 1;
-  if (h->plan_stream) cudaStreamSynchronize(h->plan_stream);
-  h->next_ready = false;
+  TRY(plan_discard(h));
   h->seed = seed;
-  h->round_counter = 0;
+  h->plan->round_counter = 0;
   return 0;
 }
 
@@ -1877,24 +1759,14 @@ int hb_setup(hb_handle* h, const double* Z, int d, int64_t N, const int32_t* phi
       inv_sort[i] = (int)s;
     }
   }
-  // static tiles (<= TM cells of one tuple) and plan chunks (<= CHUNK cells of one tuple)
-  int CHUNK = 1024;  // plan chunks: ~2000 per shard at most (the plan's scan is nb^2 x #chunks long)
-  while (CHUNK < 16384 && N / CHUNK > 2048) CHUNK <<= 1;
-  std::vector<int> t_cell0, t_len, t_tuple, c_start, t_chunk0(J, 0), c_q0, c_nq;
-  for (int q = 0; q < J; ++q) {
+  // static tiles (<= TM cells of one tuple)
+  std::vector<int> t_cell0, t_len, t_tuple;
+  for (int q = 0; q < J; ++q)
     for (int64_t s = tstart[q]; s < tstart[q + 1]; s += TM) {
       t_cell0.push_back((int)s);
       t_len.push_back((int)std::min<int64_t>(TM, tstart[q + 1] - s));
       t_tuple.push_back(q);
     }
-    t_chunk0[q] = (int)c_start.size();
-    for (int64_t s = tstart[q]; s < tstart[q + 1]; s += CHUNK) c_start.push_back((int)s);
-    const int nq = (int)c_start.size() - t_chunk0[q];
-    for (int i = 0; i < nq; ++i) {
-      c_q0.push_back(t_chunk0[q]);
-      c_nq.push_back(nq);
-    }
-  }
   std::vector<int> tc0, tcl, tct;  // 128-cell tiles for the tensor-core kernels
   for (int q = 0; q < J; ++q)
     for (int64_t s2 = tstart[q]; s2 < tstart[q + 1]; s2 += TC_TM) {
@@ -1903,15 +1775,7 @@ int hb_setup(hb_handle* h, const double* Z, int d, int64_t N, const int32_t* phi
       tct.push_back(q);
     }
   h->tc_ntiles = (int)tc0.size();
-  c_q0.push_back((int)c_start.size());  // the trailing empty chunk is a group of its own
-  c_nq.push_back(1);
-  c_start.push_back((int)N);  // start of the trailing empty chunk
-  c_start.push_back((int)N);  // and its end
   h->ntiles = (int)t_cell0.size();
-  h->nchunks = (int)c_start.size() - 1;
-  // tuples without local cells point at the first later chunk (their segments are empty)
-  for (int q = J - 1; q >= 0; --q)
-    if (tstart[q + 1] == tstart[q]) t_chunk0[q] = (q + 1 < J) ? t_chunk0[q + 1] : h->nchunks - 1;
 
   lap.mark("tuple dictionary / sort (host)");
   // ---- device allocations
@@ -1922,7 +1786,6 @@ int hb_setup(hb_handle* h, const double* Z, int d, int64_t N, const int32_t* phi
   h->paths = select_kernels(K, d, J, N, h->nb, h->coop_grid, h->kernel_set);
   h->ring_rows = sp_ring_rows(KS, SMEM_LIMIT);
   const bool single_pass = h->paths.update == UpdatePath::SinglePass;
-  h->plan_nsub = (single_pass && h->nb <= 64) ? h->nb : 1;
   CK(h->Zo.alloc(nd));
   CK(h->Zc.alloc(nd));
   CK(h->U.alloc(nK));
@@ -1958,26 +1821,8 @@ int hb_setup(hb_handle* h, const double* Z, int d, int64_t N, const int32_t* phi
   CK(h->tc_cell0.alloc(h->tc_ntiles));
   CK(h->tc_len.alloc(h->tc_ntiles));
   CK(h->tc_tuple.alloc(h->tc_ntiles));
-  h->pt_cap = (size_t)N / TC_TM + (size_t)h->nb * J + 2;
-  if (h->paths.mm.k1_stages && single_pass) {
-    CK(h->pt_p0.alloc(2 * h->pt_cap));
-    CK(h->pt_len.alloc(2 * h->pt_cap));
-    CK(h->pt_tuple.alloc(2 * h->pt_cap));
-    CK(h->pt_blk.alloc(2 * h->pt_cap));
-    CK(h->pt_count.alloc(2));
-    CK(h->pt_base.alloc((size_t)h->nb * J + 2));
-  }
-  CK(h->chunk_start.alloc(h->nchunks + 1));
-  CK(h->tuple_chunk0.alloc(J));
-  TRY(alloc_plan_rounds(h, Tplan));
-  {  // histogram scratch of the plan's counting sort: as many rounds per launch as fit 64 MB (at most 8)
-    const size_t per_round = (size_t)h->nb * h->plan_nsub * h->nchunks;
-    h->plan_batch = (int)std::max<size_t>(1, std::min<size_t>({(size_t)8, (size_t)Tplan, ((size_t)16 << 20) / std::max<size_t>(1, per_round)}));
-    CK(h->H.alloc(per_round * h->plan_batch));
-    CK(h->scan_state.alloc((size_t)h->plan_batch * ((per_round + SCAN_TILE - 1) / SCAN_TILE + 1)));
-  }
-  CK(h->chunk_q0.alloc(h->nchunks));
-  CK(h->chunk_nq.alloc(h->nchunks));
+  TRY(plan_setup(h, tstart, Tplan));
+  TRY(ensure_plan_rounds(h, Tplan));
   if (h->paths.update != UpdatePath::PerStep) {
     CK(h->ring.alloc(4 * BK));
     CK(h->Psave.alloc(single_pass ? 1 : 2 * (size_t)h->nb * BK));
@@ -2027,10 +1872,6 @@ int hb_setup(hb_handle* h, const double* Z, int d, int64_t N, const int32_t* phi
   UP(tc_cell0, tc0);
   UP(tc_len, tcl);
   UP(tc_tuple, tct);
-  UP(chunk_start, c_start);
-  UP(chunk_q0, c_q0);
-  UP(chunk_nq, c_nq);
-  UP(tuple_chunk0, t_chunk0);
   {
     std::vector<float> f(K);
     for (int k = 0; k < K; ++k) f[k] = (float)sigma[k];
@@ -2242,16 +2083,6 @@ int legacy_centroid_step(hb_handle* h) {
   return 0;
 }
 
-int ensure_plan_rounds(hb_handle* h, int T) {
-  if (T <= h->plan_rounds) return 0;
-  if (h->plan_stream) CK(cudaStreamSynchronize(h->plan_stream));
-  CK(cudaStreamSynchronize(h->stream));
-  h->next_ready = false;
-  h->plan_set = 0;
-  TRY(alloc_plan_rounds(h, T));
-  if (h->use_xch) TRY(setup_peer_exchange(h, T));  // collective: every rank grows its plan in the same call
-  return 0;
-}
 
 int hb_cluster(hb_handle* h, const int64_t* update_orders) {
   if (!h) return 1;
@@ -2274,16 +2105,12 @@ int hb_cluster(hb_handle* h, const int64_t* update_orders) {
   if (h->abort_cb && h->abort_cb(h->abort_user)) return -1;  // Progress::check_abort (:233)
   unsigned iter = 0;
   if (call.update == UpdatePath::PerStep) {
-    if (h->next_ready) {  // a plan prebuilt by an earlier call on the side stream is not used here
-      CK(cudaStreamWaitEvent(h->stream, h->plan_done, 0));
-      h->round_counter -= (uint64_t)h->next_T;
-      h->next_ready = false;
-    }
+    TRY(plan_discard(h));  // a plan prebuilt by an earlier call is not used here
     for (iter = 0; iter < T; iter++) {
       if (iter > 0 && h->abort_cb && h->abort_cb(h->abort_user)) return -1;
       if (h->legacy_centroid) TRY(legacy_centroid_step(h));  // :235-238
-      TRY(build_plan_single(h, update_orders ? h->perms_d.p + (size_t)iter * (size_t)h->N_global : nullptr, h->stream));
-      TRY(run_update_per_step(h, 0));  // :241
+      TRY(build_plans(h, 1, update_orders ? h->perms_d.p + (size_t)iter * (size_t)h->N_global : nullptr, 0, h->stream, true));
+      TRY(run_update_per_step(h));  // :241
       TRY(push_objective(h));          // :248
       if (iter > h->window_size) {  // :250-256
         int conv = 0;
@@ -2297,20 +2124,7 @@ int hb_cluster(hb_handle* h, const int64_t* update_orders) {
   } else {
     // all T update orders are drawn up front (they do not depend on the data), then the rounds run in
     // chunks: [0, window_size + 2) in one launch, afterwards one round per launch (convergence checks)
-    // The native orders of a call depend only on (seed, round counter), so the plan of the NEXT call is
-    // prebuilt on a side stream while this call's correction / the next assignment run (two buffer sets).
-    if (h->next_ready) {
-      CK(cudaStreamWaitEvent(h->stream, h->plan_done, 0));  // also serialises the use of the scan scratch
-      if (!update_orders && h->next_T >= (int)T) {
-        h->plan_set ^= 1;  // adopt the prebuilt plan
-      } else {
-        h->round_counter -= (uint64_t)h->next_T;  // discard it: its rounds were never run
-        TRY(build_plans(h, (int)T, update_orders ? h->perms_d.p : nullptr, h->plan_set, h->stream));
-      }
-      h->next_ready = false;
-    } else {
-      TRY(build_plans(h, (int)T, update_orders ? h->perms_d.p : nullptr, h->plan_set, h->stream));
-    }
+    TRY(plan_acquire(h, (int)T, update_orders ? h->perms_d.p : nullptr));
     if (T > 0) TRY(update_begin_zero(h, (int)T));
     if (plan_assign) {
       TRY(run_assign(h, true, true, false));
@@ -2337,16 +2151,8 @@ int hb_cluster(hb_handle* h, const int64_t* update_orders) {
       t0 = t1;
     }
   }
-  if (call.update != UpdatePath::PerStep && !update_orders && T > 0 && !h->timing) {
-    // prebuild the next call's plan into the other buffer set on the side stream; it starts once this
-    // call's own (main-stream) plan build and update kernel are done with the shared scan scratch
-    CK(cudaEventRecord(h->ev0, h->stream));
-    CK(cudaStreamWaitEvent(h->plan_stream, h->ev0, 0));
-    TRY(build_plans(h, (int)T, nullptr, h->plan_set ^ 1, h->plan_stream));
-    CK(cudaEventRecord(h->plan_done, h->plan_stream));
-    h->next_ready = true;
-    h->next_T = (int)T;
-  }
+  if (call.update != UpdatePath::PerStep && !update_orders && T > 0 && !h->timing)
+    TRY(plan_prebuild(h, (int)T));  // the next call's plan, while this call's correction and the next assignment run
   if (T > 0) h->R_user_set = false;
   if (update_orders) TRY(check_err_flag(h));
   h->kmeans_rounds.push_back((int)iter);         // :259

@@ -535,361 +535,6 @@ __global__ void k_assign_finalize_plan(const float* __restrict__ acc, int nb, co
   }
 }
 
-// ------------------------------------------------------------------------------------------------
-// update-order plan (replaces the physical shuffles of harmony.cpp:272-291)
-// ------------------------------------------------------------------------------------------------
-// Injected order: for global position p, cell update_order[p] belongs to block min(p/cpb, nb-1).
-__global__ void k_plan_block_injected(const int64_t* __restrict__ update_order, int64_t N_global, int64_t cell_offset,
-                                      int64_t n_local, const int* __restrict__ inv_sort, uint32_t cpb, int nb,
-                                      int* __restrict__ blk_of, int* __restrict__ err_flag) {
-  update_order += (size_t)blockIdx.y * (size_t)N_global;  // blockIdx.y: round of the call
-  blk_of += (size_t)blockIdx.y * (size_t)n_local;
-  for (int64_t p = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; p < N_global;
-       p += (int64_t)gridDim.x * blockDim.x) {
-    int64_t g = update_order[p];
-    if (g < 0 || g >= N_global) {
-      atomicExch(err_flag, 1);
-      continue;
-    }
-    int64_t l = g - cell_offset;
-    if (l < 0 || l >= n_local) continue;
-    int64_t b = p / cpb;
-    if (b > nb - 1) b = nb - 1;
-    blk_of[inv_sort[l]] = (int)b;
-  }
-}
-// Native order: position of global cell g is hb_permute(g) (a keyed bijection of [0, N)); the key of a round
-// depends on (seed, round counter) only.  blockIdx.y: round of the call.
-__host__ __device__ __forceinline__ uint64_t plan_round_key(uint64_t seed, uint64_t round_counter) {
-  return hb_mix64(seed ^ hb_mix64(round_counter + 0x1234567ull));
-}
-__global__ void k_plan_block_native(int64_t N_global, int64_t cell_offset, int64_t n_local,
-                                    const int* __restrict__ sort_perm, uint32_t cpb, int nb, int half_bits,
-                                    uint64_t seed, uint64_t round_counter0, int* __restrict__ blk_of) {
-  const uint64_t key = plan_round_key(seed, round_counter0 + blockIdx.y);
-  blk_of += (size_t)blockIdx.y * (size_t)n_local;
-  for (int64_t s = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; s < n_local;
-       s += (int64_t)gridDim.x * blockDim.x) {
-    uint64_t g = (uint64_t)(cell_offset + sort_perm[s]);
-    uint64_t pos = hb_permute(g, (uint64_t)N_global, half_bits, key);
-    uint64_t b = pos / cpb;
-    if (b > (uint64_t)(nb - 1)) b = nb - 1;
-    blk_of[s] = (int)b;
-  }
-}
-// Sort key of a cell in round t: (block in round t, tuple, block in round t+1, chunk, cell).  Chunks are runs of
-// consecutive (tuple-sorted) cells of one tuple, so with the histogram laid out as
-//   H[blk][ nsub * cq0[c] + sub * cnq[c] + (c - cq0[c]) ]      (cq0 / cnq: first chunk / #chunks of c's tuple)
-// one plain exclusive scan of H yields the offsets of that order (nsub = nb, sub = next-round block; nsub = 1
-// switches the third key off).
-__device__ __forceinline__ size_t plan_hidx(int blk, int sub, int c, int nchunks, int nsub, const int* __restrict__ cq0,
-                                            const int* __restrict__ cnq) {
-  const int c0 = cq0[c];
-  return (size_t)blk * nsub * nchunks + (size_t)nsub * c0 + (size_t)sub * cnq[c] + (c - c0);
-}
-// One warp per chunk: H[..] = #cells of the chunk with (block, next-round block) = (blk, sub).
-__global__ void k_plan_hist(const int* __restrict__ blk_of, const int* __restrict__ blk_next,
-                            const int* __restrict__ chunk_start, const int* __restrict__ cq0, const int* __restrict__ cnq,
-                            int nchunks, int nb, int nsub, int* __restrict__ H, int* __restrict__ err_flag, int64_t n_local,
-                            int rounds_with_next) {
-  extern __shared__ int sh[];
-  int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  int* cnt = sh + warp * nb * nsub;
-  int c = blockIdx.x * (blockDim.x >> 5) + warp;
-  if (c >= nchunks) return;
-  // blockIdx.y: round of the batch (rounds are n_local apart in blk_of; blk_next of round y is blk_of of round y + 1)
-  blk_of += (size_t)blockIdx.y * (size_t)n_local;
-  blk_next = ((int)blockIdx.y < rounds_with_next) ? blk_of + n_local : nullptr;
-  H += (size_t)blockIdx.y * (size_t)nb * nsub * nchunks;
-  for (int j = lane; j < nb * nsub; j += 32) cnt[j] = 0;
-  __syncwarp();
-  int s0 = chunk_start[c], s1 = chunk_start[c + 1];
-  for (int s = s0 + lane; s < s1; s += 32) {
-    const int b = blk_of[s];
-    if (b < 0 || b >= nb) {  // an injected update order that is not a permutation left this cell without a block
-      atomicCAS(err_flag, 0, 3);  // an out-of-range index (flag 1) is the more specific report
-      continue;
-    }
-    const int sub = (nsub > 1 && blk_next) ? blk_next[s] : 0;
-    atomicAdd(cnt + b * nsub + ((sub >= 0 && sub < nsub) ? sub : 0), 1);
-  }
-  __syncwarp();
-  for (int j = lane; j < nb * nsub; j += 32) H[plan_hidx(j / nsub, j % nsub, c, nchunks, nsub, cq0, cnq)] = cnt[j];
-}
-// Single-CTA exclusive scan of an int array (in place), total written to *total.  Every warp owns a contiguous
-// range and walks it 32 consecutive elements at a time (coalesced): pass 1 sums, pass 2 scans with a carry.
-__global__ void __launch_bounds__(1024) k_scan_exclusive(int* __restrict__ data, int64_t n, int* __restrict__ total) {
-  data += (size_t)blockIdx.x * (size_t)n;  // blockIdx.x: independent arrays of n elements, back to back
-  if (total) total += blockIdx.x;
-  __shared__ int wsum[32];
-  __shared__ int carry_all;
-  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, nw = blockDim.x >> 5;
-  const int64_t per = ((n + nw - 1) / nw + 31) & ~(int64_t)31;
-  const int64_t lo = (int64_t)warp * per, hi = (lo + per < n) ? lo + per : n;
-  int s = 0;
-  for (int64_t i = lo + lane; i < hi; i += 32) s += data[i];
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
-  if (lane == 0) wsum[warp] = s;
-  __syncthreads();
-  if (warp == 0) {
-    int v = (lane < nw) ? wsum[lane] : 0;
-    int inc = v;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-      int t = __shfl_up_sync(0xffffffffu, inc, o);
-      if (lane >= o) inc += t;
-    }
-    wsum[lane] = inc - v;
-    if (lane == 31) carry_all = inc;
-  }
-  __syncthreads();
-  int carry = wsum[warp];
-  for (int64_t i0 = lo; i0 < hi; i0 += 32) {
-    const int64_t i = i0 + lane;
-    const int v = (i < hi) ? data[i] : 0;
-    int inc = v;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-      int t = __shfl_up_sync(0xffffffffu, inc, o);
-      if (lane >= o) inc += t;
-    }
-    if (i < hi) data[i] = carry + inc - v;
-    carry += __shfl_sync(0xffffffffu, inc, 31);
-  }
-  if (tid == 0 && total) *total = carry_all;
-}
-// Exclusive scan of `nseg` independent int arrays of n elements (back to back in `data`, in place) by many CTAs:
-// chained scan with dynamic tile numbers.  A CTA draws the next tile (8192 elements) of its segment from a counter
-// — so a tile's predecessor has always been drawn, i.e. runs or has run: no deadlock whatever the dispatch order —,
-// scans it locally, waits for the inclusive prefix of the tile before it, publishes its own (value and flag in one
-// 64-bit word) and writes the results.  state: [nseg][1 + tiles] words, zeroed by the caller (word 0: the counter).
-constexpr int SCAN_TILE = 8192;  // 1024 threads x 8 elements
-__global__ void __launch_bounds__(1024) k_scan_chained(int* __restrict__ data, int64_t n, unsigned long long* __restrict__ state,
-                                                       int tiles_per_seg) {
-  __shared__ int wsum[32];
-  __shared__ int sh_tile, sh_carry;
-  const int seg = blockIdx.y;
-  data += (size_t)seg * (size_t)n;
-  unsigned long long* st = state + (size_t)seg * (tiles_per_seg + 1);
-  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  if (tid == 0) sh_tile = (int)atomicAdd(st, 1ull);
-  __syncthreads();
-  const int tile = sh_tile;
-  if (tile >= tiles_per_seg) return;
-  const int64_t base = (int64_t)tile * SCAN_TILE + (int64_t)tid * 8;
-  int v[8];
-  int s = 0;
-#pragma unroll
-  for (int i = 0; i < 8; ++i) {
-    v[i] = (base + i < n) ? data[base + i] : 0;
-    s += v[i];
-  }
-  // exclusive scan of the threads' sums within the CTA
-  int inc = s;
-#pragma unroll
-  for (int o = 1; o < 32; o <<= 1) {
-    const int t = __shfl_up_sync(0xffffffffu, inc, o);
-    if (lane >= o) inc += t;
-  }
-  if (lane == 31) wsum[warp] = inc;
-  __syncthreads();
-  if (warp == 0) {
-    const int w = wsum[lane];
-    int winc = w;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-      const int t = __shfl_up_sync(0xffffffffu, winc, o);
-      if (lane >= o) winc += t;
-    }
-    wsum[lane] = winc - w;  // exclusive prefix of the warps
-    if (lane == 31) {
-      // tile aggregate = winc; chain: inclusive prefix of this tile = prefix of the previous one + aggregate
-      int carry = 0;
-      if (tile > 0) {
-        unsigned long long p;
-        do {
-          asm volatile("ld.acquire.gpu.global.u64 %0, [%1];" : "=l"(p) : "l"(st + tile) : "memory");  // word 1 + (tile - 1)
-        } while ((p >> 32) == 0ull);
-        carry = (int)(unsigned)(p & 0xffffffffull);
-      }
-      const unsigned long long mine = (1ull << 32) | (unsigned)(carry + winc);
-      asm volatile("st.release.gpu.global.u64 [%0], %1;" ::"l"(st + tile + 1), "l"(mine) : "memory");
-      sh_carry = carry;
-    }
-  }
-  __syncthreads();
-  int run = sh_carry + wsum[warp] + (inc - s);
-#pragma unroll
-  for (int i = 0; i < 8; ++i) {
-    if (base + i < n) data[base + i] = run;
-    run += v[i];
-  }
-}
-// Stable scatter: order[offset(key, chunk) + rank] = cell, cells of a chunk visited in ascending order;
-// next_at[same position] = block of the cell in the next round.
-__global__ void k_plan_scatter(const int* __restrict__ blk_of, const int* __restrict__ blk_next,
-                               const int* __restrict__ chunk_start, const int* __restrict__ cq0, const int* __restrict__ cnq,
-                               int nchunks, int nb, int nsub, const int* __restrict__ Hoff, int* __restrict__ order,
-                               const int* __restrict__ blk_prev, int* __restrict__ prev_at, int* __restrict__ next_at,
-                               int64_t n_local, int rounds_with_next, int first_has_prev) {
-  extern __shared__ int sh[];
-  int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  int* cur = sh + warp * nb * nsub;
-  int c = blockIdx.x * (blockDim.x >> 5) + warp;
-  if (c >= nchunks) return;
-  {  // blockIdx.y: round of the batch
-    const size_t ro = (size_t)blockIdx.y * (size_t)n_local;
-    blk_of += ro;
-    blk_next = ((int)blockIdx.y < rounds_with_next) ? blk_of + n_local : nullptr;
-    blk_prev = (blockIdx.y > 0 || first_has_prev) ? blk_of - n_local : nullptr;
-    Hoff += (size_t)blockIdx.y * (size_t)nb * nsub * nchunks;
-    order += ro;
-    if (prev_at) prev_at += ro;
-    if (next_at) next_at += ro;
-  }
-  for (int j = lane; j < nb * nsub; j += 32) cur[j] = Hoff[plan_hidx(j / nsub, j % nsub, c, nchunks, nsub, cq0, cnq)];
-  __syncwarp();
-  int s0 = chunk_start[c], s1 = chunk_start[c + 1];
-  for (int base = s0; base < s1; base += 32) {
-    int s = base + lane;
-    bool act = s < s1;
-    int b = act ? blk_of[s] : -1;
-    act = act && b >= 0 && b < nb;  // cells without a block were flagged by k_plan_hist
-    int nx = (act && blk_next) ? blk_next[s] : 0;
-    if (nx < 0 || nx >= nb) nx = 0;
-    int key = act ? b * nsub + (nsub > 1 ? nx : 0) : -1 - lane;  // inactive lanes get unique keys
-    unsigned m = __match_any_sync(0xffffffffu, key);
-    int rank = __popc(m & ((1u << lane) - 1u));
-    int leader = __ffs(m) - 1;
-    int start = 0;
-    if (act && lane == leader) {
-      start = cur[key];
-      cur[key] = start + __popc(m);
-    }
-    start = __shfl_sync(0xffffffffu, start, leader);
-    if (act) {
-      order[start + rank] = s;
-      if (prev_at) prev_at[start + rank] = blk_prev ? blk_prev[s] : 0;
-      if (next_at) next_at[start + rank] = nx;
-    }
-    __syncwarp();
-  }
-}
-// Segment (block, tuple) boundaries: seg s = blk*J + q starts at the offset of (blk, first chunk of q, sub 0).
-__global__ void k_plan_segments(const int* __restrict__ Hoff, const int* __restrict__ tuple_chunk0, int nchunks,
-                                int nb, int nsub, int J, int n_local, int* __restrict__ seg_start,
-                                int* __restrict__ tile_base) {
-  int S = nb * J;
-  Hoff += (size_t)blockIdx.y * (size_t)nb * nsub * nchunks;  // blockIdx.y: round of the batch
-  seg_start += (size_t)blockIdx.y * (S + 1);
-  for (int s = blockIdx.x * blockDim.x + threadIdx.x; s <= S; s += gridDim.x * blockDim.x) {
-    int v;
-    if (s == S) {
-      v = n_local;
-    } else {
-      int blk = s / J, q = s - blk * J;
-      int c = tuple_chunk0[q];  // first chunk of tuple q (tuples without local cells point at the first later chunk)
-      v = Hoff[(size_t)blk * nsub * nchunks + (size_t)nsub * c];
-    }
-    seg_start[s] = v;
-  }
-}
-// Tuple-aligned work split of every block for the persistent update kernel (G CTAs): each CTA gets a contiguous
-// slice of ONE (block, tuple) segment.  The block step ends when its most loaded CTA does, so the CTAs are dealt out
-// to minimise the largest slice: every non-empty segment starts with one CTA and the remaining ones go, one at a
-// time, to the segment with the most rows per CTA (exact comparison L_a n_b > L_b n_a; ties to the lower tuple).
-// One CTA (256 threads) per (block j = blockIdx.x, round = blockIdx.y); J <= 2 J <= G <= 1024.
-constexpr int PLAN_MAXJ = 512;
-__global__ void __launch_bounds__(256) k_plan_ranges(const int* __restrict__ seg_start, int nb, int J, int G,
-                                                     int4* __restrict__ ranges) {
-  __shared__ int L[PLAN_MAXJ], nq[PLAN_MAXJ], first[PLAN_MAXJ + 1];
-  seg_start += (size_t)blockIdx.y * ((size_t)nb * J + 1);  // blockIdx.y: round of the batch
-  ranges += (size_t)blockIdx.y * (size_t)nb * G;
-  const int j = blockIdx.x;
-  const int* segs = seg_start + (size_t)j * J;
-  const int tid = threadIdx.x, lane = tid & 31;
-  for (int q = tid; q < J; q += blockDim.x) {
-    L[q] = segs[q + 1] - segs[q];
-    nq[q] = L[q] > 0 ? 1 : 0;
-  }
-  __syncthreads();
-  if (tid < 32) {
-    int nonempty = 0;
-    for (int q = lane; q < J; q += 32) nonempty += nq[q];
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) nonempty += __shfl_xor_sync(0xffffffffu, nonempty, o);
-    for (int rem = (nonempty > 0) ? G - nonempty : 0; rem > 0; --rem) {
-      long long bl = 0, bn = 1;  // best ratio bl / bn of this lane
-      int bq = J;
-      for (int q = lane; q < J; q += 32)
-        if (nq[q] > 0 && (long long)L[q] * bn > bl * (long long)nq[q]) {
-          bl = L[q];
-          bn = nq[q];
-          bq = q;
-        }
-#pragma unroll
-      for (int o = 16; o > 0; o >>= 1) {
-        const long long ol = __shfl_xor_sync(0xffffffffu, bl, o), on = __shfl_xor_sync(0xffffffffu, bn, o);
-        const int oq = __shfl_xor_sync(0xffffffffu, bq, o);
-        const long long lhs = ol * bn, rhs = bl * on;
-        if (lhs > rhs || (lhs == rhs && oq < bq)) {
-          bl = ol;
-          bn = on;
-          bq = oq;
-        }
-      }
-      if (lane == 0 && bq < J) nq[bq]++;
-      __syncwarp();
-    }
-    if (lane == 0) {
-      int c = 0;
-      for (int q = 0; q < J; ++q) {
-        first[q] = c;
-        c += nq[q];
-      }
-      first[J] = c;
-    }
-  }
-  __syncthreads();
-  const int b0 = segs[0];
-  for (int c = tid; c < G; c += blockDim.x) {
-    int4 out = make_int4(b0, b0, 0, 0);
-    if (c < first[J]) {
-      int q = 0;
-      while (first[q + 1] <= c) ++q;  // J is small
-      const int n = nq[q], me = c - first[q];
-      out = make_int4(segs[q] + (int)(((long long)L[q] * me) / n), segs[q] + (int)(((long long)L[q] * (me + 1)) / n), q, 0);
-    }
-    ranges[(size_t)j * G + c] = out;
-  }
-}
-// 128-row tiles of the (block, tuple) segments of a round (the assignment step in plan order)
-__global__ void k_plan_tilecount128(const int* __restrict__ seg_start, int S, int* __restrict__ tile_base) {
-  for (int s = blockIdx.x * blockDim.x + threadIdx.x; s <= S; s += gridDim.x * blockDim.x)
-    tile_base[s] = (s < S) ? (seg_start[s + 1] - seg_start[s] + 127) / 128 : 0;
-}
-__global__ void k_plan_tilefill128(const int* __restrict__ seg_start, const int* __restrict__ tile_base, int S, int J,
-                                   int* __restrict__ p0, int* __restrict__ len, int* __restrict__ tuple,
-                                   int* __restrict__ blk) {
-  for (int s = blockIdx.x * blockDim.x + threadIdx.x; s < S; s += gridDim.x * blockDim.x) {
-    const int a = seg_start[s], e = seg_start[s + 1];
-    int i = tile_base[s];
-    for (int p = a; p < e; p += 128, ++i) {
-      p0[i] = p;
-      len[i] = min(128, e - p);
-      tuple[i] = s % J;
-      blk[i] = s / J;
-    }
-  }
-}
-__global__ void k_plan_tilecount(const int* __restrict__ seg_start, int S, int* __restrict__ tile_base) {
-  for (int s = blockIdx.x * blockDim.x + threadIdx.x; s <= S; s += gridDim.x * blockDim.x) {
-    int len = (s < S) ? seg_start[s + 1] - seg_start[s] : 0;
-    tile_base[s] = (len + TM - 1) / TM;
-  }
-}
-
 // compute_objective (harmony.cpp:158-170) once the per-cell sums are known:
 //   cross = sum_kb sigma_k theta_b log((O+E+1)/(2E+1)) O_kb   (== the reference's N-pass, SURVEY §8a')
 // Appends (total, dist, entropy, cross) * 2000/N to the device trace at slot `slot` and clears obj_acc.
