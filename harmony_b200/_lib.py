@@ -11,7 +11,7 @@ import subprocess
 _HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(_HERE)
 SO_PATH = os.path.join(_HERE, "libharmony_b200.so")
-SOURCES = [os.path.join(_HERE, "csrc", f) for f in ("harmony_b200.cu", "kernels.cuh", "common.cuh", "update_slots.cuh", "update_per_step.cuh",
+SOURCES = [os.path.join(_HERE, "csrc", f) for f in ("harmony_b200.cu", "kernels.cuh", "io.cuh", "common.cuh", "update_slots.cuh", "update_per_step.cuh",
                                                      "update_two_pass.cuh", "update_single_pass.cuh", "plan.cuh", "umma.cuh", "assign_tc3.cuh", "logits_tc.cuh", "stats_tc3.cuh", "apply_tc3.cuh")]
 HEADER = os.path.join(ROOT, "include", "harmony_b200.h")
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17", "-shared",
@@ -67,6 +67,7 @@ def lib():
     L.hb_comm_init.argtypes = [P, I, I, ctypes.c_char_p]
     L.hb_set_shard.argtypes = [P, I64, I64]
     L.hb_setup.argtypes = [P, P, I, I64, P, P, I, P, P, P, D, I, D, D, I, D, D, I]
+    L.hb_setup_device.argtypes = [P, P, I, I64, P, I, I64, P, P, I, P, P, P, D, I, D, D, I, D, D, I]
     L.hb_set_seed.argtypes = [P, ctypes.c_uint64]
     L.hb_set_abort_callback.argtypes = [P, P, P]
     L.hb_init_cluster.argtypes = [P, P]
@@ -77,6 +78,7 @@ def lib():
     L.hb_field_size.restype = I64
     L.hb_field_size.argtypes = [P, I]
     L.hb_get_field.argtypes = [P, I, P]
+    L.hb_get_field_device.argtypes = [P, I, P, I, I64, P]
     L.hb_set_field.argtypes = [P, I, P]
     L.hb_get_scalar.argtypes = [P, I, ctypes.POINTER(D)]
     L.hb_set_scalar.argtypes = [P, I, D]

@@ -28,6 +28,7 @@
 #include <vector>
 
 #include "kernels.cuh"
+#include "io.cuh"
 #include "update_per_step.cuh"
 #include "update_two_pass.cuh"
 #include "update_single_pass.cuh"
@@ -1386,8 +1387,7 @@ int download_rows_mt(hb_handle* h, const float* src, int cols, int ld, double* o
   auto enqueue = [&](int64_t i) -> int {
     const int64_t r0 = i * rows_per, rows = std::min(rows_per, n - r0);
     float* d = dev + (size_t)(i & 1) * dev_half;
-    k_download_rows_f<<<grid_for(rows * cols, 256, h->num_sms * 8), 256, 0, h->stream>>>(src, d, h->inv_sort.p, r0, rows,
-                                                                                         cols, ld);
+    copy_rows(src, ld, d, cols, h->inv_sort.p, r0, false, rows, cols, h->num_sms, h->stream);
     CKL();
     CK(cudaMemcpyAsync(pinned[i & 1], d, sizeof(float) * (size_t)rows * cols, cudaMemcpyDeviceToHost, h->stream));
     CK(cudaEventRecord(ev[i & 1], h->stream));
@@ -1411,6 +1411,7 @@ int download_rows_mt(hb_handle* h, const float* src, int cols, int ld, double* o
   return rc;
 }
 int download_rows(hb_handle* h, const float* src, int cols, int ld, double* out) {
+  RegionScope rs(h, "download");
   {
     bool done = false;
     TRY(download_rows_mt(h, src, cols, ld, out, &done));
@@ -1420,8 +1421,7 @@ int download_rows(hb_handle* h, const float* src, int cols, int ld, double* out)
   const int64_t rows_per = std::max<int64_t>(1, (int64_t)(h->stage.n / (size_t)cols));
   for (int64_t r0 = 0; r0 < n; r0 += rows_per) {
     int64_t rows = std::min(rows_per, n - r0);
-    k_download_rows<<<grid_for(rows * cols, 256, h->num_sms * 8), 256, 0, h->stream>>>(src, h->stage.p, h->inv_sort.p,
-                                                                                        r0, rows, cols, ld);
+    copy_rows(src, ld, h->stage.p, cols, h->inv_sort.p, r0, false, rows, cols, h->num_sms, h->stream);
     CKL();
     CK(cudaMemcpyAsync(out + r0 * cols, h->stage.p, sizeof(double) * (size_t)rows * cols, cudaMemcpyDeviceToHost,
                        h->stream));
@@ -1430,17 +1430,63 @@ int download_rows(hb_handle* h, const float* src, int cols, int ld, double* out)
   return 0;
 }
 int upload_rows(hb_handle* h, const double* in, int cols, int ld, float* dst) {
+  RegionScope rs(h, "upload");
   const int64_t n = h->n;
   const int64_t rows_per = std::max<int64_t>(1, (int64_t)(h->stage.n / (size_t)cols));
   for (int64_t r0 = 0; r0 < n; r0 += rows_per) {
     int64_t rows = std::min(rows_per, n - r0);
     CK(cudaMemcpyAsync(h->stage.p, in + r0 * cols, sizeof(double) * (size_t)rows * cols, cudaMemcpyHostToDevice,
                        h->stream));
-    k_upload_rows<<<grid_for(rows * cols, 256, h->num_sms * 8), 256, 0, h->stream>>>(h->stage.p, dst, h->inv_sort.p, r0,
-                                                                                      rows, cols, ld);
+    copy_rows<double, float>(h->stage.p, cols, dst, ld, h->inv_sort.p, r0, true, rows, cols, h->num_sms, h->stream);
     CKL();
     CK(cudaStreamSynchronize(h->stream));
   }
+  return 0;
+}
+
+// ---- device-memory boundary (hb_setup_device / hb_get_field_device) -------------------------------------------------
+// Source of Z for setup: host doubles (d per row, dense) or a device array of `dtype` with row stride `ld`, read on the
+// library stream after the work queued on `stream`.
+struct ZInput {
+  const double* host = nullptr;
+  const void* dev = nullptr;
+  int dtype = HB_FLOAT64;
+  int64_t ld = 0;
+  cudaStream_t stream = nullptr;
+};
+// A caller buffer must be device or managed memory of the handle's device: the kernels dereference it directly.
+int check_device_ptr(hb_handle* h, const void* p, const char* what) {
+  if (!p) return fail(h, 2, "null %s", what);
+  cudaPointerAttributes a{};
+  const cudaError_t e = cudaPointerGetAttributes(&a, p);
+  cudaGetLastError();
+  if (e != cudaSuccess || (a.type != cudaMemoryTypeDevice && a.type != cudaMemoryTypeManaged))
+    return fail(h, 2, "%s is not device or managed memory (host buffers go through hb_setup / hb_get_field)", what);
+  if (a.device != h->device)
+    return fail(h, 2, "%s lives on device %d, the handle on device %d", what, a.device, h->device);
+  return 0;
+}
+// `later` waits for the work queued on `earlier` so far (no host synchronisation)
+int stream_after(hb_handle* h, cudaStream_t later, cudaStream_t earlier) {
+  if (later == earlier) return 0;
+  cudaEvent_t ev;
+  CK(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
+  const cudaError_t e1 = cudaEventRecord(ev, earlier);
+  const cudaError_t e2 = e1 == cudaSuccess ? cudaStreamWaitEvent(later, ev, 0) : e1;
+  cudaEventDestroy(ev);
+  CK(e2);
+  return 0;
+}
+// Z (n rows of d values, row stride ld elements, fp32 / fp64 device memory) -> Zo in tuple-sorted order, on the
+// library stream after the work queued on `caller`
+int upload_rows_device(hb_handle* h, const void* Z, int dtype, int64_t ld, cudaStream_t caller) {
+  RegionScope rs(h, "upload");
+  TRY(stream_after(h, h->stream, caller));
+  if (dtype == HB_FLOAT32)
+    copy_rows((const float*)Z, ld, h->Zo.p, h->DS, h->inv_sort.p, 0, true, h->n, h->d, h->num_sms, h->stream);
+  else
+    copy_rows((const double*)Z, ld, h->Zo.p, h->DS, h->inv_sort.p, 0, true, h->n, h->d, h->num_sms, h->stream);
+  CKL();
   return 0;
 }
 // K x B tables are stored [B][KS]; the boundary wants them dense
@@ -1483,7 +1529,7 @@ int upload_small(hb_handle* h, const double* in, size_t count, float* dst) {
 // =================================================================================================
 extern "C" {
 
-int hb_version(void) { return 100; }
+int hb_version(void) { return 200; }
 
 int hb_create(hb_handle** out, int device) {
   if (!out) return 1;
@@ -1589,13 +1635,14 @@ int hb_set_abort_callback(hb_handle* h, int (*cb)(void*), void* user) {
   return 0;
 }
 
-int hb_setup(hb_handle* h, const double* Z, int d, int64_t N, const int32_t* phi_i, const int32_t* B_vec, int C,
-             const double* sigma, const double* theta, const double* lambda, double alpha, int max_iter_kmeans,
-             double epsilon_kmeans, double epsilon_harmony, int K, double block_size,
-             double batch_proportion_cutoff, int verbose) {
+// hb_setup and hb_setup_device: everything but the source of Z
+static int setup_common(hb_handle* h, const ZInput& Z, int d, int64_t N, const int32_t* phi_i, const int32_t* B_vec,
+                        int C, const double* sigma, const double* theta, const double* lambda, double alpha,
+                        int max_iter_kmeans, double epsilon_kmeans, double epsilon_harmony, int K, double block_size,
+                        double batch_proportion_cutoff, int verbose) {
   if (!h) return 1;
   if (h->ran_setup) return fail(h, 3, "setup was already run on this object");
-  if (!Z || !phi_i || !B_vec || !sigma || !theta) return fail(h, 2, "null argument");
+  if (!(Z.host || Z.dev) || !phi_i || !B_vec || !sigma || !theta) return fail(h, 2, "null argument");
   if (d < 1 || N < 1 || C < 1 || K < 1) return fail(h, 2, "bad dimensions");
   if (K > 1024) return fail(h, 2, "K = %d is not supported (K <= 1024)", K);
   if (N > 2000000000LL) return fail(h, 2, "more than 2e9 cells per GPU are not supported");
@@ -1898,13 +1945,44 @@ int hb_setup(hb_handle* h, const double* Z, int d, int64_t N, const int32_t* phi
 #undef UP
   lap.mark("memsets + small uploads");
   // Z: double -> float, into tuple-sorted order (harmony.cpp:41); Z_corr = normalise(Z_orig) (:42)
-  TRY(upload_rows(h, Z, d, h->DS, h->Zo.p));
+  if (Z.dev)
+    TRY(upload_rows_device(h, Z.dev, Z.dtype, Z.ld, Z.stream));
+  else
+    TRY(upload_rows(h, Z.host, d, h->DS, h->Zo.p));
   k_normalise_rows<<<grid_for(N * 32, 256, h->num_sms * 8), 256, 0, h->stream>>>(h->Zo.p, h->Zc.p, N, d, h->DS);
   CKL();
   CK(cudaStreamSynchronize(h->stream));
   lap.mark("Z upload + normalise");
   h->ran_setup = true;
   return 0;
+}
+
+int hb_setup(hb_handle* h, const double* Z, int d, int64_t N, const int32_t* phi_i, const int32_t* B_vec, int C,
+             const double* sigma, const double* theta, const double* lambda, double alpha, int max_iter_kmeans,
+             double epsilon_kmeans, double epsilon_harmony, int K, double block_size,
+             double batch_proportion_cutoff, int verbose) {
+  ZInput z;
+  z.host = Z;
+  return setup_common(h, z, d, N, phi_i, B_vec, C, sigma, theta, lambda, alpha, max_iter_kmeans, epsilon_kmeans,
+                      epsilon_harmony, K, block_size, batch_proportion_cutoff, verbose);
+}
+
+int hb_setup_device(hb_handle* h, const void* Z, int z_dtype, int64_t z_ld, void* stream, int d, int64_t N,
+                    const int32_t* phi_i, const int32_t* B_vec, int C, const double* sigma, const double* theta,
+                    const double* lambda, double alpha, int max_iter_kmeans, double epsilon_kmeans,
+                    double epsilon_harmony, int K, double block_size, double batch_proportion_cutoff, int verbose) {
+  if (!h) return 1;
+  if (h->ran_setup) return fail(h, 3, "setup was already run on this object");
+  if (z_dtype != HB_FLOAT32 && z_dtype != HB_FLOAT64) return fail(h, 2, "unknown dtype %d of Z", z_dtype);
+  if (z_ld < d) return fail(h, 2, "row stride of Z (%lld) is smaller than d = %d", (long long)z_ld, d);
+  TRY(check_device_ptr(h, Z, "Z"));
+  ZInput z;
+  z.dev = Z;
+  z.dtype = z_dtype;
+  z.ld = z_ld;
+  z.stream = (cudaStream_t)stream;
+  return setup_common(h, z, d, N, phi_i, B_vec, C, sigma, theta, lambda, alpha, max_iter_kmeans, epsilon_kmeans,
+                      epsilon_harmony, K, block_size, batch_proportion_cutoff, verbose);
 }
 
 int hb_init_cluster(hb_handle* h, const double* Y0) {
@@ -2208,6 +2286,15 @@ int64_t hb_field_size(const hb_handle* h, int field) {
   return 0;
 }
 
+// cluster_cpp leaves Z_corr cosine-normalised (harmony.cpp:220); the library normalises on the first read of Z_corr
+static int normalise_pending_zc(hb_handle* h) {
+  if (!h->zc_pending_norm) return 0;
+  k_normalise_rows<<<grid_for((int64_t)h->n * 32, 256, h->num_sms * 8), 256, 0, h->stream>>>(h->Zc.p, h->Zc.p, h->n, h->d, h->DS);
+  CKL();
+  h->zc_pending_norm = false;
+  return 0;
+}
+
 int hb_get_field(hb_handle* h, int field, double* out) {
   if (!h) return 1;
   if (!h->ran_setup) return fail(h, 3, "setup has not been run");
@@ -2217,11 +2304,7 @@ int hb_get_field(hb_handle* h, int field, double* out) {
   switch (field) {
     case HB_Z_CORR: {
       HostLap lap(h->stream, "hb_get_field");
-      if (h->zc_pending_norm) {  // cluster_cpp leaves Z_corr cosine-normalised (harmony.cpp:220); done on first demand
-        k_normalise_rows<<<grid_for((int64_t)h->n * 32, 256, h->num_sms * 8), 256, 0, h->stream>>>(h->Zc.p, h->Zc.p, h->n, d, h->DS);
-        CKL();
-        h->zc_pending_norm = false;
-      }
+      TRY(normalise_pending_zc(h));
       const int rc = download_rows(h, h->Zc.p, d, h->DS, out);
       lap.mark("Z_corr download");
       return rc;
@@ -2262,6 +2345,32 @@ int hb_get_field(hb_handle* h, int field, double* out) {
     }
   }
   return fail(h, 2, "unknown field %d", field);
+}
+
+int hb_get_field_device(hb_handle* h, int field, void* out, int dtype, int64_t ld, void* stream) {
+  if (!h) return 1;
+  if (!h->ran_setup) return fail(h, 3, "setup has not been run");
+  if (field != HB_Z_CORR && field != HB_Z_ORIG && field != HB_R)
+    return fail(h, 2, "field %d has no device getter (HB_Z_CORR, HB_Z_ORIG, HB_R)", field);
+  if (dtype != HB_FLOAT32 && dtype != HB_FLOAT64) return fail(h, 2, "unknown dtype %d", dtype);
+  const int cols = field == HB_R ? h->K : h->d;
+  if (ld < cols) return fail(h, 2, "row stride %lld is smaller than the field's %d columns", (long long)ld, cols);
+  TRY(check_device_ptr(h, out, "output"));
+  CK(cudaSetDevice(h->device));
+  const cudaStream_t caller = (cudaStream_t)stream;
+  TRY(stream_after(h, h->stream, caller));  // the caller's earlier work on `out` comes first
+  if (field == HB_Z_CORR) TRY(normalise_pending_zc(h));
+  {
+    RegionScope rs(h, "download");
+    const float* src = field == HB_Z_CORR ? h->Zc.p : field == HB_Z_ORIG ? h->Zo.p : h->R.p;
+    const int src_ld = field == HB_R ? h->KS : h->DS;
+    if (dtype == HB_FLOAT32)
+      copy_rows(src, src_ld, (float*)out, ld, h->inv_sort.p, 0, false, h->n, cols, h->num_sms, h->stream);
+    else
+      copy_rows(src, src_ld, (double*)out, ld, h->inv_sort.p, 0, false, h->n, cols, h->num_sms, h->stream);
+    CKL();
+  }
+  return stream_after(h, caller, h->stream);
 }
 
 int hb_set_field(hb_handle* h, int field, const double* in) {
@@ -2311,6 +2420,7 @@ int hb_get_scalar(const hb_handle* h, int which, double* out) {
     case HB_WINDOW_SIZE: *out = h->window_size; return 0;
     case HB_LEGACY_CENTROID_STEP: *out = h->legacy_centroid ? 1 : 0; return 0;
     case HB_KERNEL_SET: *out = h->kernel_set; return 0;
+    case HB_DEVICE: *out = h->device; return 0;
   }
   return 2;
 }

@@ -21,29 +21,7 @@ constexpr int NWARP = ROW_THREADS / 32;
 // ------------------------------------------------------------------------------------------------
 // setup helpers
 // ------------------------------------------------------------------------------------------------
-// dst[dst_row[r0 + r]][c] = (float)src[r][c]   (double -> float conversion of harmony.cpp:41 fused
-// with the scatter into tuple-sorted order)
-__global__ void k_upload_rows(const double* __restrict__ src, float* __restrict__ dst,
-                              const int* __restrict__ dst_row, int64_t r0, int64_t rows, int cols, int ld) {
-  int64_t total = rows * cols;
-  for (int64_t idx = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; idx < total;
-       idx += (int64_t)gridDim.x * blockDim.x) {
-    int64_t r = idx / cols;
-    int c = (int)(idx - r * cols);
-    dst[(int64_t)dst_row[r0 + r] * ld + c] = (float)src[idx];
-  }
-}
-// out[r][c] = (double) src[src_row[r0 + r]][c]   (conv_to<RMAT>::from of harmony.cpp:640-650 + un-sort)
-__global__ void k_download_rows(const float* __restrict__ src, double* __restrict__ out,
-                                const int* __restrict__ src_row, int64_t r0, int64_t rows, int cols, int ld) {
-  int64_t total = rows * cols;
-  for (int64_t idx = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; idx < total;
-       idx += (int64_t)gridDim.x * blockDim.x) {
-    int64_t r = idx / cols;
-    int c = (int)(idx - r * cols);
-    out[idx] = (double)src[(int64_t)src_row[r0 + r] * ld + c];
-  }
-}
+// The per-cell row uploads and downloads are k_copy_rows (io.cuh).
 // Legacy centroid step (harmony.cpp:235-238, commented out in 2.0.4): Y_k = normalise(sum_i R_ik z_i) from the
 // per-tuple sums S[q][k][0..d) of the statistics kernels run on Z_corr.  One block per cluster.
 __global__ void k_centroids_from_stats(const float* __restrict__ S, float* __restrict__ Y, int J, int K, int d) {
@@ -60,17 +38,6 @@ __global__ void k_centroids_from_stats(const float* __restrict__ S, float* __res
   float nrm = sqrtf(ss);
   if (nrm == 0.f) nrm = 1.f;
   for (int c = threadIdx.x; c < d; c += blockDim.x) Y[(size_t)k * d + c] = ysum[c] / nrm;
-}
-// float variant for the threaded download path (the host workers widen to double while they scatter)
-__global__ void k_download_rows_f(const float* __restrict__ src, float* __restrict__ out, const int* __restrict__ src_row,
-                                  int64_t r0, int64_t rows, int cols, int ld) {
-  int64_t total = rows * cols;
-  for (int64_t idx = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; idx < total;
-       idx += (int64_t)gridDim.x * blockDim.x) {
-    int64_t r = idx / cols;
-    int c = (int)(idx - r * cols);
-    out[idx] = src[(int64_t)src_row[r0 + r] * ld + c];
-  }
 }
 __global__ void k_fill_f(float* __restrict__ out, int64_t n, float v) {
   for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) out[i] = v;

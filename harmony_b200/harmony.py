@@ -13,19 +13,24 @@ import warnings
 import numpy as np
 
 from . import _lib
+from .utils import is_cuda_tensor
 
 FIELD = {"Z_corr": 0, "Z_orig": 1, "R": 2, "Y": 3, "O": 4, "E": 5, "W": 6, "Pr_b": 7, "theta": 8, "sigma": 9,
          "lambda_mat": 10, "lambda": 11}
 SCALAR = {"N": 0, "B": 1, "K": 2, "d": 3, "C": 4, "alpha": 5, "max_iter_kmeans": 6, "block_size": 7,
           "epsilon_kmeans": 8, "epsilon_harmony": 9, "N_local": 10, "lambda_estimation": 11, "window_size": 12,
-          "legacy_centroid_step": 13, "kernel_set": 14}
+          "legacy_centroid_step": 13, "kernel_set": 14, "device": 15}
 TRACE = {"objective_kmeans": 0, "objective_kmeans_dist": 1, "objective_kmeans_entropy": 2,
          "objective_kmeans_cross": 3, "objective_harmony": 4, "kmeans_rounds": 5}
-_INT_SCALARS = ("N", "B", "K", "d", "C", "max_iter_kmeans", "N_local", "window_size", "legacy_centroid_step", "kernel_set")
+_INT_SCALARS = ("N", "B", "K", "d", "C", "max_iter_kmeans", "N_local", "window_size", "legacy_centroid_step", "kernel_set",
+                "device")
 
 
 def _ptr(a):
     return a.ctypes.data_as(ctypes.c_void_p)
+
+
+_DTYPE = {"float32": 0, "float64": 1}   # enum hb_dtype
 
 
 class HarmonyError(RuntimeError):
@@ -89,8 +94,13 @@ class harmony:
               block_size, B_vec, batch_proportion_cutoff, verbose=False):
         """harmony::setup (harmony.h:25-30).  ``Z``: [N, d] C-order (== the d x N column-major matrix
         of the reference) or [d, N] F-order; ``Phi``: the row-index slot of the B x N design matrix,
-        int array [N, C]; ``lambda_``: B+1 values or None / -1 for automatic estimation."""
-        Z = np.asarray(Z)
+        int array [N, C]; ``lambda_``: B+1 values or None / -1 for automatic estimation.
+
+        ``Z`` may also be a float32 / float64 CUDA tensor on the object's device, in either orientation: it is read
+        where it lies (no host round trip), after the work queued on the device's current torch stream."""
+        dev = is_cuda_tensor(Z)
+        if not dev:
+            Z = np.asarray(Z)
         phi_i = np.ascontiguousarray(Phi, dtype=np.int32)
         if phi_i.ndim == 1:
             phi_i = phi_i.reshape(-1, 1)
@@ -99,9 +109,12 @@ class harmony:
             raise ValueError("Z must be a matrix")
         if Z.shape[0] != n and Z.shape[1] == n:
             Z = Z.T                                   # d x N given: its transpose view is the same memory order
-        Z = np.ascontiguousarray(Z, dtype=np.float64)
         if Z.shape[0] != n:
             raise ValueError("number of cells in Z and Phi differ")
+        if dev:
+            Z, z_args = self._device_Z(Z)             # Z: the tensor read, alive until the call returns
+        else:
+            Z = np.ascontiguousarray(Z, dtype=np.float64)
         B_vec = np.ascontiguousarray(np.atleast_1d(B_vec), dtype=np.int32)
         K = int(K)
         sigma = np.ascontiguousarray(np.broadcast_to(np.asarray(sigma, dtype=np.float64), (K,)))
@@ -115,10 +128,27 @@ class harmony:
                 lam = None
             elif len(lam) != int(B_vec.sum()) + 1:
                 raise ValueError("lambda must hold B+1 values")
-        self._check(self._L.hb_setup(self._h, _ptr(Z), Z.shape[1], n, _ptr(phi_i), _ptr(B_vec), len(B_vec),
-                                     _ptr(sigma), _ptr(theta), None if lam is None else _ptr(lam), float(alpha),
-                                     int(max_iter_kmeans), float(epsilon_kmeans), float(epsilon_harmony), K,
-                                     float(block_size), float(batch_proportion_cutoff), int(bool(verbose))))
+        rest = (Z.shape[1], n, _ptr(phi_i), _ptr(B_vec), len(B_vec), _ptr(sigma), _ptr(theta),
+                None if lam is None else _ptr(lam), float(alpha), int(max_iter_kmeans), float(epsilon_kmeans),
+                float(epsilon_harmony), K, float(block_size), float(batch_proportion_cutoff), int(bool(verbose)))
+        if dev:
+            self._check(self._L.hb_setup_device(self._h, *z_args, *rest))
+        else:
+            self._check(self._L.hb_setup(self._h, _ptr(Z), *rest))
+
+    def _device_Z(self, Z):
+        """An [N, d] CUDA tensor -> (the tensor to read, (pointer, dtype, row stride, stream) of hb_setup_device)).
+        Rows with unit column stride are read in place; any other layout is made contiguous on the device first."""
+        import torch
+        if Z.dtype not in (torch.float32, torch.float64):
+            raise TypeError(f"Z must be float32 or float64, not {Z.dtype}")
+        if Z.device.index != self._scalar("device"):
+            raise ValueError(f"Z is on {Z.device}, the harmony object on cuda:{self._scalar('device')}")
+        if Z.shape[0] > 1 and not (Z.stride(1) == 1 and Z.stride(0) >= Z.shape[1]):
+            Z = Z.contiguous()
+        ld = Z.stride(0) if Z.shape[0] > 1 else Z.shape[1]
+        stream = torch.cuda.current_stream(Z.device).cuda_stream
+        return Z, (ctypes.c_void_p(Z.data_ptr()), _DTYPE[str(Z.dtype)[6:]], int(ld), ctypes.c_void_p(stream))
 
     def set_seed(self, seed):
         self._check(self._L.hb_set_seed(self._h, int(seed) & 0xFFFFFFFFFFFFFFFF))
@@ -195,6 +225,25 @@ class harmony:
 
     def getLambda(self):
         return self._field("lambda_mat", (self._scalar("K"), self._scalar("B") + 1))
+
+    def get_tensor(self, name, dtype=None):
+        """``name`` ("Z_corr", "Z_orig" or "R") as a new [N_local, cols] CUDA tensor on the object's device: the bytes
+        of the [cols, N_local] array getZcorr() / getZorig() / getR() return, without leaving the device.
+        ``dtype``: torch.float32 (default) or torch.float64.  The copy is ordered on the device's current torch stream
+        (work queued there afterwards sees it); the host is not blocked."""
+        import torch
+        dtype = torch.float32 if dtype is None else dtype
+        if name not in ("Z_corr", "Z_orig", "R"):
+            raise ValueError(f"get_tensor: no per-cell field {name!r} (Z_corr, Z_orig, R)")
+        if dtype not in (torch.float32, torch.float64):
+            raise TypeError(f"get_tensor: dtype must be torch.float32 or torch.float64, not {dtype}")
+        cols = self._scalar("K" if name == "R" else "d")
+        device = torch.device("cuda", self._scalar("device"))
+        out = torch.empty((self._scalar("N_local"), cols), dtype=dtype, device=device)
+        stream = torch.cuda.current_stream(device).cuda_stream
+        self._check(self._L.hb_get_field_device(self._h, FIELD[name], ctypes.c_void_p(out.data_ptr()),
+                                                _DTYPE[str(dtype)[6:]], cols, ctypes.c_void_p(stream)))
+        return out
 
     # ---- fields of the Rcpp module (harmony.cpp:675-696) ---------------------------------------
     def __getattr__(self, name):

@@ -10,7 +10,7 @@ import sys
 import numpy as np
 
 from .harmony_option import HarmonyOptions, check_legacy_args, harmony_options
-from .utils import harmonize
+from .utils import harmonize, is_cuda_tensor
 
 
 def _as_columns(meta_data, n_hint):
@@ -38,7 +38,9 @@ def prepare_inputs(data_mat, meta_data, vars_use=None, theta=None, sigma=0.1, la
     if not isinstance(options, HarmonyOptions):
         raise TypeError("Error: .options must be created from harmony_options()!")
     epsilon_harmony = options.epsilon_harmony if early_stop else -math.inf
-    data_mat = np.asarray(data_mat)
+    on_device = is_cuda_tensor(data_mat)   # stays where it is: setup reads it on its device
+    if not on_device:
+        data_mat = np.asarray(data_mat)
     if data_mat.ndim != 2:
         raise ValueError("data_mat must be a matrix")
     cols, forced = _as_columns(meta_data, data_mat.shape)
@@ -102,7 +104,9 @@ def prepare_inputs(data_mat, meta_data, vars_use=None, theta=None, sigma=0.1, la
     tau = options.tau
     with np.errstate(divide="ignore", invalid="ignore"):              # tau = 0 -> N_b/0 = Inf -> factor 1
         theta_vec = theta_vec * (1 - np.exp(-(N_b / (nclust * tau)) ** 2)) if tau != 0 else theta_vec * 1.0
-    return dict(Z=np.ascontiguousarray(Z, dtype=np.float64), phi_i=phi_i, B_vec=np.asarray(B_vec, dtype=np.int32),
+    if not on_device:
+        Z = np.ascontiguousarray(Z, dtype=np.float64)
+    return dict(Z=Z, phi_i=phi_i, B_vec=np.asarray(B_vec, dtype=np.int32),
                 sigma=sigma, theta=theta_vec, lambda_=lambda_vec, alpha=float(options.alpha),
                 max_iter_kmeans=int(options.max_iter_cluster), epsilon_kmeans=float(options.epsilon_cluster),
                 epsilon_harmony=float(epsilon_harmony), K=int(nclust), block_size=float(options.block_size),
@@ -119,6 +123,9 @@ def RunHarmony(data_mat, meta_data, vars_use=None, theta=None, sigma=0.1, lambda
     ``set.seed`` for the k-means initialisation and the per-round update orders.  Returns the
     corrected embedding [N, d] (same orientation rule as the reference: the transpose of what
     ``getZcorr()`` holds) or the ``harmony`` object when ``return_object`` is true.
+
+    ``data_mat`` may be a float32 / float64 CUDA tensor (either orientation): the object is created on its device
+    and the result is a [N, d] tensor of the same dtype on that device; the embedding never visits the host.
     """
     from .harmony import harmony  # needs the CUDA extension; fails loudly when it is missing
 
@@ -126,6 +133,10 @@ def RunHarmony(data_mat, meta_data, vars_use=None, theta=None, sigma=0.1, lambda
     a = prepare_inputs(data_mat, meta_data, vars_use, theta, sigma, lambda_, nclust, early_stop, options, verbose)
     if verbose and a["lambda_"] is None:
         print("Using automatic lambda estimation", file=sys.stderr)
+    if is_cuda_tensor(data_mat):
+        if device is not None and int(device) != data_mat.device.index:
+            raise ValueError(f"device={device} differs from the device of data_mat ({data_mat.device})")
+        device = data_mat.device.index
     obj = harmony(device=device)
     obj.setup(a["Z"], a["phi_i"], a["sigma"], a["theta"], a["lambda_"], a["alpha"], a["max_iter_kmeans"],
               a["epsilon_kmeans"], a["epsilon_harmony"], a["K"], a["block_size"], a["B_vec"],
@@ -142,4 +153,6 @@ def RunHarmony(data_mat, meta_data, vars_use=None, theta=None, sigma=0.1, lambda
         HarmonyConvergencePlot(obj)
     if return_object:
         return obj
+    if is_cuda_tensor(data_mat):
+        return obj.get_tensor("Z_corr", dtype=data_mat.dtype)
     return np.ascontiguousarray(obj.getZcorr().T)   # t(harmonyObj$getZcorr()), R/ui.R:292-295: cells x PCs

@@ -4,6 +4,12 @@ import sys
 import numpy as np
 
 
+def is_cuda_tensor(x):
+    """True for a torch tensor on a CUDA device.  Never imports torch: a tensor exists only if torch is loaded."""
+    torch = sys.modules.get("torch")
+    return torch is not None and isinstance(x, torch.Tensor) and x.is_cuda
+
+
 def harmonize(harmonyObj, iter_harmony, verbose=True):
     """R/utils.R:15-46: cluster_cpp -> moe_correct_ridge_cpp -> check_convergence(1)."""
     if iter_harmony < 1:

@@ -16,6 +16,9 @@
  *     phi_i[n*C + c] is the (global, 0-based) row of the c-th non-zero of column n.
  *   - all buffers are caller-owned host memory; inputs are copied during the call
  *     (like harmony::setup, harmony.cpp:41,44), outputs are written into caller-allocated arrays.
+ *     The exceptions are hb_setup_device and hb_get_field_device, which take the per-cell matrices
+ *     in the caller's device memory (fp32 or fp64, any row stride) and order themselves on a
+ *     caller's CUDA stream.
  *   - a handle must be driven from one host thread at a time (the reference is single-threaded).
  */
 #ifndef HARMONY_B200_H
@@ -64,6 +67,19 @@ int hb_setup(hb_handle* h, const double* Z, int d, int64_t N, const int32_t* phi
              double epsilon_kmeans, double epsilon_harmony, int K, double block_size,
              double batch_proportion_cutoff, int verbose);
 
+/* Element types of device-memory matrices (hb_setup_device, hb_get_field_device). */
+enum hb_dtype { HB_FLOAT32 = 0, HB_FLOAT64 = 1 };
+
+/* hb_setup with Z in device memory: N(local) rows of d values of z_dtype, row stride z_ld >= d elements (the bytes of a
+ * d x N column-major matrix when z_ld == d), in device or managed memory of the handle's device.  Every other argument
+ * is hb_setup's, on the host.  Z is read after the work already queued on `stream` (a cudaStream_t; NULL: the legacy
+ * default stream) and the call returns once it has been copied.  Status 2 before any launch for a NULL, host or
+ * other-device Z, an unknown dtype or z_ld < d. */
+int hb_setup_device(hb_handle* h, const void* Z, int z_dtype, int64_t z_ld, void* stream, int d, int64_t N,
+                    const int32_t* phi_i, const int32_t* B_vec, int C, const double* sigma, const double* theta,
+                    const double* lambda, double alpha, int max_iter_kmeans, double epsilon_kmeans,
+                    double epsilon_harmony, int K, double block_size, double batch_proportion_cutoff, int verbose);
+
 /* Seed of the native generators (k-means initialisation, per-round update orders).  The reference
  * draws both from R's RNG (utils.cpp:10-64, harmony.cpp:272-273); the shim may instead inject them. */
 int hb_set_seed(hb_handle* h, uint64_t seed);
@@ -110,13 +126,20 @@ int64_t hb_field_size(const hb_handle* h, int field);
 /* Device -> host copy-out with float -> double conversion (conv_to<RMAT>::from, harmony.cpp:640-650).
  * With a sharded handle the per-cell fields return the local shard. */
 int hb_get_field(hb_handle* h, int field, double* out);
+/* Device-memory hb_get_field for HB_Z_CORR, HB_Z_ORIG and HB_R: writes the N_local rows (cells in the caller's order) of
+ * d or K values of `dtype` with row stride ld >= cols elements into `out`, device or managed memory of the handle's
+ * device.  Does not block the host: the copy runs after the work queued on `stream` so far, and work queued on
+ * `stream` afterwards sees the result.  Status 2 before any launch for a NULL, host or other-device `out`, another
+ * field, an unknown dtype or ld < cols. */
+int hb_get_field_device(hb_handle* h, int field, void* out, int dtype, int64_t ld, void* stream);
 /* Writable fields (the Rcpp module's .field() members are read-write): HB_Y, HB_R, HB_O, HB_E,
  * HB_THETA, HB_SIGMA, HB_LAMBDA_VEC, HB_Z_CORR. */
 int hb_set_field(hb_handle* h, int field, const double* in);
 
 enum hb_scalar { HB_N = 0, HB_B = 1, HB_K = 2, HB_D = 3, HB_C = 4, HB_ALPHA = 5, HB_MAX_ITER_KMEANS = 6,
                  HB_BLOCK_SIZE = 7, HB_EPSILON_KMEANS = 8, HB_EPSILON_HARMONY = 9, HB_N_LOCAL = 10,
-                 HB_LAMBDA_ESTIMATION = 11, HB_WINDOW_SIZE = 12, HB_LEGACY_CENTROID_STEP = 13, HB_KERNEL_SET = 14 };
+                 HB_LAMBDA_ESTIMATION = 11, HB_WINDOW_SIZE = 12, HB_LEGACY_CENTROID_STEP = 13, HB_KERNEL_SET = 14,
+                 HB_DEVICE = 15 /* CUDA device of the handle (read-only) */ };
 /* HB_KERNEL_SET (test hook, default 0, read by the next hb_setup): the library picks its kernels from the problem's
  * shape alone; these bits force the kernels that serve shapes outside the default ones' limits onto ANY shape so that
  * the parity suite can hold them to the same bar (tests/test_gpu_parity.py::test_fallback_kernels_match_oracle). */
@@ -147,7 +170,8 @@ void* hb_stream(const hb_handle* h);
 /* Blocks until all queued work of the handle has finished; returns the sticky CUDA status as 0/>0. */
 int hb_synchronize(hb_handle* h);
 /* Accumulated device time (ms) and launch count of a named region ("assign", "update_R",
- * "ridge_stats", "ridge_solve", "ridge_apply", "plan"); returns 0 if the region exists. */
+ * "ridge_stats", "ridge_solve", "ridge_apply", "plan", and "upload" / "download": the per-cell row transfers of setup,
+ * the getters and hb_set_field, host copies included); returns 0 if the region exists. */
 int hb_region_time(hb_handle* h, const char* region, double* ms, int64_t* launches);
 /* Enables per-region CUDA-event timing (adds synchronisation; off by default). */
 int hb_enable_timing(hb_handle* h, int on);
