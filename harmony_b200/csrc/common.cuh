@@ -18,6 +18,38 @@ __device__ __forceinline__ float warp_sum(float v) {
   return v;
 }
 
+// Row norms in fp32.  The plain sum of squares underflows for rows below |v| ~ 1e-19 (the squares fall under the
+// smallest normal float) and overflows above |v| ~ 1.8e19.  Such sums are rejected by norm_sq_ok, and the row is measured
+// again after dividing by its largest magnitude.  That path is rare and costs nothing on ordinary rows.
+__device__ __forceinline__ bool norm_sq_ok(float ss) { return ss >= 1.17549435e-38f && ss <= 3.40282347e38f; }
+// |x| of n values v(0) .. v(n - 1) held by one thread; 0 for a zero row
+template <typename Get>
+__device__ __forceinline__ float norm_rescaled(int n, Get v) {
+  float m = 0.f;
+  for (int i = 0; i < n; ++i) m = fmaxf(m, fabsf(v(i)));
+  if (m == 0.f || !isfinite(m)) return m;
+  float s = 0.f;
+  for (int i = 0; i < n; ++i) {
+    const float t = v(i) / m;
+    s += t * t;
+  }
+  return m * sqrtf(s);
+}
+// the same for a row x[0 .. d) read by a whole warp (lane l reads x[l], x[l + 32], ..); every lane gets the result
+__device__ __forceinline__ float warp_norm_rescaled(const float* x, int d, int lane) {
+  float m = 0.f;
+  for (int c = lane; c < d; c += 32) m = fmaxf(m, fabsf(x[c]));
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
+  if (m == 0.f || !isfinite(m)) return m;
+  float s = 0.f;
+  for (int c = lane; c < d; c += 32) {
+    const float t = x[c] / m;
+    s += t * t;
+  }
+  return m * sqrtf(warp_sum(s));
+}
+
 // Single-instruction transcendental approximations (MUFU, flush-to-zero): the intrinsics __expf / __logf /
 // __frcp_rn expand to range-handling sequences (extra FSETP / FMUL / branches) that the issue-bound row
 // loops cannot afford.  Relative error ~2^-22.

@@ -53,7 +53,8 @@ __global__ void k_expand(const float* __restrict__ src, float* __restrict__ out,
 }
 
 // arma::normalise(X, 2, 0) on the rows of X[n][d] (= columns of the reference's d x N matrix); a zero
-// norm divides by 1.  One warp per row.  dst may alias src.
+// norm divides by 1; rows too small or too large for a plain fp32 sum of squares are rescaled first.  One warp per
+// row.  dst may alias src.
 __global__ void k_normalise_rows(const float* __restrict__ src, float* __restrict__ dst, int64_t n, int d, int ld) {
   int lane = threadIdx.x & 31;
   int64_t w = (blockIdx.x * (int64_t)blockDim.x + threadIdx.x) >> 5;
@@ -66,7 +67,7 @@ __global__ void k_normalise_rows(const float* __restrict__ src, float* __restric
       s += v * v;
     }
     s = warp_sum(s);
-    float nrm = sqrtf(s);
+    float nrm = norm_sq_ok(s) ? sqrtf(s) : warp_norm_rescaled(x, d, lane);
     if (nrm == 0.f) nrm = 1.f;
     for (int c = lane; c < d; c += 32) dst[r * ld + c] = x[c] / nrm;
   }
@@ -353,7 +354,7 @@ __global__ void __launch_bounds__(ASSIGN_THREADS) k_assign(AssignArgs a) {
             s += v * v;
           }
           s = warp_sum(s);
-          nrm = sqrtf(s);
+          nrm = norm_sq_ok(s) ? sqrtf(s) : warp_norm_rescaled(zrow, d, lane);
           if (nrm == 0.f) nrm = 1.f;
         }
         for (int c = lane; c < DP4; c += 32) {

@@ -111,7 +111,9 @@ __global__ void __launch_bounds__(LG_THREADS, 1) k_logits_tc(LogitsArgs a) {
       }
       float rn = 1.f;
       if (a.normalise) {
-        float nrm = sqrtf(ss);
+        float nrm = (norm_sq_ok(ss) || !live)
+                        ? sqrtf(ss)
+                        : norm_rescaled(4 * DS4, [&](int i) { return Ahi[((size_t)(i >> 2) * LG_TM + r) * 4 + (i & 3)]; });
         if (nrm == 0.f) nrm = 1.f;  // arma::normalise: zero norm divides by 1
         rn = 1.f / nrm;
       }

@@ -664,6 +664,10 @@ template <typename T>
 void copy_out(const std::vector<T>& v, double* out) {
   for (size_t i = 0; i < v.size(); ++i) out[i] = (double)v[i];
 }
+template <typename T>
+void copy_in(std::vector<T>& v, const double* in) {
+  for (size_t i = 0; i < v.size(); ++i) v[i] = (T)in[i];
+}
 
 }  // namespace
 
@@ -793,6 +797,27 @@ int ho_get(void* hv, int field, double* out) {
     GET(h->f)
   }
 #undef GET
+  return 0;
+}
+
+// writable fields (same ids and layouts as ho_get): 2 R, 3 Y, 4 O, 5 E.  Lets a test plant the state a step starts
+// from, like the `.field<-` writes of the reference's Rcpp module.
+int ho_set(void* hv, int field, const double* in) {
+  Handle* h = (Handle*)hv;
+#define SET(obj)                                \
+  switch (field) {                              \
+    case 2: copy_in(obj->R, in); break;         \
+    case 3: copy_in(obj->Y, in); break;         \
+    case 4: copy_in(obj->O, in); break;         \
+    case 5: copy_in(obj->E, in); break;         \
+    default: return 1;                          \
+  }
+  if (h->use_double) {
+    SET(h->dd)
+  } else {
+    SET(h->f)
+  }
+#undef SET
   return 0;
 }
 

@@ -53,6 +53,7 @@ def lib():
         L.ho_set_max_iter_kmeans.argtypes = [P, ctypes.c_int]
         L.ho_set_legacy_centroid_step.argtypes = [P, ctypes.c_int]
         L.ho_get.argtypes = [P, ctypes.c_int, P]
+        L.ho_set.argtypes = [P, ctypes.c_int, P]
         L.ho_trace.restype = ctypes.c_int64
         L.ho_trace.argtypes = [P, ctypes.c_int, P, ctypes.c_int64]
         _LIB = L
@@ -164,6 +165,13 @@ class OracleHarmony:
         st = self.L.ho_get(self.h, FIELDS[name], _ptr(out))
         assert st == 0
         return out
+
+    def set(self, name, value):
+        """Write R [N, K], Y [K, d], O or E [B, K] (the layouts get() returns)."""
+        shapes = {"R": (self.N, self.K), "Y": (self.K, self.d), "O": (self.B, self.K), "E": (self.B, self.K)}
+        v = np.ascontiguousarray(value, dtype=np.float64)
+        assert v.shape == shapes[name], (name, v.shape)
+        self._check(self.L.ho_set(self.h, FIELDS[name], _ptr(v)))
 
     def trace(self, name):
         n = self.L.ho_trace(self.h, TRACES[name], None, 0)

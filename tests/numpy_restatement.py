@@ -21,7 +21,7 @@ def my_ceil(x):
 
 
 class NumpyHarmony:
-    def __init__(self, Z, phi_i, B_vec, sigma, theta, lambda_, alpha, T, K, block_size, cutoff):
+    def __init__(self, Z, phi_i, B_vec, sigma, theta, lambda_, alpha, T, K, block_size, cutoff, epsilon_kmeans=1e-3):
         self.Z_orig = np.asarray(Z, dtype=np.float64)
         self.N, self.d = self.Z_orig.shape
         self.lev = np.asarray(phi_i, dtype=np.int64).reshape(self.N, -1)
@@ -42,7 +42,9 @@ class NumpyHarmony:
         for c in range(self.C):
             self.Phi[self.lev[:, c], np.arange(self.N)] = 1.0
         self.Z_corr = self._l2(self.Z_orig)
+        self.epsilon_kmeans = epsilon_kmeans
         self.obj_kmeans, self.obj_harmony = [], []
+        self.obj_parts = []   # (distance, entropy, cross-entropy) terms of every objective_kmeans entry
 
     @staticmethod
     def _l2(X):
@@ -70,6 +72,7 @@ class NumpyHarmony:
         L = self.theta[None, :] * np.log((self.O + self.E + 1) / (2 * self.E + 1))    # [K, B]
         cross = ((R * self.sigma[None, :]) * (self.Phi.T @ L.T)).sum()
         self.obj_kmeans.append((kerr + ent + cross) * 2000.0 / self.N)
+        self.obj_parts.append((kerr * 2000.0 / self.N, ent * 2000.0 / self.N, cross * 2000.0 / self.N))
 
     def update_R(self, order):
         N = self.N
@@ -95,7 +98,7 @@ class NumpyHarmony:
             self.O += Rn.T @ Pb.T
 
     legacy_centroid_step = False   # STEP 1 of harmony.cpp:235-238, commented out in 2.0.4
-    window_size, epsilon_kmeans = 3, 1e-3
+    window_size = 3
 
     def cluster(self, perms):
         if len(self.obj_harmony) != 1:
@@ -115,10 +118,18 @@ class NumpyHarmony:
         self.obj_harmony.append(self.obj_kmeans[-1])
 
     def moe_correct_ridge(self):
-        """Batched: sufficient statistics per (cluster, level), then tiny solves, then one apply."""
+        """Batched: sufficient statistics per (cluster, level), then tiny solves, then one apply.  Also records
+        ``lambda_mat`` (K x (B+1), getLambda of harmony.cpp:657-669) and ``W`` ((B+1) x d: the betas of the last
+        corrected cluster, row 0 and the rows of dropped levels zero)."""
         K, B, d, N = self.K, self.B, self.d, self.N
         Zc = self.Z_orig.copy()
         Ynew = self.Y.copy()
+        self.lambda_mat = np.zeros((K, B + 1))
+        if self.lam is None:
+            self.lambda_mat[:, 1:] = self.alpha * self.E
+        else:
+            self.lambda_mat[:] = self.lam[None, :]
+        self.W = np.zeros((B + 1, d))
         avg = self.O / self.N_b[None, :]                                                 # [K, B]
         over = avg > np.float32(self.cutoff)
         for k in range(K):
@@ -136,6 +147,8 @@ class NumpyHarmony:
             Wk = np.linalg.solve(cov, (Phis * Rk[None, :]) @ self.Z_orig[part])           # [B'+1, d]
             Ynew[k] = Wk[0]
             Wk[0] = 0
+            self.W = np.zeros((B + 1, d))
+            self.W[keep + 1] = Wk[1:]
             Zc[part] -= (Phis * Rk[None, :]).T @ Wk
         self.Z_corr = Zc
         self.Y = self._l2(Ynew)
