@@ -48,8 +48,11 @@ struct ApplyTcArgs {
   int k_off, Kp, KD;  // this launch: clusters [k_off, k_off + Kp) (k_off a multiple of 8), KD = Kp rounded up to 8
   const float* minuend;  // Zo for the first cluster range, Zc (the partial result) for the following ones
   int tiles_per_cta;
+  int c_off, DC;  // k_apply_tc_cols: embedding columns [c_off, c_off + DC) (multiples of 4; the last range ends at DS)
 };
 
+// k_apply_tc takes all of d in one launch up to d = 128 (NH = 2)
+inline bool apply_tc_fits(int d) { return d <= 128; }
 __host__ __device__ inline int apply_tc_nb(int d) { return d <= 64 ? 64 : 128; }
 // floats of R per row of a raw stage: the launch's cluster range (the rest of the row when it is the last range)
 __host__ __device__ inline int apply_tc_rs(int KD, int KS, int k_off) { return KS - k_off < KD ? KS - k_off : KD; }
@@ -70,15 +73,32 @@ __host__ __device__ inline size_t apply_tc_smem_bytes(int RS, int d, int DS) {
   return apply_tc_fixed_bytes(d) + apply_tc_stages(RS, d, DS) * apply_tc_stage_bytes(RS, DS);
 }
 
+// Column ranges (d > 256, or K x d beyond the FFMA apply): one launch per <= 128 embedding columns [c_off, c_off + DC)
+// and cluster range, B = 128 columns of V_q^T.  A stage's minuend rows are the range's DC floats of each row (row-by-row
+// bulk copies in and out, as the R rows of a narrow cluster range); the first cluster range of each column range
+// subtracts from Zo.  Bytes per cell over the whole grid: 4 KS per column range (R) + 8 DS per cluster range (minuend
+// in, Zc out).
+__host__ __device__ inline size_t apply_cols_fixed_bytes() { return sizeof(float) * 2 * (size_t)128 * AP_MAXK + AP_MAXST * sizeof(uint64_t); }
+__host__ __device__ inline int apply_cols_stages(int RS, int DC) {
+  const size_t fixed = apply_cols_fixed_bytes(), st = apply_tc_stage_bytes(RS, DC);
+  const int n = fixed < SMEM_LIMIT ? (int)((SMEM_LIMIT - fixed) / st) : 0;
+  return (n < AP_MAXST ? n : AP_MAXST) & ~1;  // even: see apply_tc_stages
+}
+__host__ __device__ inline size_t apply_cols_smem_bytes(int RS, int DC) {
+  return apply_cols_fixed_bytes() + apply_cols_stages(RS, DC) * apply_tc_stage_bytes(RS, DC);
+}
+
 // NH: 64-column halves of B = embedding columns (1: d <= 64, 2: d <= 128), fixed at compile time so that the
-// accumulators stay in registers
-template <int NH>
-__global__ void __launch_bounds__(AP_THREADS, 1) k_apply_tc(ApplyTcArgs a) {
+// accumulators stay in registers.  CR: one column range of the embedding per launch (NH = 2).
+template <int NH, bool CR>
+__device__ __forceinline__ void apply_tc_body(const ApplyTcArgs& a) {
   extern __shared__ __align__(128) unsigned char smem_raw[];
   constexpr int NB = 64 * NH;
-  const int KD = a.KD, K = a.K, d = a.d, KS = a.KS, DS = a.DS, Kp = a.Kp;
+  const int KD = a.KD, K = a.K, KS = a.KS, Kp = a.Kp;
+  const int d = CR ? (a.d - a.c_off < a.DC ? a.d - a.c_off : a.DC) : a.d;  // columns of this launch
+  const int DS = CR ? a.DC : a.DS;                                          // floats of a minuend row in a stage
   const int RS = apply_tc_rs(KD, KS, a.k_off);
-  const int NST = apply_tc_stages(RS, d, DS);
+  const int NST = CR ? apply_cols_stages(RS, DS) : apply_tc_stages(RS, d, DS);
   const int SST = AP_TN * (RS + DS);                 // floats per raw stage: R rows [64][RS], then minuend rows [64][DS]
   float* Bhi = reinterpret_cast<float*>(smem_raw);   // [AP_MAXK/4][NB][4]  V_q^T
   float* Blo = Bhi + (size_t)NB * AP_MAXK;
@@ -97,13 +117,18 @@ __global__ void __launch_bounds__(AP_THREADS, 1) k_apply_tc(ApplyTcArgs a) {
     float* rZ = rR + AP_TN * RS;
     if (lane == 0) {
       umma::mbar_arrive_expect_tx(full + s, (uint32_t)(sizeof(float) * len * (RS + DS)));
-      umma::bulk_g2s(rZ, a.minuend + (size_t)cell0 * DS, (uint32_t)(sizeof(float) * len * DS), full + s);
+      if constexpr (!CR) umma::bulk_g2s(rZ, a.minuend + (size_t)cell0 * DS, (uint32_t)(sizeof(float) * len * DS), full + s);
       if (RS == KS) umma::bulk_g2s(rR, a.R + (size_t)cell0 * KS, (uint32_t)(sizeof(float) * len * KS), full + s);
     }
     if (RS != KS) {  // a cluster range narrower than the row: row by row
       __syncwarp();  // the expected bytes are registered before any row completes
       for (int j = lane; j < len; j += 32)
         umma::bulk_g2s(rR + (size_t)j * RS, a.R + (size_t)(cell0 + j) * KS + a.k_off, (uint32_t)(sizeof(float) * RS), full + s);
+    }
+    if constexpr (CR) {  // the column range of each minuend row
+      __syncwarp();
+      for (int j = lane; j < len; j += 32)
+        umma::bulk_g2s(rZ + (size_t)j * DS, a.minuend + (size_t)(cell0 + j) * a.DS + a.c_off, (uint32_t)(sizeof(float) * DS), full + s);
     }
   };
 
@@ -127,10 +152,10 @@ __global__ void __launch_bounds__(AP_THREADS, 1) k_apply_tc(ApplyTcArgs a) {
     if (q != cur_q) {
       // new tuple: B = V_q^T (k contiguous per embedding column c), tf32 hi/lo — after both warpgroups' MMAs
       umma::named_sync(1, 256);
-      const float* Vq = a.V + ((size_t)q * K + a.k_off) * d;
+      const float* Vq = a.V + ((size_t)q * K + a.k_off) * a.d + (CR ? a.c_off : 0);
       for (int idx = tid; idx < NB * AP_MAXK; idx += 256) {
         const int k = idx / NB, c = idx - k * NB;
-        const float v = (k < Kp && c < d) ? Vq[(size_t)k * d + c] : 0.f;
+        const float v = (k < Kp && c < d) ? Vq[(size_t)k * a.d + c] : 0.f;
         float hi, lo;
         umma::split_tf32(v, hi, lo);
         const int off = ((k >> 2) * NB + c) * 4 + (k & 3);
@@ -195,7 +220,11 @@ __global__ void __launch_bounds__(AP_THREADS, 1) k_apply_tc(ApplyTcArgs a) {
     umma::fence_proxy_async();  // the rows written above -> the bulk store
     umma::named_sync(2 + e, 128);
     if (w == 0) {
-      if (lane == 0) {
+      if constexpr (CR) {
+        for (int j = lane; j < len; j += 32)
+          umma::bulk_s2g(a.Zc + (size_t)(cell0 + j) * a.DS + a.c_off, rZ + (size_t)j * DS, (uint32_t)(sizeof(float) * DS));
+        umma::bulk_wait_read0();
+      } else if (lane == 0) {
         umma::bulk_s2g(a.Zc + (size_t)cell0 * DS, rZ, (uint32_t)(sizeof(float) * len * DS));
         umma::bulk_wait_read0();
       }
@@ -203,7 +232,13 @@ __global__ void __launch_bounds__(AP_THREADS, 1) k_apply_tc(ApplyTcArgs a) {
       if (tile + NST < t_end) load(it + NST);  // the stage is free: refill it
     }
   }
-  if (wt == 0) umma::bulk_wait0();
+  if (CR ? w == 0 : wt == 0) umma::bulk_wait0();
 }
+
+template <int NH>
+__global__ void __launch_bounds__(AP_THREADS, 1) k_apply_tc(ApplyTcArgs a) {
+  apply_tc_body<NH, false>(a);
+}
+__global__ void __launch_bounds__(AP_THREADS, 1) k_apply_tc_cols(ApplyTcArgs a) { apply_tc_body<2, true>(a); }
 
 }  // namespace hb

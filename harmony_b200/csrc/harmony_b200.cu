@@ -34,6 +34,7 @@
 #include "update_single_pass.cuh"
 #include "assign_tc3.cuh"
 #include "logits_tc.cuh"
+#include "logits_wide.cuh"
 #include "apply_tc3.cuh"
 #include "stats_tc3.cuh"
 
@@ -221,10 +222,21 @@ struct Contractions {
   bool kmeans = false;  // native k-means initialisation from logits with sigma = 1 (logits_tc.cuh)
 };
 
+// Kernels of the shapes past the FFMA kernels' limits (or of every shape under HB_KS_WIDE); each is taken only where
+// the kernel that serves the stage otherwise does not fit (assign_ffma_fits, apply_ffma_fits, kmeans_ffma_fits).
+struct WidePaths {
+  bool assign = false;  // natural-order assignment: logits + k_softmax_tiles instead of FFMA k_assign
+  bool cold = false;    // plan-order cold start from logits + k_softmax_block_sums where k_logits_tc does not fit
+  bool logits = false;  // the logits of these paths come from k_logits_wide (d-chunked) instead of k_logits_tc
+  bool apply = false;   // ridge apply over column ranges (k_apply_tc_cols) instead of FFMA k_ridge_apply
+  bool kmeans = false;  // native k-means initialisation from logits with up to 8 pieces per lane instead of FFMA
+};
+
 struct KernelPaths {
   UpdatePath update = UpdatePath::PerStep;
   bool tuple_ranges = false;  // 2 J <= #SMs: the plan gives every CTA a slice of a block inside one tuple
   Contractions mm;
+  WidePaths wide;
 };
 
 int two_pass_nv(int KS) {
@@ -251,14 +263,20 @@ KernelPaths select_kernels(int K, int d, int J, int64_t n, int nb, int num_sms, 
     p.update = UpdatePath::SinglePass;
   else if (KS <= 256 && J <= 8192 && two_pass_smem_bytes(KS, nb, J) <= SMEM_LIMIT)
     p.update = UpdatePath::TwoPass;
-  if (!(kernel_set & HB_KS_FFMA_CONTRACTIONS)) {
+  if (!(kernel_set & (HB_KS_FFMA_CONTRACTIONS | HB_KS_WIDE))) {
     const int ns = assign3_smem_bytes(2, KD, NP, KS) <= SMEM_LIMIT ? 2 : 1;
     if (d <= 64 && K <= 128 && assign3_smem_bytes(ns, KD, NP, KS) <= SMEM_LIMIT) p.mm.k1_stages = ns;
-    const bool logits_fit = d <= 128 && logits_smem_bytes(KD) <= SMEM_LIMIT;
+    const bool logits_fit = logits_tc_fits(d);
     p.mm.logits = p.mm.k1_stages == 0 && logits_fit;
-    p.mm.apply = d <= 128;  // cluster ranges of <= AP_MAXK per launch
+    p.mm.apply = apply_tc_fits(d);  // cluster ranges of <= AP_MAXK per launch
     p.mm.kmeans = logits_fit && KS <= 256;
   }
+  const bool wide = kernel_set & HB_KS_WIDE;
+  p.wide.logits = wide || !logits_tc_fits(d);
+  p.wide.assign = p.mm.k1_stages == 0 && (wide || !assign_ffma_fits(K, d));
+  p.wide.cold = p.wide.assign && !p.mm.logits;
+  p.wide.apply = !p.mm.apply && (wide || !apply_ffma_fits(K, d));
+  p.wide.kmeans = !p.mm.kmeans && (wide || !kmeans_ffma_fits(K, d));
   return p;
 }
 
@@ -273,7 +291,7 @@ struct CallPath {
 CallPath call_path(const KernelPaths& p, unsigned T, bool legacy_centroid) {
   CallPath c{p.update, false};
   if (legacy_centroid || (p.update == UpdatePath::TwoPass && T > 31)) c.update = UpdatePath::PerStep;
-  c.plan_order_assign = c.update == UpdatePath::SinglePass && (p.mm.k1_stages > 0 || p.mm.logits) && T > 0;
+  c.plan_order_assign = c.update == UpdatePath::SinglePass && (p.mm.k1_stages > 0 || p.mm.logits || p.wide.cold) && T > 0;
   return c;
 }
 
@@ -376,6 +394,7 @@ struct hb_handle {
   int kernel_set = 0;            // HB_KERNEL_SET test hook (bits HB_KS_*), read by hb_setup
   bool legacy_centroid = false;  // HB_LEGACY_CENTROID_STEP: centroid update at the top of every clustering round
   DevBuf<float> Rkeep, OEkeep;   // R / O,E saved around the distance-only assignment of that step
+  DevBuf<float> Ypad;            // Y padded for k_logits_wide
   DevBuf<double> objkeep;
   int ring_rows = 0;     // rows of a warp's private ring in the single-pass update kernel
   bool use_xch = false;  // sharded cells: block steps exchanged through peer memory (one cooperative launch per call)
@@ -508,9 +527,39 @@ int dispatch_kq(hb_handle* h, int K, F&& f) {
   return fail(h, 2, "K = %d is not supported (K <= 1024)", K);
 }
 
+// U[i][k] = (2 / sigma_k) (z_i . y_k / |z_i| - 1) for all clusters on the tensor cores, 128 clusters per launch and d
+// in chunks (logits_wide.cuh), after one pass that pads Y
+int launch_logits_wide(hb_handle* h, const float* sigma, bool normalise) {
+  const int KDc = (h->d + LW_DC - 1) / LW_DC * LW_DC, rows = (h->K + LW_NP - 1) / LW_NP * LW_NP;
+  if (h->Ypad.n < (size_t)rows * KDc) CK(h->Ypad.alloc((size_t)rows * KDc));
+  k_pad_rows<<<grid_for((int64_t)rows * KDc, 256, h->num_sms * 4), 256, 0, h->stream>>>(h->Y.p, h->Ypad.p, h->K, h->d, rows, KDc);
+  CKL();
+  LogitsWideArgs t{};
+  t.Zc = h->Zc.p;
+  t.Ypad = h->Ypad.p;
+  t.sigma = sigma;
+  t.U = h->U.p;
+  t.n = h->n;
+  t.d = h->d;
+  t.K = h->K;
+  t.DS = h->DS;
+  t.KS = h->KS;
+  t.KDc = KDc;
+  t.normalise = normalise ? 1 : 0;
+  const size_t smem = logits_wide_smem_bytes();
+  CK(cudaFuncSetAttribute(k_logits_wide, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  const int grid = (int)std::max<int64_t>(1, std::min<int64_t>((h->n + LW_TM - 1) / LW_TM, h->num_sms));
+  for (t.n_off = 0; t.n_off < h->K; t.n_off += LW_NP) {
+    k_logits_wide<<<grid, LW_THREADS, smem, h->stream>>>(t);
+    CKL();
+  }
+  return 0;
+}
+
 // U[i][k] = (2 / sigma_k) (z_i . y_k / |z_i| - 1) for all clusters on the tensor cores, 64 clusters per launch
-// (logits_tc.cuh); `sigma`: device array of K values
+// (logits_tc.cuh), or from launch_logits_wide where the paths of the wide shapes use it; `sigma`: device array of K values
 int launch_logits(hb_handle* h, const float* sigma, bool normalise) {
+  if (h->paths.wide.logits) return launch_logits_wide(h, sigma, normalise);
   LogitsArgs t{};
   t.Zc = h->Zc.p;
   t.Y = h->Y.p;
@@ -544,7 +593,7 @@ namespace {
 int run_assign(hb_handle* h, bool normalise, bool plan_mode = false, bool want_obj = true) {
   RegionScope rs(h, "assign");
   const int K = h->K, d = h->d, B = h->B, KS = h->KS;
-  const int KP = (K + 63) & ~63, DP4 = (d + 3) & ~3;
+  const int KP = (K + 63) & ~63;
   CK(cudaMemsetAsync(h->Oacc.p, 0, sizeof(float) * ((size_t)B * KS + KS), h->stream));
   AssignArgs a;
   a.Zc = h->Zc.p;
@@ -643,7 +692,7 @@ int run_assign(hb_handle* h, bool normalise, bool plan_mode = false, bool want_o
     CKL();
     return 0;
   }
-  if (plan_mode && h->paths.mm.logits) {
+  if (plan_mode && (h->paths.mm.logits || h->paths.wide.cold)) {
     // shapes the fused kernel cannot hold (d > 64 or K > 128): logits per 64-cluster range on the tensor cores, then
     // one gather pass over U in the order of round 0 for the softmax + the blocks' removal sums (harmony.cpp:312-313)
     TRY(launch_logits(h, h->sigma.p, normalise));
@@ -666,8 +715,35 @@ int run_assign(hb_handle* h, bool normalise, bool plan_mode = false, bool want_o
     return 0;
   }
   if (plan_mode) return fail(h, 3, "internal: plan-order assignment without the tensor-core kernel");
-  size_t smem = sizeof(float) * ((size_t)DP4 * KP + (size_t)TM * DP4 + (size_t)TM * (KP + 4) + KP + (size_t)NWARP * KP);
-  if (smem > 227 * 1024) return fail(h, 2, "K*d too large for the assignment kernel (needs %zu B shared memory)", smem);
+  if (h->paths.wide.assign) {
+    // shapes whose FFMA k_assign does not fit: logits on the tensor cores, then the softmax over the natural-order tiles
+    TRY(launch_logits(h, h->sigma.p, normalise));
+    const int nv = sp_nv(KS);
+    const size_t smem_sm = sizeof(float) * 8 * 128 * (size_t)nv;
+    const int grid = std::max(1, std::min(h->ntiles, h->num_sms * 8));
+    auto go = [&](auto nvc) {
+      constexpr int NV = decltype(nvc)::value;
+      k_softmax_tiles<NV><<<grid, 256, smem_sm, h->stream>>>(h->U.p, h->R.p, h->sigma.p, h->tile_cell0.p, h->tile_len.p,
+                                                             h->tile_tuple.p, h->tuple_levels.p, a.O_acc, a.rs_acc,
+                                                             h->obj_acc.p, h->ntiles, K, KS, h->C, want_obj ? 1 : 0);
+    };
+    if (nv == 1) go(std::integral_constant<int, 1>());
+    else if (nv == 2) go(std::integral_constant<int, 2>());
+    else if (nv == 4) go(std::integral_constant<int, 4>());
+    else go(std::integral_constant<int, 8>());
+    CKL();
+    if (normalise) {  // the cold start leaves the normalised embedding in Z_corr (harmony.cpp:220)
+      k_normalise_rows<<<grid_for((int64_t)h->n * 32, 256, h->num_sms * 8), 256, 0, h->stream>>>(h->Zc.p, h->Zc.p, h->n, d, h->DS);
+      CKL();
+    }
+    h->R_user_set = false;
+    TRY(allreduce_f(h, h->Oacc.p, (size_t)B * KS + KS));
+    k_assign_finalize<<<(B * KS + 255) / 256, 256, 0, h->stream>>>(h->Oacc.p, h->Oacc.p + (size_t)B * KS, h->Pr_b.p,
+                                                                    h->O.p, h->E.p, B, K, KS);
+    CKL();
+    return 0;
+  }
+  const size_t smem = assign_ffma_smem_bytes(K, d);
   int st = dispatch_kq(h, K, [&](auto kq) -> int {
     constexpr int KQ = decltype(kq)::value;
     CK(cudaFuncSetAttribute(k_assign<KQ>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
@@ -1305,6 +1381,44 @@ int run_correct(hb_handle* h) {
     }
     return 0;
   }
+  if (h->paths.wide.apply) {
+    // d > 256, or K x d beyond the FFMA apply: column ranges of <= 128 embedding columns, each split into cluster ranges
+    // like the launches above (the first cluster range of a column range subtracts from Zo)
+    RegionScope rs(h, "ridge_apply");
+    ApplyTcArgs a;
+    a.R = h->R.p;
+    a.V = h->V.p;
+    a.Zc = h->Zc.p;
+    a.tile_cell0 = h->tile_cell0.p;
+    a.tile_len = h->tile_len.p;
+    a.tile_tuple = h->tile_tuple.p;
+    a.ntiles = h->ntiles;
+    a.d = d;
+    a.K = K;
+    a.KS = h->KS;
+    a.DS = h->DS;
+    a.tiles_per_cta = std::max(1, (h->ntiles + h->num_sms - 1) / h->num_sms);
+    const int grid = (h->ntiles + a.tiles_per_cta - 1) / a.tiles_per_cta;
+    for (a.c_off = 0; a.c_off < h->DS; a.c_off += 128) {
+      a.DC = std::min(128, h->DS - a.c_off);
+      int npass = (K + AP_MAXK - 1) / AP_MAXK, Kpass = 0;
+      for (;; ++npass) {
+        Kpass = (((K + npass - 1) / npass) + 7) & ~7;
+        if (apply_cols_stages(apply_tc_rs(Kpass, h->KS, 0), a.DC) >= 2) break;
+      }
+      for (int k_off = 0; k_off < K; k_off += Kpass) {
+        a.k_off = k_off;
+        a.Kp = std::min(Kpass, K - k_off);
+        a.KD = (a.Kp + 7) & ~7;
+        a.minuend = (k_off == 0) ? h->Zo.p : h->Zc.p;
+        const size_t smem = apply_cols_smem_bytes(apply_tc_rs(a.KD, h->KS, k_off), a.DC);
+        CK(cudaFuncSetAttribute(k_apply_tc_cols, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        k_apply_tc_cols<<<grid, AP_THREADS, smem, h->stream>>>(a);
+        CKL();
+      }
+    }
+    return 0;
+  }
   {
     RegionScope rs(h, "ridge_apply");
     ApplyArgs a;
@@ -1320,11 +1434,9 @@ int run_correct(hb_handle* h) {
     a.K = K;
     a.ldR = h->KS;
     a.ldZ = h->DS;
-    const int DP = (d + 3) & ~3, KP4 = (K + 3) & ~3;
+    const int DP = (d + 3) & ~3;
     dim3 block(DP / 4, TM / 4);
-    if (block.x * block.y > 1024) return fail(h, 2, "d = %d is too large for the apply kernel", d);
-    size_t smem = sizeof(float) * ((size_t)KP4 * DP + (size_t)TM * KP4);
-    if (smem > 227 * 1024) return fail(h, 2, "K*d too large for the apply kernel (needs %zu B shared memory)", smem);
+    const size_t smem = apply_ffma_smem_bytes(K, d);
     CK(cudaFuncSetAttribute(k_ridge_apply, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     a.tiles_per_cta = std::max(1, (h->ntiles + h->num_sms * 4 - 1) / (h->num_sms * 4));
     int grid = (h->ntiles + a.tiles_per_cta - 1) / a.tiles_per_cta;
@@ -2026,17 +2138,16 @@ int hb_init_cluster(hb_handle* h, const double* Y0) {
     // both steps run from tensor-core logits U = 2 (z . y - 1) (k_logits_tc, sigma = 1) when that kernel takes the
     // shape; else from the FFMA kernels (thread per cell)
     DevBuf<float> ones, yy;
-    if (h->paths.mm.kmeans) {
+    const bool km_logits = h->paths.mm.kmeans || h->paths.wide.kmeans;
+    const int km_nv = sp_nv(h->KS);
+    if (km_logits) {
       CK(ones.alloc(K));
       CK(yy.alloc(K));
       k_fill_f<<<1, 256, 0, h->stream>>>(ones.p, (int64_t)K, 1.0f);
       CKL();
     }
     const size_t smem_pp = sizeof(float) * Kd;
-    if (!h->paths.mm.kmeans) {
-      if (smem_pp > 200 * 1024) return fail(h, 2, "K*d too large for the native k-means initialisation; pass Y0");
-      CK(cudaFuncSetAttribute(k_kmeans_race, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_pp));
-    }
+    if (!km_logits) CK(cudaFuncSetAttribute(k_kmeans_race, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_pp));
     std::vector<unsigned long long> best(K);
     bool logits_of_start = false;  // U holds the logits of the start cells
     auto race = [&](int i0, int i1, const std::vector<int64_t>& taken) -> int {
@@ -2046,18 +2157,21 @@ int hb_init_cluster(hb_handle* h, const double* Y0) {
         CK(cudaMemcpyAsync(taken_d.p, taken.data(), sizeof(int64_t) * taken.size(), cudaMemcpyHostToDevice, h->stream));
       }
       CK(cudaMemsetAsync(best_d.p + i0, 0xff, sizeof(unsigned long long) * (i1 - i0), h->stream));
-      if (h->paths.mm.kmeans) {
+      if (km_logits) {
         if (!logits_of_start) {
           TRY(launch_logits(h, ones.p, false));
           logits_of_start = true;
         }
         const int grid_r = grid_for(h->n * 32, 256, h->num_sms * 8);
-        if (sp_nv(h->KS) == 1)
-          k_kmeans_race_u<1><<<grid_r, 256, 0, h->stream>>>(h->U.p, h->sort_perm.p, best_d.p, taken.empty() ? nullptr : taken_d.p,
-                                                          (int)taken.size(), h->n, K, h->KS, h->cell_offset, seed, i0, i1);
-        else
-          k_kmeans_race_u<2><<<grid_r, 256, 0, h->stream>>>(h->U.p, h->sort_perm.p, best_d.p, taken.empty() ? nullptr : taken_d.p,
-                                                          (int)taken.size(), h->n, K, h->KS, h->cell_offset, seed, i0, i1);
+        auto go = [&](auto nvc) {
+          constexpr int NV = decltype(nvc)::value;
+          k_kmeans_race_u<NV><<<grid_r, 256, 0, h->stream>>>(h->U.p, h->sort_perm.p, best_d.p, taken.empty() ? nullptr : taken_d.p,
+                                                           (int)taken.size(), h->n, K, h->KS, h->cell_offset, seed, i0, i1);
+        };
+        if (km_nv == 1) go(std::integral_constant<int, 1>());
+        else if (km_nv == 2) go(std::integral_constant<int, 2>());
+        else if (km_nv == 4) go(std::integral_constant<int, 4>());
+        else go(std::integral_constant<int, 8>());
         CKL();
       } else {
         k_kmeans_race<<<grid_for(h->n, 128, h->num_sms * 4), 128, sizeof(float) * (size_t)(i1 - i0) * d, h->stream>>>(
@@ -2088,18 +2202,22 @@ int hb_init_cluster(hb_handle* h, const double* Y0) {
     h->kmeans_cells = cells;
     TRY(gather(-1));
     const size_t smem = sizeof(float) * Kd;
-    if (!h->paths.mm.kmeans) CK(cudaFuncSetAttribute(k_kmeans_assign, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    if (!km_logits) CK(cudaFuncSetAttribute(k_kmeans_assign, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     for (int iter = 0; iter < 10; ++iter) {
-      if (h->paths.mm.kmeans) {
+      if (km_logits) {
         // Lloyd iteration on the tensor cores: logits -> one-hot rows of R -> members' sums and counts (K3) -> means
         TRY(launch_logits(h, ones.p, false));
         k_kmeans_norms<<<(K + 127) / 128, 128, 0, h->stream>>>(h->Y.p, yy.p, K, d);
         CKL();
         const int grid_p = grid_for(h->n * 32, 256, h->num_sms * 8);
-        if (sp_nv(h->KS) == 1)
-          k_kmeans_pick<1><<<grid_p, 256, 0, h->stream>>>(h->U.p, yy.p, h->R.p, h->n, K, h->KS);
-        else
-          k_kmeans_pick<2><<<grid_p, 256, 0, h->stream>>>(h->U.p, yy.p, h->R.p, h->n, K, h->KS);
+        auto go = [&](auto nvc) {
+          constexpr int NV = decltype(nvc)::value;
+          k_kmeans_pick<NV><<<grid_p, 256, 0, h->stream>>>(h->U.p, yy.p, h->R.p, h->n, K, h->KS);
+        };
+        if (km_nv == 1) go(std::integral_constant<int, 1>());
+        else if (km_nv == 2) go(std::integral_constant<int, 2>());
+        else if (km_nv == 4) go(std::integral_constant<int, 4>());
+        else go(std::integral_constant<int, 8>());
         CKL();
         CK(cudaMemsetAsync(h->S.p, 0, sizeof(float) * (size_t)h->J * K * (d + 1), h->stream));
         TRY(run_stats_tc(h, h->Zc.p));
@@ -2527,6 +2645,22 @@ int hb_debug_kernel_paths(int K, int d, int J, int64_t n, int nb, int num_sms, i
                         call_path(p, 20, false).plan_order_assign, (int64_t)call_path(p, 40, false).update,
                         (int64_t)call_path(p, 20, true).update};
   for (int i = 0; i < 8; ++i) out[i] = v[i];
+  return 0;
+}
+
+// The kernels of the stages whose FFMA kernels stop at a shared-memory limit, and the kernels that take those shapes
+// instead (test hook, host only).  out = {natural-order assignment: 1 fused wgmma, 2 FFMA k_assign, 3 k_logits_tc +
+// softmax pass, 4 k_logits_wide + softmax pass; plan-order cold start of a 20-round call: 0 none (natural order),
+// 1 fused wgmma, 2 k_logits_tc + block sums, 3 k_logits_wide + block sums; ridge apply: 1 wgmma, 2 FFMA, 3 column
+// ranges; native k-means initialisation: 1 FFMA, 2 k_logits_tc logits (KS <= 256), 3 k_logits_tc logits, 4
+// k_logits_wide logits}.
+int hb_debug_wide_paths(int K, int d, int J, int64_t n, int nb, int num_sms, int kernel_set, int64_t out[4]) {
+  const KernelPaths p = select_kernels(K, d, J, n, nb, num_sms, kernel_set);
+  const int lw = p.wide.logits ? 1 : 0;
+  out[0] = p.mm.k1_stages ? 1 : p.wide.assign ? 3 + lw : 2;
+  out[1] = !call_path(p, 20, false).plan_order_assign ? 0 : p.mm.k1_stages ? 1 : p.mm.logits ? 2 : 2 + lw;
+  out[2] = p.mm.apply ? 1 : p.wide.apply ? 3 : 2;
+  out[3] = p.mm.kmeans ? 2 : p.wide.kmeans ? 3 + lw : 1;
   return 0;
 }
 

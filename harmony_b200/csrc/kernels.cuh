@@ -101,6 +101,8 @@ __global__ void k_kmeans_gather(const float* __restrict__ Zc, const int* __restr
 // for the centroids i in [i0, i1) (all values are >= 0, so the bit patterns order like the floats; ties go to the
 // smaller cell index).  Cells listed in `taken` (ntaken global indices) do not take part.  Thread per cell, start
 // centroids in shared memory.
+// k_kmeans_race and k_kmeans_assign hold all K x d centroids in shared memory
+inline bool kmeans_ffma_fits(int K, int d) { return sizeof(float) * (size_t)K * d <= (size_t)200 * 1024; }
 __global__ void __launch_bounds__(128) k_kmeans_race(const float* __restrict__ Zc, const int* __restrict__ sort_perm,
                                                      const float* __restrict__ Y, unsigned long long* __restrict__ best,
                                                      const int64_t* __restrict__ taken, int ntaken, int64_t n, int K, int d,
@@ -319,6 +321,13 @@ struct AssignArgs {
   int DS, KS;               // row strides of Z and of U/R/O (multiples of 4 floats)
   int normalise;
 };
+
+// shared memory of k_assign (Ys, Zs, Ls, sig, part below); the kernel serves the shapes where this fits
+inline size_t assign_ffma_smem_bytes(int K, int d) {
+  const size_t KP = (K + 63) & ~63, DP4 = (d + 3) & ~3;
+  return sizeof(float) * (DP4 * KP + (size_t)TM * DP4 + (size_t)TM * (KP + 4) + KP + (size_t)NWARP * KP);
+}
+inline bool assign_ffma_fits(int K, int d) { return assign_ffma_smem_bytes(K, d) <= (size_t)227 * 1024; }
 
 template <int KQ>
 __global__ void __launch_bounds__(ASSIGN_THREADS) k_assign(AssignArgs a) {
@@ -818,6 +827,16 @@ struct ApplyArgs {
   int ntiles, d, K, tiles_per_cta;
   int ldR, ldZ;
 };
+
+// k_ridge_apply runs one thread per 4 cells x 4 columns of a 64-cell tile (at most 1024 threads: d <= 256) with V_q and
+// the tile of R in shared memory
+inline size_t apply_ffma_smem_bytes(int K, int d) {
+  const size_t DP = (d + 3) & ~3, KP4 = (K + 3) & ~3;
+  return sizeof(float) * (KP4 * DP + (size_t)TM * KP4);
+}
+inline bool apply_ffma_fits(int K, int d) {
+  return ((d + 3) & ~3) / 4 * (TM / 4) <= 1024 && apply_ffma_smem_bytes(K, d) <= (size_t)227 * 1024;
+}
 
 __global__ void k_ridge_apply(ApplyArgs a) {
   extern __shared__ __align__(16) float smem[];

@@ -40,6 +40,9 @@ __host__ __device__ inline size_t logits_smem_bytes(int KD) {
   return sizeof(float) * (2 * (size_t)LG_TM * KD + 2 * (size_t)LG_NP * KD + (size_t)LG_TM * LG_SS + LG_NP + 4 * (size_t)LG_TM) + 256;
 }
 
+// k_logits_tc holds the whole rows of its operands: d <= 120 on sm_90 (KD = 128 needs 233 984 B)
+__host__ __device__ inline bool logits_tc_fits(int d) { return d <= 128 && logits_smem_bytes((d + 7) & ~7) <= SMEM_LIMIT; }
+
 __global__ void __launch_bounds__(LG_THREADS, 1) k_logits_tc(LogitsArgs a) {
   extern __shared__ __align__(128) unsigned char smem_raw[];
   const int KD = a.KD, KS = a.KS, K = a.K, d = a.d, DS = a.DS;

@@ -146,7 +146,10 @@ enum hb_scalar { HB_N = 0, HB_B = 1, HB_K = 2, HB_D = 3, HB_C = 4, HB_ALPHA = 5,
 enum hb_kernel_set { HB_KS_FFMA_CONTRACTIONS = 1, /* fp32 FFMA assignment / apply / k-means initialisation instead of wgmma */
                      HB_KS_UPDATE_PER_STEP = 2,   /* update_R in three launches per block step */
                      HB_KS_UPDATE_TWO_PASS = 4,   /* update_R in the two-pass persistent kernel (look-ahead + update groups) */
-                     HB_KS_NO_PEER_EXCHANGE = 8   /* sharded cells: one NCCL all-reduce per block step */ };
+                     HB_KS_NO_PEER_EXCHANGE = 8,  /* sharded cells: one NCCL all-reduce per block step */
+                     HB_KS_WIDE = 16              /* the kernels of the shapes past the FFMA kernels' shared-memory limits:
+                                                     d-chunked logits + softmax passes for the assignment, column-range
+                                                     ridge apply, k-means initialisation from those logits */ };
 int hb_get_scalar(const hb_handle* h, int which, double* out);
 /* Settable: HB_ALPHA, HB_MAX_ITER_KMEANS (vignettes/detailedWalkthrough.Rmd:364), HB_EPSILON_*, HB_KERNEL_SET and
  * HB_LEGACY_CENTROID_STEP (0/1): run STEP 1 of harmony::cluster_cpp — Y = normalise(Z_corr * R.t()),
@@ -198,6 +201,12 @@ int hb_debug_update_geometry(int KS, int nb, int64_t out[9]);
  * initialisation, cold-start assignment of a 20-round cluster_cpp call in the plan's order, update_R path of a
  * 40-round call, update_R path of a call with HB_LEGACY_CENTROID_STEP}.  Returns 0. */
 int hb_debug_kernel_paths(int K, int d, int J, int64_t n, int nb, int num_sms, int kernel_set, int64_t out[8]);
+/* Test hook (host only): the kernel of each stage whose FFMA kernel stops at a shared-memory limit, for the same
+ * arguments: out = {natural-order assignment (1 fused wgmma, 2 FFMA, 3 wgmma logits + softmax pass, 4 d-chunked wgmma
+ * logits + softmax pass), plan-order cold start of a 20-round call (0 natural order, 1 fused wgmma, 2 wgmma logits +
+ * block sums, 3 d-chunked logits + block sums), ridge apply (1 wgmma, 2 FFMA, 3 wgmma over column ranges), native k-means
+ * initialisation (1 FFMA, 2 wgmma logits with KS <= 256, 3 wgmma logits, 4 d-chunked logits)}.  Returns 0. */
+int hb_debug_wide_paths(int K, int d, int J, int64_t n, int nb, int num_sms, int kernel_set, int64_t out[4]);
 
 #ifdef __cplusplus
 }
