@@ -12,7 +12,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(_HERE)
 SO_PATH = os.path.join(_HERE, "libharmony_b200.so")
 SOURCES = [os.path.join(_HERE, "csrc", f) for f in ("harmony_b200.cu", "kernels.cuh", "io.cuh", "common.cuh", "update_slots.cuh", "update_per_step.cuh",
-                                                     "update_two_pass.cuh", "update_single_pass.cuh", "plan.cuh", "umma.cuh", "assign_tc3.cuh", "logits_tc.cuh", "logits_wide.cuh", "stats_tc3.cuh",
+                                                     "update_two_pass.cuh", "update_single_pass.cuh", "plan.cuh", "tuples.cuh", "umma.cuh", "assign_tc3.cuh", "logits_tc.cuh", "logits_wide.cuh", "stats_tc3.cuh",
                                                      "apply_tc3.cuh")]
 HEADER = os.path.join(ROOT, "include", "harmony_b200.h")
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17", "-shared",
@@ -101,6 +101,7 @@ def lib():
     L.hb_debug_kmeans_uniform.restype = D
     L.hb_debug_kmeans_uniform.argtypes = [P, ctypes.c_uint64, ctypes.c_uint64]
     L.hb_debug_kmeans_cells.argtypes = [P, P]
+    L.hb_debug_tuple_index.argtypes = [P, P, P, P]
     L.hb_debug_widen.argtypes = [P, P, I64, I]
     _LIB = L
     return L

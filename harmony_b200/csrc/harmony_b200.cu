@@ -407,7 +407,7 @@ struct hb_handle {
   int ntiles = 0;
   int trace_cap = 0;
   std::vector<int> tuple_levels_h;  // [J][C]
-  std::vector<int> sort_perm_h;
+  std::vector<int64_t> tuple_start_h;  // [J + 1] first sorted position of each tuple
   std::vector<int64_t> kmeans_cells;  // global cells chosen by the native initialize_centroids (test hook)
 
   // traces (harmony.h:55-56); values are produced on the device and pulled lazily
@@ -585,6 +585,7 @@ int launch_logits(hb_handle* h, const float* sigma, bool normalise) {
 }  // namespace
 
 #include "plan.cuh"
+#include "tuples.cuh"
 
 namespace {
 
@@ -1578,6 +1579,20 @@ int check_device_ptr(hb_handle* h, const void* p, const char* what) {
     return fail(h, 2, "%s lives on device %d, the handle on device %d", what, a.device, h->device);
   return 0;
 }
+// Where the labels phi_i lie, found with check_device_ptr's query: *type = cudaMemoryTypeDevice or
+// cudaMemoryTypeManaged of the handle's device, else cudaMemoryTypeHost (pageable or pinned).  Another device's
+// memory: status 2.  NULL is left to setup's checks.
+int phi_location(hb_handle* h, const void* p, cudaMemoryType* type) {
+  *type = cudaMemoryTypeHost;
+  if (!p) return 0;
+  cudaPointerAttributes a{};
+  const cudaError_t e = cudaPointerGetAttributes(&a, p);
+  cudaGetLastError();
+  if (e != cudaSuccess || (a.type != cudaMemoryTypeDevice && a.type != cudaMemoryTypeManaged)) return 0;
+  if (a.device != h->device) return fail(h, 2, "phi_i lives on device %d, the handle on device %d", a.device, h->device);
+  *type = a.type;
+  return 0;
+}
 // `later` waits for the work queued on `earlier` so far (no host synchronisation)
 int stream_after(hb_handle* h, cudaStream_t later, cudaStream_t earlier) {
   if (later == earlier) return 0;
@@ -1641,7 +1656,7 @@ int upload_small(hb_handle* h, const double* in, size_t count, float* dst) {
 // =================================================================================================
 extern "C" {
 
-int hb_version(void) { return 200; }
+int hb_version(void) { return 300; }
 
 int hb_create(hb_handle** out, int device) {
   if (!out) return 1;
@@ -1748,8 +1763,8 @@ int hb_set_abort_callback(hb_handle* h, int (*cb)(void*), void* user) {
 }
 
 // hb_setup and hb_setup_device: everything but the source of Z
-static int setup_common(hb_handle* h, const ZInput& Z, int d, int64_t N, const int32_t* phi_i, const int32_t* B_vec,
-                        int C, const double* sigma, const double* theta, const double* lambda, double alpha,
+static int setup_common(hb_handle* h, const ZInput& Z, int d, int64_t N, const int32_t* phi_i, bool phi_on_device,
+                        const int32_t* B_vec, int C, const double* sigma, const double* theta, const double* lambda, double alpha,
                         int max_iter_kmeans, double epsilon_kmeans, double epsilon_harmony, int K, double block_size,
                         double batch_proportion_cutoff, int verbose) {
   if (!h) return 1;
@@ -1806,118 +1821,47 @@ static int setup_common(hb_handle* h, const ZInput& Z, int d, int64_t N, const i
   }
 
   HostLap lap(h->stream, "hb_setup");
-  // ---- joint covariate tuples; cells get sorted by tuple (stable)
-  std::vector<int64_t> lvl_count(B, 0);
-  std::vector<uint64_t> key(N);
+  // ---- joint covariate tuples; cells get sorted by tuple (stable), on the device (tuples.cuh)
   std::vector<uint64_t> radix(C);
+  uint64_t key_space = 1;
   {
     long double prod = 1;
     for (int c = 0; c < C; ++c) prod *= (long double)B_vec[c];
     if (prod > 9e18L) return fail(h, 2, "covariate level product overflows 64 bits");
-    uint64_t r = 1;
     for (int c = C - 1; c >= 0; --c) {
-      radix[c] = r;
-      r *= (uint64_t)B_vec[c];
+      radix[c] = key_space;
+      key_space *= (uint64_t)B_vec[c];
     }
   }
+  std::vector<int> base(C, 0);
+  for (int c = 1; c < C; ++c) base[c] = base[c - 1] + B_vec[c - 1];
+  TupleIndex ti;
   {
-    std::vector<int> base(C, 0);
-    for (int c = 1; c < C; ++c) base[c] = base[c - 1] + B_vec[c - 1];
-    for (int64_t i = 0; i < N; ++i) {
-      uint64_t kk = 0;
-      for (int c = 0; c < C; ++c) {
-        int b = phi_i[i * C + c];
-        if (b < base[c] || b >= base[c] + B_vec[c]) return fail(h, 2, "phi row index %d of cell %lld is not a level of covariate %d", b, (long long)i, c);
-        lvl_count[b]++;
-        kk += (uint64_t)(b - base[c]) * radix[c];
-      }
-      key[i] = kk;
+    RegionScope rs(h, "tuple_index");
+    DevBuf<int> phi_up;  // host labels: one upload, then the same kernels
+    const int* phi_d = phi_i;
+    if (phi_on_device) {
+      TRY(stream_after(h, h->stream, Z.stream));  // read after the caller's work, like Z
+    } else {
+      CK(phi_up.alloc((size_t)N * C));
+      CK(cudaMemcpyAsync(phi_up.p, phi_i, sizeof(int) * (size_t)N * C, cudaMemcpyDefault, h->stream));
+      phi_d = phi_up.p;
     }
+    TRY(build_tuple_index(h, phi_d, N, base, radix, key_space, ti));
   }
-  std::vector<uint64_t> uniq;
-  uint64_t key_space = 1;
-  for (int c = 0; c < C; ++c) key_space *= (uint64_t)B_vec[c];
-  const bool small_space = key_space <= (1ull << 22);  // the usual case: a direct table beats sorting N keys
-  if (small_space) {
-    std::vector<uint8_t> seen((size_t)key_space, 0);
-    for (int64_t i = 0; i < N; ++i) seen[key[i]] = 1;
-    for (uint64_t k2 = 0; k2 < key_space; ++k2)
-      if (seen[k2]) uniq.push_back(k2);
-  } else {
-    uniq = key;
-    std::sort(uniq.begin(), uniq.end());
-    uniq.erase(std::unique(uniq.begin(), uniq.end()), uniq.end());
-  }
-  if (h->world > 1) {
-    // global tuple dictionary = union over ranks; level counts summed over ranks
-    long long cnt = (long long)uniq.size(), maxcnt = 0;
-    DevBuf<long long> dcnt;
-    CK(dcnt.alloc(1));
-    CK(cudaMemcpyAsync(dcnt.p, &cnt, sizeof(cnt), cudaMemcpyHostToDevice, h->stream));
-    CKN(g_nccl.AllReduce(dcnt.p, dcnt.p, 1, ncclInt64, ncclMax, h->comm, h->stream));
-    CK(cudaMemcpyAsync(&maxcnt, dcnt.p, sizeof(cnt), cudaMemcpyDeviceToHost, h->stream));
-    CK(cudaStreamSynchronize(h->stream));
-    std::vector<uint64_t> sendbuf((size_t)maxcnt, ~0ull), recvbuf((size_t)maxcnt * h->world);
-    std::copy(uniq.begin(), uniq.end(), sendbuf.begin());
-    DevBuf<uint64_t> ds, dr;
-    CK(ds.alloc((size_t)maxcnt));
-    CK(dr.alloc((size_t)maxcnt * h->world));
-    CK(cudaMemcpyAsync(ds.p, sendbuf.data(), sizeof(uint64_t) * (size_t)maxcnt, cudaMemcpyHostToDevice, h->stream));
-    CKN(g_nccl.AllGather(ds.p, dr.p, (size_t)maxcnt, ncclUint64, h->comm, h->stream));
-    CK(cudaMemcpyAsync(recvbuf.data(), dr.p, sizeof(uint64_t) * recvbuf.size(), cudaMemcpyDeviceToHost, h->stream));
-    DevBuf<long long> dl;
-    CK(dl.alloc(B));
-    std::vector<long long> lc(lvl_count.begin(), lvl_count.end());
-    CK(cudaMemcpyAsync(dl.p, lc.data(), sizeof(long long) * B, cudaMemcpyHostToDevice, h->stream));
-    CKN(g_nccl.AllReduce(dl.p, dl.p, B, ncclInt64, ncclSum, h->comm, h->stream));
-    CK(cudaMemcpyAsync(lc.data(), dl.p, sizeof(long long) * B, cudaMemcpyDeviceToHost, h->stream));
-    CK(cudaStreamSynchronize(h->stream));
-    for (int b = 0; b < B; ++b) lvl_count[b] = lc[b];
-    uniq.assign(recvbuf.begin(), recvbuf.end());
-    std::sort(uniq.begin(), uniq.end());
-    uniq.erase(std::unique(uniq.begin(), uniq.end()), uniq.end());
-    if (!uniq.empty() && uniq.back() == ~0ull) uniq.pop_back();
-  }
-  if (uniq.size() > 1000000) return fail(h, 2, "more than 1e6 distinct covariate tuples are not supported");
-  const int J = (int)uniq.size();
+  const std::vector<int64_t>& lvl_count = ti.lvl_count;
+  const std::vector<int64_t>& tstart = ti.tstart;
+  const int J = (int)ti.uniq.size();
   h->J = J;
   h->tuple_levels_h.resize((size_t)J * C);
-  {
-    std::vector<int> base(C, 0);
-    for (int c = 1; c < C; ++c) base[c] = base[c - 1] + B_vec[c - 1];
-    for (int q = 0; q < J; ++q) {
-      uint64_t kk = uniq[q];
-      for (int c = 0; c < C; ++c) {
-        h->tuple_levels_h[(size_t)q * C + c] = base[c] + (int)(kk / radix[c]);
-        kk %= radix[c];
-      }
+  for (int q = 0; q < J; ++q) {
+    uint64_t kk = ti.uniq[q];
+    for (int c = 0; c < C; ++c) {
+      h->tuple_levels_h[(size_t)q * C + c] = base[c] + (int)(kk / radix[c]);
+      kk %= radix[c];
     }
   }
-  std::vector<int> tuple_of(N);
-  std::vector<int64_t> tstart(J + 1, 0);
-  {
-    std::vector<int> lut;
-    if (small_space) {
-      lut.assign((size_t)key_space, -1);
-      for (int q = 0; q < J; ++q) lut[uniq[q]] = q;
-    }
-    for (int64_t i = 0; i < N; ++i) {
-      int q = small_space ? lut[key[i]] : (int)(std::lower_bound(uniq.begin(), uniq.end(), key[i]) - uniq.begin());
-      tuple_of[i] = q;
-      tstart[q + 1]++;
-    }
-  }
-  for (int q = 0; q < J; ++q) tstart[q + 1] += tstart[q];
-  h->sort_perm_h.resize(N);
-  std::vector<int> inv_sort(N);
-  {
-    std::vector<int64_t> cur(tstart.begin(), tstart.end() - 1);
-    for (int64_t i = 0; i < N; ++i) {
-      int64_t s = cur[tuple_of[i]]++;
-      h->sort_perm_h[s] = (int)i;
-      inv_sort[i] = (int)s;
-    }
-  }
+  h->tuple_start_h = tstart;
   // static tiles (<= TM cells of one tuple)
   std::vector<int> t_cell0, t_len, t_tuple;
   for (int q = 0; q < J; ++q)
@@ -1936,7 +1880,7 @@ static int setup_common(hb_handle* h, const ZInput& Z, int d, int64_t N, const i
   h->tc_ntiles = (int)tc0.size();
   h->ntiles = (int)t_cell0.size();
 
-  lap.mark("tuple dictionary / sort (host)");
+  lap.mark("tuple index (device)");
   // ---- device allocations
   const int KS = h->KS, DS = h->DS;
   const size_t nK = (size_t)N * KS, nd = (size_t)N * DS, BK = (size_t)B * KS;
@@ -1970,8 +1914,6 @@ static int setup_common(hb_handle* h, const ZInput& Z, int d, int64_t N, const i
   CK(h->err_flag.alloc(1));
   CK(h->obj_acc.alloc(2));
   CK(h->stage.alloc((size_t)8 << 20));  // 64 MiB of doubles
-  CK(h->sort_perm.alloc(N));
-  CK(h->inv_sort.alloc(N));
   CK(h->tuple_levels.alloc((size_t)J * C));
   CK(h->cov_of_d.alloc(B));
   CK(h->tile_cell0.alloc(h->ntiles));
@@ -2007,8 +1949,6 @@ static int setup_common(hb_handle* h, const ZInput& Z, int d, int64_t N, const i
   CKL();
   CK(cudaMemsetAsync(h->Y.p, 0, sizeof(float) * (size_t)K * d, h->stream));
 #define UP(buf, vec) CK(cudaMemcpyAsync(h->buf.p, (vec).data(), sizeof((vec)[0]) * (vec).size(), cudaMemcpyHostToDevice, h->stream))
-  UP(sort_perm, h->sort_perm_h);
-  UP(inv_sort, inv_sort);
   UP(tuple_levels, h->tuple_levels_h);
   // CSR level -> tuples containing it, ascending tuple order; trailing word: the number of levels of covariate 0
   std::vector<int> lvl_ptr_h(B + 2, 0), lvl_tup_h((size_t)J * C);
@@ -2073,9 +2013,14 @@ int hb_setup(hb_handle* h, const double* Z, int d, int64_t N, const int32_t* phi
              const double* sigma, const double* theta, const double* lambda, double alpha, int max_iter_kmeans,
              double epsilon_kmeans, double epsilon_harmony, int K, double block_size,
              double batch_proportion_cutoff, int verbose) {
+  if (!h) return 1;
+  cudaMemoryType phi_type;  // managed labels are read like host ones (one copy to the device)
+  TRY(phi_location(h, phi_i, &phi_type));
+  if (phi_type == cudaMemoryTypeDevice)
+    return fail(h, 2, "phi_i is device memory: hb_setup takes host labels (device labels go through hb_setup_device)");
   ZInput z;
   z.host = Z;
-  return setup_common(h, z, d, N, phi_i, B_vec, C, sigma, theta, lambda, alpha, max_iter_kmeans, epsilon_kmeans,
+  return setup_common(h, z, d, N, phi_i, false, B_vec, C, sigma, theta, lambda, alpha, max_iter_kmeans, epsilon_kmeans,
                       epsilon_harmony, K, block_size, batch_proportion_cutoff, verbose);
 }
 
@@ -2088,12 +2033,14 @@ int hb_setup_device(hb_handle* h, const void* Z, int z_dtype, int64_t z_ld, void
   if (z_dtype != HB_FLOAT32 && z_dtype != HB_FLOAT64) return fail(h, 2, "unknown dtype %d of Z", z_dtype);
   if (z_ld < d) return fail(h, 2, "row stride of Z (%lld) is smaller than d = %d", (long long)z_ld, d);
   TRY(check_device_ptr(h, Z, "Z"));
+  cudaMemoryType phi_type;
+  TRY(phi_location(h, phi_i, &phi_type));
   ZInput z;
   z.dev = Z;
   z.dtype = z_dtype;
   z.ld = z_ld;
   z.stream = (cudaStream_t)stream;
-  return setup_common(h, z, d, N, phi_i, B_vec, C, sigma, theta, lambda, alpha, max_iter_kmeans, epsilon_kmeans,
+  return setup_common(h, z, d, N, phi_i, phi_type != cudaMemoryTypeHost, B_vec, C, sigma, theta, lambda, alpha, max_iter_kmeans, epsilon_kmeans,
                       epsilon_harmony, K, block_size, batch_proportion_cutoff, verbose);
 }
 
@@ -2662,6 +2609,19 @@ int hb_debug_wide_paths(int K, int d, int J, int64_t n, int nb, int num_sms, int
   out[2] = p.mm.apply ? 1 : p.wide.apply ? 3 : 2;
   out[3] = p.mm.kmeans ? 2 : p.wide.kmeans ? 3 + lw : 1;
   return 0;
+}
+
+// The covariate-tuple index setup built (test hook): J, and the non-null ones of sort_perm (N_local cells, sorted
+// position -> caller's cell), tuple_levels (J x C global levels) and tuple_start (J + 1 first sorted positions).
+int hb_debug_tuple_index(const hb_handle* h, int32_t* sort_perm, int32_t* tuple_levels, int64_t* tuple_start) {
+  if (!h || !h->ran_setup) return -1;
+  if (sort_perm &&
+      (cudaSetDevice(h->device) != cudaSuccess ||
+       cudaMemcpy(sort_perm, h->sort_perm.p, sizeof(int32_t) * (size_t)h->n, cudaMemcpyDeviceToHost) != cudaSuccess))
+    return -1;
+  if (tuple_levels) std::copy(h->tuple_levels_h.begin(), h->tuple_levels_h.end(), tuple_levels);
+  if (tuple_start) std::copy(h->tuple_start_h.begin(), h->tuple_start_h.end(), tuple_start);
+  return h->J;
 }
 
 // Test hooks of the native kmeans_centers: the uniform of (centroid i, global cell g) under the handle's seed, and

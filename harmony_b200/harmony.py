@@ -97,13 +97,19 @@ class harmony:
         int array [N, C]; ``lambda_``: B+1 values or None / -1 for automatic estimation.
 
         ``Z`` may also be a float32 / float64 CUDA tensor on the object's device, in either orientation: it is read
-        where it lies (no host round trip), after the work queued on the device's current torch stream."""
+        where it lies (no host round trip), after the work queued on the device's current torch stream.  With such a
+        ``Z``, ``Phi`` may be an int32 / int64 CUDA tensor ([N] or [N, C]) on the same device, read the same way."""
         dev = is_cuda_tensor(Z)
         if not dev:
             Z = np.asarray(Z)
-        phi_i = np.ascontiguousarray(Phi, dtype=np.int32)
-        if phi_i.ndim == 1:
-            phi_i = phi_i.reshape(-1, 1)
+        if is_cuda_tensor(Phi):
+            if not dev:
+                raise ValueError("Phi is a CUDA tensor but Z is not: device labels go with a device embedding")
+            phi_i = self._device_Phi(Phi)             # alive until the call returns
+        else:
+            phi_i = np.ascontiguousarray(Phi, dtype=np.int32)
+            if phi_i.ndim == 1:
+                phi_i = phi_i.reshape(-1, 1)
         n = phi_i.shape[0]
         if Z.ndim != 2:
             raise ValueError("Z must be a matrix")
@@ -128,7 +134,8 @@ class harmony:
                 lam = None
             elif len(lam) != int(B_vec.sum()) + 1:
                 raise ValueError("lambda must hold B+1 values")
-        rest = (Z.shape[1], n, _ptr(phi_i), _ptr(B_vec), len(B_vec), _ptr(sigma), _ptr(theta),
+        phi_ptr = ctypes.c_void_p(phi_i.data_ptr()) if is_cuda_tensor(phi_i) else _ptr(phi_i)
+        rest = (Z.shape[1], n, phi_ptr, _ptr(B_vec), len(B_vec), _ptr(sigma), _ptr(theta),
                 None if lam is None else _ptr(lam), float(alpha), int(max_iter_kmeans), float(epsilon_kmeans),
                 float(epsilon_harmony), K, float(block_size), float(batch_proportion_cutoff), int(bool(verbose)))
         if dev:
@@ -149,6 +156,20 @@ class harmony:
         ld = Z.stride(0) if Z.shape[0] > 1 else Z.shape[1]
         stream = torch.cuda.current_stream(Z.device).cuda_stream
         return Z, (ctypes.c_void_p(Z.data_ptr()), _DTYPE[str(Z.dtype)[6:]], int(ld), ctypes.c_void_p(stream))
+
+    def _device_Phi(self, Phi):
+        """An [N] or [N, C] int32 / int64 CUDA tensor -> contiguous [N, C] int32 on the object's device (converted, if
+        need be, on the current torch stream, which hb_setup_device orders its read after)."""
+        import torch
+        if Phi.dtype not in (torch.int32, torch.int64):
+            raise TypeError(f"Phi must be int32 or int64, not {Phi.dtype}")
+        if Phi.device.index != self._scalar("device"):
+            raise ValueError(f"Phi is on {Phi.device}, the harmony object on cuda:{self._scalar('device')}")
+        if Phi.ndim == 1:
+            Phi = Phi.reshape(-1, 1)
+        if Phi.ndim != 2:
+            raise ValueError("Phi must be [N] or [N, C]")
+        return Phi.to(torch.int32).contiguous()
 
     def set_seed(self, seed):
         self._check(self._L.hb_set_seed(self._h, int(seed) & 0xFFFFFFFFFFFFFFFF))

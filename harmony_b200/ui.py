@@ -13,17 +13,43 @@ from .harmony_option import HarmonyOptions, check_legacy_args, harmony_options
 from .utils import harmonize, is_cuda_tensor
 
 
+def _column(v):
+    return v if is_cuda_tensor(v) else np.asarray(v)
+
+
 def _as_columns(meta_data, n_hint):
-    """meta_data -> dict name -> 1-D array.  Accepts a dict, a pandas DataFrame or one vector
-    (R/ui.R:157-165: a bare vector becomes data.frame(batch_variable = ...))."""
+    """meta_data -> dict name -> 1-D array (CUDA tensors stay where they are).  Accepts a dict, a pandas DataFrame
+    or one vector (R/ui.R:157-165: a bare vector becomes data.frame(batch_variable = ...))."""
     if hasattr(meta_data, "columns") and hasattr(meta_data, "__getitem__") and not isinstance(meta_data, dict):
         return {str(c): np.asarray(meta_data[c]) for c in meta_data.columns}, None
     if isinstance(meta_data, dict):
-        return {str(k): np.asarray(v) for k, v in meta_data.items()}, None
-    v = np.asarray(meta_data)
+        return {str(k): _column(v) for k, v in meta_data.items()}, None
+    v = _column(meta_data)
     if v.ndim == 1 and len(v) in n_hint:
         return {"batch_variable": v}, "batch_variable"
     raise ValueError("meta_data must be either a data.frame or a vector with batch values for each cell")
+
+
+def _label_device(cols, vars_use, data_mat, on_device):
+    """The device of the used label columns that are CUDA tensors (None: all are host arrays).  They must be integer
+    or bool tensors on data_mat's device."""
+    device = None
+    for v in vars_use:
+        col = cols[v]
+        if not is_cuda_tensor(col):
+            continue
+        import torch
+        if col.dtype not in (torch.bool, torch.uint8, torch.int8, torch.int16, torch.int32, torch.int64):
+            raise TypeError(f"labels {v!r} on the GPU must be an integer or bool tensor, not {col.dtype}")
+        if not on_device:
+            raise ValueError(f"labels {v!r} are a CUDA tensor but data_mat is not: device labels go with a device "
+                             f"embedding")
+        if col.device != data_mat.device:
+            raise ValueError(f"labels {v!r} are on {col.device}, data_mat on {data_mat.device}")
+        if col.ndim != 1:
+            raise ValueError(f"labels {v!r} must be a vector")
+        device = col.device
+    return device
 
 
 def prepare_inputs(data_mat, meta_data, vars_use=None, theta=None, sigma=0.1, lambda_=None, nclust=None,
@@ -33,6 +59,10 @@ def prepare_inputs(data_mat, meta_data, vars_use=None, theta=None, sigma=0.1, la
     Returns a dict with the exact argument list of ``harmony::setup`` (src/harmony.h:25-30), with
     the sparse ``phi`` expressed as its row-index slot: ``phi_i[n, c]`` = row of the c-th non-zero of
     column n (each cell has exactly one level per covariate, so columns hold C non-zeros).
+
+    With a CUDA ``data_mat``, a used metadata column (or the bare vector) may be an integer or bool CUDA tensor on the
+    same device: it is factorised there, and ``phi_i`` is then an [N, C] int32 CUDA tensor (host columns are
+    factorised as usual and copied over).  ``level_names`` are always host arrays.
     """
     options = harmony_options() if options is None else options
     if not isinstance(options, HarmonyOptions):
@@ -77,15 +107,32 @@ def prepare_inputs(data_mat, meta_data, vars_use=None, theta=None, sigma=0.1, la
     # phi / B_vec: as.factor levels = sorted unique values (R/ui.R:210-221)
     phi_cols, B_vec, level_names = [], [], []
     offset = 0
+    device = _label_device(cols, vars_use, data_mat, on_device)
     for v in vars_use:
-        levels, codes = np.unique(cols[v], return_inverse=True)
-        phi_cols.append(codes.astype(np.int32) + offset)
+        if device is not None and is_cuda_tensor(cols[v]):
+            # integer / bool labels: torch's sorted unique levels are np.unique's (and as.factor's) for these dtypes
+            import torch
+            levels, codes = torch.unique(cols[v], sorted=True, return_inverse=True)
+            phi_cols.append(codes.to(torch.int32) + offset)
+            levels = levels.cpu().numpy()
+        else:
+            levels, codes = np.unique(cols[v], return_inverse=True)
+            codes = codes.reshape(-1).astype(np.int32) + offset
+            if device is not None:
+                import torch
+                codes = torch.from_numpy(codes).to(device)
+            phi_cols.append(codes)
         B_vec.append(len(levels))
         level_names.append(levels)
         offset += len(levels)
-    phi_i = np.ascontiguousarray(np.stack(phi_cols, axis=1))          # [N, C]
     B = offset
-    N_b = np.bincount(phi_i.reshape(-1), minlength=B).astype(np.float64)
+    if device is None:
+        phi_i = np.ascontiguousarray(np.stack(phi_cols, axis=1))      # [N, C]
+        N_b = np.bincount(phi_i.reshape(-1), minlength=B).astype(np.float64)
+    else:
+        import torch
+        phi_i = torch.stack(phi_cols, dim=1).contiguous()             # [N, C] int32 on the embedding's device
+        N_b = torch.bincount(phi_i.reshape(-1), minlength=B).cpu().numpy().astype(np.float64)
     if lambda_ is None:                                               # R/ui.R:224-229
         lambda_vec = None
     else:

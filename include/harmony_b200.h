@@ -17,8 +17,8 @@
  *   - all buffers are caller-owned host memory; inputs are copied during the call
  *     (like harmony::setup, harmony.cpp:41,44), outputs are written into caller-allocated arrays.
  *     The exceptions are hb_setup_device and hb_get_field_device, which take the per-cell matrices
- *     in the caller's device memory (fp32 or fp64, any row stride) and order themselves on a
- *     caller's CUDA stream.
+ *     (and, for hb_setup_device, optionally the labels phi_i) in the caller's device memory (fp32 or
+ *     fp64, any row stride) and order themselves on a caller's CUDA stream.
  *   - a handle must be driven from one host thread at a time (the reference is single-threaded).
  */
 #ifndef HARMONY_B200_H
@@ -42,7 +42,7 @@ const char* hb_last_error(const hb_handle* h);
 /* Pops one pending warning (e.g. "Too few cells. Setting block_size to 0.2", harmony.cpp:86-88) into
  * buf; returns 1 if a warning was written, 0 if none is pending.  The shim turns it into Rcpp::warning. */
 int hb_pop_warning(hb_handle* h, char* buf, size_t cap);
-/* Library/ABI version: major*10000 + minor*100 + patch. */
+/* Library/ABI version: major*10000 + minor*100 + patch (0.3.0: labels in device memory). */
 int hb_version(void);
 
 /* ---- multi-GPU (one process per GPU; cells sharded contiguously; SURVEY §8e) ------------------- */
@@ -61,7 +61,10 @@ int hb_set_shard(hb_handle* h, int64_t N_global, int64_t cell_offset);
 /* ---- harmony::setup (harmony.h:25-30, harmony.cpp:29-111; called at R/ui.R:271-275) ---------- */
 /* Z: d x N(local) column-major doubles.  lambda: B+1 values, or NULL / lambda[0] == -1 for the
  * reference's automatic estimation (harmony.cpp:75-76).  Errors: N < 6 -> status 1 with the
- * reference's message (harmony.cpp:83-85); 6 <= N < 40 -> warning + block_size 0.2 (:86-88). */
+ * reference's message (harmony.cpp:83-85); 6 <= N < 40 -> warning + block_size 0.2 (:86-88).
+ * phi_i must be host (or managed) memory: there is no stream to order a device read against; a device
+ * pointer -> status 2 before any launch.  The covariate-tuple index (cells stably sorted by their tuple
+ * of levels) is built on the device from either. */
 int hb_setup(hb_handle* h, const double* Z, int d, int64_t N, const int32_t* phi_i, const int32_t* B_vec, int C,
              const double* sigma, const double* theta, const double* lambda, double alpha, int max_iter_kmeans,
              double epsilon_kmeans, double epsilon_harmony, int K, double block_size,
@@ -71,10 +74,11 @@ int hb_setup(hb_handle* h, const double* Z, int d, int64_t N, const int32_t* phi
 enum hb_dtype { HB_FLOAT32 = 0, HB_FLOAT64 = 1 };
 
 /* hb_setup with Z in device memory: N(local) rows of d values of z_dtype, row stride z_ld >= d elements (the bytes of a
- * d x N column-major matrix when z_ld == d), in device or managed memory of the handle's device.  Every other argument
- * is hb_setup's, on the host.  Z is read after the work already queued on `stream` (a cudaStream_t; NULL: the legacy
- * default stream) and the call returns once it has been copied.  Status 2 before any launch for a NULL, host or
- * other-device Z, an unknown dtype or z_ld < d. */
+ * d x N column-major matrix when z_ld == d), in device or managed memory of the handle's device.  phi_i may lie in
+ * host memory or in device or managed memory of the handle's device; every other argument is hb_setup's, on the host.
+ * Z and a device phi_i are read after the work already queued on `stream` (a cudaStream_t; NULL: the legacy default
+ * stream) and the call returns once they have been copied.  Status 2 before any launch for a NULL, host or
+ * other-device Z, an other-device phi_i, an unknown dtype or z_ld < d. */
 int hb_setup_device(hb_handle* h, const void* Z, int z_dtype, int64_t z_ld, void* stream, int d, int64_t N,
                     const int32_t* phi_i, const int32_t* B_vec, int C, const double* sigma, const double* theta,
                     const double* lambda, double alpha, int max_iter_kmeans, double epsilon_kmeans,
@@ -173,8 +177,9 @@ void* hb_stream(const hb_handle* h);
 /* Blocks until all queued work of the handle has finished; returns the sticky CUDA status as 0/>0. */
 int hb_synchronize(hb_handle* h);
 /* Accumulated device time (ms) and launch count of a named region ("assign", "update_R",
- * "ridge_stats", "ridge_solve", "ridge_apply", "plan", and "upload" / "download": the per-cell row transfers of setup,
- * the getters and hb_set_field, host copies included); returns 0 if the region exists. */
+ * "ridge_stats", "ridge_solve", "ridge_apply", "plan", "upload" / "download": the per-cell row transfers of setup,
+ * the getters and hb_set_field, host copies included, and "tuple_index": setup's covariate-tuple index, the upload
+ * of host labels and the host's O(J) part included); returns 0 if the region exists. */
 int hb_region_time(hb_handle* h, const char* region, double* ms, int64_t* launches);
 /* Enables per-region CUDA-event timing (adds synchronisation; off by default). */
 int hb_enable_timing(hb_handle* h, int on);
@@ -190,6 +195,11 @@ int hb_debug_widen(double* out, const float* in, int64_t n, int threads);
  * cells initialize_centroids chose (returns their number, 0 if the native initialisation has not run). */
 double hb_debug_kmeans_uniform(const hb_handle* h, uint64_t i, uint64_t g);
 int hb_debug_kmeans_cells(const hb_handle* h, int64_t* out);
+/* Test hook: the covariate-tuple index hb_setup built.  Returns J (the number of tuples; -1 before setup) and writes
+ * the non-null outputs: sort_perm (N_local values: the caller's cell at each tuple-sorted position), tuple_levels
+ * (J x C global levels, tuples in ascending mixed-radix order with covariate 0 most significant) and tuple_start
+ * (J + 1 values: the first sorted position of each tuple, then N_local). */
+int hb_debug_tuple_index(const hb_handle* h, int32_t* sort_perm, int32_t* tuple_levels, int64_t* tuple_start);
 /* Test hook (host only): ring geometry of the persistent update_R kernel for rows of KS floats:
  * out = {float4 per lane, row groups per warp ring (a power of two), rows per group, shared-memory bytes, warps per
  * CTA, 0, 0, 0, 0}.  Returns 1 if the shape is supported, 0 if the library would use the other update kernels. */
