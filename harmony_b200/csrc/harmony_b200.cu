@@ -2246,6 +2246,8 @@ int hb_cluster(hb_handle* h, const int64_t* update_orders) {
     CK(cudaMemcpyAsync(h->perms_d.p, update_orders, sizeof(int64_t) * cnt, cudaMemcpyHostToDevice, h->stream));
   }
   if (h->abort_cb && h->abort_cb(h->abort_user)) return -1;  // Progress::check_abort (:233)
+  // the call's first native round: a prebuilt plan drew its rounds from here on
+  const uint64_t first_round = h->plan->round_counter - (h->plan->next_ready ? (uint64_t)h->plan->next_T : 0);
   unsigned iter = 0;
   if (call.update == UpdatePath::PerStep) {
     TRY(plan_discard(h));  // a plan prebuilt by an earlier call is not used here
@@ -2294,6 +2296,9 @@ int hb_cluster(hb_handle* h, const int64_t* update_orders) {
       t0 = t1;
     }
   }
+  // the reference draws one shuffle per executed update_R (:268): rounds drawn but not run, after an early stop or in
+  // an adopted plan longer than the call, go back to the counter, so the orders do not depend on the update path
+  if (!update_orders) h->plan->round_counter = first_round + iter;
   if (call.update != UpdatePath::PerStep && !update_orders && T > 0 && !h->timing)
     TRY(plan_prebuild(h, (int)T));  // the next call's plan, while this call's correction and the next assignment run
   if (T > 0) h->R_user_set = false;
@@ -2455,11 +2460,29 @@ int hb_set_field(hb_handle* h, int field, const double* in) {
     case HB_O: return upload_table(h, in, h->O.p);
     case HB_E: return upload_table(h, in, h->E.p);
     case HB_THETA: return upload_small(h, in, B, h->theta.p);
-    case HB_SIGMA:
+    case HB_SIGMA: {
+      for (int k = 0; k < K; ++k)
+        if (!(std::isfinite(in[k]) && (float)in[k] > 0.f))
+          return fail(h, 2, "sigma[%d] = %g: sigma must be finite and positive", k, in[k]);
+      if (h->ran_init) {
+        // U holds -dist / sigma_old (the reference keeps dist_mat and divides by the current sigma in every update_R and
+        // compute_objective, harmony.cpp:158-162, 318-319): rescale column k by sigma_old[k] / sigma_new[k]
+        std::vector<double> old(K);
+        TRY(download_small(h, h->sigma.p, K, old.data()));
+        std::vector<double> ratio(K);
+        for (int k = 0; k < K; ++k) ratio[k] = old[k] / (double)(float)in[k];
+        DevBuf<float> s;
+        CK(s.alloc(K));
+        TRY(upload_small(h, ratio.data(), K, s.p));
+        k_scale_cols<<<grid_for(h->n * K, 256, h->num_sms * 8), 256, 0, h->stream>>>(h->U.p, s.p, h->n, K, h->KS);
+        CKL();
+        CK(cudaStreamSynchronize(h->stream));
+      }
       h->sigma0 = (float)in[0];
       h->sigma_uniform = true;
       for (int k = 1; k < K; ++k) h->sigma_uniform = h->sigma_uniform && ((float)in[k] == (float)in[0]);
       return upload_small(h, in, K, h->sigma.p);
+    }
     case HB_LAMBDA_VEC:
       h->lambda_estimation = false;
       return upload_small(h, in, B + 1, h->lambda.p);

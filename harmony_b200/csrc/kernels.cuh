@@ -51,6 +51,12 @@ __global__ void k_expand(const float* __restrict__ src, float* __restrict__ out,
   int idx = blockIdx.x * blockDim.x + threadIdx.x;
   if (idx < rows * cols) out[(idx / cols) * ld + (idx % cols)] = src[idx];
 }
+// X[i][k] *= s[k] for the first `cols` columns of the rows of X[n][ld] (U = -dist / sigma after a write of sigma)
+__global__ void k_scale_cols(float* __restrict__ X, const float* __restrict__ s, int64_t n, int cols, int ld) {
+  const int64_t total = n * cols;
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x)
+    X[(i / cols) * ld + i % cols] *= s[i % cols];
+}
 
 // arma::normalise(X, 2, 0) on the rows of X[n][d] (= columns of the reference's d x N matrix); a zero
 // norm divides by 1; rows too small or too large for a plain fp32 sum of squares are rescaled first.  One warp per

@@ -327,7 +327,7 @@ struct Plan {
   DevBuf<unsigned long long> scan_state;  // state of the chained scans
   int nchunks = 0;                        // chunks: <= CHUNK consecutive cells of one tuple, + a trailing empty one
   DevBuf<int> chunk_start, chunk_q0, chunk_nq, tuple_chunk0;
-  uint64_t round_counter = 0;  // native rounds drawn since the seed was set (a round's key: seed, counter)
+  uint64_t round_counter = 0;  // native rounds run since the seed was set, plus any prebuilt (a round's key: seed, counter)
   int set = 0;                 // set of the running cluster_cpp call
   bool next_ready = false;     // the other set holds a prebuilt native plan of next_T rounds
   int next_T = 0;
@@ -475,7 +475,7 @@ int build_plans(hb_handle* h, int T, const int64_t* orders_d, int set, cudaStrea
         h->N_global, h->cell_offset, n, h->sort_perm.p, h->cpb, h->nb, h->half_bits, h->seed, p.round_counter, blk_of);
   }
   CKL();
-  p.round_counter += (uint64_t)T;
+  if (!orders_d) p.round_counter += (uint64_t)T;  // injected orders take no native rounds
   for (int t = 0; t < T; t += p.batch) TRY(plan_sort(h, t, std::min(p.batch, T - t), t + p.batch < T, set, st));
   const PlanRound0 r = plan_round0(h, set);
   int* base = step ? p.tile_base.p : p.pt_base.p + (size_t)set * (S + 1);

@@ -315,7 +315,12 @@ class harmony:
             self._check(self._L.hb_set_field(self._h, FIELD[f], _ptr(v)))
             return
         if name in ("theta", "sigma", "lambda_"):
-            v = np.ascontiguousarray(value, dtype=np.float64)
+            v = np.ascontiguousarray(value, dtype=np.float64).ravel()
+            n = {"theta": self._scalar("B"), "sigma": self._scalar("K"), "lambda_": self._scalar("B") + 1}[name]
+            if name == "sigma" and v.size == 1:
+                v = np.full(n, v[0])   # a scalar sigma is broadcast to the K clusters, as in setup
+            if v.size != n:
+                raise ValueError(f"{name} must have {n} values, got {v.size}")
             self._check(self._L.hb_set_field(self._h, FIELD["lambda" if name == "lambda_" else name], _ptr(v)))
             return
         raise AttributeError(f"field {name} is not writable")

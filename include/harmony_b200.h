@@ -137,7 +137,10 @@ int hb_get_field(hb_handle* h, int field, double* out);
  * field, an unknown dtype or ld < cols. */
 int hb_get_field_device(hb_handle* h, int field, void* out, int dtype, int64_t ld, void* stream);
 /* Writable fields (the Rcpp module's .field() members are read-write): HB_Y, HB_R, HB_O, HB_E,
- * HB_THETA, HB_SIGMA, HB_LAMBDA_VEC, HB_Z_CORR. */
+ * HB_THETA, HB_SIGMA, HB_LAMBDA_VEC, HB_Z_CORR.  `in` holds hb_field_size(h, field) values.
+ * A written HB_SIGMA takes effect at the next update_R and compute_objective, as in the reference, which keeps the
+ * distances and divides by the current sigma (harmony.cpp:158-162, 318-319): the distances of the last assignment are
+ * kept, divided by the new sigma.  Status 2 if a sigma value is not finite or not positive. */
 int hb_set_field(hb_handle* h, int field, const double* in);
 
 enum hb_scalar { HB_N = 0, HB_B = 1, HB_K = 2, HB_D = 3, HB_C = 4, HB_ALPHA = 5, HB_MAX_ITER_KMEANS = 6,

@@ -800,8 +800,9 @@ int ho_get(void* hv, int field, double* out) {
   return 0;
 }
 
-// writable fields (same ids and layouts as ho_get): 2 R, 3 Y, 4 O, 5 E.  Lets a test plant the state a step starts
-// from, like the `.field<-` writes of the reference's Rcpp module.
+// writable fields (same ids and layouts as ho_get): 2 R, 3 Y, 4 O, 5 E, 8 theta, 9 sigma.  Lets a test plant the
+// state a step starts from, like the `.field<-` writes of the reference's Rcpp module (a written sigma divides the
+// kept dist_mat in the next update_R and compute_objective).
 int ho_set(void* hv, int field, const double* in) {
   Handle* h = (Handle*)hv;
 #define SET(obj)                                \
@@ -810,6 +811,8 @@ int ho_set(void* hv, int field, const double* in) {
     case 3: copy_in(obj->Y, in); break;         \
     case 4: copy_in(obj->O, in); break;         \
     case 5: copy_in(obj->E, in); break;         \
+    case 8: copy_in(obj->theta, in); break;     \
+    case 9: copy_in(obj->sigma, in); break;     \
     default: return 1;                          \
   }
   if (h->use_double) {

@@ -167,8 +167,9 @@ class OracleHarmony:
         return out
 
     def set(self, name, value):
-        """Write R [N, K], Y [K, d], O or E [B, K] (the layouts get() returns)."""
-        shapes = {"R": (self.N, self.K), "Y": (self.K, self.d), "O": (self.B, self.K), "E": (self.B, self.K)}
+        """Write R [N, K], Y [K, d], O or E [B, K], theta [B] or sigma [K] (the layouts get() returns)."""
+        shapes = {"R": (self.N, self.K), "Y": (self.K, self.d), "O": (self.B, self.K), "E": (self.B, self.K),
+                  "theta": (self.B,), "sigma": (self.K,)}
         v = np.ascontiguousarray(value, dtype=np.float64)
         assert v.shape == shapes[name], (name, v.shape)
         self._check(self.L.ho_set(self.h, FIELDS[name], _ptr(v)))

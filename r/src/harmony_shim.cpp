@@ -8,6 +8,7 @@
 // Build (on a machine with R): R CMD SHLIB harmony_shim.cpp -I../../include -L<libdir> -lharmony_b200
 // and keep R/harmony-package.R's `loadModule("harmony_module", TRUE)` unchanged.
 #include <Rcpp.h>
+#include <string>
 #include <vector>
 #include "harmony_b200.h"
 
@@ -90,9 +91,9 @@ class harmony {
   void set_R(NumericMatrix m) { hb_check(h_, hb_set_field(h_, HB_R, m.begin())); }
   void set_O(NumericMatrix m) { hb_check(h_, hb_set_field(h_, HB_O, m.begin())); }
   void set_E(NumericMatrix m) { hb_check(h_, hb_set_field(h_, HB_E, m.begin())); }
-  void set_theta(NumericVector v) { hb_check(h_, hb_set_field(h_, HB_THETA, v.begin())); }
-  void set_sigma(NumericVector v) { hb_check(h_, hb_set_field(h_, HB_SIGMA, v.begin())); }
-  void set_lambda(NumericVector v) { hb_check(h_, hb_set_field(h_, HB_LAMBDA_VEC, v.begin())); }
+  void set_theta(NumericVector v) { set_vec(HB_THETA, v, dim(HB_B), "theta"); }
+  void set_sigma(NumericVector v) { set_vec(HB_SIGMA, v, dim(HB_K), "sigma"); }
+  void set_lambda(NumericVector v) { set_vec(HB_LAMBDA_VEC, v, dim(HB_B) + 1, "lambda"); }
   std::vector<double> trace(int id) {
     int64_t n = hb_trace(h_, id, nullptr, 0);
     std::vector<double> v(n > 0 ? n : 0);
@@ -112,6 +113,14 @@ class harmony {
     return 0;
   }
   int dim(int which) { double v = 0; hb_get_scalar(h_, which, &v); return (int)v; }
+  // the library reads exactly n values
+  void set_vec(int field, NumericVector& v, int n, const char* name) {
+    if (v.size() != n) {
+      const std::string msg = std::string(name) + " must have " + std::to_string(n) + " values, got " + std::to_string(v.size());
+      Rcpp::stop("%s", msg.c_str());
+    }
+    hb_check(h_, hb_set_field(h_, field, v.begin()));
+  }
   NumericMatrix mat(int field, int nr, int nc) {
     NumericMatrix m(nr, nc);                                            // column-major doubles: the ABI's layout
     hb_check(h_, hb_get_field(h_, field, m.begin()));

@@ -13,9 +13,9 @@ import pytest
 
 from harmony_b200 import _lib
 from helpers import make_perms, rel_l2
-from test_gpu_kernel_edges import (ALPHA, BLOCK, CUTOFF, NB, SIGMA, T, TOL_OBJ, TOL_OE, TOL_R, TOL_R1, TOL_Y,
-                                   TOL_Y_FIXED, TOL_Z, TOL_ZN, _launches, _nested, _obj_err, _one_cov, _set_zcorr,
-                                   _sizes, _table_err, f32, kernel_paths, make_Y0, numpy_model, planted_R, tables_of)
+from stages import (ALPHA, BLOCK, CUTOFF, NB, SIGMA, T, TOL_OBJ, TOL_OE, TOL_R, TOL_R1, TOL_Y, TOL_Y_FIXED, TOL_Z,
+                    TOL_ZN, _launches, _mix64, _nested, _obj_err, _one_cov, _set_zcorr, _sizes, _table_err, f32,
+                    kernel_paths, make_Y0, native_order, numpy_model, planted_R, tables_of)
 
 PER_STEP, TWO_PASS, SINGLE_PASS = 0, 1, 2
 HB_KS_WIDE = 16
@@ -377,47 +377,6 @@ def test_parity_d300_K100():
 
 
 # ---- RunHarmony on a CUDA tensor against the oracles, with the library's native update orders replayed ----------------
-_M64 = (1 << 64) - 1
-
-
-def _mix64(x):
-    """hb_mix64 (common.cuh) on uint64 arrays."""
-    with np.errstate(over="ignore"):
-        x = x + np.uint64(0x9E3779B97F4A7C15)
-        x = (x ^ (x >> np.uint64(30))) * np.uint64(0xBF58476D1CE4E5B9)
-        x = (x ^ (x >> np.uint64(27))) * np.uint64(0x94D049BB133111EB)
-        return x ^ (x >> np.uint64(31))
-
-
-def _half_bits(n):
-    bits = 1
-    while (1 << bits) < n:
-        bits += 1
-    return (bits + 1) // 2
-
-
-def native_order(n, seed, round_counter):
-    """Cells in update order of a native round (plan.cuh: key = plan_round_key(seed, counter), the cell at position p is
-    hb_permute_inv(p)): the Feistel network of common.cuh, inverted, with cycle walking, in numpy."""
-    key = int(_mix64(np.array([seed ^ int(_mix64(np.array([round_counter + 0x1234567], dtype=np.uint64))[0])],
-                              dtype=np.uint64))[0])
-    hb = _half_bits(n)
-    mask = np.uint64((1 << hb) - 1)
-    rk = [np.uint64((key + 0x632BE59BD9B4E019 * (r + 1)) & _M64) for r in range(6)]
-    x = np.arange(n, dtype=np.uint64)
-    todo = np.ones(n, dtype=bool)
-    while todo.any():
-        v = x[todo]
-        l, r = v >> np.uint64(hb), v & mask
-        for rnd in range(5, -1, -1):
-            f = _mix64(l ^ rk[rnd]) & mask
-            l, r = r ^ f, l
-        v = (l << np.uint64(hb)) | r
-        x[todo] = v
-        todo[todo] = v >= np.uint64(n)
-    return x.astype(np.int64)
-
-
 def test_native_order_replay_matches_the_library():
     """native_order restates hb_permute_inv exactly (checked through hb_debug_permute, host only)."""
     L = _lib.lib()
