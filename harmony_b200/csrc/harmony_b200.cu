@@ -208,35 +208,28 @@ int my_ceil(float num) {
 }
 
 // ---- kernel selection --------------------------------------------------------------------------------------
-// update_R runs the single-pass persistent kernel (update_single_pass.cuh) when every CTA's slice of a block can lie
-// inside one covariate tuple (2 J <= #SMs), its ring fits shared memory and n KS < 2^32; else the two-pass
-// persistent kernel (update_two_pass.cuh) when KS <= 256, J <= 8192 and its buffers fit shared memory; else three
-// launches per block step (update_per_step.cuh).
-enum class UpdatePath { PerStep, TwoPass, SinglePass };
-
-// Contractions that run on the tensor cores (wgmma); the others run the FFMA kernels of kernels.cuh.
-struct Contractions {
-  int k1_stages = 0;    // operand stages (1, 2) of the fused assignment kernel (assign_tc3.cuh); 0: not fused
-  bool logits = false;  // plan-order assignment of shapes the fused kernel cannot hold: logits_tc.cuh + softmax pass
-  bool apply = false;   // ridge apply (apply_tc3.cuh)
-  bool kmeans = false;  // native k-means initialisation from logits with sigma = 1 (logits_tc.cuh)
-};
-
-// Kernels of the shapes past the FFMA kernels' limits (or of every shape under HB_KS_WIDE); each is taken only where
-// the kernel that serves the stage otherwise does not fit (assign_ffma_fits, apply_ffma_fits, kmeans_ffma_fits).
-struct WidePaths {
-  bool assign = false;  // natural-order assignment: logits + k_softmax_tiles instead of FFMA k_assign
-  bool cold = false;    // plan-order cold start from logits + k_softmax_block_sums where k_logits_tc does not fit
-  bool logits = false;  // the logits of these paths come from k_logits_wide (d-chunked) instead of k_logits_tc
-  bool apply = false;   // ridge apply over column ranges (k_apply_tc_cols) instead of FFMA k_ridge_apply
-  bool kmeans = false;  // native k-means initialisation from logits with up to 8 pieces per lane instead of FFMA
-};
+// One kernel per stage, chosen by select_kernels.  The values of UpdatePath are hb_debug_kernel_paths' numbers, those
+// of Assign, ColdStart and Apply hb_debug_wide_paths'.
+enum class UpdatePath { PerStep = 0, TwoPass = 1, SinglePass = 2 };
+// assignment in natural order (init, legacy centroid step, cold start of the calls that do not run it in plan order):
+// fused wgmma (assign_tc3.cuh), FFMA k_assign, or logits (logits_tc.cuh / logits_wide.cuh) + k_softmax_tiles
+enum class Assign { FusedTc = 1, Ffma = 2, LogitsTc = 3, LogitsWide = 4 };
+// cold-start assignment in the order of round 0 of the plan: fused wgmma, or logits + k_softmax_block_sums;
+// None: no kernel for the shape, the cold start runs in natural order
+enum class ColdStart { None = 0, FusedTc = 1, LogitsTc = 2, LogitsWide = 3 };
+// ridge apply: wgmma k_apply_tc (one column range), FFMA k_ridge_apply, or k_apply_tc_cols over 128-column ranges
+enum class Apply { Tc = 1, Ffma = 2, TcCols = 3 };
+// native k-means initialisation: FFMA race and Lloyd steps, or both from logits with sigma = 1
+enum class KmeansInit { Ffma, LogitsTc, LogitsWide };
 
 struct KernelPaths {
   UpdatePath update = UpdatePath::PerStep;
   bool tuple_ranges = false;  // 2 J <= #SMs: the plan gives every CTA a slice of a block inside one tuple
-  Contractions mm;
-  WidePaths wide;
+  int k1_stages = 0;          // operand stages (1, 2) of the fused assignment kernel; 0: not fused
+  Assign assign = Assign::Ffma;
+  ColdStart cold = ColdStart::None;
+  Apply apply = Apply::Ffma;
+  KmeansInit kmeans = KmeansInit::Ffma;
 };
 
 int two_pass_nv(int KS) {
@@ -252,6 +245,15 @@ size_t two_pass_smem_bytes(int KS, int nb, int J) {
 }
 
 // The kernels of a shape (n: local cells, nb: update blocks); kernel_set: the HB_KS_* bits of the test hook.
+// update_R runs the single-pass persistent kernel (update_single_pass.cuh) when every CTA's slice of a block can lie
+// inside one covariate tuple (2 J <= #SMs), its ring fits shared memory and n KS < 2^32; else the two-pass
+// persistent kernel (update_two_pass.cuh) when KS <= 256, J <= 8192 and its buffers fit shared memory; else three
+// launches per block step (update_per_step.cuh).
+// The other stages take their wgmma kernel where it fits, else their FFMA kernel where it fits (assign_ffma_fits,
+// apply_ffma_fits, kmeans_ffma_fits), else the kernel of the wide shapes.  HB_KS_FFMA_CONTRACTIONS rules out the
+// wgmma kernels, HB_KS_WIDE the wgmma and FFMA ones.  A stage that runs from logits takes k_logits_tc where it fits
+// (not under HB_KS_WIDE), else the d-chunked k_logits_wide.  The plan-order cold start has no FFMA kernel: it runs
+// from logits where k_logits_tc is among the wgmma kernels or the natural-order assignment runs from logits.
 KernelPaths select_kernels(int K, int d, int J, int64_t n, int nb, int num_sms, int kernel_set) {
   const int KS = (K + 3) & ~3, KD = (d + 7) & ~7, NP = (K + 15) & ~15;
   KernelPaths p;
@@ -263,20 +265,28 @@ KernelPaths select_kernels(int K, int d, int J, int64_t n, int nb, int num_sms, 
     p.update = UpdatePath::SinglePass;
   else if (KS <= 256 && J <= 8192 && two_pass_smem_bytes(KS, nb, J) <= SMEM_LIMIT)
     p.update = UpdatePath::TwoPass;
-  if (!(kernel_set & (HB_KS_FFMA_CONTRACTIONS | HB_KS_WIDE))) {
-    const int ns = assign3_smem_bytes(2, KD, NP, KS) <= SMEM_LIMIT ? 2 : 1;
-    if (d <= 64 && K <= 128 && assign3_smem_bytes(ns, KD, NP, KS) <= SMEM_LIMIT) p.mm.k1_stages = ns;
-    const bool logits_fit = logits_tc_fits(d);
-    p.mm.logits = p.mm.k1_stages == 0 && logits_fit;
-    p.mm.apply = apply_tc_fits(d);  // cluster ranges of <= AP_MAXK per launch
-    p.mm.kmeans = logits_fit && KS <= 256;
-  }
   const bool wide = kernel_set & HB_KS_WIDE;
-  p.wide.logits = wide || !logits_tc_fits(d);
-  p.wide.assign = p.mm.k1_stages == 0 && (wide || !assign_ffma_fits(K, d));
-  p.wide.cold = p.wide.assign && !p.mm.logits;
-  p.wide.apply = !p.mm.apply && (wide || !apply_ffma_fits(K, d));
-  p.wide.kmeans = !p.mm.kmeans && (wide || !kmeans_ffma_fits(K, d));
+  const bool tc = !(kernel_set & (HB_KS_FFMA_CONTRACTIONS | HB_KS_WIDE));
+  const bool logits_tc = !wide && logits_tc_fits(d);
+  if (tc) {
+    const int ns = assign3_smem_bytes(2, KD, NP, KS) <= SMEM_LIMIT ? 2 : 1;
+    if (d <= 64 && K <= 128 && assign3_smem_bytes(ns, KD, NP, KS) <= SMEM_LIMIT) p.k1_stages = ns;
+  }
+  if (p.k1_stages) {
+    p.assign = Assign::FusedTc;
+    p.cold = ColdStart::FusedTc;
+  } else {
+    if (wide || !assign_ffma_fits(K, d)) p.assign = logits_tc ? Assign::LogitsTc : Assign::LogitsWide;
+    if ((tc && logits_tc) || p.assign != Assign::Ffma) p.cold = logits_tc ? ColdStart::LogitsTc : ColdStart::LogitsWide;
+  }
+  if (tc && apply_tc_fits(d))
+    p.apply = Apply::Tc;  // cluster ranges of <= AP_MAXK per launch
+  else if (wide || !apply_ffma_fits(K, d))
+    p.apply = Apply::TcCols;
+  if (tc && logits_tc && KS <= 256)
+    p.kmeans = KmeansInit::LogitsTc;
+  else if (wide || !kmeans_ffma_fits(K, d))
+    p.kmeans = logits_tc ? KmeansInit::LogitsTc : KmeansInit::LogitsWide;
   return p;
 }
 
@@ -291,7 +301,7 @@ struct CallPath {
 CallPath call_path(const KernelPaths& p, unsigned T, bool legacy_centroid) {
   CallPath c{p.update, false};
   if (legacy_centroid || (p.update == UpdatePath::TwoPass && T > 31)) c.update = UpdatePath::PerStep;
-  c.plan_order_assign = c.update == UpdatePath::SinglePass && (p.mm.k1_stages > 0 || p.mm.logits || p.wide.cold) && T > 0;
+  c.plan_order_assign = c.update == UpdatePath::SinglePass && p.cold != ColdStart::None && T > 0;
   return c;
 }
 
@@ -456,9 +466,9 @@ int fail(hb_handle* h, int code, const char* fmt, ...) {
     cudaError_t e__ = cudaGetLastError();                                                          \
     if (e__ != cudaSuccess) return fail(h, 10, "kernel launch failed: %s at %s:%d", cudaGetErrorString(e__), __FILE__, __LINE__); \
   } while (0)
-#define TRY(expr)            \
+#define TRY(...)             \
   do {                       \
-    int st__ = (expr);       \
+    int st__ = (__VA_ARGS__); \
     if (st__ != 0) return st__; \
   } while (0)
 
@@ -514,18 +524,16 @@ int kq_for(int K) {
   return kq;
 }
 
-template <typename F>
-int dispatch_kq(hb_handle* h, int K, F&& f) {
-  switch (kq_for(K)) {
-    case 1: return f(std::integral_constant<int, 1>());
-    case 2: return f(std::integral_constant<int, 2>());
-    case 4: return f(std::integral_constant<int, 4>());
-    case 8: return f(std::integral_constant<int, 8>());
-    case 16: return f(std::integral_constant<int, 16>());
-    case 32: return f(std::integral_constant<int, 32>());
-  }
-  return fail(h, 2, "K = %d is not supported (K <= 1024)", K);
+// Run-time value -> template argument: f(std::integral_constant<int, V>()) for the V of the list equal to v, whose
+// status it returns; `unsupported` (formatted with K) when the list has no such V.
+template <int... Vs, typename F>
+int dispatch(hb_handle* h, int v, const char* unsupported, F&& f) {
+  int st = 0;
+  if (((v == Vs && ((st = f(std::integral_constant<int, Vs>())), true)) || ...)) return st;
+  return fail(h, 2, unsupported, h->K);
 }
+constexpr const char* kUnsupportedK = "K = %d is not supported (K <= 1024)";
+constexpr const char* kUnsupportedUpdateK = "K = %d is not supported by the persistent update kernel";
 
 // U[i][k] = (2 / sigma_k) (z_i . y_k / |z_i| - 1) for all clusters on the tensor cores, 128 clusters per launch and d
 // in chunks (logits_wide.cuh), after one pass that pads Y
@@ -557,9 +565,9 @@ int launch_logits_wide(hb_handle* h, const float* sigma, bool normalise) {
 }
 
 // U[i][k] = (2 / sigma_k) (z_i . y_k / |z_i| - 1) for all clusters on the tensor cores, 64 clusters per launch
-// (logits_tc.cuh), or from launch_logits_wide where the paths of the wide shapes use it; `sigma`: device array of K values
-int launch_logits(hb_handle* h, const float* sigma, bool normalise) {
-  if (h->paths.wide.logits) return launch_logits_wide(h, sigma, normalise);
+// (logits_tc.cuh), or from launch_logits_wide when `wide`; `sigma`: device array of K values
+int launch_logits(hb_handle* h, const float* sigma, bool normalise, bool wide) {
+  if (wide) return launch_logits_wide(h, sigma, normalise);
   LogitsArgs t{};
   t.Zc = h->Zc.p;
   t.Y = h->Y.p;
@@ -589,180 +597,171 @@ int launch_logits(hb_handle* h, const float* sigma, bool normalise) {
 
 namespace {
 
-// ---- K1 launcher: assignment from centroids (init + cold start) -------------------------------
-// plan_mode: tiles follow round 0 of the current plan set (tensor-core kernel only); want_obj: objective sums (init)
-int run_assign(hb_handle* h, bool normalise, bool plan_mode = false, bool want_obj = true) {
+// ---- K1 launchers: assignment from centroids (init + cold start) -------------------------------
+// the fused kernel (assign_tc3.cuh) over the tiles, R / Z_corr outputs and accumulators the caller set in t
+int launch_assign_tc3(hb_handle* h, Assign3Args& t, int grid, bool normalise, bool want_obj) {
+  t.Zc = h->Zc.p;
+  t.Y = h->Y.p;
+  t.sigma = h->sigma.p;
+  t.U = h->U.p;
+  t.tuple_levels = h->tuple_levels.p;
+  t.obj_acc = h->obj_acc.p;
+  t.d = h->d;
+  t.K = h->K;
+  t.C = h->C;
+  t.B = h->B;
+  t.DS = h->DS;
+  t.KS = h->KS;
+  t.KD = (h->d + 7) & ~7;
+  t.NP = (h->K + 15) & ~15;
+  t.SS = assign3_stage_stride(h->KS);
+  t.ns = h->paths.k1_stages;
+  t.normalise = normalise ? 1 : 0;
+  t.want_obj = want_obj ? 1 : 0;
+  const size_t smem = assign3_smem_bytes(t.ns, t.KD, t.NP, t.KS);
+  if (want_obj) {
+    CK(cudaFuncSetAttribute(k_assign_tc3<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    k_assign_tc3<true><<<grid, A3_THREADS, smem, h->stream>>>(t);
+  } else {
+    CK(cudaFuncSetAttribute(k_assign_tc3<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    k_assign_tc3<false><<<grid, A3_THREADS, smem, h->stream>>>(t);
+  }
+  CKL();
+  return 0;
+}
+
+// natural order: R, the per-tile sums of O and of the row sums, then O and E; want_obj: objective sums (init)
+int run_assign(hb_handle* h, bool normalise, bool want_obj) {
   RegionScope rs(h, "assign");
   const int K = h->K, d = h->d, B = h->B, KS = h->KS;
-  const int KP = (K + 63) & ~63;
+  float* O_acc = h->Oacc.p;
+  float* rs_acc = h->Oacc.p + (size_t)B * KS;
   CK(cudaMemsetAsync(h->Oacc.p, 0, sizeof(float) * ((size_t)B * KS + KS), h->stream));
-  AssignArgs a;
-  a.Zc = h->Zc.p;
-  a.Y = h->Y.p;
-  a.sigma = h->sigma.p;
-  a.U = h->U.p;
-  a.R = h->R.p;
-  a.tile_cell0 = h->tile_cell0.p;
-  a.tile_len = h->tile_len.p;
-  a.tile_tuple = h->tile_tuple.p;
-  a.tuple_levels = h->tuple_levels.p;
-  a.O_acc = h->Oacc.p;
-  a.rs_acc = h->Oacc.p + (size_t)B * KS;
-  a.obj_acc = h->obj_acc.p;
-  a.ntiles = h->ntiles;
-  a.d = d;
-  a.K = K;
-  a.C = h->C;
-  a.KP = KP;
-  a.DS = h->DS;
-  a.KS = KS;
-  a.normalise = normalise ? 1 : 0;
-  if (h->paths.mm.k1_stages) {
-    Assign3Args t{};
-    t.Zc = a.Zc;
-    t.Y = a.Y;
-    t.sigma = a.sigma;
-    t.U = a.U;
-    t.tuple_levels = a.tuple_levels;
-    t.obj_acc = a.obj_acc;
-    t.d = d;
-    t.K = K;
-    t.C = h->C;
-    t.B = B;
-    t.DS = h->DS;
-    t.KS = KS;
-    t.KD = (d + 7) & ~7;
-    t.NP = (K + 15) & ~15;
-    t.SS = assign3_stage_stride(KS);
-    t.ns = h->paths.mm.k1_stages;
-    t.normalise = a.normalise;
-    t.want_obj = want_obj ? 1 : 0;
-    int grid_tc;
-    if (plan_mode) {
-      // rows in the order of round 0 of the coming cluster_cpp call: a tile's column sums are a share of its block's
-      // removal sums and go to the update kernel's accumulator slots; R is not stored
-      const PlanRound0 r = plan_round0(h, h->plan->set);
-      t.R = nullptr;
+  switch (h->paths.assign) {
+    case Assign::FusedTc: {
+      Assign3Args t{};
+      t.R = h->R.p;
+      t.tile_p0 = h->tc_cell0.p;
+      t.tile_len = h->tc_len.p;
+      t.tile_tuple = h->tc_tuple.p;
+      t.ntiles = h->tc_ntiles;
+      t.O_acc = O_acc;
+      t.rs_acc = rs_acc;
+      t.Zc_out = normalise ? h->Zc.p : nullptr;  // the compatibility paths read the normalised embedding back
+      TRY(launch_assign_tc3(h, t, std::max(1, std::min(h->tc_ntiles, h->num_sms)), normalise, want_obj));
+      break;
+    }
+    case Assign::LogitsTc:
+    case Assign::LogitsWide: {
+      // shapes whose FFMA k_assign does not fit: logits on the tensor cores, then the softmax over the natural-order tiles
+      TRY(launch_logits(h, h->sigma.p, normalise, h->paths.assign == Assign::LogitsWide));
+      const int nv = sp_nv(KS);
+      const size_t smem_sm = sizeof(float) * 8 * 128 * (size_t)nv;
+      const int grid = std::max(1, std::min(h->ntiles, h->num_sms * 8));
+      TRY(dispatch<1, 2, 4, 8>(h, nv, kUnsupportedK, [&](auto nvc) -> int {
+        constexpr int NV = decltype(nvc)::value;
+        k_softmax_tiles<NV><<<grid, 256, smem_sm, h->stream>>>(h->U.p, h->R.p, h->sigma.p, h->tile_cell0.p, h->tile_len.p,
+                                                               h->tile_tuple.p, h->tuple_levels.p, O_acc, rs_acc,
+                                                               h->obj_acc.p, h->ntiles, K, KS, h->C, want_obj ? 1 : 0);
+        CKL();
+        return 0;
+      }));
+      if (normalise) {  // the cold start leaves the normalised embedding in Z_corr (harmony.cpp:220)
+        k_normalise_rows<<<grid_for((int64_t)h->n * 32, 256, h->num_sms * 8), 256, 0, h->stream>>>(h->Zc.p, h->Zc.p, h->n, d, h->DS);
+        CKL();
+      }
+      break;
+    }
+    case Assign::Ffma: {
+      AssignArgs a;
+      a.Zc = h->Zc.p;
+      a.Y = h->Y.p;
+      a.sigma = h->sigma.p;
+      a.U = h->U.p;
+      a.R = h->R.p;
+      a.tile_cell0 = h->tile_cell0.p;
+      a.tile_len = h->tile_len.p;
+      a.tile_tuple = h->tile_tuple.p;
+      a.tuple_levels = h->tuple_levels.p;
+      a.O_acc = O_acc;
+      a.rs_acc = rs_acc;
+      a.obj_acc = h->obj_acc.p;
+      a.ntiles = h->ntiles;
+      a.d = d;
+      a.K = K;
+      a.C = h->C;
+      a.KP = (K + 63) & ~63;
+      a.DS = h->DS;
+      a.KS = KS;
+      a.normalise = normalise ? 1 : 0;
+      const size_t smem = assign_ffma_smem_bytes(K, d);
+      TRY(dispatch<1, 2, 4, 8, 16, 32>(h, kq_for(K), kUnsupportedK, [&](auto kq) -> int {
+        constexpr int KQ = decltype(kq)::value;
+        CK(cudaFuncSetAttribute(k_assign<KQ>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        int occ = 1;
+        CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k_assign<KQ>, ASSIGN_THREADS, smem));
+        if (occ < 1) occ = 1;
+        int grid = std::min(h->ntiles, h->num_sms * occ);
+        if (grid < 1) grid = 1;
+        k_assign<KQ><<<grid, ASSIGN_THREADS, smem, h->stream>>>(a);
+        CKL();
+        return 0;
+      }));
+      break;
+    }
+  }
+  h->R_user_set = false;
+  TRY(allreduce_f(h, h->Oacc.p, (size_t)B * KS + KS));
+  k_assign_finalize<<<(B * KS + 255) / 256, 256, 0, h->stream>>>(O_acc, rs_acc, h->Pr_b.p, h->O.p, h->E.p, B, K, KS);
+  CKL();
+  return 0;
+}
+
+// cold start in the order of round 0 of the coming cluster_cpp call, where call_path chose that order
+// (paths.cold != None): a tile's column sums are a share of its block's removal sums and go to the update kernel's
+// accumulator slots; R is not stored and the objective is not evaluated
+int run_assign_plan_order(hb_handle* h, bool normalise) {
+  RegionScope rs(h, "assign");
+  const int K = h->K, B = h->B, KS = h->KS;
+  const PlanRound0 r = plan_round0(h, h->plan->set);
+  switch (h->paths.cold) {
+    case ColdStart::FusedTc: {
+      Assign3Args t{};
       t.row_index = r.order;
       t.tile_p0 = r.tile_p0;
       t.tile_len = r.tile_len;
       t.tile_tuple = r.tile_tuple;
       t.tile_blk = r.tile_blk;
       t.ntiles_ptr = r.tile_count;
-      t.ntiles = 0;
       t.acc = h->acc2.p;
-      t.Zc_out = nullptr;
-      grid_tc = h->num_sms;
-    } else {
-      t.R = a.R;
-      t.row_index = nullptr;
-      t.tile_p0 = h->tc_cell0.p;
-      t.tile_len = h->tc_len.p;
-      t.tile_tuple = h->tc_tuple.p;
-      t.tile_blk = nullptr;
-      t.ntiles_ptr = nullptr;
-      t.ntiles = h->tc_ntiles;
-      t.O_acc = a.O_acc;
-      t.rs_acc = a.rs_acc;
-      t.Zc_out = normalise ? h->Zc.p : nullptr;  // the compatibility paths read the normalised embedding back
-      grid_tc = std::max(1, std::min(h->tc_ntiles, h->num_sms));
+      TRY(launch_assign_tc3(h, t, h->num_sms, normalise, false));
+      break;
     }
-    const size_t smem_tc = assign3_smem_bytes(t.ns, t.KD, t.NP, KS);
-    if (want_obj) {
-      CK(cudaFuncSetAttribute(k_assign_tc3<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_tc));
-      k_assign_tc3<true><<<grid_tc, A3_THREADS, smem_tc, h->stream>>>(t);
-    } else {
-      CK(cudaFuncSetAttribute(k_assign_tc3<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_tc));
-      k_assign_tc3<false><<<grid_tc, A3_THREADS, smem_tc, h->stream>>>(t);
+    case ColdStart::LogitsTc:
+    case ColdStart::LogitsWide: {
+      // shapes the fused kernel cannot hold (d > 64 or K > 128): logits on the tensor cores, then one gather pass over
+      // U in the order of round 0 for the softmax + the blocks' removal sums (harmony.cpp:312-313)
+      TRY(launch_logits(h, h->sigma.p, normalise, h->paths.cold == ColdStart::LogitsWide));
+      const int nv = sp_nv(KS);
+      const size_t smem_sm = sizeof(float) * 8 * 128 * (size_t)nv;
+      TRY(dispatch<1, 2>(h, nv, kUnsupportedUpdateK, [&](auto nvc) -> int {
+        constexpr int NV = decltype(nvc)::value;
+        k_softmax_block_sums<NV><<<dim3(h->coop_grid, h->nb), 256, smem_sm, h->stream>>>(
+            h->U.p, r.order, r.ranges, h->tuple_levels.p, h->acc2.p, h->coop_grid, K, KS, h->C, B);
+        CKL();
+        return 0;
+      }));
+      break;
     }
-    CKL();
-    h->R_user_set = false;
-    if (plan_mode) {
-      // O, E of the assignment = the sums of the blocks' removal terms (harmony.cpp:226-227)
-      const size_t XH = (size_t)B * KS + KS;
-      // sharded cells: the rem halves of slots 1 .. nb in ONE all-reduce (their add halves are still zero here)
-      if (h->world > 1) TRY(allreduce_f(h, h->acc2.p + 2 * XH, 2 * XH * (size_t)h->nb));
-      k_assign_finalize_plan<<<(B * KS + 255) / 256, 256, 0, h->stream>>>(h->acc2.p, h->nb, h->Pr_b.p, h->O.p, h->E.p, B, K, KS);
-      CKL();
-      h->zc_pending_norm = normalise;  // the normalised embedding (harmony.cpp:220) is materialised on demand
-      return 0;
-    }
-    TRY(allreduce_f(h, h->Oacc.p, (size_t)B * KS + KS));
-    k_assign_finalize<<<(B * KS + 255) / 256, 256, 0, h->stream>>>(h->Oacc.p, h->Oacc.p + (size_t)B * KS, h->Pr_b.p,
-                                                                    h->O.p, h->E.p, B, K, KS);
-    CKL();
-    return 0;
   }
-  if (plan_mode && (h->paths.mm.logits || h->paths.wide.cold)) {
-    // shapes the fused kernel cannot hold (d > 64 or K > 128): logits per 64-cluster range on the tensor cores, then
-    // one gather pass over U in the order of round 0 for the softmax + the blocks' removal sums (harmony.cpp:312-313)
-    TRY(launch_logits(h, h->sigma.p, normalise));
-    const PlanRound0 r = plan_round0(h, h->plan->set);
-    const int nv = sp_nv(KS);
-    const size_t smem_sm = sizeof(float) * 8 * 128 * (size_t)nv;
-    if (nv == 1)
-      k_softmax_block_sums<1><<<dim3(h->coop_grid, h->nb), 256, smem_sm, h->stream>>>(
-          h->U.p, r.order, r.ranges, h->tuple_levels.p, h->acc2.p, h->coop_grid, K, KS, h->C, B);
-    else
-      k_softmax_block_sums<2><<<dim3(h->coop_grid, h->nb), 256, smem_sm, h->stream>>>(
-          h->U.p, r.order, r.ranges, h->tuple_levels.p, h->acc2.p, h->coop_grid, K, KS, h->C, B);
-    CKL();
-    h->R_user_set = false;
-    const size_t XH = (size_t)B * KS + KS;
-    if (h->world > 1) TRY(allreduce_f(h, h->acc2.p + 2 * XH, 2 * XH * (size_t)h->nb));
-    k_assign_finalize_plan<<<(B * KS + 255) / 256, 256, 0, h->stream>>>(h->acc2.p, h->nb, h->Pr_b.p, h->O.p, h->E.p, B, K, KS);
-    CKL();
-    h->zc_pending_norm = normalise;
-    return 0;
-  }
-  if (plan_mode) return fail(h, 3, "internal: plan-order assignment without the tensor-core kernel");
-  if (h->paths.wide.assign) {
-    // shapes whose FFMA k_assign does not fit: logits on the tensor cores, then the softmax over the natural-order tiles
-    TRY(launch_logits(h, h->sigma.p, normalise));
-    const int nv = sp_nv(KS);
-    const size_t smem_sm = sizeof(float) * 8 * 128 * (size_t)nv;
-    const int grid = std::max(1, std::min(h->ntiles, h->num_sms * 8));
-    auto go = [&](auto nvc) {
-      constexpr int NV = decltype(nvc)::value;
-      k_softmax_tiles<NV><<<grid, 256, smem_sm, h->stream>>>(h->U.p, h->R.p, h->sigma.p, h->tile_cell0.p, h->tile_len.p,
-                                                             h->tile_tuple.p, h->tuple_levels.p, a.O_acc, a.rs_acc,
-                                                             h->obj_acc.p, h->ntiles, K, KS, h->C, want_obj ? 1 : 0);
-    };
-    if (nv == 1) go(std::integral_constant<int, 1>());
-    else if (nv == 2) go(std::integral_constant<int, 2>());
-    else if (nv == 4) go(std::integral_constant<int, 4>());
-    else go(std::integral_constant<int, 8>());
-    CKL();
-    if (normalise) {  // the cold start leaves the normalised embedding in Z_corr (harmony.cpp:220)
-      k_normalise_rows<<<grid_for((int64_t)h->n * 32, 256, h->num_sms * 8), 256, 0, h->stream>>>(h->Zc.p, h->Zc.p, h->n, d, h->DS);
-      CKL();
-    }
-    h->R_user_set = false;
-    TRY(allreduce_f(h, h->Oacc.p, (size_t)B * KS + KS));
-    k_assign_finalize<<<(B * KS + 255) / 256, 256, 0, h->stream>>>(h->Oacc.p, h->Oacc.p + (size_t)B * KS, h->Pr_b.p,
-                                                                    h->O.p, h->E.p, B, K, KS);
-    CKL();
-    return 0;
-  }
-  const size_t smem = assign_ffma_smem_bytes(K, d);
-  int st = dispatch_kq(h, K, [&](auto kq) -> int {
-    constexpr int KQ = decltype(kq)::value;
-    CK(cudaFuncSetAttribute(k_assign<KQ>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    int occ = 1;
-    CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k_assign<KQ>, ASSIGN_THREADS, smem));
-    if (occ < 1) occ = 1;
-    int grid = std::min(h->ntiles, h->num_sms * occ);
-    if (grid < 1) grid = 1;
-    k_assign<KQ><<<grid, ASSIGN_THREADS, smem, h->stream>>>(a);
-    CKL();
-    return 0;
-  });
-  TRY(st);
   h->R_user_set = false;
-  TRY(allreduce_f(h, h->Oacc.p, (size_t)B * KS + KS));
-  k_assign_finalize<<<(B * KS + 255) / 256, 256, 0, h->stream>>>(h->Oacc.p, h->Oacc.p + (size_t)B * KS, h->Pr_b.p,
-                                                                  h->O.p, h->E.p, B, K, KS);
+  // O, E of the assignment = the sums of the blocks' removal terms (harmony.cpp:226-227)
+  const size_t XH = (size_t)B * KS + KS;
+  // sharded cells: the rem halves of slots 1 .. nb in ONE all-reduce (their add halves are still zero here)
+  if (h->world > 1) TRY(allreduce_f(h, h->acc2.p + 2 * XH, 2 * XH * (size_t)h->nb));
+  k_assign_finalize_plan<<<(B * KS + 255) / 256, 256, 0, h->stream>>>(h->acc2.p, h->nb, h->Pr_b.p, h->O.p, h->E.p, B, K, KS);
   CKL();
+  h->zc_pending_norm = normalise;  // the normalised embedding (harmony.cpp:220) is materialised on demand
   return 0;
 }
 
@@ -860,7 +859,7 @@ int run_update_per_step(hb_handle* h) {
   const int grid = std::max(1, tiles_bound);
   const size_t sm_col = sizeof(float) * (size_t)NWARP * KP;
   const size_t sm_upd = sizeof(float) * ((size_t)NWARP * KP + 3 * (size_t)KP);
-  return dispatch_kq(h, K, [&](auto kq) -> int {
+  return dispatch<1, 2, 4, 8, 16, 32>(h, kq_for(K), kUnsupportedK, [&](auto kq) -> int {
     constexpr int KQ = decltype(kq)::value;
     for (int j = 0; j <= nb; ++j) {
       float* sl = h->acc.p + (size_t)(j & 1) * slot;  // slot j = [add_{j-1} | rem_j]
@@ -1011,15 +1010,6 @@ int setup_peer_exchange(hb_handle* h, int Tplan) {
 float* remT_ptr(hb_handle* h) { return h->use_xch ? h->xch.peer_remT[h->rank] : h->remT.p; }
 
 // ---- persistent update kernels over rounds [t0, t1) of this cluster_cpp call ---------------------------
-template <typename F>
-int dispatch_two_pass_nv(hb_handle* h, int KS, F&& f) {
-  switch (two_pass_nv(KS)) {
-    case 1: return f(std::integral_constant<int, 1>());
-    case 2: return f(std::integral_constant<int, 2>());
-    case 4: return f(std::integral_constant<int, 4>());
-  }
-  return fail(h, 2, "K = %d is not supported by the persistent update kernel", h->K);
-}
 TwoPassArgs make_two_pass_args(hb_handle* h, int T) {
   TwoPassArgs a;
   a.U = h->U.p;
@@ -1131,7 +1121,7 @@ int update_begin_seed(hb_handle* h) {
 }
 int launch_two_pass(hb_handle* h, TwoPassArgs a, bool cooperative) {
   const size_t smem = two_pass_smem_bytes(h->KS, h->nb, h->J);
-  return dispatch_two_pass_nv(h, h->KS, [&](auto nvc) -> int {
+  return dispatch<1, 2, 4>(h, two_pass_nv(h->KS), kUnsupportedUpdateK, [&](auto nvc) -> int {
     constexpr int NV = decltype(nvc)::value;
     CK(cudaFuncSetAttribute(k_update_two_pass<NV>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     a.use_barrier = cooperative ? 1 : 0;
@@ -1164,12 +1154,11 @@ int launch_single_pass_nv(hb_handle* h, SinglePassArgs& a, bool cooperative) {
   return 0;
 }
 int launch_single_pass(hb_handle* h, SinglePassArgs a, bool cooperative) {
-  const bool su = h->sigma_uniform;  // the default: scalar sigma (objective terms simplify)
-  switch (sp_nv(h->KS)) {
-    case 1: return su ? launch_single_pass_nv<1, true>(h, a, cooperative) : launch_single_pass_nv<1, false>(h, a, cooperative);
-    case 2: return su ? launch_single_pass_nv<2, true>(h, a, cooperative) : launch_single_pass_nv<2, false>(h, a, cooperative);
-  }
-  return fail(h, 2, "K = %d is not supported by the persistent update kernel", h->K);
+  return dispatch<1, 2>(h, sp_nv(h->KS), kUnsupportedUpdateK, [&](auto nvc) -> int {
+    constexpr int NV = decltype(nvc)::value;
+    // sigma_uniform, the default: scalar sigma (objective terms simplify)
+    return h->sigma_uniform ? launch_single_pass_nv<NV, true>(h, a, cooperative) : launch_single_pass_nv<NV, false>(h, a, cooperative);
+  });
 }
 // compute_objective() of every round in [t0, t1) (harmony.cpp:248) from the kernels' per-round sums and tables
 int push_round_objectives(hb_handle* h, int t0, int t1) {
@@ -1339,110 +1328,77 @@ int run_correct(hb_handle* h) {
     k_ridge_solve<<<K, 256, sizeof(int) * (size_t)(B + C), h->stream>>>(a);
     CKL();
   }
-  if (h->paths.mm.apply) {
-    RegionScope rs(h, "ridge_apply");
-    ApplyTcArgs a;
-    a.R = h->R.p;
-    a.V = h->V.p;
-    a.Zc = h->Zc.p;
-    a.tile_cell0 = h->tile_cell0.p;
-    a.tile_len = h->tile_len.p;
-    a.tile_tuple = h->tile_tuple.p;
-    a.ntiles = h->ntiles;
-    a.d = d;
-    a.K = K;
-    a.KS = h->KS;
-    a.DS = h->DS;
-    a.tiles_per_cta = std::max(1, (h->ntiles + h->num_sms - 1) / h->num_sms);
-    const int grid = (h->ntiles + a.tiles_per_cta - 1) / a.tiles_per_cta;
-    {
-      // cluster ranges of at most AP_MAXK clusters, equal sizes, multiples of 8, and small enough for two raw stages
-      // of shared memory: the first launch subtracts its share from Zo, the following ones from the partial result
-      // in Zc
-      int npass = (K + AP_MAXK - 1) / AP_MAXK, Kpass = 0;
-      for (;; ++npass) {
-        Kpass = (((K + npass - 1) / npass) + 7) & ~7;
-        if (apply_tc_stages(apply_tc_rs(Kpass, h->KS, 0), d, h->DS) >= 2) break;
-      }
-      for (int k_off = 0; k_off < K; k_off += Kpass) {
-        a.k_off = k_off;
-        a.Kp = std::min(Kpass, K - k_off);
-        a.KD = (a.Kp + 7) & ~7;
-        a.minuend = (k_off == 0) ? h->Zo.p : h->Zc.p;
-        const size_t smem = apply_tc_smem_bytes(apply_tc_rs(a.KD, h->KS, k_off), d, h->DS);
-        if (d <= 64) {
-          CK(cudaFuncSetAttribute(k_apply_tc<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-          k_apply_tc<1><<<grid, AP_THREADS, smem, h->stream>>>(a);
-        } else {
-          CK(cudaFuncSetAttribute(k_apply_tc<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-          k_apply_tc<2><<<grid, AP_THREADS, smem, h->stream>>>(a);
+  RegionScope rs(h, "ridge_apply");
+  switch (h->paths.apply) {
+    case Apply::Tc:
+    case Apply::TcCols: {
+      // Tc: one range of all columns; TcCols (d > 256, or K x d beyond the FFMA apply): ranges of <= 128 columns.
+      // Each column range runs in cluster ranges of at most AP_MAXK clusters, equal sizes, multiples of 8, and small
+      // enough for two raw stages of shared memory: the first launch subtracts its share from Zo, the following ones
+      // from the partial result in Zc
+      const bool cols = h->paths.apply == Apply::TcCols;
+      ApplyTcArgs a;
+      a.R = h->R.p;
+      a.V = h->V.p;
+      a.Zc = h->Zc.p;
+      a.tile_cell0 = h->tile_cell0.p;
+      a.tile_len = h->tile_len.p;
+      a.tile_tuple = h->tile_tuple.p;
+      a.ntiles = h->ntiles;
+      a.d = d;
+      a.K = K;
+      a.KS = h->KS;
+      a.DS = h->DS;
+      a.tiles_per_cta = std::max(1, (h->ntiles + h->num_sms - 1) / h->num_sms);
+      const int grid = (h->ntiles + a.tiles_per_cta - 1) / a.tiles_per_cta;
+      const int DC = cols ? 128 : h->DS;
+      auto kernel = cols ? k_apply_tc_cols : d <= 64 ? k_apply_tc<1> : k_apply_tc<2>;
+      for (a.c_off = 0; a.c_off < h->DS; a.c_off += DC) {
+        a.DC = std::min(DC, h->DS - a.c_off);
+        auto stages = [&](int RS) { return cols ? apply_cols_stages(RS, a.DC) : apply_tc_stages(RS, d, h->DS); };
+        int npass = (K + AP_MAXK - 1) / AP_MAXK, Kpass = 0;
+        for (;; ++npass) {
+          Kpass = (((K + npass - 1) / npass) + 7) & ~7;
+          if (stages(apply_tc_rs(Kpass, h->KS, 0)) >= 2) break;
         }
-        CKL();
+        for (int k_off = 0; k_off < K; k_off += Kpass) {
+          a.k_off = k_off;
+          a.Kp = std::min(Kpass, K - k_off);
+          a.KD = (a.Kp + 7) & ~7;
+          a.minuend = (k_off == 0) ? h->Zo.p : h->Zc.p;
+          const int RS = apply_tc_rs(a.KD, h->KS, k_off);
+          const size_t smem = cols ? apply_cols_smem_bytes(RS, a.DC) : apply_tc_smem_bytes(RS, d, h->DS);
+          CK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+          kernel<<<grid, AP_THREADS, smem, h->stream>>>(a);
+          CKL();
+        }
       }
+      break;
     }
-    return 0;
-  }
-  if (h->paths.wide.apply) {
-    // d > 256, or K x d beyond the FFMA apply: column ranges of <= 128 embedding columns, each split into cluster ranges
-    // like the launches above (the first cluster range of a column range subtracts from Zo)
-    RegionScope rs(h, "ridge_apply");
-    ApplyTcArgs a;
-    a.R = h->R.p;
-    a.V = h->V.p;
-    a.Zc = h->Zc.p;
-    a.tile_cell0 = h->tile_cell0.p;
-    a.tile_len = h->tile_len.p;
-    a.tile_tuple = h->tile_tuple.p;
-    a.ntiles = h->ntiles;
-    a.d = d;
-    a.K = K;
-    a.KS = h->KS;
-    a.DS = h->DS;
-    a.tiles_per_cta = std::max(1, (h->ntiles + h->num_sms - 1) / h->num_sms);
-    const int grid = (h->ntiles + a.tiles_per_cta - 1) / a.tiles_per_cta;
-    for (a.c_off = 0; a.c_off < h->DS; a.c_off += 128) {
-      a.DC = std::min(128, h->DS - a.c_off);
-      int npass = (K + AP_MAXK - 1) / AP_MAXK, Kpass = 0;
-      for (;; ++npass) {
-        Kpass = (((K + npass - 1) / npass) + 7) & ~7;
-        if (apply_cols_stages(apply_tc_rs(Kpass, h->KS, 0), a.DC) >= 2) break;
-      }
-      for (int k_off = 0; k_off < K; k_off += Kpass) {
-        a.k_off = k_off;
-        a.Kp = std::min(Kpass, K - k_off);
-        a.KD = (a.Kp + 7) & ~7;
-        a.minuend = (k_off == 0) ? h->Zo.p : h->Zc.p;
-        const size_t smem = apply_cols_smem_bytes(apply_tc_rs(a.KD, h->KS, k_off), a.DC);
-        CK(cudaFuncSetAttribute(k_apply_tc_cols, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        k_apply_tc_cols<<<grid, AP_THREADS, smem, h->stream>>>(a);
-        CKL();
-      }
+    case Apply::Ffma: {
+      ApplyArgs a;
+      a.R = h->R.p;
+      a.Zo = h->Zo.p;
+      a.V = h->V.p;
+      a.Zc = h->Zc.p;
+      a.tile_cell0 = h->tile_cell0.p;
+      a.tile_len = h->tile_len.p;
+      a.tile_tuple = h->tile_tuple.p;
+      a.ntiles = h->ntiles;
+      a.d = d;
+      a.K = K;
+      a.ldR = h->KS;
+      a.ldZ = h->DS;
+      const int DP = (d + 3) & ~3;
+      dim3 block(DP / 4, TM / 4);
+      const size_t smem = apply_ffma_smem_bytes(K, d);
+      CK(cudaFuncSetAttribute(k_ridge_apply, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+      a.tiles_per_cta = std::max(1, (h->ntiles + h->num_sms * 4 - 1) / (h->num_sms * 4));
+      int grid = (h->ntiles + a.tiles_per_cta - 1) / a.tiles_per_cta;
+      k_ridge_apply<<<grid, block, smem, h->stream>>>(a);
+      CKL();
+      break;
     }
-    return 0;
-  }
-  {
-    RegionScope rs(h, "ridge_apply");
-    ApplyArgs a;
-    a.R = h->R.p;
-    a.Zo = h->Zo.p;
-    a.V = h->V.p;
-    a.Zc = h->Zc.p;
-    a.tile_cell0 = h->tile_cell0.p;
-    a.tile_len = h->tile_len.p;
-    a.tile_tuple = h->tile_tuple.p;
-    a.ntiles = h->ntiles;
-    a.d = d;
-    a.K = K;
-    a.ldR = h->KS;
-    a.ldZ = h->DS;
-    const int DP = (d + 3) & ~3;
-    dim3 block(DP / 4, TM / 4);
-    const size_t smem = apply_ffma_smem_bytes(K, d);
-    CK(cudaFuncSetAttribute(k_ridge_apply, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    a.tiles_per_cta = std::max(1, (h->ntiles + h->num_sms * 4 - 1) / (h->num_sms * 4));
-    int grid = (h->ntiles + a.tiles_per_cta - 1) / a.tiles_per_cta;
-    k_ridge_apply<<<grid, block, smem, h->stream>>>(a);
-    CKL();
   }
   return 0;
 }
@@ -2082,19 +2038,21 @@ int hb_init_cluster(hb_handle* h, const double* Y0) {
       cells[k] = (int64_t)std::floor((double)kmeans_uniform(seed, (uint64_t)K, (uint64_t)k) * (double)(h->N_global - 1));
     TRY(gather(-1));
     // (2) the races of all centroids in one pass over the cells (a centroid's race only looks at its own start cell)
-    // both steps run from tensor-core logits U = 2 (z . y - 1) (k_logits_tc, sigma = 1) when that kernel takes the
-    // shape; else from the FFMA kernels (thread per cell)
+    // both steps run from tensor-core logits U = 2 (z . y - 1) (sigma = 1) when select_kernels chose them; else from
+    // the FFMA kernels (thread per cell)
     DevBuf<float> ones, yy;
-    const bool km_logits = h->paths.mm.kmeans || h->paths.wide.kmeans;
+    const KmeansInit km = h->paths.kmeans;
     const int km_nv = sp_nv(h->KS);
-    if (km_logits) {
+    const size_t smem = sizeof(float) * Kd;
+    if (km == KmeansInit::Ffma) {
+      CK(cudaFuncSetAttribute(k_kmeans_race, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+      CK(cudaFuncSetAttribute(k_kmeans_assign, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    } else {
       CK(ones.alloc(K));
       CK(yy.alloc(K));
       k_fill_f<<<1, 256, 0, h->stream>>>(ones.p, (int64_t)K, 1.0f);
       CKL();
     }
-    const size_t smem_pp = sizeof(float) * Kd;
-    if (!km_logits) CK(cudaFuncSetAttribute(k_kmeans_race, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_pp));
     std::vector<unsigned long long> best(K);
     bool logits_of_start = false;  // U holds the logits of the start cells
     auto race = [&](int i0, int i1, const std::vector<int64_t>& taken) -> int {
@@ -2104,27 +2062,29 @@ int hb_init_cluster(hb_handle* h, const double* Y0) {
         CK(cudaMemcpyAsync(taken_d.p, taken.data(), sizeof(int64_t) * taken.size(), cudaMemcpyHostToDevice, h->stream));
       }
       CK(cudaMemsetAsync(best_d.p + i0, 0xff, sizeof(unsigned long long) * (i1 - i0), h->stream));
-      if (km_logits) {
-        if (!logits_of_start) {
-          TRY(launch_logits(h, ones.p, false));
-          logits_of_start = true;
+      switch (km) {
+        case KmeansInit::Ffma:
+          k_kmeans_race<<<grid_for(h->n, 128, h->num_sms * 4), 128, sizeof(float) * (size_t)(i1 - i0) * d, h->stream>>>(
+              h->Zc.p, h->sort_perm.p, h->Y.p, best_d.p, taken.empty() ? nullptr : taken_d.p, (int)taken.size(), h->n, K, d, h->DS,
+              h->cell_offset, seed, i0, i1);
+          CKL();
+          break;
+        case KmeansInit::LogitsTc:
+        case KmeansInit::LogitsWide: {
+          if (!logits_of_start) {
+            TRY(launch_logits(h, ones.p, false, km == KmeansInit::LogitsWide));
+            logits_of_start = true;
+          }
+          const int grid_r = grid_for(h->n * 32, 256, h->num_sms * 8);
+          TRY(dispatch<1, 2, 4, 8>(h, km_nv, kUnsupportedK, [&](auto nvc) -> int {
+            constexpr int NV = decltype(nvc)::value;
+            k_kmeans_race_u<NV><<<grid_r, 256, 0, h->stream>>>(h->U.p, h->sort_perm.p, best_d.p, taken.empty() ? nullptr : taken_d.p,
+                                                             (int)taken.size(), h->n, K, h->KS, h->cell_offset, seed, i0, i1);
+            CKL();
+            return 0;
+          }));
+          break;
         }
-        const int grid_r = grid_for(h->n * 32, 256, h->num_sms * 8);
-        auto go = [&](auto nvc) {
-          constexpr int NV = decltype(nvc)::value;
-          k_kmeans_race_u<NV><<<grid_r, 256, 0, h->stream>>>(h->U.p, h->sort_perm.p, best_d.p, taken.empty() ? nullptr : taken_d.p,
-                                                           (int)taken.size(), h->n, K, h->KS, h->cell_offset, seed, i0, i1);
-        };
-        if (km_nv == 1) go(std::integral_constant<int, 1>());
-        else if (km_nv == 2) go(std::integral_constant<int, 2>());
-        else if (km_nv == 4) go(std::integral_constant<int, 4>());
-        else go(std::integral_constant<int, 8>());
-        CKL();
-      } else {
-        k_kmeans_race<<<grid_for(h->n, 128, h->num_sms * 4), 128, sizeof(float) * (size_t)(i1 - i0) * d, h->stream>>>(
-            h->Zc.p, h->sort_perm.p, h->Y.p, best_d.p, taken.empty() ? nullptr : taken_d.p, (int)taken.size(), h->n, K, d, h->DS,
-            h->cell_offset, seed, i0, i1);
-        CKL();
       }
       if (h->world > 1) CKN(g_nccl.AllReduce(best_d.p + i0, best_d.p + i0, (size_t)(i1 - i0), ncclUint64, ncclMin, h->comm, h->stream));
       CK(cudaMemcpyAsync(best.data() + i0, best_d.p + i0, sizeof(unsigned long long) * (i1 - i0), cudaMemcpyDeviceToHost, h->stream));
@@ -2148,38 +2108,38 @@ int hb_init_cluster(hb_handle* h, const double* Y0) {
     }
     h->kmeans_cells = cells;
     TRY(gather(-1));
-    const size_t smem = sizeof(float) * Kd;
-    if (!km_logits) CK(cudaFuncSetAttribute(k_kmeans_assign, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     for (int iter = 0; iter < 10; ++iter) {
-      if (km_logits) {
-        // Lloyd iteration on the tensor cores: logits -> one-hot rows of R -> members' sums and counts (K3) -> means
-        TRY(launch_logits(h, ones.p, false));
-        k_kmeans_norms<<<(K + 127) / 128, 128, 0, h->stream>>>(h->Y.p, yy.p, K, d);
-        CKL();
-        const int grid_p = grid_for(h->n * 32, 256, h->num_sms * 8);
-        auto go = [&](auto nvc) {
-          constexpr int NV = decltype(nvc)::value;
-          k_kmeans_pick<NV><<<grid_p, 256, 0, h->stream>>>(h->U.p, yy.p, h->R.p, h->n, K, h->KS);
-        };
-        if (km_nv == 1) go(std::integral_constant<int, 1>());
-        else if (km_nv == 2) go(std::integral_constant<int, 2>());
-        else if (km_nv == 4) go(std::integral_constant<int, 4>());
-        else go(std::integral_constant<int, 8>());
-        CKL();
-        CK(cudaMemsetAsync(h->S.p, 0, sizeof(float) * (size_t)h->J * K * (d + 1), h->stream));
-        TRY(run_stats_tc(h, h->Zc.p));
-        TRY(allreduce_f(h, h->S.p, (size_t)h->J * K * (d + 1)));
-        k_kmeans_means_from_stats<<<(int)((Kd + 255) / 256), 256, 0, h->stream>>>(h->S.p, h->Y.p, h->J, K, d);
-        CKL();
-        continue;
+      switch (km) {
+        case KmeansInit::Ffma:
+          CK(cudaMemsetAsync(ysum.p, 0, sizeof(float) * (Kd + K), h->stream));
+          k_kmeans_assign<<<grid_for(h->n, 128, h->num_sms * 4), 128, smem, h->stream>>>(h->Zc.p, h->Y.p, ysum.p, ysum.p + Kd,
+                                                                                           h->n, K, d, h->DS);
+          CKL();
+          TRY(allreduce_f(h, ysum.p, Kd + K));
+          k_kmeans_update<<<(int)((Kd + 255) / 256), 256, 0, h->stream>>>(h->Y.p, ysum.p, ysum.p + Kd, K, d);
+          CKL();
+          break;
+        case KmeansInit::LogitsTc:
+        case KmeansInit::LogitsWide: {
+          // Lloyd iteration on the tensor cores: logits -> one-hot rows of R -> members' sums and counts (K3) -> means
+          TRY(launch_logits(h, ones.p, false, km == KmeansInit::LogitsWide));
+          k_kmeans_norms<<<(K + 127) / 128, 128, 0, h->stream>>>(h->Y.p, yy.p, K, d);
+          CKL();
+          const int grid_p = grid_for(h->n * 32, 256, h->num_sms * 8);
+          TRY(dispatch<1, 2, 4, 8>(h, km_nv, kUnsupportedK, [&](auto nvc) -> int {
+            constexpr int NV = decltype(nvc)::value;
+            k_kmeans_pick<NV><<<grid_p, 256, 0, h->stream>>>(h->U.p, yy.p, h->R.p, h->n, K, h->KS);
+            CKL();
+            return 0;
+          }));
+          CK(cudaMemsetAsync(h->S.p, 0, sizeof(float) * (size_t)h->J * K * (d + 1), h->stream));
+          TRY(run_stats_tc(h, h->Zc.p));
+          TRY(allreduce_f(h, h->S.p, (size_t)h->J * K * (d + 1)));
+          k_kmeans_means_from_stats<<<(int)((Kd + 255) / 256), 256, 0, h->stream>>>(h->S.p, h->Y.p, h->J, K, d);
+          CKL();
+          break;
+        }
       }
-      CK(cudaMemsetAsync(ysum.p, 0, sizeof(float) * (Kd + K), h->stream));
-      k_kmeans_assign<<<grid_for(h->n, 128, h->num_sms * 4), 128, smem, h->stream>>>(h->Zc.p, h->Y.p, ysum.p, ysum.p + Kd,
-                                                                                       h->n, K, d, h->DS);
-      CKL();
-      TRY(allreduce_f(h, ysum.p, Kd + K));
-      k_kmeans_update<<<(int)((Kd + 255) / 256), 256, 0, h->stream>>>(h->Y.p, ysum.p, ysum.p + Kd, K, d);
-      CKL();
     }
     CK(cudaStreamSynchronize(h->stream));
   }
@@ -2188,7 +2148,7 @@ int hb_init_cluster(hb_handle* h, const double* Y0) {
   k_normalise_rows<<<grid_for((int64_t)h->K * 32, 256, 64), 256, 0, h->stream>>>(h->Y.p, h->Y.p, h->K, h->d, h->d);
   CKL();
   CK(cudaMemsetAsync(h->obj_acc.p, 0, 2 * sizeof(double), h->stream));
-  TRY(run_assign(h, false, false, true));
+  TRY(run_assign(h, false, true));
   TRY(push_objective(h));                       // compute_objective() (:152)
   lap.mark("assignment + objective");
   h->harmony_slots.push_back(h->obj_count - 1);  // objective_harmony.push_back (:153)
@@ -2218,7 +2178,7 @@ int legacy_centroid_step(hb_handle* h) {
   CK(cudaMemcpyAsync(h->OEkeep.p, h->O.p, sizeof(float) * BK, cudaMemcpyDeviceToDevice, h->stream));
   CK(cudaMemcpyAsync(h->OEkeep.p + BK, h->E.p, sizeof(float) * BK, cudaMemcpyDeviceToDevice, h->stream));
   CK(cudaMemcpyAsync(h->objkeep.p, h->obj_acc.p, 2 * sizeof(double), cudaMemcpyDeviceToDevice, h->stream));
-  TRY(run_assign(h, false));
+  TRY(run_assign(h, false, true));
   CK(cudaMemcpyAsync(h->R.p, h->Rkeep.p, sizeof(float) * nK, cudaMemcpyDeviceToDevice, h->stream));
   CK(cudaMemcpyAsync(h->O.p, h->OEkeep.p, sizeof(float) * BK, cudaMemcpyDeviceToDevice, h->stream));
   CK(cudaMemcpyAsync(h->E.p, h->OEkeep.p + BK, sizeof(float) * BK, cudaMemcpyDeviceToDevice, h->stream));
@@ -2237,7 +2197,7 @@ int hb_cluster(hb_handle* h, const int64_t* update_orders) {
   const CallPath call = call_path(h->paths, T, h->legacy_centroid);
   const bool plan_assign = cold && call.plan_order_assign;
   if (cold && !plan_assign) {
-    TRY(run_assign(h, true, false, false));  // the cold start does not evaluate the objective
+    TRY(run_assign(h, true, false));  // the cold start does not evaluate the objective
     CK(cudaMemsetAsync(h->obj_acc.p, 0, 2 * sizeof(double), h->stream));
   }
   if (update_orders && T > 0) {
@@ -2272,7 +2232,7 @@ int hb_cluster(hb_handle* h, const int64_t* update_orders) {
     TRY(plan_acquire(h, (int)T, update_orders ? h->perms_d.p : nullptr));
     if (T > 0) TRY(update_begin_zero(h, (int)T));
     if (plan_assign) {
-      TRY(run_assign(h, true, true, false));
+      TRY(run_assign_plan_order(h, true));
       CK(cudaMemsetAsync(h->obj_acc.p, 0, 2 * sizeof(double), h->stream));
     }
     if (T > 0) TRY(update_begin_seed(h));
@@ -2609,9 +2569,14 @@ int hb_debug_update_geometry(int KS, int nb, int64_t out[9]) {
 }
 
 // Kernels hb_setup picks for a shape, and the update path of a cluster_cpp call (test hook, host only).
+// Fields 2 and 4 are derived from the stage choices: "wgmma logits" is a k_logits_tc cold start without
+// HB_KS_FFMA_CONTRACTIONS (with it, only shapes past FFMA k_assign take that cold start), "tensor-core k-means" a
+// k_logits_tc initialisation at KS <= 256.
 int hb_debug_kernel_paths(int K, int d, int J, int64_t n, int nb, int num_sms, int kernel_set, int64_t out[8]) {
   const KernelPaths p = select_kernels(K, d, J, n, nb, num_sms, kernel_set);
-  const int64_t v[8] = {(int64_t)p.update, p.mm.k1_stages, p.mm.logits, p.mm.apply, p.mm.kmeans,
+  const bool cold_logits_tc = p.cold == ColdStart::LogitsTc && !(kernel_set & HB_KS_FFMA_CONTRACTIONS);
+  const bool kmeans_tc = p.kmeans == KmeansInit::LogitsTc && ((K + 3) & ~3) <= 256;
+  const int64_t v[8] = {(int64_t)p.update, p.k1_stages, cold_logits_tc, p.apply == Apply::Tc, kmeans_tc,
                         call_path(p, 20, false).plan_order_assign, (int64_t)call_path(p, 40, false).update,
                         (int64_t)call_path(p, 20, true).update};
   for (int i = 0; i < 8; ++i) out[i] = v[i];
@@ -2623,14 +2588,13 @@ int hb_debug_kernel_paths(int K, int d, int J, int64_t n, int nb, int num_sms, i
 // softmax pass, 4 k_logits_wide + softmax pass; plan-order cold start of a 20-round call: 0 none (natural order),
 // 1 fused wgmma, 2 k_logits_tc + block sums, 3 k_logits_wide + block sums; ridge apply: 1 wgmma, 2 FFMA, 3 column
 // ranges; native k-means initialisation: 1 FFMA, 2 k_logits_tc logits (KS <= 256), 3 k_logits_tc logits, 4
-// k_logits_wide logits}.
+// k_logits_wide logits}.  The k-means values 2 and 3 run the same kernels; they tell KS <= 256 from KS > 256.
 int hb_debug_wide_paths(int K, int d, int J, int64_t n, int nb, int num_sms, int kernel_set, int64_t out[4]) {
   const KernelPaths p = select_kernels(K, d, J, n, nb, num_sms, kernel_set);
-  const int lw = p.wide.logits ? 1 : 0;
-  out[0] = p.mm.k1_stages ? 1 : p.wide.assign ? 3 + lw : 2;
-  out[1] = !call_path(p, 20, false).plan_order_assign ? 0 : p.mm.k1_stages ? 1 : p.mm.logits ? 2 : 2 + lw;
-  out[2] = p.mm.apply ? 1 : p.wide.apply ? 3 : 2;
-  out[3] = p.mm.kmeans ? 2 : p.wide.kmeans ? 3 + lw : 1;
+  out[0] = (int64_t)p.assign;
+  out[1] = call_path(p, 20, false).plan_order_assign ? (int64_t)p.cold : 0;
+  out[2] = (int64_t)p.apply;
+  out[3] = p.kmeans == KmeansInit::Ffma ? 1 : p.kmeans == KmeansInit::LogitsWide ? 4 : ((K + 3) & ~3) <= 256 ? 2 : 3;
   return 0;
 }
 

@@ -405,7 +405,7 @@ int plan_setup(hb_handle* h, const std::vector<int64_t>& tstart, int T) {
   const bool single_pass = h->paths.update == UpdatePath::SinglePass;
   p.nsub = (single_pass && nb <= 64) ? nb : 1;
   p.pt_cap = (size_t)n / TC_TM + (size_t)nb * J + 2;
-  if (h->paths.mm.k1_stages && single_pass)
+  if (h->paths.cold == ColdStart::FusedTc && single_pass)
     for (DevBuf<int>* b : {&p.pt_p0, &p.pt_len, &p.pt_tuple, &p.pt_blk}) CK(b->alloc(2 * p.pt_cap));
   CK(p.pt_base.alloc(2 * S1));
   CK(p.tile_base.alloc(S1));

@@ -196,6 +196,65 @@ def test_kernel_paths_per_shape(shape, kernel_set, expected):
     assert tuple(out) == expected
 
 
+PIN_SHAPES = {"c3": C3, "c5": dict(K=200, d=100, J=40, n=6_250_000), "K1024_d64": dict(K=1024, d=64, J=20, n=1_000_000),
+              "K100_d300": dict(K=100, d=300, J=20, n=1_000_000), "K300_d50": dict(K=300, d=50, J=20, n=1_000_000)}
+
+
+# shape, HB_KERNEL_SET, hb_debug_kernel_paths (as above), hb_debug_wide_paths (natural-order assignment, plan-order
+# cold start, ridge apply, k-means initialisation; numbered as in tests/test_gpu_wide_shapes.py)
+@pytest.mark.parametrize("shape, kernel_set, kernel_paths, wide_paths", [
+    ("c3", 0, (2, 2, 0, 1, 1, 1, 2, 0), (1, 1, 1, 2)),
+    ("c3", 1, (2, 0, 0, 0, 0, 0, 2, 0), (2, 0, 2, 1)),
+    ("c3", 2, (0, 2, 0, 1, 1, 0, 0, 0), (1, 0, 1, 2)),
+    ("c3", 4, (1, 2, 0, 1, 1, 0, 0, 0), (1, 0, 1, 2)),
+    ("c3", 16, (2, 0, 0, 0, 0, 1, 2, 0), (4, 3, 3, 4)),
+    ("c3", 17, (2, 0, 0, 0, 0, 1, 2, 0), (4, 3, 3, 4)),
+    ("c3", 18, (0, 0, 0, 0, 0, 0, 0, 0), (4, 0, 3, 4)),
+    ("c3", 20, (1, 0, 0, 0, 0, 0, 0, 0), (4, 0, 3, 4)),
+    ("c5", 0, (2, 0, 1, 1, 1, 1, 2, 0), (2, 2, 1, 2)),
+    ("c5", 1, (2, 0, 0, 0, 0, 0, 2, 0), (2, 0, 2, 1)),
+    ("c5", 2, (0, 0, 1, 1, 1, 0, 0, 0), (2, 0, 1, 2)),
+    ("c5", 4, (1, 0, 1, 1, 1, 0, 0, 0), (2, 0, 1, 2)),
+    ("c5", 16, (2, 0, 0, 0, 0, 1, 2, 0), (4, 3, 3, 4)),
+    ("c5", 17, (2, 0, 0, 0, 0, 1, 2, 0), (4, 3, 3, 4)),
+    ("c5", 18, (0, 0, 0, 0, 0, 0, 0, 0), (4, 0, 3, 4)),
+    ("c5", 20, (1, 0, 0, 0, 0, 0, 0, 0), (4, 0, 3, 4)),
+    ("K1024_d64", 0, (0, 0, 1, 1, 0, 0, 0, 0), (3, 0, 1, 3)),
+    ("K1024_d64", 1, (0, 0, 0, 0, 0, 0, 0, 0), (3, 0, 3, 3)),
+    ("K1024_d64", 2, (0, 0, 1, 1, 0, 0, 0, 0), (3, 0, 1, 3)),
+    ("K1024_d64", 4, (0, 0, 1, 1, 0, 0, 0, 0), (3, 0, 1, 3)),
+    ("K1024_d64", 16, (0, 0, 0, 0, 0, 0, 0, 0), (4, 0, 3, 4)),
+    ("K1024_d64", 17, (0, 0, 0, 0, 0, 0, 0, 0), (4, 0, 3, 4)),
+    ("K1024_d64", 18, (0, 0, 0, 0, 0, 0, 0, 0), (4, 0, 3, 4)),
+    ("K1024_d64", 20, (0, 0, 0, 0, 0, 0, 0, 0), (4, 0, 3, 4)),
+    ("K100_d300", 0, (2, 0, 0, 0, 0, 1, 2, 0), (4, 3, 3, 1)),
+    ("K100_d300", 1, (2, 0, 0, 0, 0, 1, 2, 0), (4, 3, 3, 1)),
+    ("K100_d300", 2, (0, 0, 0, 0, 0, 0, 0, 0), (4, 0, 3, 1)),
+    ("K100_d300", 4, (1, 0, 0, 0, 0, 0, 0, 0), (4, 0, 3, 1)),
+    ("K100_d300", 16, (2, 0, 0, 0, 0, 1, 2, 0), (4, 3, 3, 4)),
+    ("K100_d300", 17, (2, 0, 0, 0, 0, 1, 2, 0), (4, 3, 3, 4)),
+    ("K100_d300", 18, (0, 0, 0, 0, 0, 0, 0, 0), (4, 0, 3, 4)),
+    ("K100_d300", 20, (1, 0, 0, 0, 0, 0, 0, 0), (4, 0, 3, 4)),
+    ("K300_d50", 0, (0, 0, 1, 1, 0, 0, 0, 0), (2, 0, 1, 1)),
+    ("K300_d50", 1, (0, 0, 0, 0, 0, 0, 0, 0), (2, 0, 2, 1)),
+    ("K300_d50", 2, (0, 0, 1, 1, 0, 0, 0, 0), (2, 0, 1, 1)),
+    ("K300_d50", 4, (0, 0, 1, 1, 0, 0, 0, 0), (2, 0, 1, 1)),
+    ("K300_d50", 16, (0, 0, 0, 0, 0, 0, 0, 0), (4, 0, 3, 4)),
+    ("K300_d50", 17, (0, 0, 0, 0, 0, 0, 0, 0), (4, 0, 3, 4)),
+    ("K300_d50", 18, (0, 0, 0, 0, 0, 0, 0, 0), (4, 0, 3, 4)),
+    ("K300_d50", 20, (0, 0, 0, 0, 0, 0, 0, 0), (4, 0, 3, 4)),
+])
+def test_kernel_sets_per_shape(shape, kernel_set, kernel_paths, wide_paths):
+    """Both selection hooks under kernel sets 0, 1, 2, 4 and 16 and under HB_KS_WIDE combined with 1, 2 or 4, at the
+    benchmark's c3 / c5 and at three more rows of DESIGN §3's kernel-selection table."""
+    L = _lib.lib()
+    s = PIN_SHAPES[shape]
+    kp, wp = (ctypes.c_int64 * 8)(), (ctypes.c_int64 * 4)()
+    L.hb_debug_kernel_paths(s["K"], s["d"], s["J"], s["n"], 20, 132, kernel_set, kp)
+    L.hb_debug_wide_paths(s["K"], s["d"], s["J"], s["n"], 20, 132, kernel_set, wp)
+    assert (tuple(kp), tuple(wp)) == (kernel_paths, wide_paths)
+
+
 def test_host_widen_pool_matches_numpy():
     """The worker pool of the download path widens float32 to float64 exactly, for
     sizes around its slice boundaries and repeatedly (the pool is persistent)."""
