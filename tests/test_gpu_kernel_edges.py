@@ -1,6 +1,6 @@
 """Stage tests of the hot-path kernels at every kernel-selection boundary, against the fp64 numpy restatement.
 
-Each row of EDGE_ROWS is a shape that straddles one limit of select_kernels (harmony_b200.cu) or of a kernel's tiling:
+Each row of EDGE_ROWS is a shape that straddles one limit of select_kernels (select.cuh) or of a kernel's tiling:
 the fused assignment kernel at d = 64 and K = 128 and its m64n16 tail, the logits + softmax cold start past them, the
 cluster ranges of the ridge apply (K > 112 runs as several launches), the cluster and column launches of the ridge
 statistics (K > 128, d + 1 > 128), the FFMA kernels past d = 128, the per-step update past KS = 256, the single-pass /
