@@ -6,7 +6,8 @@ Importing this package does not load the CUDA library; constructing ``harmony`` 
 loudly if it is missing (there is no CPU fallback).
 """
 from .harmony_option import harmony_options  # noqa: F401
-from .ui import RunHarmony, prepare_inputs  # noqa: F401
+from .mapping import HarmonyReference  # noqa: F401
+from .ui import MapQuery, RunHarmony, prepare_inputs  # noqa: F401
 from .utils import HarmonyConvergencePlot, harmonize  # noqa: F401
 
 __version__ = "0.1.0"

@@ -14,7 +14,8 @@ SO_PATH = os.path.join(_HERE, "libharmony_b200.so")
 SOURCES = [os.path.join(_HERE, "csrc", f) for f in ("harmony_b200.cu", "kernels.cuh", "io.cuh", "common.cuh", "update_slots.cuh", "update_per_step.cuh",
                                                      "update_two_pass.cuh", "update_single_pass.cuh", "plan.cuh", "tuples.cuh", "umma.cuh", "assign_tc3.cuh", "logits_tc.cuh", "logits_wide.cuh", "stats_tc3.cuh",
                                                      "apply_tc3.cuh", "select.cuh", "handle.cuh", "comm.cuh", "trace.cuh", "transfer.cuh",
-                                                     "update_host.cuh", "correct_host.cuh", "assign_host.cuh", "kmeans_init.cuh")]
+                                                     "update_host.cuh", "correct_host.cuh", "assign_host.cuh", "kmeans_init.cuh",
+                                                     "map_host.cuh")]
 HEADER = os.path.join(ROOT, "include", "harmony_b200.h")
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17", "-shared",
               "-Xcompiler", "-fPIC"]
@@ -72,6 +73,10 @@ def lib():
     L.hb_setup_device.argtypes = [P, P, I, I64, P, I, I64, P, P, I, P, P, P, D, I, D, D, I, D, D, I]
     L.hb_set_seed.argtypes = [P, ctypes.c_uint64]
     L.hb_set_abort_callback.argtypes = [P, P, P]
+    L.hb_reference.argtypes = [P, P, P, P, P]
+    L.hb_map_setup.argtypes = [P, P, I, I64, P, P, I, P, I, P, P, P, P]
+    L.hb_map_setup_device.argtypes = [P, P, I, I64, P, I, I64, P, P, I, P, I, P, P, P, P]
+    L.hb_map.argtypes = [P]
     L.hb_init_cluster.argtypes = [P, P]
     L.hb_cluster.argtypes = [P, P]
     L.hb_moe_correct_ridge.argtypes = [P]

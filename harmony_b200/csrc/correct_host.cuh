@@ -25,43 +25,10 @@ int run_stats_tc(hb_handle* h, const float* Zsrc) {
   return 0;
 }
 
-int run_correct(hb_handle* h) {
-  const int K = h->K, d = h->d, B = h->B, J = h->J, C = h->C;
-  const int D1 = d + 1;
-  {
-    RegionScope rs(h, "ridge_stats");
-    CK(cudaMemsetAsync(h->S.p, 0, sizeof(float) * (size_t)J * K * D1, h->stream));
-    TRY(run_stats_tc(h, h->Zo.p));
-    TRY(allreduce_f(h, h->S.p, (size_t)J * K * D1));
-  }
-  {
-    RegionScope rs(h, "ridge_solve");
-    SolveArgs a;
-    a.S = h->S.p;
-    a.O = h->O.p;
-    a.E = h->E.p;
-    a.N_b = h->N_b.p;
-    a.lambda = h->lambda_estimation ? nullptr : h->lambda.p;
-    a.tuple_levels = h->tuple_levels.p;
-    a.cov_of = h->cov_of_d.p;
-    a.Y = h->Y.p;
-    a.V = h->V.p;
-    a.Wfull = h->Wfull.p;
-    a.skipped = h->skipped.p;
-    a.scratch = h->scratch.p;
-    a.iscratch = h->iscratch.p;
-    a.err_flag = h->err_flag.p;
-    a.J = J;
-    a.K = K;
-    a.B = B;
-    a.C = C;
-    a.d = d;
-    a.KS = h->KS;
-    a.alpha = h->alpha;
-    a.cutoff = h->cutoff;
-    k_ridge_solve<<<K, 256, sizeof(int) * (size_t)(B + C), h->stream>>>(a);
-    CKL();
-  }
+// Zc = Zo - sum_k R_k V[q][k] for the per-tuple corrections V a solve wrote (moe_correct_ridge_cpp, and the mapping of
+// a query in map_host.cuh)
+int run_apply(hb_handle* h) {
+  const int K = h->K, d = h->d;
   RegionScope rs(h, "ridge_apply");
   switch (h->paths.apply) {
     case Apply::Tc:
@@ -117,6 +84,46 @@ int run_correct(hb_handle* h) {
     }
   }
   return 0;
+}
+
+int run_correct(hb_handle* h) {
+  const int K = h->K, d = h->d, B = h->B, J = h->J, C = h->C;
+  const int D1 = d + 1;
+  {
+    RegionScope rs(h, "ridge_stats");
+    CK(cudaMemsetAsync(h->S.p, 0, sizeof(float) * (size_t)J * K * D1, h->stream));
+    TRY(run_stats_tc(h, h->Zo.p));
+    TRY(allreduce_f(h, h->S.p, (size_t)J * K * D1));
+  }
+  {
+    RegionScope rs(h, "ridge_solve");
+    SolveArgs a;
+    a.S = h->S.p;
+    a.O = h->O.p;
+    a.E = h->E.p;
+    a.N_b = h->N_b.p;
+    a.lambda = h->lambda_estimation ? nullptr : h->lambda.p;
+    a.tuple_levels = h->tuple_levels.p;
+    a.cov_of = h->cov_of_d.p;
+    a.Y = h->Y.p;
+    a.V = h->V.p;
+    a.Wfull = h->Wfull.p;
+    a.skipped = h->skipped.p;
+    a.scratch = h->scratch.p;
+    a.iscratch = h->iscratch.p;
+    a.err_flag = h->err_flag.p;
+    a.J = J;
+    a.K = K;
+    a.B = B;
+    a.C = C;
+    a.d = d;
+    a.KS = h->KS;
+    a.alpha = h->alpha;
+    a.cutoff = h->cutoff;
+    k_ridge_solve<<<K, 256, sizeof(int) * (size_t)(B + C), h->stream>>>(a);
+    CKL();
+  }
+  return run_apply(h);
 }
 
 }  // namespace

@@ -69,6 +69,7 @@ struct Region {
 struct Plan;         // plan.cuh
 struct UpdateState;  // update_host.cuh
 struct AssignState;  // assign_host.cuh
+struct MapState;     // map_host.cuh
 
 }  // namespace
 
@@ -99,6 +100,8 @@ struct hb_handle {
   float sigma0 = 0.f;
   bool R_user_set = false;       // R was written through hb_set_field since the last assignment step
   bool zc_pending_norm = false;  // Zc holds the un-normalised corrected embedding although cluster_cpp has run
+  bool mapping = false;          // set up by hb_map_setup: a query mapped onto a reference, not a Harmony run
+  bool ran_map = false;
   std::vector<int> tuple_levels_h;     // [J][C]
   std::vector<int64_t> tuple_start_h;  // [J + 1] first sorted position of each tuple
   std::vector<int64_t> kmeans_cells;   // global cells chosen by the native initialize_centroids (test hook)
@@ -119,6 +122,7 @@ struct hb_handle {
   std::unique_ptr<Plan> plan;
   std::unique_ptr<UpdateState> upd;
   std::unique_ptr<AssignState> asg;
+  std::unique_ptr<MapState> map;  // hb_map_setup only
 
   // traces (harmony.h:55-56); values are produced on the device and pulled lazily
   DevBuf<float> trace_d;

@@ -309,12 +309,19 @@ int setup_common(hb_handle* h, const ZInput& Z, int d, int64_t N, const int32_t*
   return 0;
 }
 
+// the Harmony steps a mapping handle refuses
+int refuse_mapping(hb_handle* h, const char* what) {
+  return fail(h, 3, "%s: this object maps a query (hb_map_setup), it does not run Harmony", what);
+}
+
 }  // namespace
+
+#include "map_host.cuh"
 
 // =================================================================================================
 extern "C" {
 
-int hb_version(void) { return 300; }
+int hb_version(void) { return 400; }
 
 int hb_create(hb_handle** out, int device) {
   if (!out) return 1;
@@ -450,8 +457,49 @@ int hb_setup_device(hb_handle* h, const void* Z, int z_dtype, int64_t z_ld, void
                       epsilon_harmony, K, block_size, batch_proportion_cutoff, verbose);
 }
 
+int hb_reference(hb_handle* h, double* centroids, double* Nr, double* Cref, double* sigma) {
+  if (!h) return 1;
+  if (h->mapping) return refuse_mapping(h, "hb_reference");
+  if (!h->ran_init) return fail(h, 3, "init_cluster_cpp has not been run");
+  if (h->world > 1) return fail(h, 3, "hb_reference does not take a sharded integration");
+  CK(cudaSetDevice(h->device));
+  return reference_stats(h, centroids, Nr, Cref, sigma);
+}
+
+int hb_map_setup(hb_handle* h, const double* Z, int d, int64_t N, const int32_t* phi_i, const int32_t* B_vec, int C,
+                 const double* lambda, int K, const double* centroids, const double* Nr, const double* Cref,
+                 const double* sigma) {
+  if (!h) return 1;
+  cudaMemoryType phi_type;
+  TRY(phi_location(h, phi_i, &phi_type));
+  if (phi_type == cudaMemoryTypeDevice)
+    return fail(h, 2, "phi_i is device memory: hb_map_setup takes host labels (device labels go through hb_map_setup_device)");
+  return map_setup(h, ZInput{Z}, d, N, phi_i, false, B_vec, C, lambda, K, centroids, Nr, Cref, sigma);
+}
+
+int hb_map_setup_device(hb_handle* h, const void* Z, int z_dtype, int64_t z_ld, void* stream, int d, int64_t N,
+                        const int32_t* phi_i, const int32_t* B_vec, int C, const double* lambda, int K,
+                        const double* centroids, const double* Nr, const double* Cref, const double* sigma) {
+  if (!h) return 1;
+  if (h->ran_setup) return fail(h, 3, "setup was already run on this object");
+  if (z_dtype != HB_FLOAT32 && z_dtype != HB_FLOAT64) return fail(h, 2, "unknown dtype %d of Z", z_dtype);
+  if (z_ld < d) return fail(h, 2, "row stride of Z (%lld) is smaller than d = %d", (long long)z_ld, d);
+  TRY(check_device_ptr(h, Z, "Z"));
+  cudaMemoryType phi_type;
+  TRY(phi_location(h, phi_i, &phi_type));
+  return map_setup(h, ZInput{nullptr, Z, z_dtype, z_ld, (cudaStream_t)stream}, d, N, phi_i,
+                   phi_type != cudaMemoryTypeHost, B_vec, C, lambda, K, centroids, Nr, Cref, sigma);
+}
+
+int hb_map(hb_handle* h) {
+  if (!h) return 1;
+  if (!h->mapping) return fail(h, 3, "hb_map needs an object set up by hb_map_setup");
+  return run_map(h);
+}
+
 int hb_init_cluster(hb_handle* h, const double* Y0) {
   if (!h) return 1;
+  if (h->mapping) return refuse_mapping(h, "init_cluster_cpp");
   if (!h->ran_setup) return fail(h, 3, "setup has not been run");
   CK(cudaSetDevice(h->device));
   HostLap lap(h->stream, "hb_init_cluster");
@@ -474,6 +522,7 @@ int hb_init_cluster(hb_handle* h, const double* Y0) {
 
 int hb_cluster(hb_handle* h, const int64_t* update_orders) {
   if (!h) return 1;
+  if (h->mapping) return refuse_mapping(h, "cluster_cpp");
   if (!h->ran_init) return fail(h, 3, "init_cluster_cpp has not been run");
   CK(cudaSetDevice(h->device));
   const unsigned T = h->max_iter_kmeans;
@@ -547,6 +596,7 @@ int hb_cluster(hb_handle* h, const int64_t* update_orders) {
 
 int hb_moe_correct_ridge(hb_handle* h) {
   if (!h) return 1;
+  if (h->mapping) return refuse_mapping(h, "moe_correct_ridge_cpp");
   if (!h->ran_init) return fail(h, 3, "init_cluster_cpp has not been run");
   CK(cudaSetDevice(h->device));
   TRY(run_correct(h));
@@ -557,6 +607,7 @@ int hb_moe_correct_ridge(hb_handle* h) {
 
 int hb_check_convergence(hb_handle* h, int type) {
   if (!h) return -1;
+  if (h->mapping) return -refuse_mapping(h, "check_convergence");
   int out = 1;
   int st = check_convergence_host(h, type, &out);
   if (st != 0) return -st;
@@ -565,6 +616,7 @@ int hb_check_convergence(hb_handle* h, int type) {
 
 int hb_compute_objective(hb_handle* h) {
   if (!h) return 1;
+  if (h->mapping) return refuse_mapping(h, "compute_objective");
   if (!h->ran_init) return fail(h, 3, "init_cluster_cpp has not been run");
   CK(cudaSetDevice(h->device));
   CK(cudaMemsetAsync(h->obj_acc.p, 0, 2 * sizeof(double), h->stream));
@@ -597,6 +649,8 @@ int hb_get_field(hb_handle* h, int field, double* out) {
   if (!h) return 1;
   if (!h->ran_setup) return fail(h, 3, "setup has not been run");
   if (!out) return fail(h, 2, "null output");
+  if (h->mapping && (field == HB_W || field == HB_THETA || field == HB_LAMBDA))
+    return fail(h, 3, "field %d belongs to a Harmony run, not to a mapped query", field);
   CK(cudaSetDevice(h->device));
   const int K = h->K, B = h->B, d = h->d;
   const RowField f = row_field(h, field);
@@ -672,6 +726,7 @@ int hb_set_field(hb_handle* h, int field, const double* in) {
   if (!h) return 1;
   if (!h->ran_setup) return fail(h, 3, "setup has not been run");
   if (!in) return fail(h, 2, "null input");
+  if (h->mapping) return fail(h, 3, "the fields of a mapped query are read-only");
   CK(cudaSetDevice(h->device));
   const int K = h->K, B = h->B, d = h->d;
   if (field == HB_Z_CORR || field == HB_R) {

@@ -600,6 +600,105 @@ struct SolveArgs {
   float alpha, cutoff;
 };
 
+// The inverse of the m x m ridge matrix G (column-major) into inv, and W = inv * s, shared by k_ridge_solve and
+// k_map_solve.  Every thread of the CTA calls them.
+// Arrowhead closed form (harmony.cpp:575-586): G is zero outside row 0, column 0 and the diagonal (one covariate).
+// sh_f: one shared float.
+__device__ void ridge_inverse_arrowhead(const float* G, float* inv, int m, float* sh_f) {
+  const int tid = threadIdx.x, nt = blockDim.x;
+  if (tid == 0) {
+    float accum = 0.f;
+    for (int j = 1; j < m; ++j) {
+      float ac = -G[(size_t)j * m];
+      float bj = 1.f / G[(size_t)j * m + j];
+      accum += (ac * ac) * bj;
+    }
+    sh_f[0] = G[0] - accum;  // u
+  }
+  __syncthreads();
+  const float u = sh_f[0];
+  for (int idx = tid; idx < m * m; idx += nt) {
+    int r = idx % m, c = idx / m;
+    float acr = (r == 0) ? 1.f : (-G[(size_t)r * m]) * (1.f / G[(size_t)r * m + r]);
+    float acc_ = (c == 0) ? 1.f : (-G[(size_t)c * m]) * (1.f / G[(size_t)c * m + c]);
+    float v = (1.f / u) * (acr * acc_);
+    if (r == c && r > 0) v += 1.f / G[(size_t)r * m + r];
+    inv[idx] = v;
+  }
+  __syncthreads();
+}
+// Gauss-Jordan with partial pivoting (arma::inv -> getrf/getri, :573); G is overwritten.  A zero or non-finite pivot
+// sets *err_flag = 2.  sh_piv: one shared int, sh_f: one shared float.
+__device__ void ridge_inverse_gj(float* G, float* inv, int m, int* sh_piv, float* sh_f, int* err_flag) {
+  const int tid = threadIdx.x, nt = blockDim.x;
+  for (int idx = tid; idx < m * m; idx += nt) inv[idx] = ((idx % m) == (idx / m)) ? 1.f : 0.f;
+  __syncthreads();
+  for (int c = 0; c < m; ++c) {
+    if (tid == 0) {
+      int piv = c;
+      float best = fabsf(G[c + (size_t)c * m]);
+      for (int r = c + 1; r < m; ++r) {
+        float v = fabsf(G[r + (size_t)c * m]);
+        if (v > best) {
+          best = v;
+          piv = r;
+        }
+      }
+      *sh_piv = piv;
+      if (!(best > 0.f) || !isfinite(best)) atomicExch(err_flag, 2);
+    }
+    __syncthreads();
+    const int piv = *sh_piv;
+    if (piv != c) {
+      for (int j = tid; j < m; j += nt) {
+        float t = G[c + (size_t)j * m];
+        G[c + (size_t)j * m] = G[piv + (size_t)j * m];
+        G[piv + (size_t)j * m] = t;
+        t = inv[c + (size_t)j * m];
+        inv[c + (size_t)j * m] = inv[piv + (size_t)j * m];
+        inv[piv + (size_t)j * m] = t;
+      }
+      __syncthreads();
+    }
+    if (tid == 0) *sh_f = G[c + (size_t)c * m];
+    __syncthreads();
+    const float p = *sh_f;
+    for (int j = tid; j < m; j += nt) {
+      G[c + (size_t)j * m] /= p;
+      inv[c + (size_t)j * m] /= p;
+    }
+    __syncthreads();
+    // eliminate column c from every other row: thread per (row, col) pair
+    for (int idx = tid; idx < m * m; idx += nt) {
+      int r = idx % m, j = idx / m;
+      if (r == c) continue;
+      float f = G[r + (size_t)c * m];
+      if (j == c) continue;  // column c itself is cleared afterwards
+      G[r + (size_t)j * m] -= f * G[c + (size_t)j * m];
+    }
+    for (int idx = tid; idx < m * m; idx += nt) {
+      int r = idx % m, j = idx / m;
+      if (r == c) continue;
+      float f = G[r + (size_t)c * m];
+      inv[r + (size_t)j * m] -= f * inv[c + (size_t)j * m];
+    }
+    __syncthreads();
+    for (int r = tid; r < m; r += nt)
+      if (r != c) G[r + (size_t)c * m] = 0.f;
+    __syncthreads();
+  }
+}
+// W = inv * s (:599-609) for s [m][d]: store(r, c, W[r][c]) for every row r < m and column c < d
+template <typename F>
+__device__ void ridge_weights(const float* inv, const float* sv, int m, int d, F store) {
+  for (int idx = threadIdx.x; idx < m * d; idx += blockDim.x) {
+    int r = idx / d, c = idx - r * d;
+    float w = 0.f;
+    for (int j = 0; j < m; ++j) w += inv[r + (size_t)j * m] * sv[(size_t)j * d + c];
+    store(r, c, w);
+  }
+}
+
 __global__ void __launch_bounds__(256) k_ridge_solve(SolveArgs a) {
   const int k = blockIdx.x, tid = threadIdx.x, nt = blockDim.x;
   const int J = a.J, K = a.K, B = a.B, C = a.C, d = a.d, D1 = d + 1, M = B + 1;
@@ -698,100 +797,19 @@ __global__ void __launch_bounds__(256) k_ridge_solve(SolveArgs a) {
   if (tid == 0 && a.lambda) G[0] += a.lambda[0];
   __syncthreads();
   // ---- inverse
-  if (C == 1) {
-    // arrowhead closed form (:575-586)
-    if (tid == 0) {
-      float accum = 0.f;
-      for (int j = 1; j < m; ++j) {
-        float ac = -G[(size_t)j * m];
-        float bj = 1.f / G[(size_t)j * m + j];
-        accum += (ac * ac) * bj;
-      }
-      sh_f[0] = G[0] - accum;  // u
-    }
-    __syncthreads();
-    const float u = sh_f[0];
-    for (int idx = tid; idx < m * m; idx += nt) {
-      int r = idx % m, c = idx / m;
-      float acr = (r == 0) ? 1.f : (-G[(size_t)r * m]) * (1.f / G[(size_t)r * m + r]);
-      float acc_ = (c == 0) ? 1.f : (-G[(size_t)c * m]) * (1.f / G[(size_t)c * m + c]);
-      float v = (1.f / u) * (acr * acc_);
-      if (r == c && r > 0) v += 1.f / G[(size_t)r * m + r];
-      inv[idx] = v;
-    }
-    __syncthreads();
-  } else {
-    // Gauss-Jordan with partial pivoting (arma::inv -> getrf/getri, :573); column-major m x m
-    for (int idx = tid; idx < m * m; idx += nt) inv[idx] = ((idx % m) == (idx / m)) ? 1.f : 0.f;
-    __syncthreads();
-    for (int c = 0; c < m; ++c) {
-      if (tid == 0) {
-        int piv = c;
-        float best = fabsf(G[c + (size_t)c * m]);
-        for (int r = c + 1; r < m; ++r) {
-          float v = fabsf(G[r + (size_t)c * m]);
-          if (v > best) {
-            best = v;
-            piv = r;
-          }
-        }
-        sh_piv = piv;
-        if (!(best > 0.f) || !isfinite(best)) atomicExch(a.err_flag, 2);
-      }
-      __syncthreads();
-      const int piv = sh_piv;
-      if (piv != c) {
-        for (int j = tid; j < m; j += nt) {
-          float t = G[c + (size_t)j * m];
-          G[c + (size_t)j * m] = G[piv + (size_t)j * m];
-          G[piv + (size_t)j * m] = t;
-          t = inv[c + (size_t)j * m];
-          inv[c + (size_t)j * m] = inv[piv + (size_t)j * m];
-          inv[piv + (size_t)j * m] = t;
-        }
-        __syncthreads();
-      }
-      if (tid == 0) sh_f[1] = G[c + (size_t)c * m];
-      __syncthreads();
-      const float p = sh_f[1];
-      for (int j = tid; j < m; j += nt) {
-        G[c + (size_t)j * m] /= p;
-        inv[c + (size_t)j * m] /= p;
-      }
-      __syncthreads();
-      // eliminate column c from every other row: thread per (row, col) pair
-      // first snapshot the factors (column c of G) into sv's tail? use registers per row instead:
-      for (int idx = tid; idx < m * m; idx += nt) {
-        int r = idx % m, j = idx / m;
-        if (r == c) continue;
-        float f = G[r + (size_t)c * m];
-        if (j == c) continue;  // column c itself is cleared afterwards
-        G[r + (size_t)j * m] -= f * G[c + (size_t)j * m];
-      }
-      for (int idx = tid; idx < m * m; idx += nt) {
-        int r = idx % m, j = idx / m;
-        if (r == c) continue;
-        float f = G[r + (size_t)c * m];
-        inv[r + (size_t)j * m] -= f * inv[c + (size_t)j * m];
-      }
-      __syncthreads();
-      for (int r = tid; r < m; r += nt)
-        if (r != c) G[r + (size_t)c * m] = 0.f;
-      __syncthreads();
-    }
-  }
+  if (C == 1)
+    ridge_inverse_arrowhead(G, inv, m, &sh_f[0]);
+  else
+    ridge_inverse_gj(G, inv, m, &sh_piv, &sh_f[1], a.err_flag);
   // ---- W = inv * s  (:599-609), Y[k] = W[0] (:610), W[0] = 0 (:611)
   for (int idx = tid; idx < M * d; idx += nt) Wk[idx] = 0.f;
   __syncthreads();
-  for (int idx = tid; idx < m * d; idx += nt) {
-    int r = idx / d, c = idx - r * d;
-    float w = 0.f;
-    for (int j = 0; j < m; ++j) w += inv[r + (size_t)j * m] * sv[(size_t)j * d + c];
+  ridge_weights(inv, sv, m, d, [&](int r, int c, float w) {
     if (r == 0)
       a.Y[(size_t)k * d + c] = w;
     else
       Wk[(size_t)(keep[r - 1] + 1) * d + c] = w;
-  }
+  });
   __syncthreads();
   // ---- Y = normalise(Y, 2, 0) (:633) for this column
   if (tid < 32) {
@@ -814,6 +832,109 @@ __global__ void __launch_bounds__(256) k_ridge_solve(SolveArgs a) {
         int b = a.tuple_levels[q * C + c1];
         if (pos[b] >= 0) v += Wk[(size_t)(b + 1) * d + c];
       }
+    a.V[((size_t)q * K + k) * d + c] = v;
+  }
+}
+
+// ------------------------------------------------------------------------------------------------
+// Mapping (map_host.cuh): the compression of a reference and the solve of a query against it.
+// ------------------------------------------------------------------------------------------------
+// out[k] = {Cref[k][0..d), Nr[k], Yref[k][0..d)} from the per-tuple sums S[q][k][0..d] of Z_corr (column d: sum R):
+// Cref_k = sum_i R_ki z_i, Nr_k = sum_i R_ki, Yref_k = Cref_k / |Cref_k| (a zero row stays zero).  One block per
+// cluster; the tuples are added in double.
+__global__ void k_reference_fold(const float* __restrict__ S, double* __restrict__ out, int J, int K, int d) {
+  extern __shared__ double fold[];  // [d + 1]
+  __shared__ double nrm;
+  const int k = blockIdx.x, D1 = d + 1;
+  for (int c = threadIdx.x; c < D1; c += blockDim.x) {
+    double t = 0.0;
+    for (int q = 0; q < J; ++q) t += (double)S[((size_t)q * K + k) * D1 + c];
+    fold[c] = t;
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    double ss = 0.0;
+    for (int c = 0; c < d; ++c) ss += fold[c] * fold[c];
+    nrm = ss > 0.0 ? sqrt(ss) : 1.0;
+  }
+  __syncthreads();
+  double* o = out + (size_t)k * (2 * d + 1);
+  for (int c = threadIdx.x; c < D1; c += blockDim.x) {
+    o[c] = fold[c];
+    if (c < d) o[D1 + c] = fold[c] / nrm;
+  }
+}
+
+// The query's ridge solve against a reference, one CTA per cluster.  With x_i = [1; one-hot levels of cell i]:
+//   G_k = sum_i R_ki x_i x_i^T + diag(0, lambda) + Nr_k e_0 e_0^T,   s_k = sum_i R_ki x_i z_i^T + e_0 Cref_k,
+//   W_k = G_k^-1 s_k with row 0 zeroed,   V[q][k] = the sum of W_k's rows of tuple q's levels.
+// Every level takes part (no cutoff filter) and lambda is fixed.  A cluster with G_k[0][0] == 0 (no reference mass,
+// the query's underflowed) gets V = 0.
+struct MapSolveArgs {
+  const float* S;           // [J][K][d+1] query statistics R^T [Z | 1] per tuple
+  const float* Nr;          // [K]
+  const float* Cref;        // [K][d]
+  const float* lambda;      // [B+1], lambda[0] = 0
+  const int* tuple_levels;  // [J][C]
+  float* V;                 // [J][K][d]
+  float* scratch;           // [K][ 2*M*M + 2*M*d ]  (G | inv | s | W),  M = B+1
+  int* err_flag;
+  int J, K, B, C, d;
+};
+
+__global__ void __launch_bounds__(256) k_map_solve(MapSolveArgs a) {
+  const int k = blockIdx.x, tid = threadIdx.x, nt = blockDim.x;
+  const int J = a.J, K = a.K, C = a.C, d = a.d, D1 = d + 1, m = a.B + 1;
+  __shared__ float sh_f;
+  __shared__ int sh_piv;
+  float* G = a.scratch + (size_t)k * (2 * (size_t)m * m + 2 * (size_t)m * d);
+  float* inv = G + (size_t)m * m;
+  float* sv = inv + (size_t)m * m;  // [m][d]
+  float* W = sv + (size_t)m * d;    // [m][d]
+  for (int idx = tid; idx < m * m; idx += nt) G[idx] = 0.f;
+  __syncthreads();
+  // ---- G from the per-tuple masses n_kq = S[q][k][d]
+  for (int q = tid; q < J; q += nt) {
+    float nq = a.S[((size_t)q * K + k) * D1 + d];
+    atomicAdd(&G[0], nq);
+    for (int c1 = 0; c1 < C; ++c1) {
+      int p1 = a.tuple_levels[q * C + c1] + 1;
+      atomicAdd(&G[(size_t)p1 * m], nq);  // row 0
+      atomicAdd(&G[(size_t)p1], nq);      // col 0
+      for (int c2 = 0; c2 < C; ++c2) atomicAdd(&G[(size_t)(a.tuple_levels[q * C + c2] + 1) * m + p1], nq);
+    }
+  }
+  // ---- s: thread per embedding column, serial over tuples; row 0 takes the reference's Cref_k
+  for (int c = tid; c < d; c += nt) {
+    for (int r = 0; r < m; ++r) sv[(size_t)r * d + c] = 0.f;
+    for (int q = 0; q < J; ++q) {
+      float v = a.S[((size_t)q * K + k) * D1 + c];
+      sv[c] += v;
+      for (int c1 = 0; c1 < C; ++c1) sv[(size_t)(a.tuple_levels[q * C + c1] + 1) * d + c] += v;
+    }
+    sv[c] += a.Cref[(size_t)k * d + c];
+  }
+  __syncthreads();
+  for (int j = tid; j < m - 1; j += nt) G[(size_t)(j + 1) * m + (j + 1)] += a.lambda[j + 1];
+  if (tid == 0) G[0] += a.Nr[k];
+  __syncthreads();
+  if (G[0] == 0.f) {
+    for (int idx = tid; idx < J * d; idx += nt) {
+      int q = idx / d, c = idx - q * d;
+      a.V[((size_t)q * K + k) * d + c] = 0.f;
+    }
+    return;
+  }
+  if (C == 1)
+    ridge_inverse_arrowhead(G, inv, m, &sh_f);
+  else
+    ridge_inverse_gj(G, inv, m, &sh_piv, &sh_f, a.err_flag);
+  ridge_weights(inv, sv, m, d, [&](int r, int c, float w) { W[(size_t)r * d + c] = r == 0 ? 0.f : w; });
+  __syncthreads();
+  for (int idx = tid; idx < J * d; idx += nt) {
+    int q = idx / d, c = idx - q * d;
+    float v = 0.f;
+    for (int c1 = 0; c1 < C; ++c1) v += W[(size_t)(a.tuple_levels[q * C + c1] + 1) * d + c];
     a.V[((size_t)q * K + k) * d + c] = v;
   }
 }

@@ -99,28 +99,7 @@ class harmony:
         ``Z`` may also be a float32 / float64 CUDA tensor on the object's device, in either orientation: it is read
         where it lies (no host round trip), after the work queued on the device's current torch stream.  With such a
         ``Z``, ``Phi`` may be an int32 / int64 CUDA tensor ([N] or [N, C]) on the same device, read the same way."""
-        dev = is_cuda_tensor(Z)
-        if not dev:
-            Z = np.asarray(Z)
-        if is_cuda_tensor(Phi):
-            if not dev:
-                raise ValueError("Phi is a CUDA tensor but Z is not: device labels go with a device embedding")
-            phi_i = self._device_Phi(Phi)             # alive until the call returns
-        else:
-            phi_i = np.ascontiguousarray(Phi, dtype=np.int32)
-            if phi_i.ndim == 1:
-                phi_i = phi_i.reshape(-1, 1)
-        n = phi_i.shape[0]
-        if Z.ndim != 2:
-            raise ValueError("Z must be a matrix")
-        if Z.shape[0] != n and Z.shape[1] == n:
-            Z = Z.T                                   # d x N given: its transpose view is the same memory order
-        if Z.shape[0] != n:
-            raise ValueError("number of cells in Z and Phi differ")
-        if dev:
-            Z, z_args = self._device_Z(Z)             # Z: the tensor read, alive until the call returns
-        else:
-            Z = np.ascontiguousarray(Z, dtype=np.float64)
+        dev, Z, z_args, phi_i, phi_ptr, n = self._cell_inputs(Z, Phi)
         B_vec = np.ascontiguousarray(np.atleast_1d(B_vec), dtype=np.int32)
         K = int(K)
         sigma = np.ascontiguousarray(np.broadcast_to(np.asarray(sigma, dtype=np.float64), (K,)))
@@ -134,7 +113,6 @@ class harmony:
                 lam = None
             elif len(lam) != int(B_vec.sum()) + 1:
                 raise ValueError("lambda must hold B+1 values")
-        phi_ptr = ctypes.c_void_p(phi_i.data_ptr()) if is_cuda_tensor(phi_i) else _ptr(phi_i)
         rest = (Z.shape[1], n, phi_ptr, _ptr(B_vec), len(B_vec), _ptr(sigma), _ptr(theta),
                 None if lam is None else _ptr(lam), float(alpha), int(max_iter_kmeans), float(epsilon_kmeans),
                 float(epsilon_harmony), K, float(block_size), float(batch_proportion_cutoff), int(bool(verbose)))
@@ -142,6 +120,72 @@ class harmony:
             self._check(self._L.hb_setup_device(self._h, *z_args, *rest))
         else:
             self._check(self._L.hb_setup(self._h, _ptr(Z), *rest))
+
+    def _cell_inputs(self, Z, Phi):
+        """The per-cell inputs of setup and map_setup: Z ([N, d] or [d, N], host array or CUDA tensor) and Phi ([N] or
+        [N, C]) -> (Z on device, Z to read, its hb_*_device arguments (None for host Z), phi_i, phi_i's pointer, N).
+        The returned arrays and tensors must stay alive until the library call returns."""
+        dev = is_cuda_tensor(Z)
+        if not dev:
+            Z = np.asarray(Z)
+        if is_cuda_tensor(Phi):
+            if not dev:
+                raise ValueError("Phi is a CUDA tensor but Z is not: device labels go with a device embedding")
+            phi_i = self._device_Phi(Phi)
+        else:
+            phi_i = np.ascontiguousarray(Phi, dtype=np.int32)
+            if phi_i.ndim == 1:
+                phi_i = phi_i.reshape(-1, 1)
+        n = phi_i.shape[0]
+        if Z.ndim != 2:
+            raise ValueError("Z must be a matrix")
+        if Z.shape[0] != n and Z.shape[1] == n:
+            Z = Z.T                                   # d x N given: its transpose view is the same memory order
+        if Z.shape[0] != n:
+            raise ValueError("number of cells in Z and Phi differ")
+        z_args = None
+        if dev:
+            Z, z_args = self._device_Z(Z)
+        else:
+            Z = np.ascontiguousarray(Z, dtype=np.float64)
+        phi_ptr = ctypes.c_void_p(phi_i.data_ptr()) if is_cuda_tensor(phi_i) else _ptr(phi_i)
+        return dev, Z, z_args, phi_i, phi_ptr, n
+
+    # ---- mapping a query onto a finished integration (DESIGN.md §8) ----------------------------
+    def reference(self):
+        """The compression of this integration (any state after init_cluster_cpp; normally after harmonize) as a
+        HarmonyReference: per cluster Nr = sum R, Cref = R Z_corr^T (the Z_corr getZcorr() returns), the normalised
+        centroids Cref / |Cref| and sigma."""
+        from .mapping import HarmonyReference
+        K, d = self._scalar("K"), self._scalar("d")
+        Y, Nr, Cref, sigma = np.empty((K, d)), np.empty(K), np.empty((K, d)), np.empty(K)
+        self._check(self._L.hb_reference(self._h, _ptr(Y), _ptr(Nr), _ptr(Cref), _ptr(sigma)))
+        return HarmonyReference(Y, Nr, Cref, sigma)
+
+    def map_setup(self, Z, Phi, B_vec, lambda_, reference):
+        """Sets this object up to map a query onto ``reference`` (a HarmonyReference), instead of ``setup``.  ``Z``
+        and ``Phi`` take setup's forms (host arrays or CUDA tensors); ``Phi`` and ``B_vec`` describe the query's own
+        covariates; ``lambda_``: a scalar or one value per query level, each finite and > 0."""
+        K, d = reference.K, reference.d
+        dev, Z, z_args, phi_i, phi_ptr, n = self._cell_inputs(Z, Phi)
+        if Z.shape[1] != d:
+            raise ValueError(f"the query has {Z.shape[1]} dimensions, the reference {d}")
+        B_vec = np.ascontiguousarray(np.atleast_1d(B_vec), dtype=np.int32)
+        lam = np.ascontiguousarray(np.broadcast_to(np.asarray(lambda_, dtype=np.float64).reshape(-1),
+                                                   (int(B_vec.sum()),)))
+        ref = [np.ascontiguousarray(a, dtype=np.float64) for a in
+               (reference.centroids, reference.Nr, reference.Cref, reference.sigma)]
+        rest = (d, n, phi_ptr, _ptr(B_vec), len(B_vec), _ptr(lam), K, *(_ptr(a) for a in ref))
+        if dev:
+            self._check(self._L.hb_map_setup_device(self._h, *z_args, *rest))
+        else:
+            self._check(self._L.hb_map_setup(self._h, _ptr(Z), *rest))
+
+    def map(self):
+        """Maps the query set up by map_setup: soft assignment to the reference's clusters, then one ridge correction
+        anchored on the reference.  getZcorr() / get_tensor("Z_corr") then hold the mapped embedding, getR() the
+        assignment."""
+        self._check(self._L.hb_map(self._h))
 
     def _device_Z(self, Z):
         """An [N, d] CUDA tensor -> (the tensor to read, (pointer, dtype, row stride, stream) of hb_setup_device)).

@@ -52,22 +52,9 @@ def _label_device(cols, vars_use, data_mat, on_device):
     return device
 
 
-def prepare_inputs(data_mat, meta_data, vars_use=None, theta=None, sigma=0.1, lambda_=None, nclust=None,
-                   early_stop=True, options=None, verbose=False):
-    """Everything RunHarmony.default computes before ``new(harmony)`` (R/ui.R:133-258).
-
-    Returns a dict with the exact argument list of ``harmony::setup`` (src/harmony.h:25-30), with
-    the sparse ``phi`` expressed as its row-index slot: ``phi_i[n, c]`` = row of the c-th non-zero of
-    column n (each cell has exactly one level per covariate, so columns hold C non-zeros).
-
-    With a CUDA ``data_mat``, a used metadata column (or the bare vector) may be an integer or bool CUDA tensor on the
-    same device: it is factorised there, and ``phi_i`` is then an [N, C] int32 CUDA tensor (host columns are
-    factorised as usual and copied over).  ``level_names`` are always host arrays.
-    """
-    options = harmony_options() if options is None else options
-    if not isinstance(options, HarmonyOptions):
-        raise TypeError("Error: .options must be created from harmony_options()!")
-    epsilon_harmony = options.epsilon_harmony if early_stop else -math.inf
+def _cells_and_columns(data_mat, meta_data, vars_use, verbose):
+    """data_mat, meta_data and vars_use of RunHarmony / MapQuery -> (on_device, data_mat, cols, vars_use, N, Z) with Z
+    the [N, d] view of data_mat (R/ui.R:157-189)."""
     on_device = is_cuda_tensor(data_mat)   # stays where it is: setup reads it on its device
     if not on_device:
         data_mat = np.asarray(data_mat)
@@ -93,18 +80,13 @@ def prepare_inputs(data_mat, meta_data, vars_use=None, theta=None, sigma=0.1, la
         Z = data_mat.T
     else:
         raise ValueError("number of labels do not correspond to number of samples in data matrix")
-    if nclust is None:
-        nclust = min(int(round(N / 30.0)), 100)
-    if theta is None:
-        theta = [2.0] * len(vars_use)
-    else:
-        theta = list(np.atleast_1d(np.asarray(theta, dtype=np.float64)))
-        if len(theta) != len(vars_use):
-            raise ValueError("Please specify theta for each variable")
-    sigma = np.atleast_1d(np.asarray(sigma, dtype=np.float64))
-    if len(sigma) == 1 and nclust > 1:
-        sigma = np.repeat(sigma, nclust)
-    # phi / B_vec: as.factor levels = sorted unique values (R/ui.R:210-221)
+    return on_device, data_mat, cols, vars_use, N, Z
+
+
+def _factorise(cols, vars_use, data_mat, on_device):
+    """The used label columns -> (phi_i [N, C], B_vec, level_names, N_b): as.factor levels = sorted unique values
+    (R/ui.R:210-221), global level ids in phi_i.  Device label columns are factorised on their device, and phi_i is
+    then an int32 CUDA tensor (host columns are copied over)."""
     phi_cols, B_vec, level_names = [], [], []
     offset = 0
     device = _label_device(cols, vars_use, data_mat, on_device)
@@ -133,6 +115,39 @@ def prepare_inputs(data_mat, meta_data, vars_use=None, theta=None, sigma=0.1, la
         import torch
         phi_i = torch.stack(phi_cols, dim=1).contiguous()             # [N, C] int32 on the embedding's device
         N_b = torch.bincount(phi_i.reshape(-1), minlength=B).cpu().numpy().astype(np.float64)
+    return phi_i, B_vec, level_names, N_b
+
+
+def prepare_inputs(data_mat, meta_data, vars_use=None, theta=None, sigma=0.1, lambda_=None, nclust=None,
+                   early_stop=True, options=None, verbose=False):
+    """Everything RunHarmony.default computes before ``new(harmony)`` (R/ui.R:133-258).
+
+    Returns a dict with the exact argument list of ``harmony::setup`` (src/harmony.h:25-30), with
+    the sparse ``phi`` expressed as its row-index slot: ``phi_i[n, c]`` = row of the c-th non-zero of
+    column n (each cell has exactly one level per covariate, so columns hold C non-zeros).
+
+    With a CUDA ``data_mat``, a used metadata column (or the bare vector) may be an integer or bool CUDA tensor on the
+    same device: it is factorised there, and ``phi_i`` is then an [N, C] int32 CUDA tensor (host columns are
+    factorised as usual and copied over).  ``level_names`` are always host arrays.
+    """
+    options = harmony_options() if options is None else options
+    if not isinstance(options, HarmonyOptions):
+        raise TypeError("Error: .options must be created from harmony_options()!")
+    epsilon_harmony = options.epsilon_harmony if early_stop else -math.inf
+    on_device, data_mat, cols, vars_use, N, Z = _cells_and_columns(data_mat, meta_data, vars_use, verbose)
+    if nclust is None:
+        nclust = min(int(round(N / 30.0)), 100)
+    if theta is None:
+        theta = [2.0] * len(vars_use)
+    else:
+        theta = list(np.atleast_1d(np.asarray(theta, dtype=np.float64)))
+        if len(theta) != len(vars_use):
+            raise ValueError("Please specify theta for each variable")
+    sigma = np.atleast_1d(np.asarray(sigma, dtype=np.float64))
+    if len(sigma) == 1 and nclust > 1:
+        sigma = np.repeat(sigma, nclust)
+    phi_i, B_vec, level_names, N_b = _factorise(cols, vars_use, data_mat, on_device)
+    B = sum(B_vec)
     if lambda_ is None:                                               # R/ui.R:224-229
         lambda_vec = None
     else:
@@ -203,3 +218,46 @@ def RunHarmony(data_mat, meta_data, vars_use=None, theta=None, sigma=0.1, lambda
     if is_cuda_tensor(data_mat):
         return obj.get_tensor("Z_corr", dtype=data_mat.dtype)
     return np.ascontiguousarray(obj.getZcorr().T)   # t(harmonyObj$getZcorr()), R/ui.R:292-295: cells x PCs
+
+
+def MapQuery(data_mat, meta_data, vars_use, reference, lambda_=1.0, return_object=False, verbose=True, device=None):
+    """Maps query cells onto a finished integration in one pass, without rerunning Harmony (DESIGN.md §8).
+
+    ``data_mat``: the query's embedding in the reference's PC space (projecting genes onto the PCs is the caller's
+    job), [Nq, d] or [d, Nq], a host array or a float32 / float64 CUDA tensor, with ``meta_data`` / ``vars_use`` naming
+    the query's own covariates exactly as in RunHarmony (device labels included).  ``reference``: a HarmonyReference
+    (``harmony.reference()``, or ``HarmonyReference.load``).  ``lambda_``: ridge penalty of the query's levels, a scalar
+    or one value per covariate, each > 0.
+
+    Every query cell is softly assigned to the reference's clusters; then one ridge correction per cluster, whose
+    intercept the reference's statistics anchor, removes the query's batch terms.  The reference's cells do not move.
+    Returns the mapped embedding [Nq, d] (numpy, or a CUDA tensor of data_mat's dtype on its device) or, with
+    ``return_object``, the harmony object (getR() is the query's assignment)."""
+    from .mapping import HarmonyReference
+    if not isinstance(reference, HarmonyReference):
+        raise TypeError("reference must be a HarmonyReference (harmony.reference() or HarmonyReference.load)")
+    on_device, data_mat, cols, vars_use, N, Z = _cells_and_columns(data_mat, meta_data, vars_use, verbose)
+    if Z.shape[1] != reference.d:
+        raise ValueError(f"the query has {Z.shape[1]} dimensions, the reference {reference.d}")
+    lam = np.atleast_1d(np.asarray(lambda_, dtype=np.float64))
+    if not np.all(np.isfinite(lam) & (lam > 0)):
+        raise ValueError("Provided lambdas must be positive")
+    if len(lam) not in (1, len(vars_use)):
+        raise ValueError(f"lambda_ must be one value or one per covariate ({len(vars_use)}), not {len(lam)}")
+    if on_device:
+        if device is not None and int(device) != data_mat.device.index:
+            raise ValueError(f"device={device} differs from the device of data_mat ({data_mat.device})")
+        device = data_mat.device.index
+    phi_i, B_vec, _, _ = _factorise(cols, vars_use, data_mat, on_device)
+    lambda_vec = np.repeat(lam, B_vec) if len(lam) > 1 else np.repeat(lam, sum(B_vec))
+    from .harmony import harmony  # needs the CUDA extension; fails loudly when it is missing
+    obj = harmony(device=device)
+    if verbose:
+        print(f"Mapping {N} cells onto a {reference.K}-cluster reference", file=sys.stderr)
+    obj.map_setup(Z, phi_i, np.asarray(B_vec, dtype=np.int32), lambda_vec, reference)
+    obj.map()
+    if return_object:
+        return obj
+    if on_device:
+        return obj.get_tensor("Z_corr", dtype=data_mat.dtype)
+    return np.ascontiguousarray(obj.getZcorr().T)

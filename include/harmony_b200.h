@@ -42,7 +42,8 @@ const char* hb_last_error(const hb_handle* h);
 /* Pops one pending warning (e.g. "Too few cells. Setting block_size to 0.2", harmony.cpp:86-88) into
  * buf; returns 1 if a warning was written, 0 if none is pending.  The shim turns it into Rcpp::warning. */
 int hb_pop_warning(hb_handle* h, char* buf, size_t cap);
-/* Library/ABI version: major*10000 + minor*100 + patch (0.3.0: labels in device memory). */
+/* Library/ABI version: major*10000 + minor*100 + patch (0.3.0: labels in device memory; 0.4.0: mapping a query onto
+ * a reference, hb_reference / hb_map_setup / hb_map). */
 int hb_version(void);
 
 /* ---- multi-GPU (one process per GPU; cells sharded contiguously; SURVEY §8e) ------------------- */
@@ -109,6 +110,37 @@ int hb_check_convergence(hb_handle* h, int type);
 
 /* ---- harmony::compute_objective (harmony.cpp:158-170): appends to the four objective traces --- */
 int hb_compute_objective(hb_handle* h);
+
+/* ---- mapping a query onto a finished integration (DESIGN.md §8) -------------------------------- */
+/* The compression of the integration the handle holds (any state after hb_init_cluster), per cluster k, from the
+ * Z_corr getZcorr() returns and R: Nr[k] = sum_n R[k,n], Cref[:,k] = sum_n R[k,n] Z_corr[:,n], centroids[:,k] =
+ * Cref[:,k] / |Cref[:,k]| (a zero column stays zero), and sigma.  centroids and Cref are d x K column-major, Nr and
+ * sigma K values; NULL outputs are skipped.  Status 3 before hb_init_cluster, on a sharded handle (world > 1) and on a
+ * mapping handle.  Region "reference". */
+int hb_reference(hb_handle* h, double* centroids, double* Nr, double* Cref, double* sigma);
+/* Sets a handle up to map Nq query cells onto a reference, instead of hb_setup.  Z: d x Nq column-major doubles in the
+ * reference's PC space; phi_i / B_vec / C: the query's own covariates (hb_setup's form, B_q = sum(B_vec) levels);
+ * lambda: B_q ridge penalties, one per query level, finite and > 0; K, centroids, Nr, Cref, sigma: hb_reference's
+ * output.  Any Nq >= 1.  Status 2 for a NULL argument, bad dimensions, lambda <= 0 or non-finite, sigma non-finite or
+ * <= 0, Nr < 0, non-finite centroids or Cref, or labels outside their covariate's levels; status 3 if the handle already
+ * ran a setup or is sharded (hb_comm_init with world > 1, or hb_set_shard).  HB_KERNEL_SET is read here as in hb_setup.
+ * phi_i must be host or managed memory. */
+int hb_map_setup(hb_handle* h, const double* Z, int d, int64_t N, const int32_t* phi_i, const int32_t* B_vec, int C,
+                 const double* lambda, int K, const double* centroids, const double* Nr, const double* Cref,
+                 const double* sigma);
+/* hb_map_setup with Z (and optionally phi_i) in device memory, with hb_setup_device's dtype, row stride, stream and
+ * pointer conventions and checks. */
+int hb_map_setup_device(hb_handle* h, const void* Z, int z_dtype, int64_t z_ld, void* stream, int d, int64_t N,
+                        const int32_t* phi_i, const int32_t* B_vec, int C, const double* lambda, int K,
+                        const double* centroids, const double* Nr, const double* Cref, const double* sigma);
+/* Maps the query of a handle set up by hb_map_setup*: R_q = softmax_k(-2 (1 - Yref_k . z_n / |z_n|) / sigma_k), then
+ * one ridge correction per cluster in which Nr_k and Cref_k anchor the intercept and only the query's level terms are
+ * fitted (no level filter, fixed lambda, the centroids unchanged).  Afterwards HB_Z_CORR is the mapped embedding
+ * (hb_get_field and hb_get_field_device), HB_Z_ORIG the input, HB_R R_q, HB_Y the reference's centroids and HB_SIGMA
+ * its sigma.  Repeatable.  Status 3 on a handle set up by hb_setup.  On a mapping handle hb_init_cluster, hb_cluster,
+ * hb_moe_correct_ridge, hb_compute_objective, hb_check_convergence, hb_set_field and the fields HB_W, HB_THETA and
+ * HB_LAMBDA return status 3.  Regions "assign", "ridge_stats", "ridge_solve", "ridge_apply". */
+int hb_map(hb_handle* h);
 
 /* ---- fields / getters (harmony.cpp:640-669, 675-696) ------------------------------------------- */
 enum hb_field {
