@@ -74,6 +74,14 @@ int check_err_flag(hb_handle* h) {
   return 0;
 }
 
+// the K values of sigma must be finite and positive as floats
+int check_sigma(hb_handle* h, const double* sigma, int K) {
+  for (int k = 0; k < K; ++k)
+    if (!(std::isfinite(sigma[k]) && (float)sigma[k] > 0.f))
+      return fail(h, 2, "sigma[%d] = %g: sigma must be finite and positive", k, sigma[k]);
+  return 0;
+}
+
 // sigma0 and sigma_uniform (the update kernels' scalar-sigma form) of the K values of sigma, as floats
 void set_sigma_scalars(hb_handle* h, const double* sigma) {
   h->sigma0 = (float)sigma[0];
@@ -89,23 +97,109 @@ int reserve_rounds(hb_handle* h, int T) {
   return update_reserve(h, T);
 }
 
-// ---- hb_setup and hb_setup_device: checks and scalars, the tuple index, the allocations, the uploads ----------------
-// Source of Z for setup: host doubles (d per row, dense) or a device array of `dtype` with row stride `ld`, read on the
-// library stream after the work queued on `stream`.
-struct ZInput {
+// ---- the setup steps of both kinds of handle: hb_setup* (Harmony) and hb_map_setup* (map_host.cuh) ------------------
+// The cells given to setup: Z as host doubles (d per row, dense) or a device array of `dtype` with row stride `ld`, and
+// the labels phi, read on the library stream after the work queued on `stream`
+struct CellInput {
   const double* host = nullptr;
   const void* dev = nullptr;
   int dtype = HB_FLOAT64;
   int64_t ld = 0;
   cudaStream_t stream = nullptr;
+  const int32_t* phi = nullptr;
+  bool phi_on_device = false;  // else one copy to the device first
 };
 
-int setup_scalars(hb_handle* h, int d, int64_t N, const int32_t* B_vec, int C, const double* lambda, int max_iter_kmeans,
-                  double epsilon_kmeans, double epsilon_harmony, double alpha, int K, double block_size,
-                  double batch_proportion_cutoff, int verbose) {
+// The checks of the cell arguments of setup entry point `entry`, whose Z lies in host or (`z_on_device`) device
+// memory.  A host entry point refuses device labels and copies managed ones; a device entry point reads them in place.
+int setup_inputs(hb_handle* h, const char* entry, const void* Z, bool z_on_device, int dtype, int64_t ld, void* stream,
+                 int d, const int32_t* phi_i, CellInput* in) {
+  if (h->ran_setup) return fail(h, 3, "setup was already run on this object");
+  if (z_on_device) {
+    if (dtype != HB_FLOAT32 && dtype != HB_FLOAT64) return fail(h, 2, "unknown dtype %d of Z", dtype);
+    if (ld < d) return fail(h, 2, "row stride of Z (%lld) is smaller than d = %d", (long long)ld, d);
+    TRY(check_device_ptr(h, Z, "Z"));
+  }
+  cudaMemoryType phi_type;
+  TRY(phi_location(h, phi_i, &phi_type));
+  if (!z_on_device && phi_type == cudaMemoryTypeDevice)
+    return fail(h, 2, "phi_i is device memory: %s takes host labels (device labels go through %s_device)", entry, entry);
+  if (z_on_device)
+    *in = CellInput{nullptr, Z, dtype, ld, (cudaStream_t)stream, phi_i, phi_type != cudaMemoryTypeHost};
+  else
+    *in = CellInput{(const double*)Z, nullptr, HB_FLOAT64, 0, nullptr, phi_i, false};
+  return 0;
+}
+
+int check_dimensions(hb_handle* h, int d, int64_t N, int C, int K) {
   if (d < 1 || N < 1 || C < 1 || K < 1) return fail(h, 2, "bad dimensions");
   if (K > 1024) return fail(h, 2, "K = %d is not supported (K <= 1024)", K);
   if (N > 2000000000LL) return fail(h, 2, "more than 2e9 cells per GPU are not supported");
+  return 0;
+}
+
+void set_shape(hb_handle* h, int d, int C, int K, const int32_t* B_vec) {
+  h->d = d;
+  h->C = C;
+  h->K = K;
+  h->KS = (K + 3) & ~3;
+  h->DS = (d + 3) & ~3;
+  h->B_vec.assign(B_vec, B_vec + C);
+  h->B = std::accumulate(h->B_vec.begin(), h->B_vec.end(), 0);
+}
+
+// the kernels of the shape, for update_R in nb blocks, and the device buffers both kinds of handle use, with the tiles
+int alloc_common(hb_handle* h, int nb) {
+  const int K = h->K, d = h->d, B = h->B, J = h->J, KS = h->KS;
+  const size_t nK = (size_t)h->n * KS, nd = (size_t)h->n * h->DS, BK = (size_t)B * KS;
+  h->coop_grid = h->num_sms;  // one persistent CTA per SM
+  h->paths = select_kernels(K, d, J, h->n, nb, h->coop_grid, h->kernel_set);
+  for (DevBuf<float>* b : {&h->Zo, &h->Zc}) CK(b->alloc(nd));
+  for (DevBuf<float>* b : {&h->U, &h->R}) CK(b->alloc(nK));
+  for (DevBuf<float>* b : {&h->O, &h->E}) CK(b->alloc(BK));
+  CK(h->Pr_b.alloc(B));
+  CK(h->Y.alloc((size_t)K * d));
+  CK(h->sigma.alloc(K));
+  CK(h->lambda.alloc(B + 1));
+  CK(h->tmpT.alloc((size_t)B * K));
+  CK(h->Oacc.alloc(BK + KS));
+  CK(h->S.alloc((size_t)J * K * (d + 1)));
+  CK(h->V.alloc((size_t)J * K * d));
+  CK(h->Wfull.alloc((size_t)K * (B + 1) * d));
+  CK(h->scratch.alloc((size_t)K * (2 * (size_t)(B + 1) * (B + 1) + (size_t)(B + 1) * d)));  // the ridge solves'
+  CK(h->err_flag.alloc(1));
+  CK(h->obj_acc.alloc(2));
+  CK(h->stage.alloc((size_t)8 << 20));  // 64 MiB of doubles
+  CK(h->tuple_levels.alloc((size_t)J * h->C));
+  TRY(build_tiles(h, h->tiles, h->tuple_start_h, TM));
+  return build_tiles(h, h->tc_tiles, h->tuple_start_h, TC_TM);
+}
+
+// the initial state both kinds of handle start from: no assignment (R = 0, U = padding), empty O / E and rows, and the
+// tuples' levels
+int init_common(hb_handle* h) {
+  const size_t nK = (size_t)h->n * h->KS, nd = (size_t)h->n * h->DS, BK = (size_t)h->B * h->KS;
+  CK(cudaMemsetAsync(h->err_flag.p, 0, sizeof(int), h->stream));
+  CK(cudaMemsetAsync(h->obj_acc.p, 0, 2 * sizeof(double), h->stream));
+  for (float* t : {h->O.p, h->E.p}) CK(cudaMemsetAsync(t, 0, sizeof(float) * BK, h->stream));
+  CK(cudaMemsetAsync(h->R.p, 0, sizeof(float) * nK, h->stream));
+  for (float* z : {h->Zo.p, h->Zc.p}) CK(cudaMemsetAsync(z, 0, sizeof(float) * nd, h->stream));
+  k_fill_f<<<grid_for((int64_t)nK, 256, h->num_sms * 8), 256, 0, h->stream>>>(h->U.p, (int64_t)nK, U_PAD);
+  CKL();
+  return upload_vector(h, h->tuple_levels, h->tuple_levels_h);
+}
+
+// Z into Zo, in tuple-sorted order (double -> float for host Z)
+int upload_z(hb_handle* h, const CellInput& in) {
+  if (in.dev) return upload_rows_device(h, in.dev, in.dtype, in.ld, in.stream);
+  return upload_rows(h, in.host, h->d, h->DS, h->Zo.p);
+}
+
+// ---- hb_setup and hb_setup_device: checks and scalars, the tuple index, the allocations, the uploads ----------------
+int setup_scalars(hb_handle* h, int d, int64_t N, const int32_t* B_vec, int C, const double* lambda, int max_iter_kmeans,
+                  double epsilon_kmeans, double epsilon_harmony, double alpha, int K, double block_size,
+                  double batch_proportion_cutoff, int verbose) {
+  TRY(check_dimensions(h, d, N, C, K));
   CK(cudaSetDevice(h->device));
   h->n = N;
   if (!h->shard_set) {
@@ -114,13 +208,7 @@ int setup_scalars(hb_handle* h, int d, int64_t N, const int32_t* B_vec, int C, c
     h->cell_offset = 0;
   }
   const int64_t NG = h->N_global;
-  h->d = d;
-  h->C = C;
-  h->K = K;
-  h->KS = (K + 3) & ~3;
-  h->DS = (d + 3) & ~3;
-  h->B_vec.assign(B_vec, B_vec + C);
-  h->B = std::accumulate(h->B_vec.begin(), h->B_vec.end(), 0);
+  set_shape(h, d, C, K, B_vec);
   h->cov_of.resize(h->B);
   {
     int b = 0;
@@ -155,7 +243,7 @@ int setup_scalars(hb_handle* h, int d, int64_t N, const int32_t* B_vec, int C, c
 }
 
 // joint covariate tuples; cells get sorted by tuple (stable), on the device (tuples.cuh)
-int setup_tuples(hb_handle* h, const int32_t* phi_i, bool phi_on_device, cudaStream_t caller, TupleIndex& ti) {
+int setup_tuples(hb_handle* h, const CellInput& in, TupleIndex& ti) {
   const int C = h->C;
   const int64_t N = h->n;
   const std::vector<int>& B_vec = h->B_vec;
@@ -175,12 +263,12 @@ int setup_tuples(hb_handle* h, const int32_t* phi_i, bool phi_on_device, cudaStr
   {
     RegionScope rs(h, "tuple_index");
     DevBuf<int> phi_up;  // host labels: one upload, then the same kernels
-    const int* phi_d = phi_i;
-    if (phi_on_device) {
-      TRY(stream_after(h, h->stream, caller));  // read after the caller's work, like Z
+    const int* phi_d = in.phi;
+    if (in.phi_on_device) {
+      TRY(stream_after(h, h->stream, in.stream));  // read after the caller's work, like Z
     } else {
       CK(phi_up.alloc((size_t)N * C));
-      CK(cudaMemcpyAsync(phi_up.p, phi_i, sizeof(int) * (size_t)N * C, cudaMemcpyDefault, h->stream));
+      CK(cudaMemcpyAsync(phi_up.p, in.phi, sizeof(int) * (size_t)N * C, cudaMemcpyDefault, h->stream));
       phi_d = phi_up.p;
     }
     TRY(build_tuple_index(h, phi_d, N, base, radix, key_space, ti));
@@ -201,57 +289,26 @@ int setup_tuples(hb_handle* h, const int32_t* phi_i, bool phi_on_device, cudaStr
 
 // the kernels of the shape and every device buffer, with the tiles and the plan's static tables
 int setup_alloc(hb_handle* h) {
-  const int K = h->K, d = h->d, B = h->B, J = h->J, KS = h->KS;
-  const size_t nK = (size_t)h->n * KS, nd = (size_t)h->n * h->DS, BK = (size_t)B * KS;
+  const int K = h->K, B = h->B, J = h->J;
   const int Tplan = std::max(1, (int)h->max_iter_kmeans);
-  h->coop_grid = h->num_sms;  // one persistent CTA per SM
-  h->paths = select_kernels(K, d, J, h->n, h->nb, h->coop_grid, h->kernel_set);
-  for (DevBuf<float>* b : {&h->Zo, &h->Zc}) CK(b->alloc(nd));
-  for (DevBuf<float>* b : {&h->U, &h->R}) CK(b->alloc(nK));
-  for (DevBuf<float>* b : {&h->theta, &h->Pr_b, &h->N_b}) CK(b->alloc(B));
-  for (DevBuf<float>* b : {&h->O, &h->E}) CK(b->alloc(BK));
-  CK(h->Y.alloc((size_t)K * d));
-  CK(h->sigma.alloc(K));
-  CK(h->lambda.alloc(B + 1));
-  CK(h->tmpT.alloc((size_t)B * K));
-  CK(h->Oacc.alloc(BK + KS));
-  CK(h->S.alloc((size_t)J * K * (d + 1)));
-  CK(h->V.alloc((size_t)J * K * d));
-  CK(h->Wfull.alloc((size_t)K * (B + 1) * d));
-  CK(h->scratch.alloc((size_t)K * (2 * (size_t)(B + 1) * (B + 1) + (size_t)(B + 1) * d)));
+  TRY(alloc_common(h, h->nb));
+  for (DevBuf<float>* b : {&h->theta, &h->N_b}) CK(b->alloc(B));
   CK(h->iscratch.alloc((size_t)K * (2 * (size_t)B + J)));
   CK(h->skipped.alloc(K));
-  CK(h->err_flag.alloc(1));
-  CK(h->obj_acc.alloc(2));
-  CK(h->stage.alloc((size_t)8 << 20));  // 64 MiB of doubles
-  CK(h->tuple_levels.alloc((size_t)J * h->C));
   CK(h->cov_of_d.alloc(B));
-  TRY(build_tiles(h, h->tiles, h->tuple_start_h, TM));
-  TRY(build_tiles(h, h->tc_tiles, h->tuple_start_h, TC_TM));
   TRY(plan_setup(h, h->tuple_start_h, Tplan));
   return reserve_rounds(h, Tplan);
 }
 
 // the initial device state, the tables of the tuples and the run parameters, then Z: double -> float, into
 // tuple-sorted order (harmony.cpp:41); Z_corr = normalise(Z_orig) (:42)
-int setup_uploads(hb_handle* h, const ZInput& Z, const double* sigma, const double* theta, const double* lambda,
+int setup_uploads(hb_handle* h, const CellInput& in, const double* sigma, const double* theta, const double* lambda,
                   const std::vector<int64_t>& lvl_count, HostLap& lap) {
   const int K = h->K, d = h->d, B = h->B, J = h->J, C = h->C;
-  const size_t nK = (size_t)h->n * h->KS, nd = (size_t)h->n * h->DS, BK = (size_t)B * h->KS;
-  CK(cudaMemsetAsync(h->err_flag.p, 0, sizeof(int), h->stream));
-  CK(cudaMemsetAsync(h->obj_acc.p, 0, 2 * sizeof(double), h->stream));
-  for (float* t : {h->O.p, h->E.p}) CK(cudaMemsetAsync(t, 0, sizeof(float) * BK, h->stream));
+  TRY(init_common(h));
   CK(cudaMemsetAsync(h->Wfull.p, 0, sizeof(float) * (size_t)K * (B + 1) * d, h->stream));
   CK(cudaMemsetAsync(h->skipped.p, 0, sizeof(int) * K, h->stream));
-  CK(cudaMemsetAsync(h->R.p, 0, sizeof(float) * nK, h->stream));
-  for (float* z : {h->Zo.p, h->Zc.p}) CK(cudaMemsetAsync(z, 0, sizeof(float) * nd, h->stream));
-  k_fill_f<<<grid_for((int64_t)nK, 256, h->num_sms * 8), 256, 0, h->stream>>>(h->U.p, (int64_t)nK, U_PAD);
-  CKL();
   CK(cudaMemsetAsync(h->Y.p, 0, sizeof(float) * (size_t)K * d, h->stream));
-  auto up = [&](auto& buf, const auto& v) {
-    return cudaMemcpyAsync(buf.p, v.data(), sizeof(v[0]) * v.size(), cudaMemcpyHostToDevice, h->stream);
-  };
-  CK(up(h->tuple_levels, h->tuple_levels_h));
   // CSR level -> tuples containing it, ascending tuple order; trailing word: the number of levels of covariate 0
   std::vector<int> lvl_ptr_h(B + 2, 0), lvl_tup_h((size_t)J * C);
   for (size_t i = 0; i < h->tuple_levels_h.size(); ++i) lvl_ptr_h[h->tuple_levels_h[i] + 1]++;
@@ -263,26 +320,23 @@ int setup_uploads(hb_handle* h, const ZInput& Z, const double* sigma, const doub
   UpdateState& u = *h->upd;
   CK(u.lvl_ptr.alloc(B + 2));
   CK(u.lvl_tup.alloc(std::max<size_t>(1, lvl_tup_h.size())));
-  CK(up(u.lvl_ptr, lvl_ptr_h));
-  CK(up(u.lvl_tup, lvl_tup_h));
-  CK(up(h->cov_of_d, h->cov_of));
+  TRY(upload_vector(h, u.lvl_ptr, lvl_ptr_h));
+  TRY(upload_vector(h, u.lvl_tup, lvl_tup_h));
+  TRY(upload_vector(h, h->cov_of_d, h->cov_of));
   std::vector<float> nbv(B), prb(B);
   for (int b = 0; b < B; ++b) {
     nbv[b] = (float)lvl_count[b];
     prb[b] = (float)lvl_count[b] / (float)h->N_global;  // harmony.cpp:67
   }
-  CK(up(h->N_b, nbv));
-  CK(up(h->Pr_b, prb));
+  TRY(upload_vector(h, h->N_b, nbv));
+  TRY(upload_vector(h, h->Pr_b, prb));
   set_sigma_scalars(h, sigma);
-  CK(up(h->sigma, std::vector<float>(sigma, sigma + K)));
-  CK(up(h->theta, std::vector<float>(theta, theta + B)));
-  CK(up(h->lambda, h->lambda_estimation ? std::vector<float>(B + 1, 0.f) : std::vector<float>(lambda, lambda + B + 1)));
+  TRY(upload_vector(h, h->sigma, std::vector<float>(sigma, sigma + K)));
+  TRY(upload_vector(h, h->theta, std::vector<float>(theta, theta + B)));
+  TRY(upload_vector(h, h->lambda, h->lambda_estimation ? std::vector<float>(B + 1, 0.f) : std::vector<float>(lambda, lambda + B + 1)));
   CK(cudaStreamSynchronize(h->stream));
   lap.mark("memsets + small uploads");
-  if (Z.dev)
-    TRY(upload_rows_device(h, Z.dev, Z.dtype, Z.ld, Z.stream));
-  else
-    TRY(upload_rows(h, Z.host, d, h->DS, h->Zo.p));
+  TRY(upload_z(h, in));
   k_normalise_rows<<<grid_for(h->n * 32, 256, h->num_sms * 8), 256, 0, h->stream>>>(h->Zo.p, h->Zc.p, h->n, d, h->DS);
   CKL();
   CK(cudaStreamSynchronize(h->stream));
@@ -290,21 +344,19 @@ int setup_uploads(hb_handle* h, const ZInput& Z, const double* sigma, const doub
   return 0;
 }
 
-int setup_common(hb_handle* h, const ZInput& Z, int d, int64_t N, const int32_t* phi_i, bool phi_on_device,
-                 const int32_t* B_vec, int C, const double* sigma, const double* theta, const double* lambda, double alpha,
-                 int max_iter_kmeans, double epsilon_kmeans, double epsilon_harmony, int K, double block_size,
-                 double batch_proportion_cutoff, int verbose) {
-  if (h->ran_setup) return fail(h, 3, "setup was already run on this object");
-  if (!(Z.host || Z.dev) || !phi_i || !B_vec || !sigma || !theta) return fail(h, 2, "null argument");
+int setup_common(hb_handle* h, const CellInput& in, int d, int64_t N, const int32_t* B_vec, int C, const double* sigma,
+                 const double* theta, const double* lambda, double alpha, int max_iter_kmeans, double epsilon_kmeans,
+                 double epsilon_harmony, int K, double block_size, double batch_proportion_cutoff, int verbose) {
+  if (!(in.host || in.dev) || !in.phi || !B_vec || !sigma || !theta) return fail(h, 2, "null argument");
   TRY(setup_scalars(h, d, N, B_vec, C, lambda, max_iter_kmeans, epsilon_kmeans, epsilon_harmony, alpha, K, block_size,
                     batch_proportion_cutoff, verbose));
   HostLap lap(h->stream, "hb_setup");
   TupleIndex ti;
-  TRY(setup_tuples(h, phi_i, phi_on_device, Z.stream, ti));
+  TRY(setup_tuples(h, in, ti));
   lap.mark("tuple index (device)");
   TRY(setup_alloc(h));
   lap.mark("device allocations");
-  TRY(setup_uploads(h, Z, sigma, theta, lambda, ti.lvl_count, lap));
+  TRY(setup_uploads(h, in, sigma, theta, lambda, ti.lvl_count, lap));
   h->ran_setup = true;
   return 0;
 }
@@ -312,6 +364,14 @@ int setup_common(hb_handle* h, const ZInput& Z, int d, int64_t N, const int32_t*
 // the Harmony steps a mapping handle refuses
 int refuse_mapping(hb_handle* h, const char* what) {
   return fail(h, 3, "%s: this object maps a query (hb_map_setup), it does not run Harmony", what);
+}
+// The guard of the Harmony step `what`: a mapping handle refuses it, and it needs init_cluster_cpp (or, for
+// init_cluster_cpp itself, setup) to have run
+int harmony_step(hb_handle* h, const char* what, bool needs_init = true) {
+  if (h->mapping) return refuse_mapping(h, what);
+  if (needs_init && !h->ran_init) return fail(h, 3, "init_cluster_cpp has not been run");
+  if (!needs_init && !h->ran_setup) return fail(h, 3, "setup has not been run");
+  return 0;
 }
 
 }  // namespace
@@ -434,11 +494,9 @@ int hb_setup(hb_handle* h, const double* Z, int d, int64_t N, const int32_t* phi
              double epsilon_kmeans, double epsilon_harmony, int K, double block_size,
              double batch_proportion_cutoff, int verbose) {
   if (!h) return 1;
-  cudaMemoryType phi_type;  // managed labels are read like host ones (one copy to the device)
-  TRY(phi_location(h, phi_i, &phi_type));
-  if (phi_type == cudaMemoryTypeDevice)
-    return fail(h, 2, "phi_i is device memory: hb_setup takes host labels (device labels go through hb_setup_device)");
-  return setup_common(h, ZInput{Z}, d, N, phi_i, false, B_vec, C, sigma, theta, lambda, alpha, max_iter_kmeans, epsilon_kmeans,
+  CellInput in;
+  TRY(setup_inputs(h, "hb_setup", Z, false, HB_FLOAT64, d, nullptr, d, phi_i, &in));
+  return setup_common(h, in, d, N, B_vec, C, sigma, theta, lambda, alpha, max_iter_kmeans, epsilon_kmeans,
                       epsilon_harmony, K, block_size, batch_proportion_cutoff, verbose);
 }
 
@@ -447,20 +505,15 @@ int hb_setup_device(hb_handle* h, const void* Z, int z_dtype, int64_t z_ld, void
                     const double* lambda, double alpha, int max_iter_kmeans, double epsilon_kmeans,
                     double epsilon_harmony, int K, double block_size, double batch_proportion_cutoff, int verbose) {
   if (!h) return 1;
-  if (h->ran_setup) return fail(h, 3, "setup was already run on this object");
-  if (z_dtype != HB_FLOAT32 && z_dtype != HB_FLOAT64) return fail(h, 2, "unknown dtype %d of Z", z_dtype);
-  if (z_ld < d) return fail(h, 2, "row stride of Z (%lld) is smaller than d = %d", (long long)z_ld, d);
-  TRY(check_device_ptr(h, Z, "Z"));
-  cudaMemoryType phi_type;
-  TRY(phi_location(h, phi_i, &phi_type));
-  return setup_common(h, ZInput{nullptr, Z, z_dtype, z_ld, (cudaStream_t)stream}, d, N, phi_i, phi_type != cudaMemoryTypeHost, B_vec, C, sigma, theta, lambda, alpha, max_iter_kmeans, epsilon_kmeans,
+  CellInput in;
+  TRY(setup_inputs(h, "hb_setup_device", Z, true, z_dtype, z_ld, stream, d, phi_i, &in));
+  return setup_common(h, in, d, N, B_vec, C, sigma, theta, lambda, alpha, max_iter_kmeans, epsilon_kmeans,
                       epsilon_harmony, K, block_size, batch_proportion_cutoff, verbose);
 }
 
 int hb_reference(hb_handle* h, double* centroids, double* Nr, double* Cref, double* sigma) {
   if (!h) return 1;
-  if (h->mapping) return refuse_mapping(h, "hb_reference");
-  if (!h->ran_init) return fail(h, 3, "init_cluster_cpp has not been run");
+  TRY(harmony_step(h, "hb_reference"));
   if (h->world > 1) return fail(h, 3, "hb_reference does not take a sharded integration");
   CK(cudaSetDevice(h->device));
   return reference_stats(h, centroids, Nr, Cref, sigma);
@@ -470,25 +523,18 @@ int hb_map_setup(hb_handle* h, const double* Z, int d, int64_t N, const int32_t*
                  const double* lambda, int K, const double* centroids, const double* Nr, const double* Cref,
                  const double* sigma) {
   if (!h) return 1;
-  cudaMemoryType phi_type;
-  TRY(phi_location(h, phi_i, &phi_type));
-  if (phi_type == cudaMemoryTypeDevice)
-    return fail(h, 2, "phi_i is device memory: hb_map_setup takes host labels (device labels go through hb_map_setup_device)");
-  return map_setup(h, ZInput{Z}, d, N, phi_i, false, B_vec, C, lambda, K, centroids, Nr, Cref, sigma);
+  CellInput in;
+  TRY(setup_inputs(h, "hb_map_setup", Z, false, HB_FLOAT64, d, nullptr, d, phi_i, &in));
+  return map_setup(h, in, d, N, B_vec, C, lambda, K, centroids, Nr, Cref, sigma);
 }
 
 int hb_map_setup_device(hb_handle* h, const void* Z, int z_dtype, int64_t z_ld, void* stream, int d, int64_t N,
                         const int32_t* phi_i, const int32_t* B_vec, int C, const double* lambda, int K,
                         const double* centroids, const double* Nr, const double* Cref, const double* sigma) {
   if (!h) return 1;
-  if (h->ran_setup) return fail(h, 3, "setup was already run on this object");
-  if (z_dtype != HB_FLOAT32 && z_dtype != HB_FLOAT64) return fail(h, 2, "unknown dtype %d of Z", z_dtype);
-  if (z_ld < d) return fail(h, 2, "row stride of Z (%lld) is smaller than d = %d", (long long)z_ld, d);
-  TRY(check_device_ptr(h, Z, "Z"));
-  cudaMemoryType phi_type;
-  TRY(phi_location(h, phi_i, &phi_type));
-  return map_setup(h, ZInput{nullptr, Z, z_dtype, z_ld, (cudaStream_t)stream}, d, N, phi_i,
-                   phi_type != cudaMemoryTypeHost, B_vec, C, lambda, K, centroids, Nr, Cref, sigma);
+  CellInput in;
+  TRY(setup_inputs(h, "hb_map_setup_device", Z, true, z_dtype, z_ld, stream, d, phi_i, &in));
+  return map_setup(h, in, d, N, B_vec, C, lambda, K, centroids, Nr, Cref, sigma);
 }
 
 int hb_map(hb_handle* h) {
@@ -499,8 +545,7 @@ int hb_map(hb_handle* h) {
 
 int hb_init_cluster(hb_handle* h, const double* Y0) {
   if (!h) return 1;
-  if (h->mapping) return refuse_mapping(h, "init_cluster_cpp");
-  if (!h->ran_setup) return fail(h, 3, "setup has not been run");
+  TRY(harmony_step(h, "init_cluster_cpp", false));
   CK(cudaSetDevice(h->device));
   HostLap lap(h->stream, "hb_init_cluster");
   if (Y0)  // Y = normalise(kmeans_centers(..)) (harmony.cpp:133-136), centroids injected by the caller
@@ -522,8 +567,7 @@ int hb_init_cluster(hb_handle* h, const double* Y0) {
 
 int hb_cluster(hb_handle* h, const int64_t* update_orders) {
   if (!h) return 1;
-  if (h->mapping) return refuse_mapping(h, "cluster_cpp");
-  if (!h->ran_init) return fail(h, 3, "init_cluster_cpp has not been run");
+  TRY(harmony_step(h, "cluster_cpp"));
   CK(cudaSetDevice(h->device));
   const unsigned T = h->max_iter_kmeans;
   const bool cold = h->harmony_slots.size() != 1;  // harmony.cpp:214-228 cold start
@@ -596,8 +640,7 @@ int hb_cluster(hb_handle* h, const int64_t* update_orders) {
 
 int hb_moe_correct_ridge(hb_handle* h) {
   if (!h) return 1;
-  if (h->mapping) return refuse_mapping(h, "moe_correct_ridge_cpp");
-  if (!h->ran_init) return fail(h, 3, "init_cluster_cpp has not been run");
+  TRY(harmony_step(h, "moe_correct_ridge_cpp"));
   CK(cudaSetDevice(h->device));
   TRY(run_correct(h));
   h->zc_pending_norm = false;  // Z_corr was rebuilt from Z_orig
@@ -616,8 +659,7 @@ int hb_check_convergence(hb_handle* h, int type) {
 
 int hb_compute_objective(hb_handle* h) {
   if (!h) return 1;
-  if (h->mapping) return refuse_mapping(h, "compute_objective");
-  if (!h->ran_init) return fail(h, 3, "init_cluster_cpp has not been run");
+  TRY(harmony_step(h, "compute_objective"));
   CK(cudaSetDevice(h->device));
   CK(cudaMemsetAsync(h->obj_acc.p, 0, 2 * sizeof(double), h->stream));
   k_objective_cells<<<grid_for(h->n * 32, ROW_THREADS, h->num_sms * 8), ROW_THREADS, 0, h->stream>>>(
@@ -743,9 +785,7 @@ int hb_set_field(hb_handle* h, int field, const double* in) {
     case HB_E: return upload_table(h, in, h->E.p);
     case HB_THETA: return upload_small(h, in, B, h->theta.p);
     case HB_SIGMA: {
-      for (int k = 0; k < K; ++k)
-        if (!(std::isfinite(in[k]) && (float)in[k] > 0.f))
-          return fail(h, 2, "sigma[%d] = %g: sigma must be finite and positive", k, in[k]);
+      TRY(check_sigma(h, in, K));
       if (h->ran_init) {
         // U holds -dist / sigma_old (the reference keeps dist_mat and divides by the current sigma in every update_R and
         // compute_objective, harmony.cpp:158-162, 318-319): rescale column k by sigma_old[k] / sigma_new[k]

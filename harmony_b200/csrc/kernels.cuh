@@ -699,9 +699,78 @@ __device__ void ridge_weights(const float* inv, const float* sv, int m, int d, F
   }
 }
 
+// The folds of the per-tuple sums S[q][k] = {sum_i R_ki z_i, sum_i R_ki} into cluster k's ridge system and the
+// expansion of its weights, shared by k_ridge_solve and k_map_solve (arguments `a`: S, tuple_levels, V, J, K, C, d).
+// Row 0 is the intercept; `rows` says whether tuple q takes part and maps level b to its row less one (-1: left out).
+struct KeptLevels {  // k_ridge_solve: the levels the filter keeps; a tuple takes part when it has one
+  const int *pos, *part;
+  __device__ bool tuple(int q) const { return part[q]; }
+  __device__ int operator()(int b) const { return pos[b]; }
+};
+struct AllLevels {  // k_map_solve: every level
+  __device__ bool tuple(int) const { return true; }
+  __device__ int operator()(int b) const { return b; }
+};
+// G += sum_q n_kq x_q x_q^T (n_kq = S[q][k][d]; thread per tuple, atomics) and s = sum_q x_q S[q][k][0..d) ([m][d];
+// thread per embedding column, serial over tuples in tuple order, no atomics), G [m][m] starting from 0
+template <typename A, typename Rows>
+__device__ void ridge_fold(const A& a, int k, Rows rows, float* G, float* sv, int m) {
+  const int C = a.C, d = a.d;
+  for (int idx = threadIdx.x; idx < m * m; idx += blockDim.x) G[idx] = 0.f;
+  __syncthreads();
+  for (int q = threadIdx.x; q < a.J; q += blockDim.x) {
+    if (!rows.tuple(q)) continue;
+    float nq = a.S[((size_t)q * a.K + k) * (d + 1) + d];
+    atomicAdd(&G[0], nq);
+    for (int c1 = 0; c1 < C; ++c1) {
+      int p1 = rows(a.tuple_levels[q * C + c1]);
+      if (p1 < 0) continue;
+      atomicAdd(&G[(size_t)(p1 + 1) * m], nq);  // row 0
+      atomicAdd(&G[(size_t)(p1 + 1)], nq);      // col 0
+      for (int c2 = 0; c2 < C; ++c2) {
+        int p2 = rows(a.tuple_levels[q * C + c2]);
+        if (p2 >= 0) atomicAdd(&G[(size_t)(p2 + 1) * m + (p1 + 1)], nq);
+      }
+    }
+  }
+  for (int c = threadIdx.x; c < d; c += blockDim.x) {
+    for (int r = 0; r < m; ++r) sv[(size_t)r * d + c] = 0.f;
+    for (int q = 0; q < a.J; ++q) {
+      if (!rows.tuple(q)) continue;
+      float v = a.S[((size_t)q * a.K + k) * (d + 1) + c];
+      sv[c] += v;
+      for (int c1 = 0; c1 < C; ++c1) {
+        int p1 = rows(a.tuple_levels[q * C + c1]);
+        if (p1 >= 0) sv[(size_t)(p1 + 1) * d + c] += v;
+      }
+    }
+  }
+}
+// V[q][k] = the sum of the weights Wk[b + 1] ([B+1][d]) of tuple q's levels b in the system (0 if q takes no part)
+template <typename A, typename Rows>
+__device__ void ridge_expand(const A& a, int k, Rows rows, const float* Wk) {
+  const int C = a.C, d = a.d;
+  for (int idx = threadIdx.x; idx < a.J * d; idx += blockDim.x) {
+    int q = idx / d, c = idx - q * d;
+    float v = 0.f;
+    if (rows.tuple(q))
+      for (int c1 = 0; c1 < C; ++c1) {
+        int b = a.tuple_levels[q * C + c1];
+        if (rows(b) >= 0) v += Wk[(size_t)(b + 1) * d + c];
+      }
+    a.V[((size_t)q * a.K + k) * d + c] = v;
+  }
+}
+
+// V[q][k] = 0 for every tuple q: cluster k corrects nothing
+template <typename A>
+__device__ void ridge_no_correction(const A& a, int k) {
+  for (int i = threadIdx.x; i < a.J * a.d; i += blockDim.x) a.V[((size_t)(i / a.d) * a.K + k) * a.d + i % a.d] = 0.f;
+}
+
 __global__ void __launch_bounds__(256) k_ridge_solve(SolveArgs a) {
   const int k = blockIdx.x, tid = threadIdx.x, nt = blockDim.x;
-  const int J = a.J, K = a.K, B = a.B, C = a.C, d = a.d, D1 = d + 1, M = B + 1;
+  const int J = a.J, B = a.B, C = a.C, d = a.d, M = B + 1;
   __shared__ int sh_m;       // kept levels + 1
   __shared__ float sh_f[4];
   __shared__ int sh_piv;
@@ -741,52 +810,19 @@ __global__ void __launch_bounds__(256) k_ridge_solve(SolveArgs a) {
   __syncthreads();
   const int m = sh_m;
   float* Wk = a.Wfull + (size_t)k * M * d;
+  for (int idx = tid; idx < M * d; idx += nt) Wk[idx] = 0.f;  // the rows of dropped levels stay 0
   if (m == 1) {  // no active covariate (:449-452): cluster untouched, Y[k] keeps its value
-    for (int idx = tid; idx < J * d; idx += nt) {
-      int q = idx / d, c = idx - q * d;
-      a.V[((size_t)q * K + k) * d + c] = 0.f;
-    }
-    for (int idx = tid; idx < M * d; idx += nt) Wk[idx] = 0.f;
+    ridge_no_correction(a, k);
     return;
   }
-  // ---- participating tuples, zero G and s
+  // ---- participating tuples
   for (int q = tid; q < J; q += nt) {
     int p = 0;
     for (int c = 0; c < C; ++c) p |= (pos[a.tuple_levels[q * C + c]] >= 0);
     part[q] = p;
   }
-  for (int idx = tid; idx < m * m; idx += nt) G[idx] = 0.f;
-  __syncthreads();
-  // ---- G = Phi* diag(R_k) Phi*^T (:561-567) folded from the per-tuple sums n_kq = S[q][k][d]
-  for (int q = tid; q < J; q += nt) {
-    if (!part[q]) continue;
-    float nq = a.S[((size_t)q * K + k) * D1 + d];
-    atomicAdd(&G[0], nq);
-    for (int c1 = 0; c1 < C; ++c1) {
-      int p1 = pos[a.tuple_levels[q * C + c1]];
-      if (p1 < 0) continue;
-      atomicAdd(&G[(size_t)(p1 + 1) * m], nq);  // row 0
-      atomicAdd(&G[(size_t)(p1 + 1)], nq);      // col 0
-      for (int c2 = 0; c2 < C; ++c2) {
-        int p2 = pos[a.tuple_levels[q * C + c2]];
-        if (p2 < 0) continue;
-        atomicAdd(&G[(size_t)(p2 + 1) * m + (p1 + 1)], nq);
-      }
-    }
-  }
-  // ---- s = Phi* diag(R_k) Zo^T: thread per embedding column, serial over tuples (no atomics)
-  for (int c = tid; c < d; c += nt) {
-    for (int r = 0; r < m; ++r) sv[(size_t)r * d + c] = 0.f;
-    for (int q = 0; q < J; ++q) {
-      if (!part[q]) continue;
-      float v = a.S[((size_t)q * K + k) * D1 + c];
-      sv[c] += v;
-      for (int c1 = 0; c1 < C; ++c1) {
-        int p1 = pos[a.tuple_levels[q * C + c1]];
-        if (p1 >= 0) sv[(size_t)(p1 + 1) * d + c] += v;
-      }
-    }
-  }
+  // ---- G = Phi* diag(R_k) Phi*^T (:561-567) and s = Phi* diag(R_k) Zo^T, folded from the per-tuple sums
+  ridge_fold(a, k, KeptLevels{pos, part}, G, sv, m);
   __syncthreads();
   // ---- + diag(lambda): lambda_0 = 0, lambda_b = alpha*E_kb (find_lambda_cpp) or the fixed vector
   for (int j = tid; j < m - 1; j += nt) {
@@ -802,8 +838,6 @@ __global__ void __launch_bounds__(256) k_ridge_solve(SolveArgs a) {
   else
     ridge_inverse_gj(G, inv, m, &sh_piv, &sh_f[1], a.err_flag);
   // ---- W = inv * s  (:599-609), Y[k] = W[0] (:610), W[0] = 0 (:611)
-  for (int idx = tid; idx < M * d; idx += nt) Wk[idx] = 0.f;
-  __syncthreads();
   ridge_weights(inv, sv, m, d, [&](int r, int c, float w) {
     if (r == 0)
       a.Y[(size_t)k * d + c] = w;
@@ -824,16 +858,7 @@ __global__ void __launch_bounds__(256) k_ridge_solve(SolveArgs a) {
     for (int c = tid; c < d; c += 32) a.Y[(size_t)k * d + c] /= nrm;
   }
   // ---- V[q][k] = sum of the kept levels' betas of tuple q (0 for tuples that do not take part)
-  for (int idx = tid; idx < J * d; idx += nt) {
-    int q = idx / d, c = idx - q * d;
-    float v = 0.f;
-    if (part[q])
-      for (int c1 = 0; c1 < C; ++c1) {
-        int b = a.tuple_levels[q * C + c1];
-        if (pos[b] >= 0) v += Wk[(size_t)(b + 1) * d + c];
-      }
-    a.V[((size_t)q * K + k) * d + c] = v;
-  }
+  ridge_expand(a, k, KeptLevels{pos, part}, Wk);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -877,66 +902,39 @@ struct MapSolveArgs {
   const float* lambda;      // [B+1], lambda[0] = 0
   const int* tuple_levels;  // [J][C]
   float* V;                 // [J][K][d]
-  float* scratch;           // [K][ 2*M*M + 2*M*d ]  (G | inv | s | W),  M = B+1
+  float* Wfull;             // [K][B+1][d], row 0 zeroed
+  float* scratch;           // [K][ 2*M*M + M*d ]  (G | inv | s),  M = B+1
   int* err_flag;
   int J, K, B, C, d;
 };
 
 __global__ void __launch_bounds__(256) k_map_solve(MapSolveArgs a) {
   const int k = blockIdx.x, tid = threadIdx.x, nt = blockDim.x;
-  const int J = a.J, K = a.K, C = a.C, d = a.d, D1 = d + 1, m = a.B + 1;
+  const int C = a.C, d = a.d, m = a.B + 1;
   __shared__ float sh_f;
   __shared__ int sh_piv;
-  float* G = a.scratch + (size_t)k * (2 * (size_t)m * m + 2 * (size_t)m * d);
+  float* G = a.scratch + (size_t)k * (2 * (size_t)m * m + (size_t)m * d);
   float* inv = G + (size_t)m * m;
   float* sv = inv + (size_t)m * m;  // [m][d]
-  float* W = sv + (size_t)m * d;    // [m][d]
-  for (int idx = tid; idx < m * m; idx += nt) G[idx] = 0.f;
-  __syncthreads();
-  // ---- G from the per-tuple masses n_kq = S[q][k][d]
-  for (int q = tid; q < J; q += nt) {
-    float nq = a.S[((size_t)q * K + k) * D1 + d];
-    atomicAdd(&G[0], nq);
-    for (int c1 = 0; c1 < C; ++c1) {
-      int p1 = a.tuple_levels[q * C + c1] + 1;
-      atomicAdd(&G[(size_t)p1 * m], nq);  // row 0
-      atomicAdd(&G[(size_t)p1], nq);      // col 0
-      for (int c2 = 0; c2 < C; ++c2) atomicAdd(&G[(size_t)(a.tuple_levels[q * C + c2] + 1) * m + p1], nq);
-    }
-  }
-  // ---- s: thread per embedding column, serial over tuples; row 0 takes the reference's Cref_k
-  for (int c = tid; c < d; c += nt) {
-    for (int r = 0; r < m; ++r) sv[(size_t)r * d + c] = 0.f;
-    for (int q = 0; q < J; ++q) {
-      float v = a.S[((size_t)q * K + k) * D1 + c];
-      sv[c] += v;
-      for (int c1 = 0; c1 < C; ++c1) sv[(size_t)(a.tuple_levels[q * C + c1] + 1) * d + c] += v;
-    }
-    sv[c] += a.Cref[(size_t)k * d + c];
-  }
+  float* Wk = a.Wfull + (size_t)k * m * d;
+  // ---- G and s from the per-tuple sums; row 0 of s takes the reference's Cref_k (same thread per column)
+  ridge_fold(a, k, AllLevels{}, G, sv, m);
+  for (int c = tid; c < d; c += nt) sv[c] += a.Cref[(size_t)k * d + c];
   __syncthreads();
   for (int j = tid; j < m - 1; j += nt) G[(size_t)(j + 1) * m + (j + 1)] += a.lambda[j + 1];
   if (tid == 0) G[0] += a.Nr[k];
   __syncthreads();
   if (G[0] == 0.f) {
-    for (int idx = tid; idx < J * d; idx += nt) {
-      int q = idx / d, c = idx - q * d;
-      a.V[((size_t)q * K + k) * d + c] = 0.f;
-    }
+    ridge_no_correction(a, k);
     return;
   }
   if (C == 1)
     ridge_inverse_arrowhead(G, inv, m, &sh_f);
   else
     ridge_inverse_gj(G, inv, m, &sh_piv, &sh_f, a.err_flag);
-  ridge_weights(inv, sv, m, d, [&](int r, int c, float w) { W[(size_t)r * d + c] = r == 0 ? 0.f : w; });
+  ridge_weights(inv, sv, m, d, [&](int r, int c, float w) { Wk[(size_t)r * d + c] = r == 0 ? 0.f : w; });
   __syncthreads();
-  for (int idx = tid; idx < J * d; idx += nt) {
-    int q = idx / d, c = idx - q * d;
-    float v = 0.f;
-    for (int c1 = 0; c1 < C; ++c1) v += W[(size_t)(a.tuple_levels[q * C + c1] + 1) * d + c];
-    a.V[((size_t)q * K + k) * d + c] = v;
-  }
+  ridge_expand(a, k, AllLevels{}, Wk);
 }
 
 // ------------------------------------------------------------------------------------------------

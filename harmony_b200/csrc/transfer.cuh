@@ -286,6 +286,12 @@ int download_small(hb_handle* h, const float* src, size_t count, double* out) {
   for (size_t i = 0; i < count; ++i) out[i] = (double)tmp[i];
   return 0;
 }
+// a host vector into the front of a device buffer of its element type, on the handle's stream
+template <typename T>
+int upload_vector(hb_handle* h, DevBuf<T>& buf, const std::vector<T>& v) {
+  CK(cudaMemcpyAsync(buf.p, v.data(), sizeof(T) * v.size(), cudaMemcpyHostToDevice, h->stream));
+  return 0;
+}
 int upload_small(hb_handle* h, const double* in, size_t count, float* dst) {
   std::vector<float> tmp(count);
   for (size_t i = 0; i < count; ++i) tmp[i] = (float)in[i];

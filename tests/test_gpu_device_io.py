@@ -39,17 +39,22 @@ def iterate(g, Y0, perms):
         g.check_convergence(1)
 
 
-def raw_setup(g, a, ptr, dtype, ld, stream=None):
-    """hb_setup_device through the ABI with an arbitrary pointer (only ever one the library must refuse)."""
+def raw_setup(g, a, ptr, dtype, ld, stream=None, host=False, d=None, N=None, C=None, K=None, phi_ptr=None):
+    """hb_setup_device through the ABI with an arbitrary pointer (only ever one the library must refuse), or hb_setup
+    on the host array a["Z"] when `host`.  d, N, C, K and phi_ptr replace what `a` gives."""
     phi = np.ascontiguousarray(a["phi_i"], dtype=np.int32)
     B_vec = np.ascontiguousarray(a["B_vec"], dtype=np.int32)
     sigma = np.ascontiguousarray(a["sigma"], dtype=np.float64)
     theta = np.ascontiguousarray(a["theta"], dtype=np.float64)
     P = ctypes.c_void_p
-    return g._L.hb_setup_device(g._h, P(ptr), dtype, ld, P(stream), a["Z"].shape[1], phi.shape[0],
-                                P(phi.ctypes.data), P(B_vec.ctypes.data), len(B_vec), P(sigma.ctypes.data),
-                                P(theta.ctypes.data), None, a["alpha"], a["max_iter_kmeans"], a["epsilon_kmeans"],
-                                a["epsilon_harmony"], a["K"], a["block_size"], a["batch_proportion_cutoff"], 0)
+    rest = (a["Z"].shape[1] if d is None else d, phi.shape[0] if N is None else N,
+            P(phi.ctypes.data if phi_ptr is None else phi_ptr), P(B_vec.ctypes.data), len(B_vec) if C is None else C,
+            P(sigma.ctypes.data), P(theta.ctypes.data), None, a["alpha"], a["max_iter_kmeans"], a["epsilon_kmeans"],
+            a["epsilon_harmony"], a["K"] if K is None else K, a["block_size"], a["batch_proportion_cutoff"], 0)
+    if host:
+        Z = np.ascontiguousarray(a["Z"], dtype=np.float64)
+        return g._L.hb_setup(g._h, P(Z.ctypes.data), *rest)
+    return g._L.hb_setup_device(g._h, P(ptr), dtype, ld, P(stream), *rest)
 
 
 @pytest.fixture(scope="module")
@@ -220,6 +225,13 @@ def test_rejected_before_any_launch(small):
                                  (Zd.data_ptr(), 7, d, "dtype")):
         assert raw_setup(g, a, ptr, dtype, ld) == 2
         assert what in g._L.hb_last_error(g._h).decode()
+    # the dimension checks of both entry points, and device labels given to the host one
+    for host in (False, True):
+        for bad in (dict(d=0), dict(N=0), dict(C=0), dict(K=0), dict(K=1025)):
+            assert raw_setup(g, a, Zd.data_ptr(), HB_FLOAT64, d, host=host, **bad) == 2, (host, bad)
+    phi_d = torch.from_numpy(np.ascontiguousarray(a["phi_i"], dtype=np.int32)).cuda()
+    assert raw_setup(g, a, None, HB_FLOAT64, d, host=True, phi_ptr=phi_d.data_ptr()) == 2
+    assert "hb_setup_device" in g._L.hb_last_error(g._h).decode()
     assert g.kernel_launches == 0
     with pytest.raises(TypeError):
         g.setup(Zd.half(), a["phi_i"], a["sigma"], a["theta"], a["lambda_"], a["alpha"], a["max_iter_kmeans"],
@@ -227,6 +239,8 @@ def test_rejected_before_any_launch(small):
                 a["batch_proportion_cutoff"])
     g = new(a, Zd)
     n0 = g.kernel_launches
+    for host in (False, True):   # a second setup
+        assert raw_setup(g, a, Zd.data_ptr(), HB_FLOAT64, d, host=host) == 3, host
     out = torch.empty((N, d), dtype=torch.float64, device="cuda")
     P, s = ctypes.c_void_p, ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
     for field, ptr, dtype, ld in ((HB_Z_CORR, pageable.ctypes.data, HB_FLOAT64, d),

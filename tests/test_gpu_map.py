@@ -251,15 +251,25 @@ def _ptr(a):
     return a.ctypes.data_as(ctypes.c_void_p)
 
 
-def _raw_map_setup(g, Z, phi, B_vec, lam, ref, K=None):
-    """Status of hb_map_setup called directly (the Python layer checks shapes first)."""
+HB_FLOAT64 = 1
+
+
+def _raw_map_setup(g, Z, phi, B_vec, lam, ref, K=None, d=None, N=None, C=None, phi_ptr=None, z_dev=None,
+                   dtype=HB_FLOAT64, ld=None):
+    """Status of hb_map_setup called directly (the Python layer checks shapes first), or of hb_map_setup_device on the
+    device pointer z_dev.  K, d, N, C, phi_ptr and ld replace what the arrays give."""
     Z = np.ascontiguousarray(Z, dtype=np.float64)
     phi = np.ascontiguousarray(phi, dtype=np.int32).reshape(len(Z), -1)
     B_vec = np.ascontiguousarray(B_vec, dtype=np.int32)
     lam = np.ascontiguousarray(lam, dtype=np.float64)
     arrs = [np.ascontiguousarray(a, dtype=np.float64) for a in (ref.centroids, ref.Nr, ref.Cref, ref.sigma)]
-    return g._L.hb_map_setup(g._h, _ptr(Z), Z.shape[1], len(Z), _ptr(phi), _ptr(B_vec), len(B_vec), _ptr(lam),
-                             ref.K if K is None else K, *(_ptr(a) for a in arrs))
+    d = Z.shape[1] if d is None else d
+    labels = _ptr(phi) if phi_ptr is None else ctypes.c_void_p(phi_ptr)
+    rest = (d, len(Z) if N is None else N, labels, _ptr(B_vec), len(B_vec) if C is None else C, _ptr(lam),
+            ref.K if K is None else K, *(_ptr(a) for a in arrs))
+    if z_dev is None:
+        return g._L.hb_map_setup(g._h, _ptr(Z), *rest)
+    return g._L.hb_map_setup_device(g._h, ctypes.c_void_p(z_dev), dtype, d if ld is None else ld, None, *rest)
 
 
 def test_map_refusals():
@@ -276,6 +286,20 @@ def test_map_refusals():
         assert _raw_map_setup(_harmony(), Z, phi, [2], lam, r) == 2
     assert _raw_map_setup(_harmony(), Z, np.where(phi == 1, 2, phi), [2], lam, ref) == 2
     assert _raw_map_setup(_harmony(), Z, phi, [2], lam, ref, K=0) == 2
+    # status 2 from the setup steps hb_setup shares, through the host and the device entry point: dimensions, K past
+    # the library's range, device labels given to the host entry point, and the device entry point's Z checks
+    import torch
+    Zt = torch.from_numpy(Z).cuda()
+    for z_dev in (None, Zt.data_ptr()):
+        for bad in (dict(d=0), dict(N=0), dict(C=0), dict(K=0), dict(K=1025)):
+            assert _raw_map_setup(_harmony(), Z, phi, [2], lam, ref, z_dev=z_dev, **bad) == 2, (z_dev, bad)
+    phi_t = torch.from_numpy(np.ascontiguousarray(phi, dtype=np.int32)).cuda()
+    h = _harmony()
+    assert _raw_map_setup(h, Z, phi, [2], lam, ref, phi_ptr=phi_t.data_ptr()) == 2
+    assert "hb_map_setup_device" in h._L.hb_last_error(h._h).decode()
+    Zh = np.ascontiguousarray(Z)
+    for z_dev, dtype, ld in ((Zt.data_ptr(), 7, None), (Zt.data_ptr(), HB_FLOAT64, 15), (Zh.ctypes.data, HB_FLOAT64, None)):
+        assert _raw_map_setup(_harmony(), Z, phi, [2], lam, ref, z_dev=z_dev, dtype=dtype, ld=ld) == 2, (dtype, ld)
     # d or K not matching the reference arrays: the Python layer refuses before the library
     with pytest.raises(ValueError):
         _harmony().map_setup(Z[:, :15], phi, [2], lam, ref)
@@ -285,6 +309,7 @@ def test_map_refusals():
     g = _harmony()
     assert _raw_map_setup(g, Z, phi, [2], lam, ref) == 0
     assert _raw_map_setup(g, Z, phi, [2], lam, ref) == 3
+    assert _raw_map_setup(g, Z, phi, [2], lam, ref, z_dev=Zt.data_ptr()) == 3
     with pytest.raises(HarmonyError):
         g.setup(Z, phi, 0.1, np.full(2, 2.0), None, 0.2, 5, 1e-5, 1e-4, 10, 0.05, [2], 1e-5)
     s = _harmony()
