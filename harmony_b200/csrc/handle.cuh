@@ -70,6 +70,7 @@ struct Plan;         // plan.cuh
 struct UpdateState;  // update_host.cuh
 struct AssignState;  // assign_host.cuh
 struct MapState;     // map_host.cuh
+struct KnnState;     // knn_host.cuh
 
 }  // namespace
 
@@ -123,6 +124,7 @@ struct hb_handle {
   std::unique_ptr<UpdateState> upd;
   std::unique_ptr<AssignState> asg;
   std::unique_ptr<MapState> map;  // hb_map_setup only
+  std::unique_ptr<KnnState> knn;  // hb_knn's scratch, from its first call
 
   // traces (harmony.h:55-56); values are produced on the device and pulled lazily
   DevBuf<float> trace_d;

@@ -37,6 +37,7 @@
 #include "logits_wide.cuh"
 #include "apply_tc3.cuh"
 #include "stats_tc3.cuh"
+#include "knn.cuh"
 
 #include "select.cuh"
 #include "handle.cuh"
@@ -377,6 +378,7 @@ int harmony_step(hb_handle* h, const char* what, bool needs_init = true) {
 }  // namespace
 
 #include "map_host.cuh"
+#include "knn_host.cuh"
 
 // =================================================================================================
 extern "C" {
@@ -541,6 +543,13 @@ int hb_map(hb_handle* h) {
   if (!h) return 1;
   if (!h->mapping) return fail(h, 3, "hb_map needs an object set up by hb_map_setup");
   return run_map(h);
+}
+
+int hb_knn(hb_handle* h, const void* Q, int q_dtype, int64_t q_ld, int64_t Nq, const void* X, int x_dtype, int64_t x_ld,
+           int64_t Nx, int d, int k, int metric, int exclude_self, int32_t* idx, float* dist, void* stream) {
+  if (!h) return 1;
+  return run_knn(h, KnnRows{Q, q_dtype, q_ld, Nq}, KnnRows{X, x_dtype, x_ld, Nx}, d, k, metric, exclude_self != 0, idx, dist,
+                 (cudaStream_t)stream);
 }
 
 int hb_init_cluster(hb_handle* h, const double* Y0) {
@@ -955,6 +964,17 @@ int hb_debug_wide_paths(int K, int d, int J, int64_t n, int nb, int num_sms, int
   out[1] = call_path(p, 20, false).plan_order_assign ? (int64_t)p.cold : 0;
   out[2] = (int64_t)p.apply;
   out[3] = p.kmeans == KmeansInit::Ffma ? 1 : p.kmeans == KmeansInit::LogitsWide ? 4 : ((K + 3) & ~3) <= 256 ? 2 : 3;
+  return 0;
+}
+
+// The launch geometry hb_knn picks (test hook, host only): out = {query rows per CTA, reference rows per tile, reference
+// operand stages, reference splits, shared-memory bytes, reference tiles per split, padded row length, threads per CTA}.
+// Status 2 (out untouched) for a d or k hb_knn refuses.
+int hb_debug_knn_geometry(int d, int k, int64_t Nq, int64_t Nx, int num_sms, int64_t out[8]) {
+  if (!knn_fits(d, k) || Nq < 1 || Nx < 1 || num_sms < 1) return 2;
+  const KnnGeometry g = knn_geometry(d, k, Nq, Nx, num_sms);
+  const int64_t v[8] = {g.tq, KNN_TN, g.stages, g.splits, (int64_t)g.smem, g.tiles_per_split, g.KD, 2 * g.tq};
+  for (int i = 0; i < 8; ++i) out[i] = v[i];
   return 0;
 }
 

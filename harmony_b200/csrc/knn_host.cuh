@@ -1,0 +1,113 @@
+// knn_host.cuh — hb_knn (DESIGN §9): the checks, the scratch a handle keeps for it and the launches of knn.cuh.  The
+// call needs no setup and touches no state of a Harmony run or a mapping.  Included by harmony_b200.cu.
+#pragma once
+
+namespace {
+
+// hb_knn's scratch; every buffer grows on demand and is kept for the next call
+struct KnnState {
+  DevBuf<float> Qp, Xp, hx;  // prepared rows [n][KD], |x|^2 / 2
+  DevBuf<int> part;          // [Nq][splits][k] listed candidates
+  DevBuf<double> centre;     // [KNN_MAX_D] column sums of X
+};
+
+template <typename T>
+int knn_reserve(hb_handle* h, DevBuf<T>& b, size_t count) {
+  if (b.n < count) CK(b.alloc(count));
+  return 0;
+}
+
+struct KnnRows {
+  const void* p;
+  int dtype;
+  int64_t ld, n;
+};
+
+// rows -> dst [n][KD] (and hx), centred on `centre` / centre_n or normalised
+int knn_prepare(hb_handle* h, const KnnRows& r, int d, int KD, bool cosine, const double* centre, double centre_n,
+                float* dst, float* hx) {
+  const int grid = grid_for(r.n * 32, 256, h->num_sms * 16);
+  if (r.dtype == HB_FLOAT32)
+    k_knn_prepare<<<grid, 256, 0, h->stream>>>((const float*)r.p, r.ld, r.n, d, KD, (int)cosine, centre, centre_n, dst, hx);
+  else
+    k_knn_prepare<<<grid, 256, 0, h->stream>>>((const double*)r.p, r.ld, r.n, d, KD, (int)cosine, centre, centre_n, dst, hx);
+  CKL();
+  return 0;
+}
+
+int knn_check_rows(hb_handle* h, const KnnRows& r, int d, const char* what) {
+  if (r.dtype != HB_FLOAT32 && r.dtype != HB_FLOAT64) return fail(h, 2, "unknown dtype %d of %s", r.dtype, what);
+  if (r.ld < d) return fail(h, 2, "row stride of %s (%lld) is smaller than d = %d", what, (long long)r.ld, d);
+  return check_device_ptr(h, r.p, what);
+}
+
+int run_knn(hb_handle* h, const KnnRows& Q, const KnnRows& X, int d, int k, int metric, bool exclude_self, int32_t* idx,
+            float* dist, cudaStream_t caller) {
+  if (Q.n < 1 || X.n < 1) return fail(h, 2, "hb_knn needs at least one query row and one reference row");
+  if (X.n >= (1LL << 31)) return fail(h, 2, "hb_knn: Nx = %lld reference rows are not supported (Nx < 2^31)", (long long)X.n);
+  if (d < 1 || d > KNN_MAX_D) return fail(h, 2, "hb_knn: d = %d is not supported (1 <= d <= %d)", d, KNN_MAX_D);
+  if (k < 1 || k > KNN_MAX_K) return fail(h, 2, "hb_knn: k = %d is not supported (1 <= k <= %d)", k, KNN_MAX_K);
+  if (k > X.n - (exclude_self ? 1 : 0))
+    return fail(h, 2, "hb_knn: k = %d exceeds the %lld candidate rows of a query row", k, (long long)(X.n - (exclude_self ? 1 : 0)));
+  if (metric != HB_EUCLIDEAN && metric != HB_COSINE) return fail(h, 2, "hb_knn: unknown metric %d", metric);
+  TRY(knn_check_rows(h, Q, d, "Q"));
+  TRY(knn_check_rows(h, X, d, "X"));
+  TRY(check_device_ptr(h, idx, "idx"));
+  if (dist) TRY(check_device_ptr(h, dist, "dist"));
+  CK(cudaSetDevice(h->device));
+  if (!h->knn) h->knn.reset(new KnnState());
+  KnnState& s = *h->knn;
+  const bool cosine = metric == HB_COSINE;
+  const KnnGeometry g = knn_geometry(d, k, Q.n, X.n, h->num_sms);
+  const bool shared_rows = Q.p == X.p && Q.dtype == X.dtype && Q.ld == X.ld && Q.n == X.n;  // one prepared copy serves
+  TRY(knn_reserve(h, s.Xp, (size_t)X.n * g.KD));
+  if (!shared_rows) TRY(knn_reserve(h, s.Qp, (size_t)Q.n * g.KD));
+  TRY(knn_reserve(h, s.hx, (size_t)X.n));
+  TRY(knn_reserve(h, s.part, (size_t)Q.n * g.splits * k));
+  TRY(knn_reserve(h, s.centre, (size_t)KNN_MAX_D));
+
+  TRY(stream_after(h, h->stream, caller));  // the caller's earlier work on Q, X and the outputs comes first
+  {
+    RegionScope rs(h, "knn");
+    const double* centre = nullptr;
+    if (!cosine) {
+      CK(cudaMemsetAsync(s.centre.p, 0, sizeof(double) * KNN_MAX_D, h->stream));
+      const int grid = grid_for(X.n, 2, h->num_sms * 8);
+      if (X.dtype == HB_FLOAT32)
+        k_knn_colsum<<<grid, 256, 0, h->stream>>>((const float*)X.p, X.ld, X.n, d, s.centre.p);
+      else
+        k_knn_colsum<<<grid, 256, 0, h->stream>>>((const double*)X.p, X.ld, X.n, d, s.centre.p);
+      CKL();
+      centre = s.centre.p;
+    }
+    TRY(knn_prepare(h, X, d, g.KD, cosine, centre, (double)X.n, s.Xp.p, s.hx.p));
+    const float* Qp = s.Xp.p;
+    if (!shared_rows) {
+      TRY(knn_prepare(h, Q, d, g.KD, cosine, centre, (double)X.n, s.Qp.p, nullptr));
+      Qp = s.Qp.p;
+    }
+    KnnArgs a;
+    a.Qp = Qp;
+    a.Xp = s.Xp.p;
+    a.hx = s.hx.p;
+    a.part_i = s.part.p;
+    a.Nq = Q.n;
+    a.Nx = X.n;
+    a.KD = g.KD;
+    a.k = k;
+    a.stages = g.stages;
+    a.exclude_self = exclude_self;
+    a.tiles_per_split = g.tiles_per_split;
+    const dim3 grid((unsigned)g.qtiles, (unsigned)g.splits);
+    if (g.tq == 128)
+      TRY(launch(h, k_knn_tc<128>, grid, dim3(256), g.smem, a));
+    else
+      TRY(launch(h, k_knn_tc<64>, grid, dim3(128), g.smem, a));
+    const int nc = g.splits * k;
+    TRY(launch(h, k_knn_merge, dim3((unsigned)((Q.n + 3) / 4)), dim3(128), (size_t)4 * 2 * nc * sizeof(float), Qp,
+               (const float*)s.Xp.p, (const int*)s.part.p, Q.n, g.KD, k, nc, (int)cosine, idx, dist));
+  }
+  return stream_after(h, caller, h->stream);
+}
+
+}  // namespace

@@ -102,4 +102,36 @@ CallPath call_path(const KernelPaths& p, unsigned T, bool legacy_centroid) {
   return c;
 }
 
+// ---- hb_knn (knn.cuh) -------------------------------------------------------------------------------------------------
+// Launch geometry of the k-nearest-neighbour sweep: query rows per CTA (tq), operand stages of the reference tiles
+// (KNN_TN rows each) and reference splits.  The first of (128, 2), (128, 1), (64, 2) whose shared memory fits: the query
+// tile and the lists stay for the CTA's life, so wide rows and long lists take it from the second reference stage first
+// and from the query tile last (a 64-row tile halves the flop per reference byte and runs one warpgroup).  (64, 2)
+// holds d = 128, k = 64.  With fewer query tiles than SMs the reference is split over grid.y so that the GPU is full, as
+// far as k_knn_merge's candidate limit and the reference's tiles allow.
+struct KnnGeometry {
+  int tq = 0, stages = 0, splits = 0, KD = 0;
+  size_t smem = 0;
+  int64_t qtiles = 0, tiles_per_split = 0;
+};
+bool knn_fits(int d, int k) { return d >= 1 && d <= KNN_MAX_D && k >= 1 && k <= KNN_MAX_K; }
+KnnGeometry knn_geometry(int d, int k, int64_t Nq, int64_t Nx, int num_sms) {
+  KnnGeometry g;
+  g.KD = (d + 7) & ~7;
+  static const int shapes[3][2] = {{128, 2}, {128, 1}, {64, 2}};
+  for (const auto& s : shapes)
+    if (knn_smem_bytes(s[0], s[1], g.KD, k) <= SMEM_LIMIT) {
+      g.tq = s[0], g.stages = s[1];
+      break;
+    }
+  g.smem = knn_smem_bytes(g.tq, g.stages, g.KD, k);
+  g.qtiles = (Nq + g.tq - 1) / g.tq;
+  const int64_t xtiles = (Nx + KNN_TN - 1) / KNN_TN;
+  int64_t splits = 1;
+  if (g.qtiles < num_sms) splits = std::max<int64_t>(1, std::min<int64_t>({num_sms / g.qtiles, xtiles, KNN_MERGE_MAX / k}));
+  g.tiles_per_split = (xtiles + splits - 1) / splits;
+  g.splits = (int)((xtiles + g.tiles_per_split - 1) / g.tiles_per_split);  // no empty split
+  return g;
+}
+
 }  // namespace

@@ -187,6 +187,13 @@ class harmony:
         assignment."""
         self._check(self._L.hb_map(self._h))
 
+    def knn(self, query, ref=None, k=15, metric="euclidean"):
+        """``harmony_b200.knn`` on this object's device and stream, without a second handle: the exact k nearest rows
+        of ``ref`` (``None``: of ``query`` itself, leaving each row out) for every row of ``query`` -> (idx, dist).
+        Works in any state of the object and changes none of it, e.g. ``obj.knn(obj.get_tensor("Z_corr"))``."""
+        from .neighbors import knn_on
+        return knn_on(self, query, ref, k, metric)
+
     def _device_Z(self, Z):
         """An [N, d] CUDA tensor -> (the tensor to read, (pointer, dtype, row stride, stream) of hb_setup_device)).
         Rows with unit column stride are read in place; any other layout is made contiguous on the device first."""

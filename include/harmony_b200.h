@@ -43,7 +43,8 @@ const char* hb_last_error(const hb_handle* h);
  * buf; returns 1 if a warning was written, 0 if none is pending.  The shim turns it into Rcpp::warning. */
 int hb_pop_warning(hb_handle* h, char* buf, size_t cap);
 /* Library/ABI version: major*10000 + minor*100 + patch (0.3.0: labels in device memory; 0.4.0: mapping a query onto
- * a reference, hb_reference / hb_map_setup / hb_map). */
+ * a reference, hb_reference / hb_map_setup / hb_map).  hb_knn and hb_debug_knn_geometry were added without moving the
+ * number. */
 int hb_version(void);
 
 /* ---- multi-GPU (one process per GPU; cells sharded contiguously; SURVEY §8e) ------------------- */
@@ -141,6 +142,33 @@ int hb_map_setup_device(hb_handle* h, const void* Z, int z_dtype, int64_t z_ld, 
  * hb_moe_correct_ridge, hb_compute_objective, hb_check_convergence, hb_set_field and the fields HB_W, HB_THETA and
  * HB_LAMBDA return status 3.  Regions "assign", "ridge_stats", "ridge_solve", "ridge_apply". */
 int hb_map(hb_handle* h);
+
+/* ---- exact k nearest neighbours in an embedding (DESIGN.md §9) ---------------------------------- */
+enum hb_metric { HB_EUCLIDEAN = 0, HB_COSINE = 1 };
+/* For every one of the Nq rows of Q the k rows of X at the smallest distance, by brute force over all pairs:
+ * idx[Nq][k] (0-based rows of X) and, unless NULL, dist[Nq][k], each row by ascending distance.  Q and X: rows of d values
+ * of q_dtype / x_dtype (hb_dtype) with row strides q_ld, x_ld >= d elements; Q, X, idx and dist in device or managed
+ * memory of the handle's device.  fp64 values are rounded to fp32 after centring (Euclidean) and before normalising.
+ * metric: HB_EUCLIDEAN (dist is the distance, not its square) or HB_COSINE (dist = 1 - cos; a zero row divides by 1 and
+ * so lies at distance 1 from every row).  exclude_self: row i of X is no candidate for row i of Q (a search of an
+ * embedding against itself).  The candidates are selected on 3xTF32 scores and the winners' distances recomputed directly
+ * in fp32, so dist is accurate per pair and only the membership of rows within a narrow band of the k-th distance is
+ * subject to rounding (DESIGN.md §9 gives the band); among exact duplicates any may be returned, no row twice.  A pair
+ * whose fp32 distance is NaN or infinite is never returned; a query row with fewer than k returnable rows ends with
+ * idx = -1, dist = +inf.
+ * Limits, status 2 with a message before any launch: 1 <= k <= 64, k <= Nx (Nx - 1 with exclude_self), 1 <= d <= 128,
+ * Nq >= 1, Nx < 2^31, an unknown metric or dtype, a row stride < d, a NULL, host or other-device pointer.
+ * Q and X are read after the work queued on `stream` (a cudaStream_t; NULL: the legacy default stream) and work queued on
+ * `stream` afterwards sees idx and dist; the host is not blocked.  Needs no setup: it runs on a fresh handle, on one that
+ * is running Harmony and on a mapping handle, whose state it leaves untouched; its scratch stays with the handle.  On a
+ * sharded handle it is a local call.  Region "knn". */
+int hb_knn(hb_handle* h, const void* Q, int q_dtype, int64_t q_ld, int64_t Nq, const void* X, int x_dtype, int64_t x_ld,
+           int64_t Nx, int d, int k, int metric, int exclude_self, int32_t* idx, float* dist, void* stream);
+/* Test hook (host only): the launch geometry hb_knn picks for (d, k, Nq, Nx) on num_sms SMs: out = {query rows per CTA,
+ * reference rows per tile, reference operand stages, reference splits (grid.y; > 1 when the query tiles alone would not
+ * fill the GPU), shared-memory bytes, reference tiles per split, padded row length in floats, threads per CTA}.
+ * Returns 0, or 2 with out untouched for a d or k hb_knn refuses. */
+int hb_debug_knn_geometry(int d, int k, int64_t Nq, int64_t Nx, int num_sms, int64_t out[8]);
 
 /* ---- fields / getters (harmony.cpp:640-669, 675-696) ------------------------------------------- */
 enum hb_field {
