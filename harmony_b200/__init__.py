@@ -6,6 +6,7 @@ Importing this package does not load the CUDA library; constructing ``harmony`` 
 loudly if it is missing (there is no CPU fallback).
 """
 from .harmony_option import harmony_options  # noqa: F401
+from .lisi import compute_lisi  # noqa: F401
 from .mapping import HarmonyReference  # noqa: F401
 from .neighbors import TransferLabels, knn  # noqa: F401
 from .ui import MapQuery, RunHarmony, prepare_inputs  # noqa: F401

@@ -71,6 +71,7 @@ struct UpdateState;  // update_host.cuh
 struct AssignState;  // assign_host.cuh
 struct MapState;     // map_host.cuh
 struct KnnState;     // knn_host.cuh
+struct LisiState;    // lisi_host.cuh
 
 }  // namespace
 
@@ -125,6 +126,7 @@ struct hb_handle {
   std::unique_ptr<AssignState> asg;
   std::unique_ptr<MapState> map;  // hb_map_setup only
   std::unique_ptr<KnnState> knn;  // hb_knn's scratch, from its first call
+  std::unique_ptr<LisiState> lisi;  // hb_lisi's neighbour lists, from its first call without idx / dist
 
   // traces (harmony.h:55-56); values are produced on the device and pulled lazily
   DevBuf<float> trace_d;

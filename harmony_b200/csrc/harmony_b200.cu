@@ -38,6 +38,7 @@
 #include "apply_tc3.cuh"
 #include "stats_tc3.cuh"
 #include "knn.cuh"
+#include "lisi.cuh"
 
 #include "select.cuh"
 #include "handle.cuh"
@@ -379,6 +380,7 @@ int harmony_step(hb_handle* h, const char* what, bool needs_init = true) {
 
 #include "map_host.cuh"
 #include "knn_host.cuh"
+#include "lisi_host.cuh"
 
 // =================================================================================================
 extern "C" {
@@ -550,6 +552,13 @@ int hb_knn(hb_handle* h, const void* Q, int q_dtype, int64_t q_ld, int64_t Nq, c
   if (!h) return 1;
   return run_knn(h, KnnRows{Q, q_dtype, q_ld, Nq}, KnnRows{X, x_dtype, x_ld, Nx}, d, k, metric, exclude_self != 0, idx, dist,
                  (cudaStream_t)stream);
+}
+
+int hb_lisi(hb_handle* h, const void* X, int x_dtype, int64_t x_ld, int64_t N, int d, const int32_t* labels,
+            int64_t labels_ld, int n_sets, double perplexity, double* lisi, int32_t* idx, float* dist, void* stream) {
+  if (!h) return 1;
+  return run_lisi(h, KnnRows{X, x_dtype, x_ld, N}, d, labels, labels_ld, n_sets, perplexity, lisi, idx, dist,
+                  (cudaStream_t)stream);
 }
 
 int hb_init_cluster(hb_handle* h, const double* Y0) {
@@ -973,6 +982,18 @@ int hb_debug_wide_paths(int K, int d, int J, int64_t n, int nb, int num_sms, int
 int hb_debug_knn_geometry(int d, int k, int64_t Nq, int64_t Nx, int num_sms, int64_t out[8]) {
   if (!knn_fits(d, k) || Nq < 1 || Nx < 1 || num_sms < 1) return 2;
   const KnnGeometry g = knn_geometry(d, k, Nq, Nx, num_sms);
+  const int64_t v[8] = {g.tq, KNN_TN, g.stages, g.splits, (int64_t)g.smem, g.tiles_per_split, g.KD, 2 * g.tq};
+  for (int i = 0; i < 8; ++i) out[i] = v[i];
+  return 0;
+}
+
+// The launch geometry of hb_lisi's neighbour search (test hook, host only): hb_debug_knn_geometry's eight values for a
+// self-search of N rows with k = floor(3 perplexity) - 1.  Status 2 (out untouched) for a d, perplexity or N hb_lisi
+// refuses.
+int hb_debug_lisi_geometry(int d, double perplexity, int64_t N, int num_sms, int64_t out[8]) {
+  int k = 0;
+  if (lisi_check_shape(nullptr, d, perplexity, N, &k) != 0 || num_sms < 1) return 2;
+  const KnnGeometry g = knn_geometry(d, k, N, N, num_sms);
   const int64_t v[8] = {g.tq, KNN_TN, g.stages, g.splits, (int64_t)g.smem, g.tiles_per_split, g.KD, 2 * g.tq};
   for (int i = 0; i < 8; ++i) out[i] = v[i];
   return 0;

@@ -21,7 +21,8 @@ namespace hb {
 constexpr int KNN_CAP = 16;          // candidate slots per query row; a fold is due above KNN_CAP - 8
 constexpr int KNN_SS = 18;           // row stride of a warp's 16 x 16 score stage (even: 8-byte stores)
 constexpr int KNN_TN = 64;           // reference rows per tile (= wgmma N)
-constexpr int KNN_MAX_K = 64;
+constexpr int KNN_MAX_K = 64;       // hb_knn's k
+constexpr int KNN_SWEEP_MAX_K = 128; // the sweep's: a list of 4 entries per lane (hb_lisi)
 constexpr int KNN_MAX_D = 128;
 constexpr int KNN_MERGE_MAX = 1024;  // candidates per query row in k_knn_merge (splits * k)
 constexpr float KNN_INF = __builtin_huge_valf();
@@ -108,12 +109,14 @@ struct KnnArgs {
 // (score, row) a before (score, row) b in a list: larger score, then smaller row
 __device__ __forceinline__ bool knn_before(float sa, int ia, float sb, int ib) { return sa > sb || (sa == sb && ia < ib); }
 
-// The warp folds the candidates of one query row into its list (k entries, best first) and returns the new threshold.
+// The warp folds the candidates of one query row into its list (k <= 32 E entries, best first; lane holds entries
+// lane + 32 u) and returns the new threshold.
+template <int E>
 __device__ __noinline__ float knn_fold(float* ls, int* li, const float* bs, const int* bi, int nb, int k, int lane) {
-  float s[2], cs = 0.f;
-  int id[2], ci = 0, rank[2], crank = 0;
+  float s[E], cs = 0.f;
+  int id[E], ci = 0, rank[E], crank = 0;
 #pragma unroll
-  for (int u = 0; u < 2; ++u) {
+  for (int u = 0; u < E; ++u) {
     const int e = lane + 32 * u;
     if (e < k) {
       s[u] = ls[e];
@@ -131,7 +134,7 @@ __device__ __noinline__ float knn_fold(float* ls, int* li, const float* bs, cons
   }
   __syncwarp();
 #pragma unroll
-  for (int u = 0; u < 2; ++u)
+  for (int u = 0; u < E; ++u)
     if (lane + 32 * u < k && rank[u] < k) {
       ls[rank[u]] = s[u];
       li[rank[u]] = id[u];
@@ -144,8 +147,9 @@ __device__ __noinline__ float knn_fold(float* ls, int* li, const float* bs, cons
   return ls[k - 1];
 }
 
-// grid = (query tiles, reference splits), 2 TQ threads: warpgroup g multiplies query rows [64 g, 64 g + 64) of the tile
-template <int TQ>
+// grid = (query tiles, reference splits), 2 TQ threads: warpgroup g multiplies query rows [64 g, 64 g + 64) of the tile.
+// E: list entries per lane, k <= 32 E (2 for hb_knn's k <= 64, 4 up to KNN_SWEEP_MAX_K)
+template <int TQ, int E>
 __global__ void __launch_bounds__(2 * TQ, 1) k_knn_tc(KnnArgs a) {
   constexpr int TN = KNN_TN;
   constexpr int THREADS = 2 * TQ, NACC = TN / 2, NG = TN / 8, NCH = TN / 16;
@@ -311,7 +315,7 @@ __global__ void __launch_bounds__(2 * TQ, 1) k_knn_tc(KnnArgs a) {
             // through a shuffle: ptxas sees the branch around the call as warp-uniform and does not serialise the wgmma
             const int nb = __shfl_sync(0xffffffffu, cnt[rr], 0);
             if (nb > KNN_CAP - 8) {
-              const float nt = knn_fold(lst_s + (size_t)rr * k, lst_i + (size_t)rr * k, buf_s + rr * KNN_CAP, buf_i + rr * KNN_CAP, nb, k, lane);
+              const float nt = knn_fold<E>(lst_s + (size_t)rr * k, lst_i + (size_t)rr * k, buf_s + rr * KNN_CAP, buf_i + rr * KNN_CAP, nb, k, lane);
               if (lane == 0) {
                 thr[rr] = nt;
                 cnt[rr] = 0;
@@ -329,7 +333,7 @@ __global__ void __launch_bounds__(2 * TQ, 1) k_knn_tc(KnnArgs a) {
   __syncwarp();
   for (int r = wrow; r < wrow + 16; ++r) {
     const int nb = cnt[r];
-    if (nb > 0) knn_fold(lst_s + (size_t)r * k, lst_i + (size_t)r * k, buf_s + r * KNN_CAP, buf_i + r * KNN_CAP, nb, k, lane);
+    if (nb > 0) knn_fold<E>(lst_s + (size_t)r * k, lst_i + (size_t)r * k, buf_s + r * KNN_CAP, buf_i + r * KNN_CAP, nb, k, lane);
     __syncwarp();
     if (q0 + r < a.Nq) {
       const size_t o = ((size_t)(q0 + r) * gridDim.y + blockIdx.y) * k;

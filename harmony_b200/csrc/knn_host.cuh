@@ -41,6 +41,66 @@ int knn_check_rows(hb_handle* h, const KnnRows& r, int d, const char* what) {
   return check_device_ptr(h, r.p, what);
 }
 
+// The search itself, for arguments the caller has checked, on h->stream: column sums (Euclidean), the preparation of X
+// (and of Q unless it is X), the sweep and the merge into idx / dist [Nq][k].  hb_knn and hb_lisi run it.
+int knn_search(hb_handle* h, const KnnRows& Q, const KnnRows& X, int d, int k, bool cosine, bool exclude_self,
+               int32_t* idx, float* dist) {
+  if (!h->knn) h->knn.reset(new KnnState());
+  KnnState& s = *h->knn;
+  const KnnGeometry g = knn_geometry(d, k, Q.n, X.n, h->num_sms);
+  const bool shared_rows = Q.p == X.p && Q.dtype == X.dtype && Q.ld == X.ld && Q.n == X.n;  // one prepared copy serves
+  TRY(knn_reserve(h, s.Xp, (size_t)X.n * g.KD));
+  if (!shared_rows) TRY(knn_reserve(h, s.Qp, (size_t)Q.n * g.KD));
+  TRY(knn_reserve(h, s.hx, (size_t)X.n));
+  TRY(knn_reserve(h, s.part, (size_t)Q.n * g.splits * k));
+  TRY(knn_reserve(h, s.centre, (size_t)KNN_MAX_D));
+
+  const double* centre = nullptr;
+  if (!cosine) {
+    CK(cudaMemsetAsync(s.centre.p, 0, sizeof(double) * KNN_MAX_D, h->stream));
+    const int grid = grid_for(X.n, 2, h->num_sms * 8);
+    if (X.dtype == HB_FLOAT32)
+      k_knn_colsum<<<grid, 256, 0, h->stream>>>((const float*)X.p, X.ld, X.n, d, s.centre.p);
+    else
+      k_knn_colsum<<<grid, 256, 0, h->stream>>>((const double*)X.p, X.ld, X.n, d, s.centre.p);
+    CKL();
+    centre = s.centre.p;
+  }
+  TRY(knn_prepare(h, X, d, g.KD, cosine, centre, (double)X.n, s.Xp.p, s.hx.p));
+  const float* Qp = s.Xp.p;
+  if (!shared_rows) {
+    TRY(knn_prepare(h, Q, d, g.KD, cosine, centre, (double)X.n, s.Qp.p, nullptr));
+    Qp = s.Qp.p;
+  }
+  KnnArgs a;
+  a.Qp = Qp;
+  a.Xp = s.Xp.p;
+  a.hx = s.hx.p;
+  a.part_i = s.part.p;
+  a.Nq = Q.n;
+  a.Nx = X.n;
+  a.KD = g.KD;
+  a.k = k;
+  a.stages = g.stages;
+  a.exclude_self = exclude_self;
+  a.tiles_per_split = g.tiles_per_split;
+  const dim3 grid((unsigned)g.qtiles, (unsigned)g.splits);
+  if (k <= 64) {
+    if (g.tq == 128)
+      TRY(launch(h, k_knn_tc<128, 2>, grid, dim3(256), g.smem, a));
+    else
+      TRY(launch(h, k_knn_tc<64, 2>, grid, dim3(128), g.smem, a));
+  } else {
+    if (g.tq == 128)
+      TRY(launch(h, k_knn_tc<128, 4>, grid, dim3(256), g.smem, a));
+    else
+      TRY(launch(h, k_knn_tc<64, 4>, grid, dim3(128), g.smem, a));
+  }
+  const int nc = g.splits * k;
+  return launch(h, k_knn_merge, dim3((unsigned)((Q.n + 3) / 4)), dim3(128), (size_t)4 * 2 * nc * sizeof(float), Qp,
+                (const float*)s.Xp.p, (const int*)s.part.p, Q.n, g.KD, k, nc, (int)cosine, idx, dist);
+}
+
 int run_knn(hb_handle* h, const KnnRows& Q, const KnnRows& X, int d, int k, int metric, bool exclude_self, int32_t* idx,
             float* dist, cudaStream_t caller) {
   if (Q.n < 1 || X.n < 1) return fail(h, 2, "hb_knn needs at least one query row and one reference row");
@@ -55,57 +115,10 @@ int run_knn(hb_handle* h, const KnnRows& Q, const KnnRows& X, int d, int k, int 
   TRY(check_device_ptr(h, idx, "idx"));
   if (dist) TRY(check_device_ptr(h, dist, "dist"));
   CK(cudaSetDevice(h->device));
-  if (!h->knn) h->knn.reset(new KnnState());
-  KnnState& s = *h->knn;
-  const bool cosine = metric == HB_COSINE;
-  const KnnGeometry g = knn_geometry(d, k, Q.n, X.n, h->num_sms);
-  const bool shared_rows = Q.p == X.p && Q.dtype == X.dtype && Q.ld == X.ld && Q.n == X.n;  // one prepared copy serves
-  TRY(knn_reserve(h, s.Xp, (size_t)X.n * g.KD));
-  if (!shared_rows) TRY(knn_reserve(h, s.Qp, (size_t)Q.n * g.KD));
-  TRY(knn_reserve(h, s.hx, (size_t)X.n));
-  TRY(knn_reserve(h, s.part, (size_t)Q.n * g.splits * k));
-  TRY(knn_reserve(h, s.centre, (size_t)KNN_MAX_D));
-
   TRY(stream_after(h, h->stream, caller));  // the caller's earlier work on Q, X and the outputs comes first
   {
     RegionScope rs(h, "knn");
-    const double* centre = nullptr;
-    if (!cosine) {
-      CK(cudaMemsetAsync(s.centre.p, 0, sizeof(double) * KNN_MAX_D, h->stream));
-      const int grid = grid_for(X.n, 2, h->num_sms * 8);
-      if (X.dtype == HB_FLOAT32)
-        k_knn_colsum<<<grid, 256, 0, h->stream>>>((const float*)X.p, X.ld, X.n, d, s.centre.p);
-      else
-        k_knn_colsum<<<grid, 256, 0, h->stream>>>((const double*)X.p, X.ld, X.n, d, s.centre.p);
-      CKL();
-      centre = s.centre.p;
-    }
-    TRY(knn_prepare(h, X, d, g.KD, cosine, centre, (double)X.n, s.Xp.p, s.hx.p));
-    const float* Qp = s.Xp.p;
-    if (!shared_rows) {
-      TRY(knn_prepare(h, Q, d, g.KD, cosine, centre, (double)X.n, s.Qp.p, nullptr));
-      Qp = s.Qp.p;
-    }
-    KnnArgs a;
-    a.Qp = Qp;
-    a.Xp = s.Xp.p;
-    a.hx = s.hx.p;
-    a.part_i = s.part.p;
-    a.Nq = Q.n;
-    a.Nx = X.n;
-    a.KD = g.KD;
-    a.k = k;
-    a.stages = g.stages;
-    a.exclude_self = exclude_self;
-    a.tiles_per_split = g.tiles_per_split;
-    const dim3 grid((unsigned)g.qtiles, (unsigned)g.splits);
-    if (g.tq == 128)
-      TRY(launch(h, k_knn_tc<128>, grid, dim3(256), g.smem, a));
-    else
-      TRY(launch(h, k_knn_tc<64>, grid, dim3(128), g.smem, a));
-    const int nc = g.splits * k;
-    TRY(launch(h, k_knn_merge, dim3((unsigned)((Q.n + 3) / 4)), dim3(128), (size_t)4 * 2 * nc * sizeof(float), Qp,
-               (const float*)s.Xp.p, (const int*)s.part.p, Q.n, g.KD, k, nc, (int)cosine, idx, dist));
+    TRY(knn_search(h, Q, X, d, k, metric == HB_COSINE, exclude_self, idx, dist));
   }
   return stream_after(h, caller, h->stream);
 }

@@ -104,11 +104,12 @@ CallPath call_path(const KernelPaths& p, unsigned T, bool legacy_centroid) {
 
 // ---- hb_knn (knn.cuh) -------------------------------------------------------------------------------------------------
 // Launch geometry of the k-nearest-neighbour sweep: query rows per CTA (tq), operand stages of the reference tiles
-// (KNN_TN rows each) and reference splits.  The first of (128, 2), (128, 1), (64, 2) whose shared memory fits: the query
-// tile and the lists stay for the CTA's life, so wide rows and long lists take it from the second reference stage first
-// and from the query tile last (a 64-row tile halves the flop per reference byte and runs one warpgroup).  (64, 2)
-// holds d = 128, k = 64.  With fewer query tiles than SMs the reference is split over grid.y so that the GPU is full, as
-// far as k_knn_merge's candidate limit and the reference's tiles allow.
+// (KNN_TN rows each) and reference splits.  The first of (128, 2), (128, 1), (64, 2), (64, 1) whose shared memory fits:
+// the query tile and the lists stay for the CTA's life, so wide rows and long lists take it from the second reference
+// stage first and from the query tile last (a 64-row tile halves the flop per reference byte and runs one warpgroup).
+// (64, 2) holds d = 128, k = 64; (64, 1), reached only by hb_lisi's k > 64, holds d = 128, k = KNN_SWEEP_MAX_K.  With
+// fewer query tiles than SMs the reference is split over grid.y so that the GPU is full, as far as k_knn_merge's
+// candidate limit and the reference's tiles allow.
 struct KnnGeometry {
   int tq = 0, stages = 0, splits = 0, KD = 0;
   size_t smem = 0;
@@ -118,7 +119,7 @@ bool knn_fits(int d, int k) { return d >= 1 && d <= KNN_MAX_D && k >= 1 && k <= 
 KnnGeometry knn_geometry(int d, int k, int64_t Nq, int64_t Nx, int num_sms) {
   KnnGeometry g;
   g.KD = (d + 7) & ~7;
-  static const int shapes[3][2] = {{128, 2}, {128, 1}, {64, 2}};
+  static const int shapes[4][2] = {{128, 2}, {128, 1}, {64, 2}, {64, 1}};
   for (const auto& s : shapes)
     if (knn_smem_bytes(s[0], s[1], g.KD, k) <= SMEM_LIMIT) {
       g.tq = s[0], g.stages = s[1];

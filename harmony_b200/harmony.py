@@ -194,6 +194,14 @@ class harmony:
         from .neighbors import knn_on
         return knn_on(self, query, ref, k, metric)
 
+    def lisi(self, X, codes, perplexity=30, return_neighbors=False):
+        """LISI of every row of ``X`` [N, d] (host array or CUDA tensor) for the label sets ``codes`` (int32 [N] or
+        [n_sets, N]; any codes, only equality counts) on this object's device and stream -> [N, n_sets] float64, with
+        ``return_neighbors`` also ``(idx, dist)``.  ``harmony_b200.compute_lisi`` takes labels by column name.  Works
+        in any state of the object and changes none of it, e.g. ``obj.lisi(obj.get_tensor("Z_corr"), batch_codes)``."""
+        from .lisi import lisi_on
+        return lisi_on(self, X, codes, perplexity, return_neighbors)
+
     def _device_Z(self, Z):
         """An [N, d] CUDA tensor -> (the tensor to read, (pointer, dtype, row stride, stream) of hb_setup_device)).
         Rows with unit column stride are read in place; any other layout is made contiguous on the device first."""

@@ -43,8 +43,8 @@ const char* hb_last_error(const hb_handle* h);
  * buf; returns 1 if a warning was written, 0 if none is pending.  The shim turns it into Rcpp::warning. */
 int hb_pop_warning(hb_handle* h, char* buf, size_t cap);
 /* Library/ABI version: major*10000 + minor*100 + patch (0.3.0: labels in device memory; 0.4.0: mapping a query onto
- * a reference, hb_reference / hb_map_setup / hb_map).  hb_knn and hb_debug_knn_geometry were added without moving the
- * number. */
+ * a reference, hb_reference / hb_map_setup / hb_map).  hb_knn, hb_debug_knn_geometry, hb_lisi and
+ * hb_debug_lisi_geometry were added without moving the number. */
 int hb_version(void);
 
 /* ---- multi-GPU (one process per GPU; cells sharded contiguously; SURVEY §8e) ------------------- */
@@ -169,6 +169,23 @@ int hb_knn(hb_handle* h, const void* Q, int q_dtype, int64_t q_ld, int64_t Nq, c
  * fill the GPU), shared-memory bytes, reference tiles per split, padded row length in floats, threads per CTA}.
  * Returns 0, or 2 with out untouched for a d or k hb_knn refuses. */
 int hb_debug_knn_geometry(int d, int k, int64_t Nq, int64_t Nx, int num_sms, int64_t out[8]);
+/* LISI, the Local Inverse Simpson's Index (DESIGN.md §10), of every row of X [N, d] for n_sets label sets: with the
+ * k = floor(3 perplexity) - 1 nearest other rows by Euclidean distance D_j (hb_knn's search with exclude_self), weights
+ * P_j ~ exp(-beta D_j) with beta bisected in fp64 until the entropy is within 1e-5 of ln(perplexity) (at most 50
+ * evaluations), and lisi[i][s] = 1 / sum over the labels of set s of (sum of P_j over the neighbours with that label)^2:
+ * the effective number of labels around row i.  -1 for a row whose final entropy is exactly 0; NaN for a row without a
+ * neighbour (every row with a non-finite value).  labels: n_sets rows of labels_ld >= N int32 codes, set s of row j at
+ * labels[s * labels_ld + j]; codes are arbitrary, only equality counts.  lisi [N][n_sets] fp64; idx [N][k] and dist
+ * [N][k] (as hb_knn returns them) when not NULL.  X of x_dtype (hb_dtype) with row stride x_ld >= d.
+ * Limits, status 2 with a message before any launch: a finite perplexity >= 1, k <= 128 (perplexity < 43 1/3),
+ * k <= N - 1, N < 2^31, 1 <= d <= 128, n_sets >= 1, labels_ld >= N, an unknown dtype, a row stride < d, a NULL (X,
+ * labels, lisi), host or other-device pointer.  Ordered on `stream` like hb_knn; needs no setup and leaves a Harmony or
+ * mapping handle's state untouched.  Region "lisi". */
+int hb_lisi(hb_handle* h, const void* X, int x_dtype, int64_t x_ld, int64_t N, int d, const int32_t* labels,
+            int64_t labels_ld, int n_sets, double perplexity, double* lisi, int32_t* idx, float* dist, void* stream);
+/* Test hook (host only): hb_debug_knn_geometry's eight values for hb_lisi's search of N rows at this perplexity on
+ * num_sms SMs.  Returns 0, or 2 with out untouched for a d, perplexity or N hb_lisi refuses. */
+int hb_debug_lisi_geometry(int d, double perplexity, int64_t N, int num_sms, int64_t out[8]);
 
 /* ---- fields / getters (harmony.cpp:640-669, 675-696) ------------------------------------------- */
 enum hb_field {
