@@ -31,7 +31,7 @@ A logits_args(hb_handle* h, const float* sigma, bool normalise) {
 int launch_logits_wide(hb_handle* h, const float* sigma, bool normalise) {
   const int KDc = (h->d + LW_DC - 1) / LW_DC * LW_DC, rows = (h->K + LW_NP - 1) / LW_NP * LW_NP;
   DevBuf<float>& Ypad = h->asg->Ypad;
-  if (Ypad.n < (size_t)rows * KDc) CK(Ypad.alloc((size_t)rows * KDc));
+  CK(Ypad.reserve((size_t)rows * KDc));
   k_pad_rows<<<grid_for((int64_t)rows * KDc, 256, h->num_sms * 4), 256, 0, h->stream>>>(h->Y.p, Ypad.p, h->K, h->d, rows, KDc);
   CKL();
   LogitsWideArgs t = logits_args<LogitsWideArgs>(h, sigma, normalise);
@@ -222,9 +222,9 @@ int legacy_centroid_step(hb_handle* h) {
   k_centroids_from_stats<<<K, 64, sizeof(float) * (size_t)d, h->stream>>>(h->S.p, h->Y.p, J, K, d);
   CKL();
   // distances to the new centroids -> U; everything else the assignment writes is put back
-  if (keep.Rkeep.n < nK) CK(keep.Rkeep.alloc(nK));
-  if (keep.OEkeep.n < 2 * BK) CK(keep.OEkeep.alloc(2 * BK));
-  if (keep.objkeep.n < 2) CK(keep.objkeep.alloc(2));
+  CK(keep.Rkeep.reserve(nK));
+  CK(keep.OEkeep.reserve(2 * BK));
+  CK(keep.objkeep.reserve(2));
   CK(cudaMemcpyAsync(keep.Rkeep.p, h->R.p, sizeof(float) * nK, cudaMemcpyDeviceToDevice, h->stream));
   CK(cudaMemcpyAsync(keep.OEkeep.p, h->O.p, sizeof(float) * BK, cudaMemcpyDeviceToDevice, h->stream));
   CK(cudaMemcpyAsync(keep.OEkeep.p + BK, h->E.p, sizeof(float) * BK, cudaMemcpyDeviceToDevice, h->stream));

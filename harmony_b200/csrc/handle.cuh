@@ -35,6 +35,8 @@ struct DevBuf {
     if (e == cudaSuccess) n = count;
     return e;
   }
+  // at least `count` elements: a smaller buffer is replaced (its contents go), a large enough one is kept as it is
+  cudaError_t reserve(size_t count) { return n < count ? alloc(count) : cudaSuccess; }
 };
 void keep_pool_memory(int device) {
   cudaMemPool_t pool;

@@ -100,36 +100,27 @@ int reserve_rounds(hb_handle* h, int T) {
 }
 
 // ---- the setup steps of both kinds of handle: hb_setup* (Harmony) and hb_map_setup* (map_host.cuh) ------------------
-// The cells given to setup: Z as host doubles (d per row, dense) or a device array of `dtype` with row stride `ld`, and
-// the labels phi, read on the library stream after the work queued on `stream`
+// The cells given to setup: Z as host doubles (d per row, dense) or device rows, and the labels phi, read on the
+// library stream after the work queued on `stream`
 struct CellInput {
   const double* host = nullptr;
-  const void* dev = nullptr;
-  int dtype = HB_FLOAT64;
-  int64_t ld = 0;
+  DevRows dev{};  // dev.p null: host Z
   cudaStream_t stream = nullptr;
   const int32_t* phi = nullptr;
   bool phi_on_device = false;  // else one copy to the device first
 };
 
-// The checks of the cell arguments of setup entry point `entry`, whose Z lies in host or (`z_on_device`) device
-// memory.  A host entry point refuses device labels and copies managed ones; a device entry point reads them in place.
-int setup_inputs(hb_handle* h, const char* entry, const void* Z, bool z_on_device, int dtype, int64_t ld, void* stream,
-                 int d, const int32_t* phi_i, CellInput* in) {
+// The checks of the cell arguments of setup entry point `entry`, whose Z lies in host memory (`host`) or is the device
+// rows *dev.  A host entry point refuses device labels and copies managed ones; a device entry point reads them in place.
+int setup_inputs(hb_handle* h, const char* entry, const double* host, const DevRows* dev, void* stream, int d,
+                 const int32_t* phi_i, CellInput* in) {
   if (h->ran_setup) return fail(h, 3, "setup was already run on this object");
-  if (z_on_device) {
-    if (dtype != HB_FLOAT32 && dtype != HB_FLOAT64) return fail(h, 2, "unknown dtype %d of Z", dtype);
-    if (ld < d) return fail(h, 2, "row stride of Z (%lld) is smaller than d = %d", (long long)ld, d);
-    TRY(check_device_ptr(h, Z, "Z"));
-  }
+  if (dev) TRY(check_rows(h, *dev, d, "Z"));
   cudaMemoryType phi_type;
   TRY(phi_location(h, phi_i, &phi_type));
-  if (!z_on_device && phi_type == cudaMemoryTypeDevice)
+  if (!dev && phi_type == cudaMemoryTypeDevice)
     return fail(h, 2, "phi_i is device memory: %s takes host labels (device labels go through %s_device)", entry, entry);
-  if (z_on_device)
-    *in = CellInput{nullptr, Z, dtype, ld, (cudaStream_t)stream, phi_i, phi_type != cudaMemoryTypeHost};
-  else
-    *in = CellInput{(const double*)Z, nullptr, HB_FLOAT64, 0, nullptr, phi_i, false};
+  *in = CellInput{host, dev ? *dev : DevRows{}, (cudaStream_t)stream, phi_i, dev && phi_type != cudaMemoryTypeHost};
   return 0;
 }
 
@@ -193,7 +184,7 @@ int init_common(hb_handle* h) {
 
 // Z into Zo, in tuple-sorted order (double -> float for host Z)
 int upload_z(hb_handle* h, const CellInput& in) {
-  if (in.dev) return upload_rows_device(h, in.dev, in.dtype, in.ld, in.stream);
+  if (in.dev.p) return upload_rows_device(h, in.dev, in.stream);
   return upload_rows(h, in.host, h->d, h->DS, h->Zo.p);
 }
 
@@ -349,7 +340,7 @@ int setup_uploads(hb_handle* h, const CellInput& in, const double* sigma, const 
 int setup_common(hb_handle* h, const CellInput& in, int d, int64_t N, const int32_t* B_vec, int C, const double* sigma,
                  const double* theta, const double* lambda, double alpha, int max_iter_kmeans, double epsilon_kmeans,
                  double epsilon_harmony, int K, double block_size, double batch_proportion_cutoff, int verbose) {
-  if (!(in.host || in.dev) || !in.phi || !B_vec || !sigma || !theta) return fail(h, 2, "null argument");
+  if (!(in.host || in.dev.p) || !in.phi || !B_vec || !sigma || !theta) return fail(h, 2, "null argument");
   TRY(setup_scalars(h, d, N, B_vec, C, lambda, max_iter_kmeans, epsilon_kmeans, epsilon_harmony, alpha, K, block_size,
                     batch_proportion_cutoff, verbose));
   HostLap lap(h->stream, "hb_setup");
@@ -499,7 +490,7 @@ int hb_setup(hb_handle* h, const double* Z, int d, int64_t N, const int32_t* phi
              double batch_proportion_cutoff, int verbose) {
   if (!h) return 1;
   CellInput in;
-  TRY(setup_inputs(h, "hb_setup", Z, false, HB_FLOAT64, d, nullptr, d, phi_i, &in));
+  TRY(setup_inputs(h, "hb_setup", Z, nullptr, nullptr, d, phi_i, &in));
   return setup_common(h, in, d, N, B_vec, C, sigma, theta, lambda, alpha, max_iter_kmeans, epsilon_kmeans,
                       epsilon_harmony, K, block_size, batch_proportion_cutoff, verbose);
 }
@@ -510,7 +501,8 @@ int hb_setup_device(hb_handle* h, const void* Z, int z_dtype, int64_t z_ld, void
                     double epsilon_harmony, int K, double block_size, double batch_proportion_cutoff, int verbose) {
   if (!h) return 1;
   CellInput in;
-  TRY(setup_inputs(h, "hb_setup_device", Z, true, z_dtype, z_ld, stream, d, phi_i, &in));
+  const DevRows z{Z, z_dtype, z_ld, N};
+  TRY(setup_inputs(h, "hb_setup_device", nullptr, &z, stream, d, phi_i, &in));
   return setup_common(h, in, d, N, B_vec, C, sigma, theta, lambda, alpha, max_iter_kmeans, epsilon_kmeans,
                       epsilon_harmony, K, block_size, batch_proportion_cutoff, verbose);
 }
@@ -528,7 +520,7 @@ int hb_map_setup(hb_handle* h, const double* Z, int d, int64_t N, const int32_t*
                  const double* sigma) {
   if (!h) return 1;
   CellInput in;
-  TRY(setup_inputs(h, "hb_map_setup", Z, false, HB_FLOAT64, d, nullptr, d, phi_i, &in));
+  TRY(setup_inputs(h, "hb_map_setup", Z, nullptr, nullptr, d, phi_i, &in));
   return map_setup(h, in, d, N, B_vec, C, lambda, K, centroids, Nr, Cref, sigma);
 }
 
@@ -537,7 +529,8 @@ int hb_map_setup_device(hb_handle* h, const void* Z, int z_dtype, int64_t z_ld, 
                         const double* centroids, const double* Nr, const double* Cref, const double* sigma) {
   if (!h) return 1;
   CellInput in;
-  TRY(setup_inputs(h, "hb_map_setup_device", Z, true, z_dtype, z_ld, stream, d, phi_i, &in));
+  const DevRows z{Z, z_dtype, z_ld, N};
+  TRY(setup_inputs(h, "hb_map_setup_device", nullptr, &z, stream, d, phi_i, &in));
   return map_setup(h, in, d, N, B_vec, C, lambda, K, centroids, Nr, Cref, sigma);
 }
 
@@ -550,14 +543,14 @@ int hb_map(hb_handle* h) {
 int hb_knn(hb_handle* h, const void* Q, int q_dtype, int64_t q_ld, int64_t Nq, const void* X, int x_dtype, int64_t x_ld,
            int64_t Nx, int d, int k, int metric, int exclude_self, int32_t* idx, float* dist, void* stream) {
   if (!h) return 1;
-  return run_knn(h, KnnRows{Q, q_dtype, q_ld, Nq}, KnnRows{X, x_dtype, x_ld, Nx}, d, k, metric, exclude_self != 0, idx, dist,
+  return run_knn(h, DevRows{Q, q_dtype, q_ld, Nq}, DevRows{X, x_dtype, x_ld, Nx}, d, k, metric, exclude_self != 0, idx, dist,
                  (cudaStream_t)stream);
 }
 
 int hb_lisi(hb_handle* h, const void* X, int x_dtype, int64_t x_ld, int64_t N, int d, const int32_t* labels,
             int64_t labels_ld, int n_sets, double perplexity, double* lisi, int32_t* idx, float* dist, void* stream) {
   if (!h) return 1;
-  return run_lisi(h, KnnRows{X, x_dtype, x_ld, N}, d, labels, labels_ld, n_sets, perplexity, lisi, idx, dist,
+  return run_lisi(h, DevRows{X, x_dtype, x_ld, N}, d, labels, labels_ld, n_sets, perplexity, lisi, idx, dist,
                   (cudaStream_t)stream);
 }
 
@@ -595,7 +588,7 @@ int hb_cluster(hb_handle* h, const int64_t* update_orders) {
   if (cold && !plan_assign) TRY(run_assign(h, true, false));
   if (update_orders && T > 0) {
     size_t cnt = (size_t)T * (size_t)h->N_global;
-    if (h->perms_d.n < cnt) CK(h->perms_d.alloc(cnt));
+    CK(h->perms_d.reserve(cnt));
     CK(cudaMemcpyAsync(h->perms_d.p, update_orders, sizeof(int64_t) * cnt, cudaMemcpyHostToDevice, h->stream));
   }
   if (h->abort_cb && h->abort_cb(h->abort_user)) return -1;  // Progress::check_abort (:233)
@@ -763,23 +756,19 @@ int hb_get_field_device(hb_handle* h, int field, void* out, int dtype, int64_t l
   if (!h->ran_setup) return fail(h, 3, "setup has not been run");
   const RowField f = row_field(h, field);
   if (!f.buf) return fail(h, 2, "field %d has no device getter (HB_Z_CORR, HB_Z_ORIG, HB_R)", field);
-  if (dtype != HB_FLOAT32 && dtype != HB_FLOAT64) return fail(h, 2, "unknown dtype %d", dtype);
-  if (ld < f.cols) return fail(h, 2, "row stride %lld is smaller than the field's %d columns", (long long)ld, f.cols);
-  TRY(check_device_ptr(h, out, "output"));
+  const DevRows rows{out, dtype, ld, h->n};
+  TRY(check_rows(h, rows, f.cols, "out"));
   CK(cudaSetDevice(h->device));
-  const cudaStream_t caller = (cudaStream_t)stream;
-  TRY(stream_after(h, h->stream, caller));  // the caller's earlier work on `out` comes first
-  if (field == HB_Z_CORR) TRY(normalise_pending_zc(h));
-  {
+  return on_caller_stream(h, (cudaStream_t)stream, [&] {
+    if (field == HB_Z_CORR) TRY(normalise_pending_zc(h));
     RegionScope rs(h, "download");
-    const float* src = f.buf;
-    if (dtype == HB_FLOAT32)
-      copy_rows(src, f.ld, (float*)out, ld, h->inv_sort.p, 0, false, h->n, f.cols, h->num_sms, h->stream);
-    else
-      copy_rows(src, f.ld, (double*)out, ld, h->inv_sort.p, 0, false, h->n, f.cols, h->num_sms, h->stream);
+    with_rows(rows, [&](auto o) {  // `out` is the caller's writable array
+      using T = std::remove_const_t<std::remove_pointer_t<decltype(o)>>;
+      copy_rows(f.buf, f.ld, const_cast<T*>(o), ld, h->inv_sort.p, 0, false, h->n, f.cols, h->num_sms, h->stream);
+    });
     CKL();
-  }
-  return stream_after(h, caller, h->stream);
+    return 0;
+  });
 }
 
 int hb_set_field(hb_handle* h, int field, const double* in) {
@@ -981,9 +970,7 @@ int hb_debug_wide_paths(int K, int d, int J, int64_t n, int nb, int num_sms, int
 // Status 2 (out untouched) for a d or k hb_knn refuses.
 int hb_debug_knn_geometry(int d, int k, int64_t Nq, int64_t Nx, int num_sms, int64_t out[8]) {
   if (!knn_fits(d, k) || Nq < 1 || Nx < 1 || num_sms < 1) return 2;
-  const KnnGeometry g = knn_geometry(d, k, Nq, Nx, num_sms);
-  const int64_t v[8] = {g.tq, KNN_TN, g.stages, g.splits, (int64_t)g.smem, g.tiles_per_split, g.KD, 2 * g.tq};
-  for (int i = 0; i < 8; ++i) out[i] = v[i];
+  knn_geometry_record(d, k, Nq, Nx, num_sms, out);
   return 0;
 }
 
@@ -993,9 +980,7 @@ int hb_debug_knn_geometry(int d, int k, int64_t Nq, int64_t Nx, int num_sms, int
 int hb_debug_lisi_geometry(int d, double perplexity, int64_t N, int num_sms, int64_t out[8]) {
   int k = 0;
   if (lisi_check_shape(nullptr, d, perplexity, N, &k) != 0 || num_sms < 1) return 2;
-  const KnnGeometry g = knn_geometry(d, k, N, N, num_sms);
-  const int64_t v[8] = {g.tq, KNN_TN, g.stages, g.splits, (int64_t)g.smem, g.tiles_per_split, g.KD, 2 * g.tq};
-  for (int i = 0; i < 8; ++i) out[i] = v[i];
+  knn_geometry_record(d, k, N, N, num_sms, out);
   return 0;
 }
 

@@ -11,58 +11,55 @@ struct KnnState {
   DevBuf<double> centre;     // [KNN_MAX_D] column sums of X
 };
 
-template <typename T>
-int knn_reserve(hb_handle* h, DevBuf<T>& b, size_t count) {
-  if (b.n < count) CK(b.alloc(count));
-  return 0;
-}
-
-struct KnnRows {
-  const void* p;
-  int dtype;
-  int64_t ld, n;
-};
-
 // rows -> dst [n][KD] (and hx), centred on `centre` / centre_n or normalised
-int knn_prepare(hb_handle* h, const KnnRows& r, int d, int KD, bool cosine, const double* centre, double centre_n,
+int knn_prepare(hb_handle* h, const DevRows& r, int d, int KD, bool cosine, const double* centre, double centre_n,
                 float* dst, float* hx) {
   const int grid = grid_for(r.n * 32, 256, h->num_sms * 16);
-  if (r.dtype == HB_FLOAT32)
-    k_knn_prepare<<<grid, 256, 0, h->stream>>>((const float*)r.p, r.ld, r.n, d, KD, (int)cosine, centre, centre_n, dst, hx);
-  else
-    k_knn_prepare<<<grid, 256, 0, h->stream>>>((const double*)r.p, r.ld, r.n, d, KD, (int)cosine, centre, centre_n, dst, hx);
+  with_rows(r, [&](auto p) {
+    k_knn_prepare<<<grid, 256, 0, h->stream>>>(p, r.ld, r.n, d, KD, (int)cosine, centre, centre_n, dst, hx);
+  });
   CKL();
   return 0;
 }
 
-int knn_check_rows(hb_handle* h, const KnnRows& r, int d, const char* what) {
-  if (r.dtype != HB_FLOAT32 && r.dtype != HB_FLOAT64) return fail(h, 2, "unknown dtype %d of %s", r.dtype, what);
-  if (r.ld < d) return fail(h, 2, "row stride of %s (%lld) is smaller than d = %d", what, (long long)r.ld, d);
-  return check_device_ptr(h, r.p, what);
+// Status 2, with the message when there is a handle: the geometry hooks run the shape checks without one
+template <typename... A>
+int refuse(hb_handle* h, const char* fmt, A... args) { return h ? fail(h, 2, fmt, args...) : 2; }
+// The search's shape limits, which hb_knn and hb_lisi (`entry`) share: fewer than 2^31 rows to search (n, named
+// `what`) and 1 <= d <= KNN_MAX_D
+int check_search_shape(hb_handle* h, const char* entry, const char* what, int64_t n, int d) {
+  if (n >= (1LL << 31)) return refuse(h, "%s: %s = %lld rows are not supported (%s < 2^31)", entry, what, (long long)n, what);
+  if (d < 1 || d > KNN_MAX_D) return refuse(h, "%s: d = %d is not supported (1 <= d <= %d)", entry, d, KNN_MAX_D);
+  return 0;
+}
+
+// The eight values of the geometry hooks (hb_debug_knn_geometry, hb_debug_lisi_geometry) for a search of Nq rows
+// against Nx
+void knn_geometry_record(int d, int k, int64_t Nq, int64_t Nx, int num_sms, int64_t out[8]) {
+  const KnnGeometry g = knn_geometry(d, k, Nq, Nx, num_sms);
+  const int64_t v[8] = {g.tq, KNN_TN, g.stages, g.splits, (int64_t)g.smem, g.tiles_per_split, g.KD, 2 * g.tq};
+  for (int i = 0; i < 8; ++i) out[i] = v[i];
 }
 
 // The search itself, for arguments the caller has checked, on h->stream: column sums (Euclidean), the preparation of X
 // (and of Q unless it is X), the sweep and the merge into idx / dist [Nq][k].  hb_knn and hb_lisi run it.
-int knn_search(hb_handle* h, const KnnRows& Q, const KnnRows& X, int d, int k, bool cosine, bool exclude_self,
+int knn_search(hb_handle* h, const DevRows& Q, const DevRows& X, int d, int k, bool cosine, bool exclude_self,
                int32_t* idx, float* dist) {
   if (!h->knn) h->knn.reset(new KnnState());
   KnnState& s = *h->knn;
   const KnnGeometry g = knn_geometry(d, k, Q.n, X.n, h->num_sms);
   const bool shared_rows = Q.p == X.p && Q.dtype == X.dtype && Q.ld == X.ld && Q.n == X.n;  // one prepared copy serves
-  TRY(knn_reserve(h, s.Xp, (size_t)X.n * g.KD));
-  if (!shared_rows) TRY(knn_reserve(h, s.Qp, (size_t)Q.n * g.KD));
-  TRY(knn_reserve(h, s.hx, (size_t)X.n));
-  TRY(knn_reserve(h, s.part, (size_t)Q.n * g.splits * k));
-  TRY(knn_reserve(h, s.centre, (size_t)KNN_MAX_D));
+  CK(s.Xp.reserve((size_t)X.n * g.KD));
+  if (!shared_rows) CK(s.Qp.reserve((size_t)Q.n * g.KD));
+  CK(s.hx.reserve((size_t)X.n));
+  CK(s.part.reserve((size_t)Q.n * g.splits * k));
+  CK(s.centre.reserve((size_t)KNN_MAX_D));
 
   const double* centre = nullptr;
   if (!cosine) {
     CK(cudaMemsetAsync(s.centre.p, 0, sizeof(double) * KNN_MAX_D, h->stream));
     const int grid = grid_for(X.n, 2, h->num_sms * 8);
-    if (X.dtype == HB_FLOAT32)
-      k_knn_colsum<<<grid, 256, 0, h->stream>>>((const float*)X.p, X.ld, X.n, d, s.centre.p);
-    else
-      k_knn_colsum<<<grid, 256, 0, h->stream>>>((const double*)X.p, X.ld, X.n, d, s.centre.p);
+    with_rows(X, [&](auto x) { k_knn_colsum<<<grid, 256, 0, h->stream>>>(x, X.ld, X.n, d, s.centre.p); });
     CKL();
     centre = s.centre.p;
   }
@@ -101,26 +98,23 @@ int knn_search(hb_handle* h, const KnnRows& Q, const KnnRows& X, int d, int k, b
                 (const float*)s.Xp.p, (const int*)s.part.p, Q.n, g.KD, k, nc, (int)cosine, idx, dist);
 }
 
-int run_knn(hb_handle* h, const KnnRows& Q, const KnnRows& X, int d, int k, int metric, bool exclude_self, int32_t* idx,
+int run_knn(hb_handle* h, const DevRows& Q, const DevRows& X, int d, int k, int metric, bool exclude_self, int32_t* idx,
             float* dist, cudaStream_t caller) {
   if (Q.n < 1 || X.n < 1) return fail(h, 2, "hb_knn needs at least one query row and one reference row");
-  if (X.n >= (1LL << 31)) return fail(h, 2, "hb_knn: Nx = %lld reference rows are not supported (Nx < 2^31)", (long long)X.n);
-  if (d < 1 || d > KNN_MAX_D) return fail(h, 2, "hb_knn: d = %d is not supported (1 <= d <= %d)", d, KNN_MAX_D);
+  TRY(check_search_shape(h, "hb_knn", "Nx", X.n, d));
   if (k < 1 || k > KNN_MAX_K) return fail(h, 2, "hb_knn: k = %d is not supported (1 <= k <= %d)", k, KNN_MAX_K);
   if (k > X.n - (exclude_self ? 1 : 0))
     return fail(h, 2, "hb_knn: k = %d exceeds the %lld candidate rows of a query row", k, (long long)(X.n - (exclude_self ? 1 : 0)));
   if (metric != HB_EUCLIDEAN && metric != HB_COSINE) return fail(h, 2, "hb_knn: unknown metric %d", metric);
-  TRY(knn_check_rows(h, Q, d, "Q"));
-  TRY(knn_check_rows(h, X, d, "X"));
+  TRY(check_rows(h, Q, d, "Q"));
+  TRY(check_rows(h, X, d, "X"));
   TRY(check_device_ptr(h, idx, "idx"));
   if (dist) TRY(check_device_ptr(h, dist, "dist"));
   CK(cudaSetDevice(h->device));
-  TRY(stream_after(h, h->stream, caller));  // the caller's earlier work on Q, X and the outputs comes first
-  {
+  return on_caller_stream(h, caller, [&] {
     RegionScope rs(h, "knn");
-    TRY(knn_search(h, Q, X, d, k, metric == HB_COSINE, exclude_self, idx, dist));
-  }
-  return stream_after(h, caller, h->stream);
+    return knn_search(h, Q, X, d, k, metric == HB_COSINE, exclude_self, idx, dist);
+  });
 }
 
 }  // namespace

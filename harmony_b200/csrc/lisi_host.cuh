@@ -22,23 +22,21 @@ int lisi_k(double p) {
 // The refusals hb_lisi and hb_debug_lisi_geometry share; h may be null (no message).
 int lisi_check_shape(hb_handle* h, int d, double p, int64_t N, int* k_out) {
   const int k = lisi_k(p);
-  auto refuse = [&](const char* fmt, auto... args) { return h ? fail(h, 2, fmt, args...) : 2; };
-  if (k == 0) return refuse("hb_lisi: perplexity %g is not supported (a finite p >= 1)", p);
-  if (k > KNN_SWEEP_MAX_K) return refuse("hb_lisi: perplexity %g needs more than %d neighbours (p < 43 1/3)", p, KNN_SWEEP_MAX_K);
-  if (N >= (1LL << 31)) return refuse("hb_lisi: N = %lld rows are not supported (N < 2^31)", (long long)N);
-  if (k > N - 1) return refuse("hb_lisi: perplexity %g needs k = %d neighbours, N = %lld rows have %lld", p, k, (long long)N, (long long)(N - 1));
-  if (d < 1 || d > KNN_MAX_D) return refuse("hb_lisi: d = %d is not supported (1 <= d <= %d)", d, KNN_MAX_D);
+  if (k == 0) return refuse(h, "hb_lisi: perplexity %g is not supported (a finite p >= 1)", p);
+  if (k > KNN_SWEEP_MAX_K) return refuse(h, "hb_lisi: perplexity %g needs more than %d neighbours (p < 43 1/3)", p, KNN_SWEEP_MAX_K);
+  if (k > N - 1) return refuse(h, "hb_lisi: perplexity %g needs k = %d neighbours, N = %lld rows have %lld", p, k, (long long)N, (long long)(N - 1));
+  TRY(check_search_shape(h, "hb_lisi", "N", N, d));  // N >= 2^31 passes the check above: the refusals keep their order
   *k_out = k;
   return 0;
 }
 
-int run_lisi(hb_handle* h, const KnnRows& X, int d, const int32_t* labels, int64_t labels_ld, int n_sets, double p,
+int run_lisi(hb_handle* h, const DevRows& X, int d, const int32_t* labels, int64_t labels_ld, int n_sets, double p,
              double* lisi, int32_t* idx, float* dist, cudaStream_t caller) {
   int k = 0;
   TRY(lisi_check_shape(h, d, p, X.n, &k));
   if (n_sets < 1) return fail(h, 2, "hb_lisi: n_sets = %d, at least one label set is needed", n_sets);
   if (labels_ld < X.n) return fail(h, 2, "hb_lisi: label stride %lld is smaller than N = %lld", (long long)labels_ld, (long long)X.n);
-  TRY(knn_check_rows(h, X, d, "X"));
+  TRY(check_rows(h, X, d, "X"));
   TRY(check_device_ptr(h, labels, "labels"));
   TRY(check_device_ptr(h, lisi, "lisi"));
   if (idx) TRY(check_device_ptr(h, idx, "idx"));
@@ -47,21 +45,19 @@ int run_lisi(hb_handle* h, const KnnRows& X, int d, const int32_t* labels, int64
   if (!h->lisi) h->lisi.reset(new LisiState());
   LisiState& s = *h->lisi;
   if (!idx) {
-    TRY(knn_reserve(h, s.idx, (size_t)X.n * k));
+    CK(s.idx.reserve((size_t)X.n * k));
     idx = s.idx.p;
   }
   if (!dist) {
-    TRY(knn_reserve(h, s.dist, (size_t)X.n * k));
+    CK(s.dist.reserve((size_t)X.n * k));
     dist = s.dist.p;
   }
-  TRY(stream_after(h, h->stream, caller));  // the caller's earlier work on X, the labels and the outputs comes first
-  {
+  return on_caller_stream(h, caller, [&] {
     RegionScope rs(h, "lisi");
     TRY(knn_search(h, X, X, d, k, false, true, idx, dist));
-    TRY(launch(h, k_lisi, dim3((unsigned)((X.n + LISI_WARPS - 1) / LISI_WARPS)), dim3(32 * LISI_WARPS), 0,
-               (const int32_t*)idx, (const float*)dist, X.n, k, labels, labels_ld, n_sets, std::log(p), lisi));
-  }
-  return stream_after(h, caller, h->stream);
+    return launch(h, k_lisi, dim3((unsigned)((X.n + LISI_WARPS - 1) / LISI_WARPS)), dim3(32 * LISI_WARPS), 0,
+                  (const int32_t*)idx, (const float*)dist, X.n, k, labels, labels_ld, n_sets, std::log(p), lisi);
+  });
 }
 
 }  // namespace

@@ -50,7 +50,7 @@ int map_setup(hb_handle* h, const CellInput& in, int d, int64_t N, const int32_t
               int K, const double* centroids, const double* Nr, const double* Cref, const double* sigma) {
   if (h->world > 1 || (h->shard_set && (h->N_global != N || h->cell_offset != 0)))
     return fail(h, 3, "mapping does not take sharded cells");
-  if (!(in.host || in.dev) || !in.phi || !B_vec || !lambda || !centroids || !Nr || !Cref || !sigma)
+  if (!(in.host || in.dev.p) || !in.phi || !B_vec || !lambda || !centroids || !Nr || !Cref || !sigma)
     return fail(h, 2, "null argument");
   TRY(check_dimensions(h, d, N, C, K));
   for (int c = 0; c < C; ++c)

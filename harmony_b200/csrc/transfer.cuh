@@ -236,6 +236,23 @@ int phi_location(hb_handle* h, const void* p, cudaMemoryType* type) {
   *type = cudaMemoryTypeHost;
   return p ? memory_type(h, p, "phi_i", type) : 0;
 }
+// A caller's device array of n rows: fp32 or fp64 (enum hb_dtype), row stride ld elements
+struct DevRows {
+  const void* p;
+  int dtype;
+  int64_t ld, n;
+};
+// Caller rows of `cols` values, which the kernels access in place: a known dtype, ld >= cols, device memory (status 2)
+int check_rows(hb_handle* h, const DevRows& r, int cols, const char* what) {
+  if (r.dtype != HB_FLOAT32 && r.dtype != HB_FLOAT64) return fail(h, 2, "unknown dtype %d of %s", r.dtype, what);
+  if (r.ld < cols) return fail(h, 2, "row stride of %s (%lld) is smaller than its %d columns", what, (long long)r.ld, cols);
+  return check_device_ptr(h, r.p, what);
+}
+// f(p) with the rows' pointer as `const float*` or `const double*`, by their checked dtype
+template <typename F>
+auto with_rows(const DevRows& r, F&& f) {
+  return r.dtype == HB_FLOAT32 ? f((const float*)r.p) : f((const double*)r.p);
+}
 // `later` waits for the work queued on `earlier` so far (no host synchronisation)
 int stream_after(hb_handle* h, cudaStream_t later, cudaStream_t earlier) {
   if (later == earlier) return 0;
@@ -247,15 +264,18 @@ int stream_after(hb_handle* h, cudaStream_t later, cudaStream_t earlier) {
   CK(e2);
   return 0;
 }
-// Z (n rows of d values, row stride ld elements, fp32 / fp64 device memory) -> Zo in tuple-sorted order, on the
-// library stream after the work queued on `caller`
-int upload_rows_device(hb_handle* h, const void* Z, int dtype, int64_t ld, cudaStream_t caller) {
+// work() on the library stream after the work queued on `caller` so far, and before the work queued there next
+template <typename F>
+int on_caller_stream(hb_handle* h, cudaStream_t caller, F&& work) {
+  TRY(stream_after(h, h->stream, caller));
+  TRY(work());
+  return stream_after(h, caller, h->stream);
+}
+// Z (h->n rows of d values) -> Zo in tuple-sorted order, on the library stream after the work queued on `caller`
+int upload_rows_device(hb_handle* h, const DevRows& Z, cudaStream_t caller) {
   RegionScope rs(h, "upload");
   TRY(stream_after(h, h->stream, caller));
-  if (dtype == HB_FLOAT32)
-    copy_rows((const float*)Z, ld, h->Zo.p, h->DS, h->inv_sort.p, 0, true, h->n, h->d, h->num_sms, h->stream);
-  else
-    copy_rows((const double*)Z, ld, h->Zo.p, h->DS, h->inv_sort.p, 0, true, h->n, h->d, h->num_sms, h->stream);
+  with_rows(Z, [&](auto z) { copy_rows(z, Z.ld, h->Zo.p, h->DS, h->inv_sort.p, 0, true, h->n, h->d, h->num_sms, h->stream); });
   CKL();
   return 0;
 }

@@ -13,6 +13,7 @@ import warnings
 import numpy as np
 
 from . import _lib
+from ._arrays import DTYPE, current_stream, device_rows
 from .utils import is_cuda_tensor
 
 FIELD = {"Z_corr": 0, "Z_orig": 1, "R": 2, "Y": 3, "O": 4, "E": 5, "W": 6, "Pr_b": 7, "theta": 8, "sigma": 9,
@@ -28,9 +29,6 @@ _INT_SCALARS = ("N", "B", "K", "d", "C", "max_iter_kmeans", "N_local", "window_s
 
 def _ptr(a):
     return a.ctypes.data_as(ctypes.c_void_p)
-
-
-_DTYPE = {"float32": 0, "float64": 1}   # enum hb_dtype
 
 
 class HarmonyError(RuntimeError):
@@ -145,7 +143,8 @@ class harmony:
             raise ValueError("number of cells in Z and Phi differ")
         z_args = None
         if dev:
-            Z, z_args = self._device_Z(Z)
+            Z, ptr, dtype, ld = device_rows(self, Z, "Z")
+            z_args = (ptr, dtype, ld, current_stream(Z.device))
         else:
             Z = np.ascontiguousarray(Z, dtype=np.float64)
         phi_ptr = ctypes.c_void_p(phi_i.data_ptr()) if is_cuda_tensor(phi_i) else _ptr(phi_i)
@@ -201,20 +200,6 @@ class harmony:
         in any state of the object and changes none of it, e.g. ``obj.lisi(obj.get_tensor("Z_corr"), batch_codes)``."""
         from .lisi import lisi_on
         return lisi_on(self, X, codes, perplexity, return_neighbors)
-
-    def _device_Z(self, Z):
-        """An [N, d] CUDA tensor -> (the tensor to read, (pointer, dtype, row stride, stream) of hb_setup_device)).
-        Rows with unit column stride are read in place; any other layout is made contiguous on the device first."""
-        import torch
-        if Z.dtype not in (torch.float32, torch.float64):
-            raise TypeError(f"Z must be float32 or float64, not {Z.dtype}")
-        if Z.device.index != self._scalar("device"):
-            raise ValueError(f"Z is on {Z.device}, the harmony object on cuda:{self._scalar('device')}")
-        if Z.shape[0] > 1 and not (Z.stride(1) == 1 and Z.stride(0) >= Z.shape[1]):
-            Z = Z.contiguous()
-        ld = Z.stride(0) if Z.shape[0] > 1 else Z.shape[1]
-        stream = torch.cuda.current_stream(Z.device).cuda_stream
-        return Z, (ctypes.c_void_p(Z.data_ptr()), _DTYPE[str(Z.dtype)[6:]], int(ld), ctypes.c_void_p(stream))
 
     def _device_Phi(self, Phi):
         """An [N] or [N, C] int32 / int64 CUDA tensor -> contiguous [N, C] int32 on the object's device (converted, if
@@ -320,9 +305,8 @@ class harmony:
         cols = self._scalar("K" if name == "R" else "d")
         device = torch.device("cuda", self._scalar("device"))
         out = torch.empty((self._scalar("N_local"), cols), dtype=dtype, device=device)
-        stream = torch.cuda.current_stream(device).cuda_stream
         self._check(self._L.hb_get_field_device(self._h, FIELD[name], ctypes.c_void_p(out.data_ptr()),
-                                                _DTYPE[str(dtype)[6:]], cols, ctypes.c_void_p(stream)))
+                                                DTYPE[str(dtype)[6:]], cols, current_stream(device)))
         return out
 
     # ---- fields of the Rcpp module (harmony.cpp:675-696) ---------------------------------------

@@ -9,7 +9,8 @@ import math
 
 import numpy as np
 
-from .neighbors import MAX_D, _device_rows
+from ._arrays import current_stream, device_rows, factorise, resolve_device, to_device
+from .neighbors import MAX_D
 from .utils import is_cuda_tensor
 
 MAX_K = 128   # the neighbour lists of hb_lisi's search: perplexity < 43 1/3
@@ -70,9 +71,9 @@ def lisi_on(obj, X, codes, perplexity=30, return_neighbors=False):
     import torch
     host = not is_cuda_tensor(X)
     device = torch.device("cuda", obj._scalar("device"))
-    if host:   # uploaded with torch; float64 stays float64 (the library rounds after centring)
-        X = torch.as_tensor(np.ascontiguousarray(X, dtype=np.float64 if X.dtype == np.float64 else np.float32)).to(device)
-    x, x_args = _device_rows(obj, X, "X")
+    if host:
+        X = to_device(obj, X)
+    x, *x_args = device_rows(obj, X, "X")
     if not is_cuda_tensor(codes):
         codes = torch.as_tensor(np.ascontiguousarray(codes, dtype=np.int32)).to(device)
     if codes.device != device:
@@ -86,9 +87,8 @@ def lisi_on(obj, X, codes, perplexity=30, return_neighbors=False):
         idx = torch.empty((N, k), dtype=torch.int32, device=device)
         dist = torch.empty((N, k), dtype=torch.float32, device=device)
     ptr = lambda t: ctypes.c_void_p(None if t is None else t.data_ptr())  # noqa: E731
-    stream = torch.cuda.current_stream(device).cuda_stream
-    obj._check(obj._L.hb_lisi(obj._h, *x_args, int(d), ptr(codes), int(ld), int(codes.shape[0]), float(perplexity),
-                              ptr(out), ptr(idx), ptr(dist), ctypes.c_void_p(stream)))
+    obj._check(obj._L.hb_lisi(obj._h, *x_args, N, int(d), ptr(codes), int(ld), int(codes.shape[0]), float(perplexity),
+                              ptr(out), ptr(idx), ptr(dist), current_stream(device)))
     if host:
         out = out.cpu().numpy()
         if return_neighbors:
@@ -136,23 +136,10 @@ def compute_lisi(X, meta_data, label_colnames, perplexity=30, device=None, retur
         if not is_cuda_tensor(cols[v]) and _missing(cols[v]):
             raise ValueError(f"column {v!r} holds missing labels")
     _label_device(cols, names, X, on_device)
-    if on_device:
-        if device is not None and int(device) != X.device.index:
-            raise ValueError(f"device={device} differs from the device of X ({X.device})")
-        device = X.device.index
+    device = resolve_device(device, X, "X")
     from .harmony import harmony  # needs the CUDA extension; fails loudly when it is missing
     obj = harmony(device=device)
-    codes = []
-    for v in names:
-        if is_cuda_tensor(cols[v]):
-            import torch
-            codes.append(torch.unique(cols[v], return_inverse=True)[1].to(torch.int32))
-        else:
-            c = np.unique(cols[v], return_inverse=True)[1].reshape(-1).astype(np.int32)
-            if on_device:
-                import torch
-                c = torch.as_tensor(c, device=X.device)
-            codes.append(c)
+    codes = [factorise(cols[v], X.device if on_device else None)[1] for v in names]
     if on_device:
         import torch
         codes = torch.stack(codes)

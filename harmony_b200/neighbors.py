@@ -8,11 +8,11 @@ import ctypes
 
 import numpy as np
 
+from ._arrays import current_stream, device_rows, factorise, resolve_device, to_device
 from .utils import is_cuda_tensor
 
 METRIC = {"euclidean": 0, "cosine": 1}   # enum hb_metric
 MAX_K, MAX_D = 64, 128
-_DTYPE = {"float32": 0, "float64": 1}    # enum hb_dtype
 
 
 def _check_args(query, ref, k, metric):
@@ -44,35 +44,21 @@ def _check_args(query, ref, k, metric):
     return query, ref
 
 
-def _device_rows(obj, Z, what):
-    import torch
-    if Z.dtype not in (torch.float32, torch.float64):
-        raise TypeError(f"{what} must be float32 or float64, not {Z.dtype}")
-    if Z.device.index != obj._scalar("device"):
-        raise ValueError(f"{what} is on {Z.device}, the harmony object on cuda:{obj._scalar('device')}")
-    if Z.shape[0] > 1 and not (Z.stride(1) == 1 and Z.stride(0) >= Z.shape[1]):
-        Z = Z.contiguous()
-    ld = Z.stride(0) if Z.shape[0] > 1 else Z.shape[1]
-    return Z, (ctypes.c_void_p(Z.data_ptr()), _DTYPE[str(Z.dtype)[6:]], int(ld), int(Z.shape[0]))
-
-
 def knn_on(obj, query, ref=None, k=15, metric="euclidean"):
     """``knn`` on an existing ``harmony`` object (any state: the search needs no setup and changes none)."""
     query, ref = _check_args(query, ref, k, metric)
     import torch
     host = not is_cuda_tensor(query)
     device = torch.device("cuda", obj._scalar("device"))
-    if host:   # uploaded and downloaded with torch; float64 stays float64 (the library rounds after centring)
-        as_dev = lambda a: torch.as_tensor(  # noqa: E731
-            np.ascontiguousarray(a, dtype=np.float64 if a.dtype == np.float64 else np.float32)).to(device)
-        query, ref = as_dev(query), None if ref is None else as_dev(ref)
-    q, q_args = _device_rows(obj, query, "query")
-    x, x_args = (q, q_args) if ref is None else _device_rows(obj, ref, "ref")
+    if host:   # uploaded and downloaded with torch
+        query, ref = to_device(obj, query), None if ref is None else to_device(obj, ref)
+    q, *q_args = device_rows(obj, query, "query")
+    x, *x_args = (q, *q_args) if ref is None else device_rows(obj, ref, "ref")
     idx = torch.empty((q.shape[0], int(k)), dtype=torch.int32, device=device)
     dist = torch.empty((q.shape[0], int(k)), dtype=torch.float32, device=device)
-    stream = torch.cuda.current_stream(device).cuda_stream
-    obj._check(obj._L.hb_knn(obj._h, *q_args, *x_args, int(q.shape[1]), int(k), METRIC[metric], int(ref is None),
-                             ctypes.c_void_p(idx.data_ptr()), ctypes.c_void_p(dist.data_ptr()), ctypes.c_void_p(stream)))
+    obj._check(obj._L.hb_knn(obj._h, *q_args, q.shape[0], *x_args, x.shape[0], int(q.shape[1]), int(k), METRIC[metric],
+                             int(ref is None), ctypes.c_void_p(idx.data_ptr()), ctypes.c_void_p(dist.data_ptr()),
+                             current_stream(device)))
     if host:
         return idx.cpu().numpy(), dist.cpu().numpy()
     return idx, dist
@@ -89,11 +75,7 @@ def knn(query, ref=None, k=15, metric="euclidean", device=None):
     with fewer than k candidates)."""
     query, ref = _check_args(query, ref, k, metric)
     from .harmony import harmony  # needs the CUDA extension; fails loudly when it is missing
-    if is_cuda_tensor(query):
-        if device is not None and int(device) != query.device.index:
-            raise ValueError(f"device={device} differs from the device of query ({query.device})")
-        device = query.device.index
-    return knn_on(harmony(device=device), query, ref, k, metric)
+    return knn_on(harmony(device=resolve_device(device, query, "query")), query, ref, k, metric)
 
 
 def vote(idx, dist, codes, n_labels):
@@ -163,14 +145,13 @@ def TransferLabels(query, ref, ref_labels, k=5, metric="euclidean", return_prob=
         given = np.asarray(ref_labels)
         if given.ndim != 1:
             raise ValueError("ref_labels must hold one label per row of ref")
-        categories, codes = np.unique(given, return_inverse=True)
+        categories, codes = factorise(given)
         n_given = len(given)
     if n_given != ref.shape[0]:
         raise ValueError(f"ref has {ref.shape[0]} rows, ref_labels {n_given} labels")
     idx, dist = knn(query, ref, k, metric, device)
     if labels_on_device:
-        import torch
-        categories, codes = torch.unique(ref_labels, return_inverse=True)
+        categories, codes = factorise(ref_labels)
     elif is_cuda_tensor(idx):
         import torch
         codes = torch.as_tensor(codes, device=idx.device)

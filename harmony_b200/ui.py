@@ -9,6 +9,7 @@ import sys
 
 import numpy as np
 
+from ._arrays import factorise, resolve_device
 from .harmony_option import HarmonyOptions, check_legacy_args, harmony_options
 from .utils import harmonize, is_cuda_tensor
 
@@ -91,19 +92,11 @@ def _factorise(cols, vars_use, data_mat, on_device):
     offset = 0
     device = _label_device(cols, vars_use, data_mat, on_device)
     for v in vars_use:
-        if device is not None and is_cuda_tensor(cols[v]):
-            # integer / bool labels: torch's sorted unique levels are np.unique's (and as.factor's) for these dtypes
-            import torch
-            levels, codes = torch.unique(cols[v], sorted=True, return_inverse=True)
-            phi_cols.append(codes.to(torch.int32) + offset)
+        # device columns hold integer / bool labels: torch's sorted unique levels are np.unique's (and as.factor's)
+        levels, codes = factorise(cols[v], device)
+        if is_cuda_tensor(levels):
             levels = levels.cpu().numpy()
-        else:
-            levels, codes = np.unique(cols[v], return_inverse=True)
-            codes = codes.reshape(-1).astype(np.int32) + offset
-            if device is not None:
-                import torch
-                codes = torch.from_numpy(codes).to(device)
-            phi_cols.append(codes)
+        phi_cols.append(codes + offset)
         B_vec.append(len(levels))
         level_names.append(levels)
         offset += len(levels)
@@ -195,11 +188,7 @@ def RunHarmony(data_mat, meta_data, vars_use=None, theta=None, sigma=0.1, lambda
     a = prepare_inputs(data_mat, meta_data, vars_use, theta, sigma, lambda_, nclust, early_stop, options, verbose)
     if verbose and a["lambda_"] is None:
         print("Using automatic lambda estimation", file=sys.stderr)
-    if is_cuda_tensor(data_mat):
-        if device is not None and int(device) != data_mat.device.index:
-            raise ValueError(f"device={device} differs from the device of data_mat ({data_mat.device})")
-        device = data_mat.device.index
-    obj = harmony(device=device)
+    obj = harmony(device=resolve_device(device, data_mat, "data_mat"))
     obj.setup(a["Z"], a["phi_i"], a["sigma"], a["theta"], a["lambda_"], a["alpha"], a["max_iter_kmeans"],
               a["epsilon_kmeans"], a["epsilon_harmony"], a["K"], a["block_size"], a["B_vec"],
               a["batch_proportion_cutoff"], verbose)
@@ -244,10 +233,7 @@ def MapQuery(data_mat, meta_data, vars_use, reference, lambda_=1.0, return_objec
         raise ValueError("Provided lambdas must be positive")
     if len(lam) not in (1, len(vars_use)):
         raise ValueError(f"lambda_ must be one value or one per covariate ({len(vars_use)}), not {len(lam)}")
-    if on_device:
-        if device is not None and int(device) != data_mat.device.index:
-            raise ValueError(f"device={device} differs from the device of data_mat ({data_mat.device})")
-        device = data_mat.device.index
+    device = resolve_device(device, data_mat, "data_mat")
     phi_i, B_vec, _, _ = _factorise(cols, vars_use, data_mat, on_device)
     lambda_vec = np.repeat(lam, B_vec) if len(lam) > 1 else np.repeat(lam, sum(B_vec))
     from .harmony import harmony  # needs the CUDA extension; fails loudly when it is missing

@@ -1,5 +1,6 @@
 """Shared helpers for the test-suite (test infrastructure; may use oracle/)."""
 import os
+import socket
 
 import numpy as np
 
@@ -95,3 +96,24 @@ def run_oracle(a, Y0, n_iter, perm_seed=0, double=False, perms=None):
 
 def rel_l2(a, b):
     return float(np.linalg.norm(np.asarray(a) - np.asarray(b)) / max(np.linalg.norm(np.asarray(b)), 1e-300))
+
+
+def num_sms():
+    """The SM count of GPU 0, which the geometry and kernel-path hooks take."""
+    import torch
+    return torch.cuda.get_device_properties(0).multi_processor_count
+
+
+def gpu_harmony():
+    """A fresh harmony object on GPU 0."""
+    from harmony_b200.harmony import harmony
+    return harmony(device=0)
+
+
+def free_port():
+    """A TCP port on 127.0.0.1 that was free a moment ago, for a test's process group."""
+    s = socket.socket()
+    s.bind(("127.0.0.1", 0))
+    p = s.getsockname()[1]
+    s.close()
+    return p

@@ -2,7 +2,6 @@
 broadcast, and that sharding the update order / the diversity statistics reproduces the unsharded
 quantities (the identities the library relies on when it all-reduces O, E and the ridge statistics)."""
 import os
-import socket
 
 import numpy as np
 import pytest
@@ -11,6 +10,7 @@ import torch.distributed as dist
 import torch.multiprocessing as mp
 
 from harmony_b200.dist import broadcast_bytes, make_comm, shard_bounds
+from helpers import free_port
 
 
 def test_shard_bounds():
@@ -20,14 +20,6 @@ def test_shard_bounds():
     assert all(0 <= x - y <= 1 for x, y in zip(np.diff(shard_bounds(1_000_003, 8))[:-1],
                                               np.diff(shard_bounds(1_000_003, 8))[1:]))
     assert shard_bounds(12, 4, rank=2) == (6, 9)
-
-
-def _free_port():
-    s = socket.socket()
-    s.bind(("127.0.0.1", 0))
-    p = s.getsockname()[1]
-    s.close()
-    return p
 
 
 def _worker(rank, world, port, N, K, B, out):
@@ -75,7 +67,7 @@ def _worker(rank, world, port, N, K, B, out):
 def test_two_rank_gloo():
     ctx = mp.get_context("spawn")
     q = ctx.Queue()
-    port = _free_port()
+    port = free_port()
     procs = [ctx.Process(target=_worker, args=(r, 2, port, 4001, 7, 3, q)) for r in range(2)]
     for p in procs:
         p.start()

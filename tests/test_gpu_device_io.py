@@ -6,14 +6,13 @@ The per-cell conversions are exact (fp32 -> fp32, fp32 <-> fp64 widening) or the
 get_tensor returns the bits of getZcorr() / getZorig() / getR()."""
 import ctypes
 import os
-import socket
 import sys
 
 import numpy as np
 import pytest
 
 from harmony_b200 import RunHarmony, prepare_inputs
-from helpers import make_perms, make_Y0, rel_l2, synthetic
+from helpers import free_port, make_perms, make_Y0, rel_l2, synthetic
 
 pytestmark = pytest.mark.gpu
 
@@ -270,14 +269,6 @@ def test_rejected_before_any_launch(small):
     assert g2.kernel_launches == 0
 
 
-def _free_port():
-    s = socket.socket()
-    s.bind(("127.0.0.1", 0))
-    p = s.getsockname()[1]
-    s.close()
-    return p
-
-
 def _shard_run(rank, world, port, q):
     sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
     import torch
@@ -326,7 +317,7 @@ def test_two_gpu_device_shards_match_host_shards():
         pytest.skip("needs 2 GPUs")
     ctx = mp.get_context("spawn")
     q = ctx.Queue()
-    port = _free_port()
+    port = free_port()
     procs = [ctx.Process(target=_shard_run, args=(r, 2, port, q)) for r in range(2)]
     for p in procs:
         p.start()

@@ -6,7 +6,6 @@ sorted by tuple id.  Host labels (hb_setup, and hb_setup_device with a host phi_
 exactly that index."""
 import ctypes
 import os
-import socket
 import sys
 import warnings
 
@@ -14,7 +13,7 @@ import numpy as np
 import pytest
 
 from harmony_b200 import RunHarmony, prepare_inputs
-from helpers import synthetic
+from helpers import free_port, synthetic
 
 pytestmark = pytest.mark.gpu
 
@@ -282,14 +281,6 @@ def test_runharmony_with_device_labels():
     assert float(np.abs(h1 - mixed).max()) <= 2 * noise + 1e-6
 
 
-def _free_port():
-    s = socket.socket()
-    s.bind(("127.0.0.1", 0))
-    p = s.getsockname()[1]
-    s.close()
-    return p
-
-
 def _shard_run(rank, world, port, q):
     sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
     import torch
@@ -348,7 +339,7 @@ def test_two_gpu_device_label_shards_match_host_shards():
         pytest.skip("needs 2 GPUs")
     ctx = mp.get_context("spawn")
     q = ctx.Queue()
-    port = _free_port()
+    port = free_port()
     procs = [ctx.Process(target=_shard_run, args=(r, 2, port, q)) for r in range(2)]
     for p in procs:
         p.start()

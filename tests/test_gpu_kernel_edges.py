@@ -16,7 +16,7 @@ with the device's SM count and counts the launches of the multi-launch ranges.
 import numpy as np
 import pytest
 
-from helpers import rel_l2
+from helpers import num_sms, rel_l2
 from stages import (ALPHA, BLOCK, CUTOFF, NB, PER_STEP, SIGMA, SINGLE_PASS, T, TOL_OBJ, TOL_OE, TOL_R, TOL_R1,  # noqa: F401
                     TOL_Y, TOL_Y_FIXED, TOL_Z, TOL_ZN, TWO_PASS, _grid, _launches, _nested, _obj_err, _one_cov,
                     _set_zcorr, _sizes, _table_err, f32, kernel_paths, level_of_single_cluster, make_Y0, numpy_model,
@@ -147,15 +147,10 @@ def test_planted_ridge_inputs_numpy_matches_oracle(name, fixed_lambda):
 
 
 # ---- GPU tests --------------------------------------------------------------------------------------------------------
-def _num_sms():
-    import torch
-    return torch.cuda.get_device_properties(0).multi_processor_count
-
-
 @pytest.mark.gpu
 @pytest.mark.parametrize("name", list(EDGE_ROWS))
 def test_edge_row_stages(name):
-    sms = _num_sms()
+    sms = num_sms()
     c = build_case(name, sms)
     K, d, N = c["K"], c["d"], c["N"]
     J = len(c["sizes"])
@@ -179,7 +174,7 @@ def test_setup_normalises_rows_at_extreme_scales(kernel_set):
     """Rows whose fp32 sum of squares overflows (|v| ~ 1e20) or underflows (|v| <= 1e-25) are normalised like any
     other row at setup, and the assignment sees them so; a zero row stays zero."""
     from harmony_b200.harmony import harmony
-    c = build_case("k1_tail_K17_d3", _num_sms())
+    c = build_case("k1_tail_K17_d3", num_sms())
     Z = c["Z"].copy()
     rng = np.random.default_rng(2)
     rows = rng.choice(c["N"], 12, replace=False)

@@ -7,27 +7,17 @@ import pytest
 
 import knn_restatement as kr
 from harmony_b200 import MapQuery, RunHarmony, TransferLabels, knn
-from helpers import synthetic
+from helpers import gpu_harmony, num_sms, synthetic
 
 pytestmark = pytest.mark.gpu
 
 EPS32 = 2.0 ** -24
 
 
-def _harmony():
-    from harmony_b200.harmony import harmony
-    return harmony(device=0)
-
-
-def _num_sms():
-    import torch
-    return torch.cuda.get_device_properties(0).multi_processor_count
-
-
 def _geometry(d, k, Nq, Nx):
     from harmony_b200 import _lib
     out = (ctypes.c_int64 * 8)()
-    assert _lib.lib().hb_debug_knn_geometry(d, k, Nq, Nx, _num_sms(), out) == 0
+    assert _lib.lib().hb_debug_knn_geometry(d, k, Nq, Nx, num_sms(), out) == 0
     return list(out)
 
 
@@ -152,7 +142,7 @@ def test_knn_table(row):
     else:
         xt = torch.as_tensor(X, device=dev)
         qt = xt if self_search else torch.as_tensor(Q, device=dev)
-    g = _harmony()
+    g = gpu_harmony()
     idx, dist = g.knn(qt, None if self_search else xt, k=k, metric=metric)
     assert idx.is_cuda and dist.is_cuda
     launches = g.region_time("knn")[1]
@@ -208,7 +198,7 @@ def test_handle_state_untouched():
     state = lambda h: (h.getZcorr(), h.getR(), h.Y)  # noqa: E731
     outs = []
     for with_knn in (False, True):
-        g = _harmony()
+        g = gpu_harmony()
         g.setup(a["Z"], a["phi_i"], a["sigma"], a["theta"], a["lambda_"], a["alpha"], a["max_iter_kmeans"],
                 a["epsilon_kmeans"], a["epsilon_harmony"], 50, a["block_size"], a["B_vec"], a["batch_proportion_cutoff"])
         g.init_cluster_cpp(Y0)
@@ -227,7 +217,7 @@ def test_handle_state_untouched():
         assert rel_l2(u, v) < 1e-4
     maps = []
     for with_knn in (False, True):
-        m = _harmony()
+        m = gpu_harmony()
         m.map_setup(Z[:6000], a["phi_i"][:6000], a["B_vec"], 1.0, ref)
         if with_knn:
             m.knn(probe, k=5, metric="cosine")
@@ -282,7 +272,7 @@ def test_refusals_launch_nothing():
     import torch
     from harmony_b200 import _lib
     L = _lib.lib()
-    g = _harmony()
+    g = gpu_harmony()
     dev = torch.device("cuda", 0)
     X, Q = torch.zeros((100, 8), device=dev), torch.zeros((10, 8), device=dev)
     idx, dist = torch.zeros((10, 5), dtype=torch.int32, device=dev), torch.zeros((10, 5), device=dev)

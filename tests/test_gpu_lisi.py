@@ -8,7 +8,7 @@ import pytest
 import knn_restatement as kr
 import lisi_restatement as lr
 from harmony_b200 import RunHarmony, compute_lisi, knn
-from helpers import load_cell_lines, synthetic
+from helpers import gpu_harmony, load_cell_lines, num_sms, synthetic
 
 pytestmark = pytest.mark.gpu
 
@@ -17,20 +17,10 @@ REL_FP64 = 1e-4     # bar (b): the restatement from scratch, rows with fp64's ne
 SET_DIFF = 0.001    # bar (b): rows whose neighbour set differs from fp64's (DESIGN §9's bar for the sweep)
 
 
-def _harmony():
-    from harmony_b200.harmony import harmony
-    return harmony(device=0)
-
-
-def _num_sms():
-    import torch
-    return torch.cuda.get_device_properties(0).multi_processor_count
-
-
 def _geometry(d, p, N):
     from harmony_b200 import _lib
     out = (ctypes.c_int64 * 8)()
-    assert _lib.lib().hb_debug_lisi_geometry(d, p, N, _num_sms(), out) == 0
+    assert _lib.lib().hb_debug_lisi_geometry(d, p, N, num_sms(), out) == 0
     return list(out)
 
 
@@ -145,7 +135,7 @@ def test_lisi_table(row):
     else:
         xt = torch.as_tensor(X, device=dev)
         ct = torch.as_tensor(codes, device=dev)
-    g = _harmony()
+    g = gpu_harmony()
     out, idx, dist = g.lisi(xt, ct, p, return_neighbors=True)
     assert out.is_cuda and out.dtype == torch.float64 and out.shape == (N, codes.shape[0])
     # column sums, one preparation, the sweep, the merge, k_lisi
@@ -222,7 +212,7 @@ def test_handle_state_untouched():
     probe = torch.as_tensor(Z[:5000], device="cuda:0")
     codes = torch.as_tensor(meta["cov0"][:5000].astype(np.int32), device="cuda:0")
     state = lambda h: (h.getZcorr(), h.getR(), h.Y)  # noqa: E731
-    g = _harmony()
+    g = gpu_harmony()
     g.setup(a["Z"], a["phi_i"], a["sigma"], a["theta"], a["lambda_"], a["alpha"], a["max_iter_kmeans"],
             a["epsilon_kmeans"], a["epsilon_harmony"], 50, a["block_size"], a["B_vec"], a["batch_proportion_cutoff"])
     g.init_cluster_cpp(Y0)
@@ -235,7 +225,7 @@ def test_handle_state_untouched():
             np.testing.assert_array_equal(u, v)
         g.moe_correct_ridge_cpp()
     ref = g.reference()
-    m = _harmony()
+    m = gpu_harmony()
     m.map_setup(Z[:6000], a["phi_i"][:6000], a["B_vec"], 1.0, ref)
     m.lisi(probe, codes, 10)
     m.map()
@@ -249,7 +239,7 @@ def test_refusals_launch_nothing():
     import torch
     from harmony_b200 import _lib
     L = _lib.lib()
-    g = _harmony()
+    g = gpu_harmony()
     dev = torch.device("cuda", 0)
     N, d = 200, 8
     X = torch.zeros((N, d), device=dev)

@@ -7,7 +7,7 @@ import numpy as np
 import pytest
 
 from harmony_b200 import HarmonyReference, MapQuery, RunHarmony, prepare_inputs
-from helpers import make_perms, make_Y0, rel_l2, synthetic
+from helpers import gpu_harmony, make_perms, make_Y0, num_sms, rel_l2, synthetic
 from map_restatement import assign, correct, lambda_levels, map_query, reference_stats, type_offset, weights_folded
 from stages import TOL_OE, TOL_R1, TOL_Y, TOL_Z, f32
 
@@ -16,20 +16,10 @@ pytestmark = pytest.mark.gpu
 KS_FFMA, KS_WIDE = 1, 16
 
 
-def _harmony():
-    from harmony_b200.harmony import harmony
-    return harmony(device=0)
-
-
-def _num_sms():
-    import torch
-    return torch.cuda.get_device_properties(0).multi_processor_count
-
-
 def _wide_paths(K, d, J, n, kernel_set):
     from harmony_b200 import _lib
     out = (ctypes.c_int64 * 4)()
-    _lib.lib().hb_debug_wide_paths(K, d, J, n, 1, _num_sms(), kernel_set, out)
+    _lib.lib().hb_debug_wide_paths(K, d, J, n, 1, num_sms(), kernel_set, out)
     return int(out[0]), int(out[2])
 
 
@@ -40,7 +30,7 @@ def test_reference_compression(d, K, N):
     d = 50 also after a further cluster_cpp, whose Z_corr the library normalises on the first read."""
     Z, meta = synthetic(N, d, [4], n_types=12, seed=d + K)
     a = prepare_inputs(Z, meta, "cov0", nclust=K, early_stop=False)
-    g = _harmony()
+    g = gpu_harmony()
     g.setup(a["Z"], a["phi_i"], a["sigma"], a["theta"], a["lambda_"], a["alpha"], 5, a["epsilon_kmeans"],
             a["epsilon_harmony"], K, a["block_size"], a["B_vec"], a["batch_proportion_cutoff"])
     g.init_cluster_cpp(make_Y0(Z, K, 1))
@@ -124,7 +114,7 @@ def _map_row(K, d, B_vec, kernel_set, Nq, opts, seed):
     sigma = rng.uniform(0.05, 0.2, K) if opts.get("sigma") == "per_cluster" else 0.1
     ref = planted_reference(rng, K, d, M, sigma, opts.get("zero"))
     lam = lambda_levels(opts.get("lam", 1.0), B_vec)
-    g = _harmony()
+    g = gpu_harmony()
     if kernel_set:
         g.kernel_set = kernel_set
     g.map_setup(Z, phi, B_vec, lam, ref)
@@ -190,7 +180,7 @@ def test_map_device_io():
     phis = {"host labels": phi, "device labels": torch.from_numpy(phi).to(dev)}
     for zname, Zt in inputs.items():
         for pname, ph in phis.items():
-            h = _harmony()
+            h = gpu_harmony()
             h.map_setup(Zt, ph, B_vec, lam, ref)
             h.map()
             for dtype in (torch.float32, torch.float64):
@@ -280,39 +270,39 @@ def test_map_refusals():
     lam = np.ones(2)
     # status 2: lambda, sigma, labels outside their levels, K beyond the library's range
     for bad_lam in ([0.0, 1.0], [1.0, -2.0], [np.nan, 1.0], [np.inf, 1.0]):
-        assert _raw_map_setup(_harmony(), Z, phi, [2], bad_lam, ref) == 2
+        assert _raw_map_setup(gpu_harmony(), Z, phi, [2], bad_lam, ref) == 2
     for bad_sigma in (0.0, -0.1, np.inf, np.nan):
         r = HarmonyReference(ref.centroids, ref.Nr, ref.Cref, np.r_[ref.sigma[:-1], bad_sigma])
-        assert _raw_map_setup(_harmony(), Z, phi, [2], lam, r) == 2
-    assert _raw_map_setup(_harmony(), Z, np.where(phi == 1, 2, phi), [2], lam, ref) == 2
-    assert _raw_map_setup(_harmony(), Z, phi, [2], lam, ref, K=0) == 2
+        assert _raw_map_setup(gpu_harmony(), Z, phi, [2], lam, r) == 2
+    assert _raw_map_setup(gpu_harmony(), Z, np.where(phi == 1, 2, phi), [2], lam, ref) == 2
+    assert _raw_map_setup(gpu_harmony(), Z, phi, [2], lam, ref, K=0) == 2
     # status 2 from the setup steps hb_setup shares, through the host and the device entry point: dimensions, K past
     # the library's range, device labels given to the host entry point, and the device entry point's Z checks
     import torch
     Zt = torch.from_numpy(Z).cuda()
     for z_dev in (None, Zt.data_ptr()):
         for bad in (dict(d=0), dict(N=0), dict(C=0), dict(K=0), dict(K=1025)):
-            assert _raw_map_setup(_harmony(), Z, phi, [2], lam, ref, z_dev=z_dev, **bad) == 2, (z_dev, bad)
+            assert _raw_map_setup(gpu_harmony(), Z, phi, [2], lam, ref, z_dev=z_dev, **bad) == 2, (z_dev, bad)
     phi_t = torch.from_numpy(np.ascontiguousarray(phi, dtype=np.int32)).cuda()
-    h = _harmony()
+    h = gpu_harmony()
     assert _raw_map_setup(h, Z, phi, [2], lam, ref, phi_ptr=phi_t.data_ptr()) == 2
     assert "hb_map_setup_device" in h._L.hb_last_error(h._h).decode()
     Zh = np.ascontiguousarray(Z)
     for z_dev, dtype, ld in ((Zt.data_ptr(), 7, None), (Zt.data_ptr(), HB_FLOAT64, 15), (Zh.ctypes.data, HB_FLOAT64, None)):
-        assert _raw_map_setup(_harmony(), Z, phi, [2], lam, ref, z_dev=z_dev, dtype=dtype, ld=ld) == 2, (dtype, ld)
+        assert _raw_map_setup(gpu_harmony(), Z, phi, [2], lam, ref, z_dev=z_dev, dtype=dtype, ld=ld) == 2, (dtype, ld)
     # d or K not matching the reference arrays: the Python layer refuses before the library
     with pytest.raises(ValueError):
-        _harmony().map_setup(Z[:, :15], phi, [2], lam, ref)
+        gpu_harmony().map_setup(Z[:, :15], phi, [2], lam, ref)
     with pytest.raises(ValueError):
         HarmonyReference(ref.centroids, ref.Nr[:-1], ref.Cref, ref.sigma)
     # status 3: a second setup, a sharded handle
-    g = _harmony()
+    g = gpu_harmony()
     assert _raw_map_setup(g, Z, phi, [2], lam, ref) == 0
     assert _raw_map_setup(g, Z, phi, [2], lam, ref) == 3
     assert _raw_map_setup(g, Z, phi, [2], lam, ref, z_dev=Zt.data_ptr()) == 3
     with pytest.raises(HarmonyError):
         g.setup(Z, phi, 0.1, np.full(2, 2.0), None, 0.2, 5, 1e-5, 1e-4, 10, 0.05, [2], 1e-5)
-    s = _harmony()
+    s = gpu_harmony()
     assert s._L.hb_set_shard(s._h, 400, 0) == 0
     assert _raw_map_setup(s, Z, phi, [2], lam, ref) == 3
     # status 3: the Harmony steps on a mapping handle, hb_map on an ordinary one, hb_reference before init
@@ -327,13 +317,13 @@ def test_map_refusals():
     out = np.empty(64)
     assert L.hb_get_field(g._h, 6, _ptr(out)) == 3            # HB_W
     assert L.hb_set_field(g._h, 9, _ptr(np.full(10, 0.1))) == 3  # HB_SIGMA
-    h = _harmony()
+    h = gpu_harmony()
     assert L.hb_reference(h._h, None, None, None, None) == 3   # before setup
     h.setup(Z, phi, 0.1, np.full(2, 2.0), None, 0.2, 5, 1e-5, 1e-4, 10, 0.05, [2], 1e-5)
     assert L.hb_reference(h._h, None, None, None, None) == 3   # before init_cluster_cpp
     assert L.hb_map(h._h) == 3
     # a query of one cell maps (no "fewer than 6 cells" refusal)
-    one = _harmony()
+    one = gpu_harmony()
     one.map_setup(Z[:1], phi[:1], [2], lam, ref)
     one.map()
     assert np.isfinite(one.getZcorr()).all()

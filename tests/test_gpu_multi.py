@@ -1,20 +1,13 @@
 """2-GPU equivalence (gpu-marked; skipped with < 2 devices): the cell-sharded run with NCCL
 all-reduces equals the single-GPU run on the same inputs up to fp32 reassociation."""
 import os
-import socket
 
 import numpy as np
 import pytest
 
+from helpers import free_port
+
 pytestmark = pytest.mark.gpu
-
-
-def _free_port():
-    s = socket.socket()
-    s.bind(("127.0.0.1", 0))
-    p = s.getsockname()[1]
-    s.close()
-    return p
 
 
 def _run(rank, world, port, case, q):
@@ -80,7 +73,7 @@ def test_two_gpu_equals_one_gpu(case):
         pytest.skip("needs 2 GPUs")
     ctx = mp.get_context("spawn")
     q = ctx.Queue()
-    port = _free_port()
+    port = free_port()
     procs = [ctx.Process(target=_run, args=(r, 2, port, case, q)) for r in range(2)]
     for p in procs:
         p.start()

@@ -25,7 +25,7 @@ oracle's error on the same inputs, computed in the test and printed.  The wide r
 import numpy as np
 import pytest
 
-from helpers import make_perms
+from helpers import make_perms, num_sms
 from numpy_restatement import my_ceil
 from stages import (ALPHA, CUTOFF, PER_STEP, SINGLE_PASS, TOL_OBJ, TOL_OE, TOL_R, TOL_R1, TWO_PASS, RunParams,
                     _nested, _obj_err, _one_cov, _sizes, build_case, cluster_and_compare, f32, kernel_paths, make_Y0,
@@ -205,11 +205,6 @@ def test_numpy_matches_oracle_on_run_parameters(what):
 
 
 # ---- GPU tests --------------------------------------------------------------------------------------------------------
-def _num_sms():
-    import torch
-    return torch.cuda.get_device_properties(0).multi_processor_count
-
-
 def _fp32_r_errors(c, p, Y0, R2, perms2, Zp, Yp, perms3, tables=False):
     """max |R32 - R64| of the fp32 and fp64 oracles after S1, S2 and S3 on the stages' inputs (the wide file's rule);
     tables: also the O and E errors (as _table_err measures them) after S2 and S3."""
@@ -244,7 +239,7 @@ def _fp32_r_errors(c, p, Y0, R2, perms2, Zp, Yp, perms3, tables=False):
 
 
 def _run_stages(name, c, p, stages, kernel_set=0, r_bars=None, objective=False, oe_bars=None):
-    sms = _num_sms()
+    sms = num_sms()
     rng = np.random.default_rng(11)
     Y0 = f32(make_Y0(c["Z"], c["K"], rng))
     g = setup_gpu(c, p, kernel_set)
@@ -274,7 +269,7 @@ def _run_stages(name, c, p, stages, kernel_set=0, r_bars=None, objective=False, 
 @pytest.mark.gpu
 @pytest.mark.parametrize("row", list(SIGMA_ROWS))
 def test_sigma_per_cluster(row):
-    c = case_of(row, _num_sms())
+    c = case_of(row, num_sms())
     p = RunParams(sigma=sigma_vec(c["K"]))
     r_bars = None
     if row in WIDE_ROWS:
@@ -294,7 +289,7 @@ def test_sigma_per_cluster(row):
 @pytest.mark.gpu
 @pytest.mark.parametrize("row", list(THETA_ROWS))
 def test_theta_per_level(row):
-    c = case_of(row, _num_sms())
+    c = case_of(row, num_sms())
     _run_stages(f"theta {row}", c, RunParams(theta=theta_levels(sum(c["B_vec"]))), ("S1", "S2", "S3"))
 
 
@@ -302,7 +297,7 @@ def test_theta_per_level(row):
 @pytest.mark.parametrize("name", list(BLOCK_ROWS))
 def test_block_counts(name):
     row, cov, nb = BLOCK_ROWS[name]
-    sms = _num_sms()
+    sms = num_sms()
     c = case_of(row, sms, cov)
     p = RunParams(block_size=block_for(nb))
     if sms == 132:
@@ -330,7 +325,7 @@ def test_block_counts(name):
 def test_call_length(row, T):
     """S2 (warm, from written R) and S3 (cold) with T rounds.  T = 0: the warm call changes nothing; the cold call leaves
     the natural-order assignment's R, O, E and the normalised Z_corr."""
-    c = case_of(row, _num_sms())
+    c = case_of(row, num_sms())
     p = RunParams(T=T)
     if T == 0:
         rng = np.random.default_rng(11)
@@ -362,7 +357,7 @@ def test_call_length(row, T):
 def test_early_stop(row, T):
     """epsilon_kmeans = +inf: both calls stop after 5 rounds, like numpy; the second (cold) call starts from the state
     the first one left when it stopped."""
-    c = case_of(row, _num_sms())
+    c = case_of(row, num_sms())
     _, _, n2, n3 = _run_stages(f"early {row} T={T}", c, RunParams(T=T, epsilon_kmeans=np.inf), ("S2", "S3"))
     assert n2 == n3 == 5
 
@@ -374,7 +369,7 @@ def test_native_orders_after_early_stop(path, kernel_set):
     """Three 8-round calls with native update orders that each stop after 5 rounds: call i runs the native rounds
     5 i .. 5 i + 4 of the seed on every update path (the reference draws one shuffle per executed update_R)."""
     SEED = 20261016
-    c = case_of("k1_K33_d63", _num_sms())
+    c = case_of("k1_K33_d63", num_sms())
     p = RunParams(T=8, epsilon_kmeans=np.inf)
     rng = np.random.default_rng(11)
     Y0 = f32(make_Y0(c["Z"], c["K"], rng))
@@ -403,7 +398,7 @@ def test_written_sigma(row):
     """setup with scalar sigma, init_cluster_cpp(Y0), sigma written per cluster, then a warm cluster_cpp and a
     standalone compute_objective; then a uniform sigma written, compute_objective and a (cold) cluster_cpp.  The
     library must divide the distances of the last assignment by the sigma written since, as the reference does."""
-    c = case_of(row, _num_sms())
+    c = case_of(row, num_sms())
     K = c["K"]
     p = RunParams()
     rng = np.random.default_rng(11)
@@ -439,7 +434,7 @@ def test_written_sigma(row):
 @pytest.mark.gpu
 def test_sigma_written_before_init():
     """A sigma written between setup and init_cluster_cpp is the sigma of the first assignment."""
-    c = case_of("k1_K33_d63", _num_sms())
+    c = case_of("k1_K33_d63", num_sms())
     s = sigma_vec(c["K"])
     rng = np.random.default_rng(11)
     Y0 = f32(make_Y0(c["Z"], c["K"], rng))
@@ -455,7 +450,7 @@ def test_vector_setters_check_lengths():
     """sigma takes K values or one (broadcast, as in setup), theta B and lambda_ B + 1; any other length raises
     ValueError before the library reads the buffer.  A sigma that is not finite and positive is rejected."""
     from harmony_b200.harmony import HarmonyError
-    c = case_of("k1_tail_K17_d3", _num_sms())
+    c = case_of("k1_tail_K17_d3", num_sms())
     K, B = c["K"], sum(c["B_vec"])
     g = setup_gpu(c, RunParams())
     g.sigma = 0.2

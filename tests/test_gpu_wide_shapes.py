@@ -12,7 +12,7 @@ import numpy as np
 import pytest
 
 from harmony_b200 import _lib
-from helpers import make_perms, rel_l2
+from helpers import free_port, make_perms, num_sms, rel_l2
 from stages import (ALPHA, BLOCK, CUTOFF, NB, SIGMA, T, TOL_OBJ, TOL_OE, TOL_R, TOL_R1, TOL_Y, TOL_Y_FIXED, TOL_Z,
                     TOL_ZN, _launches, _mix64, _nested, _obj_err, _one_cov, _set_zcorr, _sizes, _table_err, f32,
                     kernel_paths, make_Y0, native_order, numpy_model, planted_R, tables_of)
@@ -172,11 +172,6 @@ def test_wide_rows_reach_their_kernels(name):
 
 
 # ---- GPU ----------------------------------------------------------------------------------------------------------------
-def _num_sms():
-    import torch
-    return torch.cuda.get_device_properties(0).multi_processor_count
-
-
 def _prenormalised(Z):
     """Z with the rows whose fp32 sum of squares under- or overflows (|v| ~ 1e-25 or 1e20) divided by their norm in fp64:
     the reference's fp32 arithmetic does not rescale such rows, so the fp32 oracle would measure that, not the stage."""
@@ -235,7 +230,7 @@ def _assign_launches(K, wide_logits, plan, normalise):
 @pytest.mark.parametrize("name", list(ROWS))
 def test_wide_row_stages(name):
     from harmony_b200.harmony import harmony
-    sms = _num_sms()
+    sms = num_sms()
     c = build_case(name, sms)
     K, d, _, want, update, ks = ROWS[name]
     N, B, J = c["N"], sum(c["B_vec"]), len(c["sizes"])
@@ -338,7 +333,7 @@ def test_native_kmeans_wide_follows_the_reference_rule(K, d, N):
     centers = rng.standard_normal((40, d)) * 2.0
     Z = centers[rng.integers(0, 40, N)] + 0.7 * rng.standard_normal((N, d))
     phi = rng.integers(0, 3, (N, 1))
-    assert wide_paths(K, d, 3, N, _num_sms())[3] in (M_LOGITS, M_WIDE)
+    assert wide_paths(K, d, 3, N, num_sms())[3] in (M_LOGITS, M_WIDE)
     g = harmony()
     g.setup(Z, phi, SIGMA, np.full(3, 2.0), None, ALPHA, T, -np.inf, -np.inf, K, BLOCK, [3], CUTOFF)
     g.set_seed(77)
@@ -482,14 +477,13 @@ def test_two_gpu_wide_row_equals_one_gpu():
     start's removal-sum all-reduce, the column-range apply) give the single-GPU result up to fp32 reassociation."""
     import torch
     import torch.multiprocessing as mp
-    from test_gpu_multi import _free_port
     if torch.cuda.device_count() < 2:
         pytest.skip("needs 2 GPUs")
     assert wide_paths(100, 300, 8, 15006, torch.cuda.get_device_properties(0).multi_processor_count)[:3] == \
         (A_WIDE, C_WIDE, P_COLS)
     ctx = mp.get_context("spawn")
     q = ctx.Queue()
-    port = _free_port()
+    port = free_port()
     procs = [ctx.Process(target=_run_sharded, args=(r, 2, port, q)) for r in range(2)]
     for p in procs:
         p.start()
