@@ -111,6 +111,9 @@ def lib():
     L.hb_debug_kmeans_uniform.restype = D
     L.hb_debug_kmeans_uniform.argtypes = [P, ctypes.c_uint64, ctypes.c_uint64]
     L.hb_debug_kmeans_cells.argtypes = [P, P]
+    L.hb_debug_kmeans_keep_means.argtypes = [P, I]
+    L.hb_debug_kmeans_means.restype = I64
+    L.hb_debug_kmeans_means.argtypes = [P, P]
     L.hb_debug_tuple_index.argtypes = [P, P, P, P]
     L.hb_debug_widen.argtypes = [P, P, I64, I]
     _LIB = L

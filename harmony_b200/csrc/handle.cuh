@@ -109,6 +109,8 @@ struct hb_handle {
   std::vector<int> tuple_levels_h;     // [J][C]
   std::vector<int64_t> tuple_start_h;  // [J + 1] first sorted position of each tuple
   std::vector<int64_t> kmeans_cells;   // global cells chosen by the native initialize_centroids (test hook)
+  bool kmeans_keep_means = false;      // record Y after the race's gather and after every Lloyd step (test hook)
+  std::vector<float> kmeans_means;     // [steps][K][d] recorded while kmeans_keep_means is on
 
   // kernels
   KernelPaths paths;             // kernels picked by hb_setup (select_kernels)

@@ -1007,6 +1007,18 @@ int hb_debug_kmeans_cells(const hb_handle* h, int64_t* out) {
   for (size_t i = 0; i < h->kmeans_cells.size(); ++i) out[i] = h->kmeans_cells[i];
   return (int)h->kmeans_cells.size();
 }
+// ... and the means of every step of the native initialisations that run while `on` is set (off by default: the
+// record costs a copy and a synchronisation per step).
+int hb_debug_kmeans_keep_means(hb_handle* h, int on) {
+  if (!h) return 1;
+  h->kmeans_keep_means = on != 0;
+  return 0;
+}
+int64_t hb_debug_kmeans_means(const hb_handle* h, float* out) {
+  if (!h || h->kmeans_means.empty()) return 0;
+  std::copy(h->kmeans_means.begin(), h->kmeans_means.end(), out);
+  return (int64_t)h->kmeans_means.size();
+}
 
 int hb_enable_timing(hb_handle* h, int on) {
   if (!h) return 1;

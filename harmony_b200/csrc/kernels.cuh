@@ -86,10 +86,12 @@ __global__ void k_normalise_rows(const float* __restrict__ src, float* __restric
 // for every centroid i in turn, replaces it by the cell j that minimises -log(u_ij) / |2 (1 - y_i . x_j)| (a race of
 // exponentials: cell j wins with probability proportional to its distance from the START cell i), skipping cells
 // that were already taken.  R's random stream cannot be replayed; here u is a keyed hash of (seed, i, global cell),
-// so the rule itself is the reference's and tests replay it exactly (tests/numpy_restatement.py).
+// so the rule itself is the reference's and tests replay it exactly (tests/kmeans_restatement.py).
 __host__ __device__ __forceinline__ float kmeans_uniform(uint64_t seed, uint64_t i, uint64_t g) {
   const uint64_t h = hb_mix64(seed ^ hb_mix64((i << 40) ^ g ^ 0x6b6d2b2b00000000ull));
-  return ((float)(h >> 40) + 0.5f) * (1.0f / 16777216.0f);  // 24 random bits, strictly inside (0, 1)
+  // 24 random bits, strictly inside (0, 1): the top value's + 0.5f rounds to 2^24, so it is held at 1 - 2^-24 (a draw
+  // of 1 would give the key -0.0f, which the packed race keys order after every positive key, not before)
+  return fminf(((float)(h >> 40) + 0.5f) * (1.0f / 16777216.0f), 0x1.fffffep-1f);
 }
 // Y[k] <- the (cosine-normalised) cell with GLOBAL index cells[k]; each rank writes the rows it owns, the rest
 // stay 0 (the caller zeroes Y and all-reduces it).  only >= 0: just that centroid.

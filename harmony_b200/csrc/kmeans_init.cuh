@@ -19,6 +19,15 @@ int kmeans_centers(hb_handle* h) {
   CK(cells_d.alloc(K));
   CK(best_d.alloc(K));
   std::vector<int64_t> cells(K);
+  h->kmeans_means.clear();
+  auto keep_means = [&]() -> int {  // test hook: Y after the race's gather (step 0) and after each Lloyd step
+    if (!h->kmeans_keep_means) return 0;
+    const size_t at = h->kmeans_means.size();
+    h->kmeans_means.resize(at + Kd);
+    CK(cudaMemcpyAsync(h->kmeans_means.data() + at, h->Y.p, sizeof(float) * Kd, cudaMemcpyDeviceToHost, h->stream));
+    CK(cudaStreamSynchronize(h->stream));
+    return 0;
+  };
   auto gather = [&](int only) -> int {  // Y rows <- cells (all, or one centroid), summed over the ranks that own them
     CK(cudaMemcpyAsync(cells_d.p, cells.data(), sizeof(int64_t) * K, cudaMemcpyHostToDevice, h->stream));
     float* dst = (only >= 0) ? h->Y.p + (size_t)only * d : h->Y.p;
@@ -92,6 +101,7 @@ int kmeans_centers(hb_handle* h) {
   }
   h->kmeans_cells = cells;
   TRY(gather(-1));
+  TRY(keep_means());
   for (int iter = 0; iter < 10; ++iter) {
     switch (km) {
       case KmeansInit::Ffma:
@@ -120,6 +130,7 @@ int kmeans_centers(hb_handle* h) {
         break;
       }
     }
+    TRY(keep_means());
   }
   CK(cudaStreamSynchronize(h->stream));
   return 0;

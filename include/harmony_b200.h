@@ -275,6 +275,12 @@ int hb_debug_widen(double* out, const float* in, int64_t n, int threads);
  * cells initialize_centroids chose (returns their number, 0 if the native initialisation has not run). */
 double hb_debug_kmeans_uniform(const hb_handle* h, uint64_t i, uint64_t g);
 int hb_debug_kmeans_cells(const hb_handle* h, int64_t* out);
+/* Test hook: with on != 0, the native initialisations that follow record Y (K x d row-major floats) after the race's
+ * gather (step 0) and after each of the 10 Lloyd steps (steps 1..10); each native initialisation clears the record
+ * first, hb_init_cluster with Y0 records nothing.  hb_debug_kmeans_means copies the record (11 K d floats) and
+ * returns its length, 0 if there is none.  Off by default. */
+int hb_debug_kmeans_keep_means(hb_handle* h, int on);
+int64_t hb_debug_kmeans_means(const hb_handle* h, float* out);
 /* Test hook: the covariate-tuple index hb_setup built.  Returns J (the number of tuples; -1 before setup) and writes
  * the non-null outputs: sort_perm (N_local values: the caller's cell at each tuple-sorted position), tuple_levels
  * (J x C global levels, tuples in ascending mixed-radix order with covariate 0 most significant) and tuple_start

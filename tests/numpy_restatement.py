@@ -153,38 +153,3 @@ class NumpyHarmony:
         self.Z_corr = Zc
         self.Y = self._l2(Ynew)
 
-
-def kmeans_centers(X, K, uniform):
-    """kmeans_centers of the reference (src/utils.cpp:10-64) in float64, with the uniforms injected:
-    ``uniform(i, j)`` stands in for arma::randu at (centroid i, cell j); i = K addresses the K start-cell draws.
-
-    initialize_centroids (:10-49): K start cells floor(u (N - 1)); then centroid i becomes the cell that minimises
-    -log(u_ij) / |2 (1 - y_i . x_j)| with y_i its START cell, cells taken earlier skipped.  Then 10 x
-    arma::kmeans(Y, X, K, keep_existing, 1): one Lloyd iteration each — nearest mean in Euclidean distance, mean of
-    the members; a mean without members is left where it is (Armadillo's own dead-mean heuristic is not restated:
-    Armadillo is not vendored in the reference; documented deviation).  X: [N, d] rows = cosine-normalised cells.
-    Returns (Y [K, d] un-normalised means, chosen cells [K])."""
-    X = np.asarray(X, dtype=np.float64)
-    N = X.shape[0]
-    start = np.array([int(np.floor(uniform(K, k) * (N - 1))) for k in range(K)])
-    Y = X[start].copy()
-    taken = []
-    cells = np.empty(K, dtype=np.int64)
-    U = np.array([[uniform(i, j) for j in range(N)] for i in range(K)])
-    for i in range(K):
-        dist = np.abs(2.0 * (1.0 - X @ Y[i]))
-        with np.errstate(divide="ignore"):
-            prob = -np.log(U[i]) / dist
-        if taken:
-            prob[np.array(taken)] = np.inf
-        cells[i] = int(np.argmin(prob))
-        taken.append(int(cells[i]))
-    Y = X[cells].copy()
-    for _ in range(10):
-        d2 = (X * X).sum(1)[:, None] - 2.0 * X @ Y.T + (Y * Y).sum(1)[None, :]
-        a = np.argmin(d2, axis=1)
-        for k in range(K):
-            m = a == k
-            if m.any():
-                Y[k] = X[m].mean(axis=0)
-    return Y, cells

@@ -190,39 +190,6 @@ def test_library_reproduces_the_vignette_tables_after_cluster_cpp(seed):
     assert np.abs(err - g["error_rate_clustered"]).max() < 2e-3
 
 
-def test_native_kmeans_centers_follows_the_reference_rule():
-    """init_cluster_cpp() without injected centroids = kmeans_centers of the reference (src/utils.cpp:10-64):
-    start cells, the exponential race per centroid with already-taken cells skipped, 10 Lloyd iterations.  The
-    uniforms are a keyed hash of (seed, centroid, cell) exposed by the library, so the numpy restatement replays the
-    very same draws: the chosen cells must be identical (up to float32 near-ties of the race) and the centroids agree."""
-    import ctypes
-    from harmony_b200 import prepare_inputs
-    from harmony_b200.harmony import harmony
-    from harmony_b200 import _lib
-    from numpy_restatement import kmeans_centers
-    Z, meta = synthetic(3000, 12, [3], n_types=6, seed=31)
-    a = prepare_inputs(Z, meta, "cov0", nclust=12, early_stop=False)
-    g = harmony(device=0)
-    g.setup(a["Z"], a["phi_i"], a["sigma"], a["theta"], a["lambda_"], a["alpha"], a["max_iter_kmeans"],
-            a["epsilon_kmeans"], a["epsilon_harmony"], a["K"], a["block_size"], a["B_vec"], a["batch_proportion_cutoff"])
-    g.set_seed(77)
-    g.init_cluster_cpp()
-    L = _lib.lib()
-    K, N = a["K"], Z.shape[0]
-    cells = (ctypes.c_int64 * K)()
-    assert L.hb_debug_kmeans_cells(g._h, cells) == K
-    cells = np.array(list(cells))
-    assert len(set(cells.tolist())) == K                      # utils.cpp:38-45: no cell is taken twice
-    uni = lambda i, j: L.hb_debug_kmeans_uniform(g._h, i, j)
-    X = np.asarray(Z, dtype=np.float32).astype(np.float64)
-    X = X / np.linalg.norm(X, axis=1, keepdims=True)
-    Yn, cells_n = kmeans_centers(X, K, uni)
-    assert (cells == cells_n).mean() >= 0.9, (cells, cells_n)  # a float32 near-tie may pick the runner-up
-    if np.array_equal(cells, cells_n):
-        Yn = Yn / np.linalg.norm(Yn, axis=1, keepdims=True)
-        np.testing.assert_allclose(g.Y.T, Yn, atol=2e-3)       # Lloyd in fp32 with atomics vs fp64: boundary cells may flip
-
-
 def test_abort_callback_stops_cluster_cpp():
     """hb_set_abort_callback = Progress::check_abort (harmony.cpp:233): cluster_cpp returns -1 once the callback
     says so, harmonize() reports "terminated by user" like R/utils.R:27-29, and the object stays usable."""
