@@ -35,7 +35,8 @@ __global__ void k_centroids_from_stats(const float* __restrict__ S, float* __res
   __syncthreads();
   float ss = 0.f;
   for (int c = 0; c < d; ++c) ss += ysum[c] * ysum[c];  // every thread: d is small
-  float nrm = sqrtf(ss);
+  // a cluster of tiny mass (|sum| below ~1e-19) keeps a unit centroid: its norm is measured again after rescaling
+  float nrm = norm_sq_ok(ss) ? sqrtf(ss) : norm_rescaled(d, [&](int c) { return ysum[c]; });
   if (nrm == 0.f) nrm = 1.f;
   for (int c = threadIdx.x; c < d; c += blockDim.x) Y[(size_t)k * d + c] = ysum[c] / nrm;
 }

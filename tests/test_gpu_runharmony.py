@@ -159,13 +159,16 @@ def test_library_reproduces_the_tables_printed_by_the_reference_vignette():
     assert np.abs(np.round(R @ ct) - g["celltype_init"]).max() <= 1
 
 
-@pytest.mark.xfail(strict=False, reason="legacy centroid step (HB_LEGACY_CENTROID_STEP) written without a GPU, first run pending")
-@pytest.mark.parametrize("seed", [0, 1])
-def test_library_reproduces_the_vignette_tables_after_cluster_cpp(seed):
+# update orders 0-3 under the default kernels (fused wgmma at this shape; ids "0" .. "3"), the FFMA contractions
+# (HB_KS_FFMA_CONTRACTIONS = 1) and the wide kernels (HB_KS_WIDE = 16)
+@pytest.mark.parametrize("seed,kernel_set", [pytest.param(s, ks, id=str(s) if ks == 0 else f"{s}-ks{ks}")
+                                             for ks in (0, 1, 16) for s in (0, 1, 2, 3)])
+def test_library_reproduces_the_vignette_tables_after_cluster_cpp(seed, kernel_set):
     """The tables the reference's vignette prints after `max_iter_kmeans <- 10; cluster_cpp()`
     (doc/detailedWalkthrough.html:733-786) through the C ABI, with the centroid step of harmony.cpp:235-238
     switched on as in the package version that rendered them: 25 integers, exactly, for any update order, after
-    exactly 5 rounds (see tests/test_oracle.py for the same check on the restatements)."""
+    exactly 5 rounds (see tests/test_oracle.py for the same check on the restatements), whichever kernel the step's
+    assignment runs on."""
     import os
     from harmony_b200 import prepare_inputs
     from harmony_b200.harmony import harmony
@@ -174,6 +177,7 @@ def test_library_reproduces_the_vignette_tables_after_cluster_cpp(seed):
     Z, meta = load_cell_lines(small=False)
     a = prepare_inputs(Z, meta, "dataset", nclust=5, theta=1.0)
     h = harmony(device=0)
+    h.kernel_set = kernel_set
     h.setup(a["Z"], a["phi_i"], a["sigma"], a["theta"], a["lambda_"], a["alpha"], 10,
             a["epsilon_kmeans"], a["epsilon_harmony"], a["K"], a["block_size"], a["B_vec"],
             a["batch_proportion_cutoff"], False)
