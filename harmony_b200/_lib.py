@@ -15,7 +15,8 @@ SOURCES = [os.path.join(_HERE, "csrc", f) for f in ("harmony_b200.cu", "kernels.
                                                      "update_two_pass.cuh", "update_single_pass.cuh", "plan.cuh", "tuples.cuh", "umma.cuh", "assign_tc3.cuh", "logits_tc.cuh", "logits_wide.cuh", "stats_tc3.cuh",
                                                      "apply_tc3.cuh", "select.cuh", "handle.cuh", "comm.cuh", "trace.cuh", "transfer.cuh",
                                                      "update_host.cuh", "correct_host.cuh", "assign_host.cuh", "kmeans_init.cuh",
-                                                     "map_host.cuh", "knn.cuh", "knn_host.cuh", "lisi.cuh", "lisi_host.cuh")]
+                                                     "map_host.cuh", "knn.cuh", "knn_host.cuh", "lisi.cuh", "lisi_host.cuh",
+                                                     "silhouette.cuh", "silhouette_host.cuh")]
 HEADER = os.path.join(ROOT, "include", "harmony_b200.h")
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17", "-shared",
               "-Xcompiler", "-fPIC"]
@@ -81,6 +82,8 @@ def lib():
     L.hb_debug_knn_geometry.argtypes = [I, I, I64, I64, I, ctypes.POINTER(I64)]
     L.hb_lisi.argtypes = [P, P, I, I64, I64, I, P, I64, I, D, P, P, P, P]
     L.hb_debug_lisi_geometry.argtypes = [I, D, I64, I, ctypes.POINTER(I64)]
+    L.hb_silhouette.argtypes = [P, P, I, I64, I64, I, P, I, P, I, P, P]
+    L.hb_debug_silhouette_geometry.argtypes = [I, I64, I, ctypes.POINTER(I64)]
     L.hb_init_cluster.argtypes = [P, P]
     L.hb_cluster.argtypes = [P, P]
     L.hb_moe_correct_ridge.argtypes = [P]

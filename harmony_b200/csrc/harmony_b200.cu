@@ -39,6 +39,7 @@
 #include "stats_tc3.cuh"
 #include "knn.cuh"
 #include "lisi.cuh"
+#include "silhouette.cuh"
 
 #include "select.cuh"
 #include "handle.cuh"
@@ -239,20 +240,10 @@ int setup_scalars(hb_handle* h, int d, int64_t N, const int32_t* B_vec, int C, c
 int setup_tuples(hb_handle* h, const CellInput& in, TupleIndex& ti) {
   const int C = h->C;
   const int64_t N = h->n;
-  const std::vector<int>& B_vec = h->B_vec;
-  std::vector<uint64_t> radix(C);
-  uint64_t key_space = 1;
-  {
-    long double prod = 1;
-    for (int c = 0; c < C; ++c) prod *= (long double)B_vec[c];
-    if (prod > 9e18L) return fail(h, 2, "covariate level product overflows 64 bits");
-    for (int c = C - 1; c >= 0; --c) {
-      radix[c] = key_space;
-      key_space *= (uint64_t)B_vec[c];
-    }
-  }
-  std::vector<int> base(C, 0);
-  for (int c = 1; c < C; ++c) base[c] = base[c - 1] + B_vec[c - 1];
+  TupleKeys keys;
+  TRY(tuple_keys(h, h->B_vec, keys));
+  const std::vector<int>& base = keys.base;
+  const std::vector<uint64_t>& radix = keys.radix;
   {
     RegionScope rs(h, "tuple_index");
     DevBuf<int> phi_up;  // host labels: one upload, then the same kernels
@@ -264,7 +255,7 @@ int setup_tuples(hb_handle* h, const CellInput& in, TupleIndex& ti) {
       CK(cudaMemcpyAsync(phi_up.p, in.phi, sizeof(int) * (size_t)N * C, cudaMemcpyDefault, h->stream));
       phi_d = phi_up.p;
     }
-    TRY(build_tuple_index(h, phi_d, N, base, radix, key_space, ti));
+    TRY(build_tuple_index(h, phi_d, N, keys, true, h->sort_perm, h->inv_sort, ti));
   }
   const int J = (int)ti.uniq.size();
   h->J = J;
@@ -372,6 +363,7 @@ int harmony_step(hb_handle* h, const char* what, bool needs_init = true) {
 #include "map_host.cuh"
 #include "knn_host.cuh"
 #include "lisi_host.cuh"
+#include "silhouette_host.cuh"
 
 // =================================================================================================
 extern "C" {
@@ -552,6 +544,12 @@ int hb_lisi(hb_handle* h, const void* X, int x_dtype, int64_t x_ld, int64_t N, i
   if (!h) return 1;
   return run_lisi(h, DevRows{X, x_dtype, x_ld, N}, d, labels, labels_ld, n_sets, perplexity, lisi, idx, dist,
                   (cudaStream_t)stream);
+}
+
+int hb_silhouette(hb_handle* h, const void* X, int x_dtype, int64_t x_ld, int64_t N, int d, const int32_t* labels,
+                  int n_labels, const int32_t* groups, int n_groups, double* s, void* stream) {
+  if (!h) return 1;
+  return run_silhouette(h, DevRows{X, x_dtype, x_ld, N}, d, labels, n_labels, groups, n_groups, s, (cudaStream_t)stream);
 }
 
 int hb_init_cluster(hb_handle* h, const double* Y0) {
@@ -981,6 +979,15 @@ int hb_debug_lisi_geometry(int d, double perplexity, int64_t N, int num_sms, int
   int k = 0;
   if (lisi_check_shape(nullptr, d, perplexity, N, &k) != 0 || num_sms < 1) return 2;
   knn_geometry_record(d, k, N, N, num_sms, out);
+  return 0;
+}
+
+// The launch geometry of hb_silhouette's sweep (test hook, host only): out = {rows per query tile, reference rows per
+// tile, operand stages, shared-memory bytes, padded row length, threads per CTA, query tiles of N rows in one group,
+// waves of those tiles on num_sms SMs}.  Status 2 (out untouched) for a d or N hb_silhouette refuses.
+int hb_debug_silhouette_geometry(int d, int64_t N, int num_sms, int64_t out[8]) {
+  if (sil_check_shape(nullptr, N, d) != 0 || num_sms < 1) return 2;
+  sil_geometry_record(d, N, num_sms, out);
   return 0;
 }
 

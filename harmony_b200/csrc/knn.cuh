@@ -52,21 +52,24 @@ __global__ void __launch_bounds__(256) k_knn_colsum(const T* __restrict__ X, int
 }
 
 // One warp per row (d <= 128: four values per lane).  centre: column sums (divided by centre_n here) or null.
-template <typename T>
+// GATHER: row r of dst and hx is row perm[r] of src (hb_silhouette's rows in sorted order).
+template <typename T, bool GATHER = false>
 __global__ void __launch_bounds__(256) k_knn_prepare(const T* __restrict__ src, int64_t ld, int64_t n, int d, int KD,
                                                      int cosine, const double* __restrict__ centre, double centre_n,
-                                                     float* __restrict__ dst, float* __restrict__ hx) {
+                                                     float* __restrict__ dst, float* __restrict__ hx,
+                                                     const int* __restrict__ perm) {
   const int lane = threadIdx.x & 31;
   const int64_t w = (blockIdx.x * (int64_t)blockDim.x + threadIdx.x) >> 5, nw = ((int64_t)gridDim.x * blockDim.x) >> 5;
   double c[4];
 #pragma unroll
   for (int i = 0; i < 4; ++i) c[i] = (centre && lane + 32 * i < d) ? centre[lane + 32 * i] / centre_n : 0.0;
   for (int64_t r = w; r < n; r += nw) {
+    const int64_t sr = GATHER ? (int64_t)perm[r] : r;
     float v[4];
     float ss = 0.f;
 #pragma unroll
     for (int i = 0; i < 4; ++i) {
-      v[i] = lane + 32 * i < d ? (float)((double)src[r * ld + lane + 32 * i] - c[i]) : 0.f;
+      v[i] = lane + 32 * i < d ? (float)((double)src[sr * ld + lane + 32 * i] - c[i]) : 0.f;
       ss = fmaf(v[i], v[i], ss);
     }
     ss = warp_sum(ss);

@@ -11,12 +11,16 @@ struct KnnState {
   DevBuf<double> centre;     // [KNN_MAX_D] column sums of X
 };
 
-// rows -> dst [n][KD] (and hx), centred on `centre` / centre_n or normalised
+// rows -> dst [n][KD] (and hx), centred on `centre` / centre_n or normalised; with perm, row r of dst is row perm[r]
 int knn_prepare(hb_handle* h, const DevRows& r, int d, int KD, bool cosine, const double* centre, double centre_n,
-                float* dst, float* hx) {
+                float* dst, float* hx, const int* perm = nullptr) {
   const int grid = grid_for(r.n * 32, 256, h->num_sms * 16);
   with_rows(r, [&](auto p) {
-    k_knn_prepare<<<grid, 256, 0, h->stream>>>(p, r.ld, r.n, d, KD, (int)cosine, centre, centre_n, dst, hx);
+    using T = std::remove_const_t<std::remove_pointer_t<decltype(p)>>;
+    if (perm)
+      k_knn_prepare<T, true><<<grid, 256, 0, h->stream>>>(p, r.ld, r.n, d, KD, (int)cosine, centre, centre_n, dst, hx, perm);
+    else
+      k_knn_prepare<T, false><<<grid, 256, 0, h->stream>>>(p, r.ld, r.n, d, KD, (int)cosine, centre, centre_n, dst, hx, nullptr);
   });
   CKL();
   return 0;

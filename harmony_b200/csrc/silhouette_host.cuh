@@ -1,0 +1,136 @@
+// silhouette_host.cuh — hb_silhouette (DESIGN §11): the checks, the scratch a handle keeps for it and the launches of
+// silhouette.cuh: the (group, label) index (build_tuple_index, tuples.cuh, into buffers of its own), the column sums
+// and sorted preparation of knn.cuh, the finite counts, the tile list and the sweep.  The call needs no setup and
+// touches no state of a Harmony run or a mapping.  Included by harmony_b200.cu.
+#pragma once
+
+namespace {
+
+// hb_silhouette's scratch; every buffer grows on demand and is kept for the next call
+struct SilhouetteState {
+  DevBuf<float> Xp, hx;              // prepared rows [N][KD] in sorted order, |x - c|^2 / 2
+  DevBuf<int> phi;                   // [N][2] (group, label) levels
+  DevBuf<int> sort_perm, inv_sort;   // the rows sorted by (group, label)
+  DevBuf<int> pstart, count;         // [J + 1] pair starts, [J] finite rows per pair
+  DevBuf<int4> tiles;
+  DevBuf<double> centre;             // [KNN_MAX_D] column sums of X
+};
+
+// Launch geometry of k_silhouette_tc: the first of (TQ, stages) = (128, 2), (128, 1), (64, 2), (64, 1) whose shared
+// memory fits (by sil_smem_bytes, (128, 2) fits every d <= 128)
+struct SilGeometry {
+  int tq = 0, stages = 0, KD = 0;
+  size_t smem = 0;
+};
+SilGeometry sil_geometry(int d) {
+  SilGeometry g;
+  g.KD = (d + 7) & ~7;
+  static const int shapes[4][2] = {{128, 2}, {128, 1}, {64, 2}, {64, 1}};
+  for (const auto& s : shapes)
+    if (sil_smem_bytes(s[0], s[1], g.KD) <= SMEM_LIMIT) {
+      g.tq = s[0], g.stages = s[1];
+      break;
+    }
+  g.smem = sil_smem_bytes(g.tq, g.stages, g.KD);
+  return g;
+}
+
+// The shape refusals hb_silhouette and hb_debug_silhouette_geometry share; h may be null (no message)
+int sil_check_shape(hb_handle* h, int64_t N, int d) {
+  if (N < 2) return refuse(h, "hb_silhouette: N = %lld rows, at least 2 are needed", (long long)N);
+  return check_search_shape(h, "hb_silhouette", "N", N, d);
+}
+
+// The eight values of hb_debug_silhouette_geometry
+void sil_geometry_record(int d, int64_t N, int num_sms, int64_t out[8]) {
+  const SilGeometry g = sil_geometry(d);
+  const int64_t tiles = (N + g.tq - 1) / g.tq;
+  const int64_t v[8] = {g.tq, KNN_TN, g.stages, (int64_t)g.smem, g.KD, 2 * g.tq, tiles, (tiles + num_sms - 1) / num_sms};
+  for (int i = 0; i < 8; ++i) out[i] = v[i];
+}
+
+// The tiles of <= tq sorted rows, none across a group, largest group first: {first row, end row, first pair, end
+// pair of the group}.  Pair q belongs to group uniq[q] / n_labels (group most significant in the key).
+std::vector<int4> sil_tiles(const TupleIndex& ti, int n_labels, int tq) {
+  struct Group {
+    int p0, p1;
+    int64_t rows;
+  };
+  std::vector<Group> gs;
+  const int J = (int)ti.uniq.size();
+  for (int q = 0; q < J;) {
+    int e = q + 1;
+    while (e < J && ti.uniq[e] / n_labels == ti.uniq[q] / n_labels) ++e;
+    gs.push_back({q, e, ti.tstart[e] - ti.tstart[q]});
+    q = e;
+  }
+  std::stable_sort(gs.begin(), gs.end(), [](const Group& a, const Group& b) { return a.rows > b.rows; });
+  std::vector<int4> tiles;
+  for (const Group& g : gs)
+    for (int64_t r = ti.tstart[g.p0]; r < ti.tstart[g.p1]; r += tq)
+      tiles.push_back(make_int4((int)r, (int)std::min<int64_t>(r + tq, ti.tstart[g.p1]), g.p0, g.p1));
+  return tiles;
+}
+
+// The whole call on h->stream, for arguments the caller has checked
+int silhouette_run(hb_handle* h, const DevRows& X, int d, const int32_t* labels, int n_labels, const int32_t* groups,
+                   int n_groups, double* s_out) {
+  if (!h->sil) h->sil.reset(new SilhouetteState());
+  SilhouetteState& s = *h->sil;
+  const int64_t N = X.n;
+  const SilGeometry g = sil_geometry(d);
+  const cudaStream_t st = h->stream;
+  CK(s.phi.reserve(2 * (size_t)N));
+  CK(s.Xp.reserve((size_t)N * g.KD));
+  CK(s.hx.reserve((size_t)N));
+  CK(s.centre.reserve((size_t)KNN_MAX_D));
+  // ---- the index of the (group, label) pairs: the sorted order and the pair starts
+  k_silhouette_phi<<<grid_for(N, 256, h->num_sms * 8), 256, 0, st>>>(labels, groups, N, n_labels, n_groups, s.phi.p);
+  CKL();
+  TupleKeys keys;
+  TRY(tuple_keys(h, {n_groups, n_labels}, keys));
+  TupleIndex ti;
+  static const char* const names[2] = {"hb_silhouette: groups", "hb_silhouette: labels"};
+  TRY(build_tuple_index(h, s.phi.p, N, keys, false, s.sort_perm, s.inv_sort, ti, names));
+  const int J = (int)ti.uniq.size();
+  CK(s.pstart.reserve((size_t)J + 1));
+  CK(s.count.reserve((size_t)J));
+  TRY(upload_vector(h, s.pstart, std::vector<int>(ti.tstart.begin(), ti.tstart.end())));
+  CK(cudaMemsetAsync(s.count.p, 0, sizeof(int) * J, st));
+  // ---- centre, rows in sorted order, finite rows per pair
+  CK(cudaMemsetAsync(s.centre.p, 0, sizeof(double) * KNN_MAX_D, st));
+  with_rows(X, [&](auto x) { k_knn_colsum<<<grid_for(N, 2, h->num_sms * 8), 256, 0, st>>>(x, X.ld, N, d, s.centre.p); });
+  CKL();
+  TRY(knn_prepare(h, X, d, g.KD, false, s.centre.p, (double)N, s.Xp.p, s.hx.p, s.sort_perm.p));
+  k_silhouette_count<<<grid_for(N, 256, h->num_sms * 8), 256, 0, st>>>(s.hx.p, N, s.pstart.p, J, s.count.p);
+  CKL();
+  // ---- the sweep
+  const std::vector<int4> tiles = sil_tiles(ti, n_labels, g.tq);
+  CK(s.tiles.reserve(tiles.size()));
+  TRY(upload_vector(h, s.tiles, tiles));
+  SilArgs a{s.Xp.p, s.hx.p, s.pstart.p, s.count.p, s.tiles.p, s.sort_perm.p, s_out, g.KD, g.stages};
+  const dim3 grid((unsigned)tiles.size());
+  if (g.tq == 128) return launch(h, k_silhouette_tc<128>, grid, dim3(256), g.smem, a);
+  return launch(h, k_silhouette_tc<64>, grid, dim3(128), g.smem, a);
+}
+
+int run_silhouette(hb_handle* h, const DevRows& X, int d, const int32_t* labels, int n_labels, const int32_t* groups,
+                   int n_groups, double* s, cudaStream_t caller) {
+  TRY(sil_check_shape(h, X.n, d));
+  if (n_labels < 1) return fail(h, 2, "hb_silhouette: n_labels = %d, at least one label is needed", n_labels);
+  if (groups && n_groups < 1) return fail(h, 2, "hb_silhouette: n_groups = %d, at least one group is needed", n_groups);
+  if (!groups) n_groups = 1;
+  if (n_labels > X.n || n_groups > X.n)
+    return fail(h, 2, "hb_silhouette: %d labels and %d groups, more codes than the N = %lld rows", n_labels, n_groups, (long long)X.n);
+  TRY(check_rows(h, X, d, "X"));
+  TRY(check_device_ptr(h, labels, "labels"));
+  if (groups) TRY(check_device_ptr(h, groups, "groups"));
+  TRY(check_device_ptr(h, s, "s"));
+  CK(cudaSetDevice(h->device));
+  return on_caller_stream(h, caller, [&] {
+    RegionScope rs(h, "silhouette");
+    return silhouette_run(h, X, d, labels, n_labels, groups, n_groups, s);
+  });
+}
+
+}  // namespace

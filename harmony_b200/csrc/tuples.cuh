@@ -1,7 +1,7 @@
-// tuples.cuh — the covariate-tuple index of setup, built on the device: each cell's key (the mixed-radix number of
-// its C levels, covariate 0 most significant), the level counts, the dictionary of the distinct keys (tuple ids
-// 0..J-1 in ascending key order), each cell's tuple id, and the stable sort of the cells by tuple id (sort_perm,
-// inv_sort, tstart).  The kernels and the host code that drives them; included by harmony_b200.cu after plan.cuh,
+// tuples.cuh — the covariate-tuple index of setup (and of hb_silhouette's (group, label) pairs), built on the device:
+// each cell's key (the mixed-radix number of its C levels, covariate 0 most significant), the level counts, the
+// dictionary of the distinct keys (tuple ids 0..J-1 in ascending key order), each cell's tuple id, and the stable sort
+// of the cells by tuple id (sort_perm, inv_sort, tstart).  The kernels and the host code that drives them; included by harmony_b200.cu after plan.cuh,
 // whose chained scan it reuses.
 #pragma once
 #include "common.cuh"
@@ -227,11 +227,44 @@ int tuple_scan(hb_handle* h, int* data, int64_t n) {
   return 0;
 }
 
-// The index of the N local cells whose levels phi_d (device, [N][C]) holds, read on the library stream.  Writes
-// h->sort_perm / h->inv_sort (allocated here) and `out`; every other buffer is freed before it returns.
-int build_tuple_index(hb_handle* h, const int* phi_d, int64_t N, const std::vector<int>& base,
-                      const std::vector<uint64_t>& radix, uint64_t key_space, TupleIndex& out) {
-  const int C = h->C, B = h->B;
+// The key layout of C covariates of nlev[c] levels: covariate c's first global level (base), its weight in the key
+// (radix; covariate 0 most significant) and the number of keys.  Status 2 when the level product overflows 64 bits.
+struct TupleKeys {
+  std::vector<int> nlev, base;
+  std::vector<uint64_t> radix;
+  uint64_t key_space = 1;
+  int B = 0;  // levels in all
+};
+int tuple_keys(hb_handle* h, const std::vector<int>& nlev, TupleKeys& k) {
+  const int C = (int)nlev.size();
+  k.nlev = nlev;
+  k.radix.assign(C, 0);
+  k.base.assign(C, 0);
+  k.key_space = 1;
+  long double prod = 1;
+  for (int c = 0; c < C; ++c) prod *= (long double)nlev[c];
+  if (prod > 9e18L) return fail(h, 2, "covariate level product overflows 64 bits");
+  for (int c = C - 1; c >= 0; --c) {
+    k.radix[c] = k.key_space;
+    k.key_space *= (uint64_t)nlev[c];
+  }
+  for (int c = 1; c < C; ++c) k.base[c] = k.base[c - 1] + nlev[c - 1];
+  k.B = std::accumulate(nlev.begin(), nlev.end(), 0);
+  return 0;
+}
+
+// The index of the N cells whose levels phi_d (device, [N][C]) holds, read on the library stream.  global: the
+// dictionary and the level counts are the union / sum over the ranks of h's communicator (setup of a sharded handle);
+// else the cells are all there is.  Writes sort_perm / inv_sort (allocated here) and `out`; every other buffer is freed
+// before it returns.  A level outside its covariate is refused with status 2, naming the cell; `names` (C names, or
+// null for setup's message) name the covariates and report the caller's code (phi minus the covariate's base).
+int build_tuple_index(hb_handle* h, const int* phi_d, int64_t N, const TupleKeys& keys, bool global,
+                      DevBuf<int>& sort_perm, DevBuf<int>& inv_sort, TupleIndex& out, const char* const* names = nullptr) {
+  const int C = (int)keys.nlev.size(), B = keys.B;
+  const std::vector<int>& base = keys.base;
+  const std::vector<uint64_t>& radix = keys.radix;
+  const uint64_t key_space = keys.key_space;
+  const int world = global ? h->world : 1;
   const bool direct = key_space <= (1ull << 22);  // the usual case: a table over the whole key space
   const cudaStream_t st = h->stream;
   const int grid = grid_for(N, 256, h->num_sms * 8);
@@ -249,7 +282,7 @@ int build_tuple_index(hb_handle* h, const int* phi_d, int64_t N, const std::vect
     for (int c = 0; c < C; ++c) {
       sm[1 + c] = radix[c];
       g[c] = base[c];
-      g[C + c] = h->B_vec[c];
+      g[C + c] = keys.nlev[c];
     }
     CK(cudaMemcpyAsync(small.p, sm.data(), sizeof(unsigned long long) * sm.size(), cudaMemcpyHostToDevice, st));
     CK(cudaMemcpyAsync(geom.p, g.data(), sizeof(int) * g.size(), cudaMemcpyHostToDevice, st));
@@ -275,7 +308,9 @@ int build_tuple_index(hb_handle* h, const int* phi_d, int64_t N, const std::vect
     int b = 0;
     CK(cudaMemcpyAsync(&b, phi_d + bad, sizeof(int), cudaMemcpyDeviceToHost, st));
     CK(cudaStreamSynchronize(st));
-    return fail(h, 2, "phi row index %d of cell %lld is not a level of covariate %d", b, (long long)(bad / C), (int)(bad % C));
+    const int c = (int)(bad % C);
+    if (names) return fail(h, 2, "%s of cell %lld is not a code in 0..%d", names[c], (long long)(bad / C), keys.nlev[c] - 1);
+    return fail(h, 2, "phi row index %d of cell %lld is not a level of covariate %d", b, (long long)(bad / C), c);
   }
   // ---- the local dictionary: its keys on the device (uniq_d, J_local of them, ascending on the direct path)
   int J_local = 0, hash_full = 0;
@@ -298,9 +333,9 @@ int build_tuple_index(hb_handle* h, const int* phi_d, int64_t N, const std::vect
   }
   // a full hash table holds more than TI_SLOTS / 2 > 1e6 keys (or a probe sequence ran out): over the limit either way
   const bool over = hash_full || (size_t)J_local > TI_MAX_TUPLES;
-  if (h->world == 1 && over) return too_many_tuples(h);
+  if (world == 1 && over) return too_many_tuples(h);
   out.lvl_count.assign(B, 0);
-  if (h->world == 1) {
+  if (world == 1) {
     out.uniq.resize(J_local);
     CK(cudaMemcpyAsync(out.uniq.data(), uniq_d.p, sizeof(uint64_t) * J_local, cudaMemcpyDeviceToHost, st));
     CK(cudaMemcpyAsync(out.lvl_count.data(), count.p, sizeof(int64_t) * B, cudaMemcpyDeviceToHost, st));
@@ -336,7 +371,7 @@ int build_tuple_index(hb_handle* h, const int* phi_d, int64_t N, const std::vect
   if (out.uniq.size() > TI_MAX_TUPLES) return too_many_tuples(h);
   const int J = (int)out.uniq.size();
   // ---- tuple ids of the keys (the direct table of a single handle already holds them), then of the cells
-  if (!direct || h->world > 1) {
+  if (!direct || world > 1) {
     DevBuf<unsigned long long> ud;
     CK(ud.alloc(J));
     CK(cudaMemcpyAsync(ud.p, out.uniq.data(), sizeof(uint64_t) * J, cudaMemcpyHostToDevice, st));
@@ -354,14 +389,14 @@ int build_tuple_index(hb_handle* h, const int* phi_d, int64_t N, const std::vect
   slots.release();
   slot_id.release();
   // ---- stable sort by tuple id: ceil(log2(J) / 8) passes of 8 bits
-  CK(h->sort_perm.alloc(N));
-  CK(h->inv_sort.alloc(N));
+  CK(sort_perm.reserve(N));
+  CK(inv_sort.reserve(N));
   int bits = 0;
   while (bits < 31 && (1ll << bits) < (long long)J) ++bits;
   const int passes = (bits + 7) / 8;
   int* kin = tid.p;
   if (passes == 0) {
-    k_identity_perm<<<grid, 256, 0, st>>>(N, h->sort_perm.p, h->inv_sort.p);
+    k_identity_perm<<<grid, 256, 0, st>>>(N, sort_perm.p, inv_sort.p);
     CKL();
   } else {
     const int nchunks = (int)((N + TI_CHUNK - 1) / TI_CHUNK);
@@ -378,8 +413,8 @@ int build_tuple_index(hb_handle* h, const int* phi_d, int64_t N, const std::vect
       CKL();
       TRY(tuple_scan(h, H.p, (int64_t)256 * nchunks));
       k_radix_scatter<<<cta, TI_WARPS * 32, 0, st>>>(kin, p == 0 ? nullptr : vbuf[(p - 1) & 1], N, 8 * p, nchunks, H.p,
-                                                     kout, last ? h->sort_perm.p : vbuf[p & 1],
-                                                     last ? h->inv_sort.p : nullptr);
+                                                     kout, last ? sort_perm.p : vbuf[p & 1],
+                                                     last ? inv_sort.p : nullptr);
       CKL();
       std::swap(kin, kout);
     }

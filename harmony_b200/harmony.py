@@ -201,6 +201,14 @@ class harmony:
         from .lisi import lisi_on
         return lisi_on(self, X, codes, perplexity, return_neighbors)
 
+    def silhouette(self, X, labels, groups=None):
+        """Silhouette width of every row of ``X`` [N, d] (host array or CUDA tensor) for the label codes ``labels``
+        (dense codes 0..n-1, [N]; numpy or int32 CUDA tensor), only rows of one group interacting when ``groups`` (the
+        same) are given, on this object's device and stream -> [N] float64.  ``harmony_b200.silhouette_samples`` takes
+        any label values.  Works in any state of the object and changes none of it."""
+        from .silhouette import silhouette_on
+        return silhouette_on(self, X, labels, groups)
+
     def _device_Phi(self, Phi):
         """An [N] or [N, C] int32 / int64 CUDA tensor -> contiguous [N, C] int32 on the object's device (converted, if
         need be, on the current torch stream, which hb_setup_device orders its read after)."""

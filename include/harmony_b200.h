@@ -43,8 +43,8 @@ const char* hb_last_error(const hb_handle* h);
  * buf; returns 1 if a warning was written, 0 if none is pending.  The shim turns it into Rcpp::warning. */
 int hb_pop_warning(hb_handle* h, char* buf, size_t cap);
 /* Library/ABI version: major*10000 + minor*100 + patch (0.3.0: labels in device memory; 0.4.0: mapping a query onto
- * a reference, hb_reference / hb_map_setup / hb_map).  hb_knn, hb_debug_knn_geometry, hb_lisi and
- * hb_debug_lisi_geometry were added without moving the number. */
+ * a reference, hb_reference / hb_map_setup / hb_map).  hb_knn, hb_debug_knn_geometry, hb_lisi,
+ * hb_debug_lisi_geometry, hb_silhouette and hb_debug_silhouette_geometry were added without moving the number. */
 int hb_version(void);
 
 /* ---- multi-GPU (one process per GPU; cells sharded contiguously; SURVEY §8e) ------------------- */
@@ -186,6 +186,25 @@ int hb_lisi(hb_handle* h, const void* X, int x_dtype, int64_t x_ld, int64_t N, i
 /* Test hook (host only): hb_debug_knn_geometry's eight values for hb_lisi's search of N rows at this perplexity on
  * num_sms SMs.  Returns 0, or 2 with out untouched for a d, perplexity or N hb_lisi refuses. */
 int hb_debug_lisi_geometry(int d, double perplexity, int64_t N, int num_sms, int64_t out[8]);
+/* Silhouette widths (DESIGN.md §11) of every row of X [N, d] with labels[i] in 0..n_labels-1 and, when groups is not
+ * NULL, groups[i] in 0..n_groups-1 (int32 device arrays of N codes; no groups: one group).  Only rows of one group
+ * interact, and only finite rows take part (a row with a NaN or an infinity, or whose centred |x - c|^2 overflows fp32,
+ * gets NaN and is nobody's neighbour).  With D the Euclidean distance and n the finite rows of row i's (group, label):
+ * a = sum of D to the other rows of its (group, label) / (n - 1), b = the smallest mean of D to the rows of another
+ * label of its group that has a finite row, s[i] = (b - a) / max(a, b) (0 when that is 0); 0 when n = 1, NaN when its
+ * group has no other such label.  Without groups this is sklearn.metrics.silhouette_samples.  s [N] fp64 in the
+ * caller's order.  X of x_dtype (hb_dtype) with row stride x_ld >= d.  Limits, status 2 with a message before any
+ * launch: 2 <= N < 2^31, 1 <= d <= 128, n_labels >= 1, n_groups >= 1 when groups are given, n_labels and n_groups
+ * <= N, an unknown dtype, a row stride < d, a NULL (X, labels, s), host or other-device pointer; a code out of range
+ * is status 2 naming the cell, found before the sweep.  Ordered on `stream` like hb_knn; needs no setup and leaves a
+ * Harmony or mapping handle's state untouched; on a sharded handle the call is local.  Region "silhouette". */
+int hb_silhouette(hb_handle* h, const void* X, int x_dtype, int64_t x_ld, int64_t N, int d, const int32_t* labels,
+                  int n_labels, const int32_t* groups, int n_groups, double* s, void* stream);
+/* Test hook (host only): the launch geometry of hb_silhouette's sweep for (d, N) on num_sms SMs: out = {rows per query
+ * tile, reference rows per tile, operand stages, shared-memory bytes, padded row length in floats, threads per CTA,
+ * query tiles of N rows in one group, waves of those tiles}.  Returns 0, or 2 with out untouched for a d or N
+ * hb_silhouette refuses. */
+int hb_debug_silhouette_geometry(int d, int64_t N, int num_sms, int64_t out[8]);
 
 /* ---- fields / getters (harmony.cpp:640-669, 675-696) ------------------------------------------- */
 enum hb_field {
