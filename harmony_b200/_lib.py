@@ -5,18 +5,15 @@ constructors raise.  The library is built IN-TREE (harmony_b200/libharmony_b200.
 ``nvcc -gencode arch=compute_90a,code=sm_90a`` (H100) by ``build()`` / ``__graft_entry__.build()``.
 """
 import ctypes
+import glob
 import os
 import subprocess
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(_HERE)
 SO_PATH = os.path.join(_HERE, "libharmony_b200.so")
-SOURCES = [os.path.join(_HERE, "csrc", f) for f in ("harmony_b200.cu", "kernels.cuh", "io.cuh", "common.cuh", "update_slots.cuh", "update_per_step.cuh",
-                                                     "update_two_pass.cuh", "update_single_pass.cuh", "plan.cuh", "tuples.cuh", "umma.cuh", "assign_tc3.cuh", "logits_tc.cuh", "logits_wide.cuh", "stats_tc3.cuh",
-                                                     "apply_tc3.cuh", "select.cuh", "handle.cuh", "comm.cuh", "trace.cuh", "transfer.cuh",
-                                                     "update_host.cuh", "correct_host.cuh", "assign_host.cuh", "kmeans_init.cuh",
-                                                     "map_host.cuh", "knn.cuh", "knn_host.cuh", "lisi.cuh", "lisi_host.cuh",
-                                                     "silhouette.cuh", "silhouette_host.cuh")]
+# the translation unit build() compiles, then every header it may include: a new header cannot miss needs_build()
+SOURCES = [os.path.join(_HERE, "csrc", "harmony_b200.cu")] + sorted(glob.glob(os.path.join(_HERE, "csrc", "*.cuh")))
 HEADER = os.path.join(ROOT, "include", "harmony_b200.h")
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17", "-shared",
               "-Xcompiler", "-fPIC"]

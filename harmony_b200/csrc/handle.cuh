@@ -72,9 +72,7 @@ struct Plan;         // plan.cuh
 struct UpdateState;  // update_host.cuh
 struct AssignState;  // assign_host.cuh
 struct MapState;     // map_host.cuh
-struct KnnState;     // knn_host.cuh
-struct LisiState;    // lisi_host.cuh
-struct SilhouetteState;  // silhouette_host.cuh
+struct ScoreScratch;  // knn_host.cuh
 
 }  // namespace
 
@@ -130,9 +128,7 @@ struct hb_handle {
   std::unique_ptr<UpdateState> upd;
   std::unique_ptr<AssignState> asg;
   std::unique_ptr<MapState> map;  // hb_map_setup only
-  std::unique_ptr<KnnState> knn;  // hb_knn's scratch, from its first call
-  std::unique_ptr<LisiState> lisi;  // hb_lisi's neighbour lists, from its first call without idx / dist
-  std::unique_ptr<SilhouetteState> sil;  // hb_silhouette's scratch, from its first call
+  std::unique_ptr<ScoreScratch> scores;  // the scratch of hb_knn, hb_lisi and hb_silhouette, from the first such call
 
   // traces (harmony.h:55-56); values are produced on the device and pulled lazily
   DevBuf<float> trace_d;

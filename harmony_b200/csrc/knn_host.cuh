@@ -1,15 +1,26 @@
-// knn_host.cuh — hb_knn (DESIGN §9): the checks, the scratch a handle keeps for it and the launches of knn.cuh.  The
+// knn_host.cuh — hb_knn (DESIGN §9): the checks, the scratch of the score calls and the launches of knn.cuh.  The
 // call needs no setup and touches no state of a Harmony run or a mapping.  Included by harmony_b200.cu.
 #pragma once
 
 namespace {
 
-// hb_knn's scratch; every buffer grows on demand and is kept for the next call
-struct KnnState {
-  DevBuf<float> Qp, Xp, hx;  // prepared rows [n][KD], |x|^2 / 2
-  DevBuf<int> part;          // [Nq][splits][k] listed candidates
-  DevBuf<double> centre;     // [KNN_MAX_D] column sums of X
+// The scratch of the score calls (hb_knn, hb_lisi, hb_silhouette), shared by them: each runs on h->stream, and a buffer
+// that grows is freed only after the device has drained.  Every buffer grows on demand and is kept for the next call.
+struct ScoreScratch {
+  DevBuf<float> rows, query_rows, hx;  // prepared rows [n][KD] of X and of Q, |x - c|^2 / 2 (or |x|^2 / 2)
+  DevBuf<double> centre;               // [KNN_MAX_D] column sums of X
+  DevBuf<int> part;                    // knn: [Nq][splits][k] listed candidates
+  DevBuf<int32_t> idx;                 // lisi: the neighbour lists when the caller passes no idx / dist
+  DevBuf<float> dist;
+  DevBuf<int> phi;                     // silhouette: [N][2] (group, label) levels
+  DevBuf<int> sort_perm, inv_sort;     // silhouette: the rows sorted by (group, label)
+  DevBuf<int> pstart, count;           // silhouette: [J + 1] pair starts, [J] finite rows per pair
+  DevBuf<int4> tiles;                  // silhouette: the sweep's tiles
 };
+ScoreScratch& score_scratch(hb_handle* h) {
+  if (!h->scores) h->scores.reset(new ScoreScratch());
+  return *h->scores;
+}
 
 // rows -> dst [n][KD] (and hx), centred on `centre` / centre_n or normalised; with perm, row r of dst is row perm[r]
 int knn_prepare(hb_handle* h, const DevRows& r, int d, int KD, bool cosine, const double* centre, double centre_n,
@@ -24,6 +35,19 @@ int knn_prepare(hb_handle* h, const DevRows& r, int d, int KD, bool cosine, cons
   });
   CKL();
   return 0;
+}
+
+// X's rows -> dst (and hx), optionally through perm: centred on X's column means, whose sums go to `centre`
+// (Euclidean), or normalised (cosine, centre unused)
+int prepare_centred(hb_handle* h, const DevRows& X, int d, int KD, bool cosine, double* centre, float* dst, float* hx,
+                    const int* perm = nullptr) {
+  if (!cosine) {
+    CK(cudaMemsetAsync(centre, 0, sizeof(double) * KNN_MAX_D, h->stream));
+    const int grid = grid_for(X.n, 2, h->num_sms * 8);
+    with_rows(X, [&](auto x) { k_knn_colsum<<<grid, 256, 0, h->stream>>>(x, X.ld, X.n, d, centre); });
+    CKL();
+  }
+  return knn_prepare(h, X, d, KD, cosine, cosine ? nullptr : centre, (double)X.n, dst, hx, perm);
 }
 
 // Status 2, with the message when there is a handle: the geometry hooks run the shape checks without one
@@ -49,33 +73,24 @@ void knn_geometry_record(int d, int k, int64_t Nq, int64_t Nx, int num_sms, int6
 // (and of Q unless it is X), the sweep and the merge into idx / dist [Nq][k].  hb_knn and hb_lisi run it.
 int knn_search(hb_handle* h, const DevRows& Q, const DevRows& X, int d, int k, bool cosine, bool exclude_self,
                int32_t* idx, float* dist) {
-  if (!h->knn) h->knn.reset(new KnnState());
-  KnnState& s = *h->knn;
+  ScoreScratch& s = score_scratch(h);
   const KnnGeometry g = knn_geometry(d, k, Q.n, X.n, h->num_sms);
   const bool shared_rows = Q.p == X.p && Q.dtype == X.dtype && Q.ld == X.ld && Q.n == X.n;  // one prepared copy serves
-  CK(s.Xp.reserve((size_t)X.n * g.KD));
-  if (!shared_rows) CK(s.Qp.reserve((size_t)Q.n * g.KD));
+  CK(s.rows.reserve((size_t)X.n * g.KD));
+  if (!shared_rows) CK(s.query_rows.reserve((size_t)Q.n * g.KD));
   CK(s.hx.reserve((size_t)X.n));
   CK(s.part.reserve((size_t)Q.n * g.splits * k));
   CK(s.centre.reserve((size_t)KNN_MAX_D));
 
-  const double* centre = nullptr;
-  if (!cosine) {
-    CK(cudaMemsetAsync(s.centre.p, 0, sizeof(double) * KNN_MAX_D, h->stream));
-    const int grid = grid_for(X.n, 2, h->num_sms * 8);
-    with_rows(X, [&](auto x) { k_knn_colsum<<<grid, 256, 0, h->stream>>>(x, X.ld, X.n, d, s.centre.p); });
-    CKL();
-    centre = s.centre.p;
-  }
-  TRY(knn_prepare(h, X, d, g.KD, cosine, centre, (double)X.n, s.Xp.p, s.hx.p));
-  const float* Qp = s.Xp.p;
+  TRY(prepare_centred(h, X, d, g.KD, cosine, s.centre.p, s.rows.p, s.hx.p));
+  const float* Qp = s.rows.p;
   if (!shared_rows) {
-    TRY(knn_prepare(h, Q, d, g.KD, cosine, centre, (double)X.n, s.Qp.p, nullptr));
-    Qp = s.Qp.p;
+    TRY(knn_prepare(h, Q, d, g.KD, cosine, cosine ? nullptr : s.centre.p, (double)X.n, s.query_rows.p, nullptr));
+    Qp = s.query_rows.p;
   }
   KnnArgs a;
   a.Qp = Qp;
-  a.Xp = s.Xp.p;
+  a.Xp = s.rows.p;
   a.hx = s.hx.p;
   a.part_i = s.part.p;
   a.Nq = Q.n;
@@ -99,7 +114,7 @@ int knn_search(hb_handle* h, const DevRows& Q, const DevRows& X, int d, int k, b
   }
   const int nc = g.splits * k;
   return launch(h, k_knn_merge, dim3((unsigned)((Q.n + 3) / 4)), dim3(128), (size_t)4 * 2 * nc * sizeof(float), Qp,
-                (const float*)s.Xp.p, (const int*)s.part.p, Q.n, g.KD, k, nc, (int)cosine, idx, dist);
+                (const float*)s.rows.p, (const int*)s.part.p, Q.n, g.KD, k, nc, (int)cosine, idx, dist);
 }
 
 int run_knn(hb_handle* h, const DevRows& Q, const DevRows& X, int d, int k, int metric, bool exclude_self, int32_t* idx,

@@ -1,15 +1,9 @@
-// lisi_host.cuh — hb_lisi (DESIGN §10): the checks, the neighbour lists a handle keeps when the caller takes none, and
-// the launches: knn_search (knn_host.cuh) for each row's floor(3 p) - 1 nearest other rows, then k_lisi.  The call
-// needs no setup and touches no state of a Harmony run or a mapping.  Included by harmony_b200.cu.
+// lisi_host.cuh — hb_lisi (DESIGN §10): the checks and the launches: knn_search (knn_host.cuh) for each row's
+// floor(3 p) - 1 nearest other rows, then k_lisi.  The call needs no setup and touches no state of a Harmony run or a
+// mapping.  Included by harmony_b200.cu.
 #pragma once
 
 namespace {
-
-// hb_lisi's neighbour lists when the caller passes no idx / dist; grown on demand and kept for the next call
-struct LisiState {
-  DevBuf<int32_t> idx;
-  DevBuf<float> dist;
-};
 
 // The neighbours LISI weighs at perplexity p: floor(3 p) - 1 (the package searches 3 p rows with the cell itself and
 // drops the first), 0 for a p that is not finite or below 1, KNN_SWEEP_MAX_K + 1 for any k above the sweep's limit.
@@ -42,8 +36,7 @@ int run_lisi(hb_handle* h, const DevRows& X, int d, const int32_t* labels, int64
   if (idx) TRY(check_device_ptr(h, idx, "idx"));
   if (dist) TRY(check_device_ptr(h, dist, "dist"));
   CK(cudaSetDevice(h->device));
-  if (!h->lisi) h->lisi.reset(new LisiState());
-  LisiState& s = *h->lisi;
+  ScoreScratch& s = score_scratch(h);
   if (!idx) {
     CK(s.idx.reserve((size_t)X.n * k));
     idx = s.idx.p;

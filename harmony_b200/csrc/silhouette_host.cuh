@@ -1,20 +1,10 @@
-// silhouette_host.cuh — hb_silhouette (DESIGN §11): the checks, the scratch a handle keeps for it and the launches of
-// silhouette.cuh: the (group, label) index (build_tuple_index, tuples.cuh, into buffers of its own), the column sums
-// and sorted preparation of knn.cuh, the finite counts, the tile list and the sweep.  The call needs no setup and
+// silhouette_host.cuh — hb_silhouette (DESIGN §11): the checks and the launches of silhouette.cuh: the (group, label)
+// index (build_tuple_index, tuples.cuh, into the score scratch), the column sums and sorted preparation of knn.cuh, the
+// finite counts, the tile list and the sweep.  The call needs no setup and
 // touches no state of a Harmony run or a mapping.  Included by harmony_b200.cu.
 #pragma once
 
 namespace {
-
-// hb_silhouette's scratch; every buffer grows on demand and is kept for the next call
-struct SilhouetteState {
-  DevBuf<float> Xp, hx;              // prepared rows [N][KD] in sorted order, |x - c|^2 / 2
-  DevBuf<int> phi;                   // [N][2] (group, label) levels
-  DevBuf<int> sort_perm, inv_sort;   // the rows sorted by (group, label)
-  DevBuf<int> pstart, count;         // [J + 1] pair starts, [J] finite rows per pair
-  DevBuf<int4> tiles;
-  DevBuf<double> centre;             // [KNN_MAX_D] column sums of X
-};
 
 // Launch geometry of k_silhouette_tc: the first of (TQ, stages) = (128, 2), (128, 1), (64, 2), (64, 1) whose shared
 // memory fits (by sil_smem_bytes, (128, 2) fits every d <= 128)
@@ -75,13 +65,12 @@ std::vector<int4> sil_tiles(const TupleIndex& ti, int n_labels, int tq) {
 // The whole call on h->stream, for arguments the caller has checked
 int silhouette_run(hb_handle* h, const DevRows& X, int d, const int32_t* labels, int n_labels, const int32_t* groups,
                    int n_groups, double* s_out) {
-  if (!h->sil) h->sil.reset(new SilhouetteState());
-  SilhouetteState& s = *h->sil;
+  ScoreScratch& s = score_scratch(h);
   const int64_t N = X.n;
   const SilGeometry g = sil_geometry(d);
   const cudaStream_t st = h->stream;
   CK(s.phi.reserve(2 * (size_t)N));
-  CK(s.Xp.reserve((size_t)N * g.KD));
+  CK(s.rows.reserve((size_t)N * g.KD));
   CK(s.hx.reserve((size_t)N));
   CK(s.centre.reserve((size_t)KNN_MAX_D));
   // ---- the index of the (group, label) pairs: the sorted order and the pair starts
@@ -98,17 +87,14 @@ int silhouette_run(hb_handle* h, const DevRows& X, int d, const int32_t* labels,
   TRY(upload_vector(h, s.pstart, std::vector<int>(ti.tstart.begin(), ti.tstart.end())));
   CK(cudaMemsetAsync(s.count.p, 0, sizeof(int) * J, st));
   // ---- centre, rows in sorted order, finite rows per pair
-  CK(cudaMemsetAsync(s.centre.p, 0, sizeof(double) * KNN_MAX_D, st));
-  with_rows(X, [&](auto x) { k_knn_colsum<<<grid_for(N, 2, h->num_sms * 8), 256, 0, st>>>(x, X.ld, N, d, s.centre.p); });
-  CKL();
-  TRY(knn_prepare(h, X, d, g.KD, false, s.centre.p, (double)N, s.Xp.p, s.hx.p, s.sort_perm.p));
+  TRY(prepare_centred(h, X, d, g.KD, false, s.centre.p, s.rows.p, s.hx.p, s.sort_perm.p));
   k_silhouette_count<<<grid_for(N, 256, h->num_sms * 8), 256, 0, st>>>(s.hx.p, N, s.pstart.p, J, s.count.p);
   CKL();
   // ---- the sweep
   const std::vector<int4> tiles = sil_tiles(ti, n_labels, g.tq);
   CK(s.tiles.reserve(tiles.size()));
   TRY(upload_vector(h, s.tiles, tiles));
-  SilArgs a{s.Xp.p, s.hx.p, s.pstart.p, s.count.p, s.tiles.p, s.sort_perm.p, s_out, g.KD, g.stages};
+  SilArgs a{s.rows.p, s.hx.p, s.pstart.p, s.count.p, s.tiles.p, s.sort_perm.p, s_out, g.KD, g.stages};
   const dim3 grid((unsigned)tiles.size());
   if (g.tq == 128) return launch(h, k_silhouette_tc<128>, grid, dim3(256), g.smem, a);
   return launch(h, k_silhouette_tc<64>, grid, dim3(128), g.smem, a);

@@ -4,15 +4,13 @@
 ``TransferLabels`` is Symphony's ``knnPredict`` on top of it: every query cell takes the majority label of its k nearest
 reference cells.  Argument errors are raised before the CUDA library is loaded.
 """
-import ctypes
-
 import numpy as np
 
-from ._arrays import current_stream, device_rows, factorise, resolve_device, to_device
+from ._arrays import current_stream, download, embedding, factorise, ptr, resolve_device, rows_on
 from .utils import is_cuda_tensor
 
 METRIC = {"euclidean": 0, "cosine": 1}   # enum hb_metric
-MAX_K, MAX_D = 64, 128
+MAX_K = 64
 
 
 def _check_args(query, ref, k, metric):
@@ -33,8 +31,7 @@ def _check_args(query, ref, k, metric):
     nx = nq if ref is None else ref.shape[0]
     if ref is not None and ref.shape[1] != d:
         raise ValueError(f"query has {d} dimensions, ref {ref.shape[1]}")
-    if not 1 <= d <= MAX_D:
-        raise ValueError(f"d = {d} is not supported (1 <= d <= {MAX_D})")
+    embedding(query, "query")
     if nq < 1 or nx < 1:
         raise ValueError("query and ref need at least one row")
     limit = min(MAX_K, nx - (1 if ref is None else 0))
@@ -48,20 +45,14 @@ def knn_on(obj, query, ref=None, k=15, metric="euclidean"):
     """``knn`` on an existing ``harmony`` object (any state: the search needs no setup and changes none)."""
     query, ref = _check_args(query, ref, k, metric)
     import torch
-    host = not is_cuda_tensor(query)
     device = torch.device("cuda", obj._scalar("device"))
-    if host:   # uploaded and downloaded with torch
-        query, ref = to_device(obj, query), None if ref is None else to_device(obj, ref)
-    q, *q_args = device_rows(obj, query, "query")
-    x, *x_args = (q, *q_args) if ref is None else device_rows(obj, ref, "ref")
+    host, q, q_args = rows_on(obj, query, "query")
+    _, x, x_args = (host, q, q_args) if ref is None else rows_on(obj, ref, "ref")
     idx = torch.empty((q.shape[0], int(k)), dtype=torch.int32, device=device)
     dist = torch.empty((q.shape[0], int(k)), dtype=torch.float32, device=device)
     obj._check(obj._L.hb_knn(obj._h, *q_args, q.shape[0], *x_args, x.shape[0], int(q.shape[1]), int(k), METRIC[metric],
-                             int(ref is None), ctypes.c_void_p(idx.data_ptr()), ctypes.c_void_p(dist.data_ptr()),
-                             current_stream(device)))
-    if host:
-        return idx.cpu().numpy(), dist.cpu().numpy()
-    return idx, dist
+                             int(ref is None), ptr(idx), ptr(dist), current_stream(device)))
+    return tuple(download(host, idx, dist))
 
 
 def knn(query, ref=None, k=15, metric="euclidean", device=None):

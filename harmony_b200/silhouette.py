@@ -7,85 +7,34 @@ folds of these per-cell values.
 (``harmony.silhouette``) runs ``hb_silhouette`` on an existing object.  Argument errors are raised before the CUDA
 library is loaded.
 """
-import ctypes
-
 import numpy as np
 
-from ._arrays import current_stream, device_rows, factorise, resolve_device, to_device
-from .lisi import _check_rows, _missing
+from ._arrays import (codes_on, current_stream, dense_codes, download, embedding, factorise, label_columns,
+                      label_device, label_vector, ptr, resolve_device, rows_on)
 from .utils import is_cuda_tensor
-
-
-def _check_codes(codes, n, what):
-    """int32-representable codes [N] (numpy or an int32 CUDA tensor) -> the same, and their count (largest + 1)."""
-    if is_cuda_tensor(codes):
-        import torch
-        if codes.dtype != torch.int32:
-            raise TypeError(f"CUDA {what} must be int32, not {codes.dtype}")
-        if codes.ndim != 1 or codes.shape[0] != n:
-            raise ValueError(f"{what} must be [{n}], not {tuple(codes.shape)}")
-        return codes, int(codes.max()) + 1 if n else 0
-    codes = np.asarray(codes)
-    if codes.dtype.kind not in "iu":
-        raise TypeError(f"{what} must be integers, not {codes.dtype}")
-    if codes.ndim != 1 or codes.shape[0] != n:
-        raise ValueError(f"{what} must be [{n}], not {codes.shape}")
-    if codes.size and (codes.min() < 0 or codes.max() >= 2 ** 31 - 1):
-        raise ValueError(f"{what} must be codes in 0..2^31 - 2")
-    return codes, int(codes.max()) + 1 if n else 0
 
 
 def silhouette_on(obj, X, labels, groups=None):
     """``hb_silhouette`` on an existing ``harmony`` object (any state: the call needs no setup and changes none).
     ``labels`` / ``groups``: dense codes 0..n-1 (numpy or int32 CUDA tensors on the object's device)."""
-    X = _check_rows(X)
+    X = embedding(X, "X")
     N, d = X.shape
     if N < 2:
         raise ValueError(f"X has {N} rows, at least 2 are needed")
-    labels, n_labels = _check_codes(labels, N, "labels")
+    labels, n_labels = dense_codes(labels, N, "labels")
     n_groups = 0
     if groups is not None:
-        groups, n_groups = _check_codes(groups, N, "groups")
+        groups, n_groups = dense_codes(groups, N, "groups")
     import torch
-    host = not is_cuda_tensor(X)
     device = torch.device("cuda", obj._scalar("device"))
-    if host:
-        X = to_device(obj, X)
-    x, *x_args = device_rows(obj, X, "X")
-    codes = []
-    for c in (labels, groups):
-        if c is not None and not is_cuda_tensor(c):
-            c = torch.as_tensor(np.ascontiguousarray(c, dtype=np.int32)).to(device)
-        if c is not None:
-            if c.device != device:
-                raise ValueError(f"codes are on {c.device}, the harmony object on {device}")
-            c = c.contiguous()
-        codes.append(c)
+    host, x, x_args = rows_on(obj, X, "X")
+    labels = codes_on(obj, labels).contiguous()
+    if groups is not None:
+        groups = codes_on(obj, groups).contiguous()
     out = torch.empty(N, dtype=torch.float64, device=device)
-    ptr = lambda t: ctypes.c_void_p(None if t is None else t.data_ptr())  # noqa: E731
-    obj._check(obj._L.hb_silhouette(obj._h, *x_args, N, int(d), ptr(codes[0]), int(n_labels), ptr(codes[1]),
+    obj._check(obj._L.hb_silhouette(obj._h, *x_args, N, int(d), ptr(labels), int(n_labels), ptr(groups),
                                     int(n_groups), ptr(out), current_stream(device)))
-    return out.cpu().numpy() if host else out
-
-
-def _column(cols, name, n):
-    if name not in cols:
-        raise ValueError(f"meta_data has no column {name!r}")
-    if cols[name].ndim != 1 or len(cols[name]) != n:
-        raise ValueError(f"column {name!r} must hold one label per row of X ({n})")
-    if not is_cuda_tensor(cols[name]) and _missing(cols[name]):
-        raise ValueError(f"column {name!r} holds missing labels")
-    return cols[name]
-
-
-def _vector(v, n, what):
-    if not is_cuda_tensor(v):
-        v = np.asarray(v)
-    if v.ndim != 1 or len(v) != n:
-        raise ValueError(f"{what} must hold one label per row of X ({n})")
-    if not is_cuda_tensor(v) and _missing(v):
-        raise ValueError(f"{what} holds missing labels")
-    return v
+    return download(host, out)[0]
 
 
 def _n_levels(codes):
@@ -103,15 +52,14 @@ def silhouette_samples(X, labels, groups=None, device=None):
     tensor).  Host ``X`` in -> numpy out; a CUDA ``X`` (float32 / float64) -> a CUDA tensor, ordered on the device's
     current torch stream.  A row with a non-finite value gets NaN and takes no part.  d <= 128."""
     on_device = is_cuda_tensor(X)
-    X = _check_rows(X)
+    X = embedding(X, "X")
     N = X.shape[0]
     if N < 2:
         raise ValueError(f"X has {N} rows, at least 2 are needed")
-    cols = {"labels": _vector(labels, N, "labels")}
+    cols = {"labels": label_vector(labels, N, "labels")}
     if groups is not None:
-        cols["groups"] = _vector(groups, N, "groups")
-    from .ui import _label_device
-    _label_device(cols, list(cols), X, on_device)
+        cols["groups"] = label_vector(groups, N, "groups")
+    label_device(cols, list(cols), X, on_device)
     device = resolve_device(device, X, "X")
     dev = X.device if on_device else None
     codes = factorise(cols["labels"], dev)[1]
@@ -123,22 +71,11 @@ def silhouette_samples(X, labels, groups=None, device=None):
     return silhouette_on(harmony(device=device), X, codes, gcodes)
 
 
-def _columns(X, meta_data, names):
-    on_device = is_cuda_tensor(X)
-    X = _check_rows(X)
-    if not isinstance(meta_data, dict) and not hasattr(meta_data, "columns"):
-        raise ValueError("meta_data must be a DataFrame or a dict of columns")
-    from .ui import _as_columns, _label_device
-    cols, _ = _as_columns(meta_data, ())
-    used = [_column(cols, v, X.shape[0]) for v in names]
-    _label_device(cols, names, X, on_device)
-    return X, used
-
-
 def silhouette_label(X, meta_data, label_key, scale=True):
     """Cell-type ASW, scib's ``silhouette``: the mean silhouette width of ``meta_data[label_key]`` over ``X``,
     scaled to ``(s + 1) / 2`` (1 best) unless ``scale`` is False.  Labels are taken as ``compute_lisi`` takes them."""
-    X, (labels,) = _columns(X, meta_data, [label_key])
+    X = embedding(X, "X")
+    (labels,) = label_columns(meta_data, [label_key], X)
     s = silhouette_samples(X, labels)
     asw = float(s.mean())
     return (asw + 1) / 2 if scale else asw
@@ -168,7 +105,8 @@ def silhouette_batch(X, meta_data, batch_key, label_key, scale=True, return_all=
     batches (``batch_key``) of its cells, taken as ``1 - |s|`` (``|s|`` unless ``scale``), averaged per cell type and
     then over the cell types.  A cell type with one batch, or with as many batches as cells, is skipped; NaN when all
     are.  One device call scores every cell type.  With ``return_all`` also ``{cell type: its mean}``."""
-    X, (batch, label) = _columns(X, meta_data, [batch_key, label_key])
+    X = embedding(X, "X")
+    batch, label = label_columns(meta_data, [batch_key, label_key], X)
     s = silhouette_samples(X, batch, groups=label)
     host = lambda v: v.cpu().numpy() if is_cuda_tensor(v) else np.asarray(v)  # noqa: E731
     asw, means = batch_fold(host(s), host(batch), host(label), scale)

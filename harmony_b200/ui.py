@@ -9,48 +9,9 @@ import sys
 
 import numpy as np
 
-from ._arrays import factorise, resolve_device
+from ._arrays import as_columns, factorise, label_device, resolve_device
 from .harmony_option import HarmonyOptions, check_legacy_args, harmony_options
 from .utils import harmonize, is_cuda_tensor
-
-
-def _column(v):
-    return v if is_cuda_tensor(v) else np.asarray(v)
-
-
-def _as_columns(meta_data, n_hint):
-    """meta_data -> dict name -> 1-D array (CUDA tensors stay where they are).  Accepts a dict, a pandas DataFrame
-    or one vector (R/ui.R:157-165: a bare vector becomes data.frame(batch_variable = ...))."""
-    if hasattr(meta_data, "columns") and hasattr(meta_data, "__getitem__") and not isinstance(meta_data, dict):
-        return {str(c): np.asarray(meta_data[c]) for c in meta_data.columns}, None
-    if isinstance(meta_data, dict):
-        return {str(k): _column(v) for k, v in meta_data.items()}, None
-    v = _column(meta_data)
-    if v.ndim == 1 and len(v) in n_hint:
-        return {"batch_variable": v}, "batch_variable"
-    raise ValueError("meta_data must be either a data.frame or a vector with batch values for each cell")
-
-
-def _label_device(cols, vars_use, data_mat, on_device):
-    """The device of the used label columns that are CUDA tensors (None: all are host arrays).  They must be integer
-    or bool tensors on data_mat's device."""
-    device = None
-    for v in vars_use:
-        col = cols[v]
-        if not is_cuda_tensor(col):
-            continue
-        import torch
-        if col.dtype not in (torch.bool, torch.uint8, torch.int8, torch.int16, torch.int32, torch.int64):
-            raise TypeError(f"labels {v!r} on the GPU must be an integer or bool tensor, not {col.dtype}")
-        if not on_device:
-            raise ValueError(f"labels {v!r} are a CUDA tensor but data_mat is not: device labels go with a device "
-                             f"embedding")
-        if col.device != data_mat.device:
-            raise ValueError(f"labels {v!r} are on {col.device}, data_mat on {data_mat.device}")
-        if col.ndim != 1:
-            raise ValueError(f"labels {v!r} must be a vector")
-        device = col.device
-    return device
 
 
 def _cells_and_columns(data_mat, meta_data, vars_use, verbose):
@@ -61,7 +22,7 @@ def _cells_and_columns(data_mat, meta_data, vars_use, verbose):
         data_mat = np.asarray(data_mat)
     if data_mat.ndim != 2:
         raise ValueError("data_mat must be a matrix")
-    cols, forced = _as_columns(meta_data, data_mat.shape)
+    cols, forced = as_columns(meta_data, data_mat.shape)
     if forced is not None:
         vars_use = forced
     if vars_use is None:
@@ -90,7 +51,7 @@ def _factorise(cols, vars_use, data_mat, on_device):
     then an int32 CUDA tensor (host columns are copied over)."""
     phi_cols, B_vec, level_names = [], [], []
     offset = 0
-    device = _label_device(cols, vars_use, data_mat, on_device)
+    device = label_device(cols, vars_use, data_mat, on_device)
     for v in vars_use:
         # device columns hold integer / bool labels: torch's sorted unique levels are np.unique's (and as.factor's)
         levels, codes = factorise(cols[v], device)

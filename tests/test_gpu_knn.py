@@ -7,18 +7,13 @@ import pytest
 
 import knn_restatement as kr
 from harmony_b200 import MapQuery, RunHarmony, TransferLabels, knn
-from helpers import gpu_harmony, num_sms, synthetic
+from harmony_b200._arrays import ptr
+from helpers import gpu_harmony
+from score_helpers import check_band, generic, geometry, handle_state_untouched, refusals_launch_nothing, strided
 
 pytestmark = pytest.mark.gpu
 
 EPS32 = 2.0 ** -24
-
-
-def _geometry(d, k, Nq, Nx):
-    from harmony_b200 import _lib
-    out = (ctypes.c_int64 * 8)()
-    assert _lib.lib().hb_debug_knn_geometry(d, k, Nq, Nx, num_sms(), out) == 0
-    return list(out)
 
 
 def check(Q, X, k, metric, exclude_self, idx, dist, max_set_diff=0.001, block=1000):
@@ -37,13 +32,8 @@ def check(Q, X, k, metric, exclude_self, idx, dist, max_set_diff=0.001, block=10
         D = kr.distances(Q64[r0:r1], X64, metric)
         if exclude_self:
             D[np.arange(r1 - r0), np.arange(r0, r1)] = np.inf
-        Dk = np.partition(D, k - 1, axis=1)[:, k - 1]
-        b = kr.band(qn[r0:r1], xn, d, metric)
         got = np.take_along_axis(D, idx[r0:r1].astype(np.int64), 1)
-        must = (D < (Dk - b)[:, None]).sum(axis=1)
-        have = (got < (Dk - b)[:, None]).sum(axis=1)
-        assert (have == must).all(), f"rows {r0 + np.nonzero(have != must)[0][:5]} miss a neighbour inside the band"
-        assert (got <= (Dk + b)[:, None]).all(), "a row outside the band was returned"
+        check_band(D, got, k, kr.band(qn[r0:r1], xn, d, metric))
         want = got if metric == "cosine" else np.sqrt(got)
         floor = 16 * EPS32 * (1.0 if metric == "cosine" else (qn[r0:r1, None] + xn))
         err = np.abs(dist[r0:r1] - want)
@@ -55,11 +45,6 @@ def check(Q, X, k, metric, exclude_self, idx, dist, max_set_diff=0.001, block=10
     if max_set_diff is not None:
         assert share <= max_set_diff, f"{share:.4%} of the rows differ from fp64's neighbours"
     return share
-
-
-def generic(rng, n, d, types=12):
-    M = rng.standard_normal((types, d)) * 3.0
-    return M[rng.integers(0, types, n)] + rng.standard_normal((n, d))
 
 
 ROWS = [
@@ -99,7 +84,7 @@ def test_knn_table(row):
     import torch
     name, d, k, Nq, Nx, metric, dtype, o = row
     rng = np.random.default_rng(sum(map(ord, name)))
-    X = generic(rng, Nx, d)
+    X = generic(rng, Nx, d)[0]
     if o.get("offset"):
         X += o["offset"]
     if o.get("duplicates"):
@@ -125,20 +110,15 @@ def test_knn_table(row):
     X, Q = X.astype(dtype), (X if self_search else Q).astype(dtype)
     if self_search:
         Q = X
-    tq, tn, stages, splits, smem, per, KD, threads = _geometry(d, k, len(Q), Nx)
+    tq, tn, stages, splits, smem, per, KD, threads = geometry("hb_debug_knn_geometry", d, k, len(Q), Nx)
     if "splits" in o:
         assert (splits > 1) == o["splits"], (splits, o)
     if "stages" in o:
         assert stages == o["stages"]
     assert tq == o.get("tq", 128)
     dev = torch.device("cuda", 0)
-    if o.get("strided"):   # views that end exactly where their allocation does
-        ld = d + 3
-        bx = torch.zeros(Nx * ld - 3, dtype=torch.float32, device=dev)
-        bq = torch.zeros(Nq * ld - 3, dtype=torch.float32, device=dev)
-        xt, qt = torch.as_strided(bx, (Nx, d), (ld, 1)), torch.as_strided(bq, (Nq, d), (ld, 1))
-        xt.copy_(torch.as_tensor(X, device=dev))
-        qt.copy_(torch.as_tensor(Q, device=dev))
+    if o.get("strided"):
+        xt, qt = strided(X), strided(Q)
     else:
         xt = torch.as_tensor(X, device=dev)
         qt = xt if self_search else torch.as_tensor(Q, device=dev)
@@ -156,7 +136,7 @@ def test_knn_table(row):
 def test_non_finite_rows():
     """A NaN or infinite reference row is nobody's neighbour; such a query row has none (idx -1, dist inf)."""
     rng = np.random.default_rng(5)
-    X, Q = generic(rng, 3000, 20).astype(np.float32), generic(rng, 300, 20).astype(np.float32)
+    X, Q = generic(rng, 3000, 20)[0].astype(np.float32), generic(rng, 300, 20)[0].astype(np.float32)
     X[7, 3], X[100, 0], Q[5, 1], Q[9, 19] = np.nan, np.inf, np.nan, -np.inf
     for metric in ("euclidean", "cosine"):
         idx, dist = knn(Q, X, k=5, metric=metric)
@@ -176,7 +156,7 @@ def test_non_finite_rows():
 def test_numpy_and_tensor_paths_agree():
     import torch
     rng = np.random.default_rng(2)
-    X, Q = generic(rng, 20000, 30), generic(rng, 500, 30)
+    X, Q = generic(rng, 20000, 30)[0], generic(rng, 500, 30)[0]
     i0, d0 = knn(Q, X, k=10)
     i1, d1 = knn(torch.as_tensor(Q, device="cuda:0"), torch.as_tensor(X, device="cuda:0"), k=10)
     assert isinstance(i0, np.ndarray) and i1.is_cuda
@@ -188,48 +168,17 @@ def test_handle_state_untouched():
     """hb_knn between cluster_cpp and moe_correct_ridge_cpp, and on a mapping handle before and after hb_map: Z_corr, R
     and Y read bit for bit the same before and after the call, and the run ends where a run without it ends (to the
     run-to-run noise of the atomics' order)."""
-    import torch
-    from harmony_b200 import prepare_inputs
-    from helpers import make_perms, make_Y0, rel_l2
-    Z, meta = synthetic(20000, 50, [4], n_types=10, seed=3)
-    a = prepare_inputs(Z, meta, "cov0", nclust=50, early_stop=False)
-    Y0, perms = make_Y0(Z, 50, 1), make_perms(20000, 2 * a["max_iter_kmeans"], 2).reshape(2, a["max_iter_kmeans"], -1)
-    probe = torch.as_tensor(Z[:5000], device="cuda:0")
-    state = lambda h: (h.getZcorr(), h.getR(), h.Y)  # noqa: E731
-    outs = []
-    for with_knn in (False, True):
-        g = gpu_harmony()
-        g.setup(a["Z"], a["phi_i"], a["sigma"], a["theta"], a["lambda_"], a["alpha"], a["max_iter_kmeans"],
-                a["epsilon_kmeans"], a["epsilon_harmony"], 50, a["block_size"], a["B_vec"], a["batch_proportion_cutoff"])
-        g.init_cluster_cpp(Y0)
-        for it in range(2):
-            assert g.cluster_cpp(perms[it]) == 0
-            if with_knn:
-                before = state(g)
-                idx, _ = g.knn(probe, k=15)
-                assert int(idx.min()) >= 0
-                for u, v in zip(before, state(g)):
-                    np.testing.assert_array_equal(u, v)
-            g.moe_correct_ridge_cpp()
-        outs.append(state(g))
-        ref = g.reference()
-    for u, v in zip(*outs):
-        assert rel_l2(u, v) < 1e-4
-    maps = []
-    for with_knn in (False, True):
-        m = gpu_harmony()
-        m.map_setup(Z[:6000], a["phi_i"][:6000], a["B_vec"], 1.0, ref)
-        if with_knn:
-            m.knn(probe, k=5, metric="cosine")
-        m.map()
-        if with_knn:
-            before = state(m)
-            m.knn(m.get_tensor("Z_corr"), probe, k=5)
-            for u, v in zip(before, state(m)):
-                np.testing.assert_array_equal(u, v)
-        maps.append(state(m))
-    for u, v in zip(*maps):
-        assert rel_l2(u, v) < 1e-4
+
+    def call(h, phase, data):
+        if phase == "run":
+            idx, _ = h.knn(data.probe, k=15)
+            assert int(idx.min()) >= 0
+        elif phase == "setup":
+            h.knn(data.probe, k=5, metric="cosine")
+        else:
+            h.knn(h.get_tensor("Z_corr"), data.probe, k=5)
+
+    handle_state_untouched(call, baseline=True)
 
 
 def test_label_transfer_end_to_end():
@@ -276,19 +225,16 @@ def test_refusals_launch_nothing():
     dev = torch.device("cuda", 0)
     X, Q = torch.zeros((100, 8), device=dev), torch.zeros((10, 8), device=dev)
     idx, dist = torch.zeros((10, 5), dtype=torch.int32, device=dev), torch.zeros((10, 5), device=dev)
-    P = lambda t: ctypes.c_void_p(t.data_ptr())  # noqa: E731
     host = np.zeros((100, 8), np.float32)
-    good = dict(Q=P(Q), qt=0, qld=8, Nq=10, X=P(X), xt=0, xld=8, Nx=100, d=8, k=5, metric=0, excl=0, idx=P(idx), dist=P(dist))
+    good = dict(Q=ptr(Q), qt=0, qld=8, Nq=10, X=ptr(X), xt=0, xld=8, Nx=100, d=8, k=5, metric=0, excl=0, idx=ptr(idx),
+                dist=ptr(dist))
     bad = [dict(k=0), dict(k=65), dict(k=101, Nx=100), dict(k=5, Nx=5, excl=1), dict(d=0), dict(d=129, qld=129, xld=129),
            dict(Nq=0), dict(Nx=0), dict(Nx=2 ** 31), dict(metric=2), dict(qt=2), dict(xt=-1), dict(qld=7), dict(xld=7),
            dict(Q=None), dict(X=None), dict(idx=None), dict(X=host.ctypes.data_as(ctypes.c_void_p)),
            dict(dist=host.ctypes.data_as(ctypes.c_void_p))]
-    for change in bad:
-        a = dict(good, **change)
-        st = L.hb_knn(g._h, a["Q"], a["qt"], a["qld"], a["Nq"], a["X"], a["xt"], a["xld"], a["Nx"], a["d"], a["k"],
-                      a["metric"], a["excl"], a["idx"], a["dist"], None)
-        assert st == 2 and L.hb_last_error(g._h), change
-        assert g.kernel_launches == 0, change
+    refusals_launch_nothing(g, lambda a: L.hb_knn(g._h, a["Q"], a["qt"], a["qld"], a["Nq"], a["X"], a["xt"], a["xld"],
+                                                  a["Nx"], a["d"], a["k"], a["metric"], a["excl"], a["idx"], a["dist"],
+                                                  None), good, bad)
     a = good
     assert L.hb_knn(g._h, a["Q"], 0, 8, 10, a["X"], 0, 8, 100, 8, 5, 0, 0, a["idx"], None, None) == 0   # dist may be NULL
     assert g.kernel_launches > 0

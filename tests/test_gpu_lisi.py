@@ -8,20 +8,16 @@ import pytest
 import knn_restatement as kr
 import lisi_restatement as lr
 from harmony_b200 import RunHarmony, compute_lisi, knn
-from helpers import gpu_harmony, load_cell_lines, num_sms, synthetic
+from harmony_b200._arrays import ptr
+from helpers import gpu_harmony, load_cell_lines
+from score_helpers import Frame, generic, geometry, handle_state_untouched, refusals_launch_nothing, strided
+from score_helpers import check_band as in_band
 
 pytestmark = pytest.mark.gpu
 
 REL_OWN = 1e-9      # bar (a): the call's own neighbours through the restatement
 REL_FP64 = 1e-4     # bar (b): the restatement from scratch, rows with fp64's neighbour set (DESIGN §10)
 SET_DIFF = 0.001    # bar (b): rows whose neighbour set differs from fp64's (DESIGN §9's bar for the sweep)
-
-
-def _geometry(d, p, N):
-    from harmony_b200 import _lib
-    out = (ctypes.c_int64 * 8)()
-    assert _lib.lib().hb_debug_lisi_geometry(d, p, N, num_sms(), out) == 0
-    return list(out)
 
 
 def same_lisi(got, want, rel):
@@ -49,17 +45,7 @@ def check_band(X, k, idx, block=2000):
         r1 = min(len(F), r0 + block)
         D = kr.distances(F[r0:r1], F, "euclidean")
         D[np.arange(r1 - r0), np.arange(r0, r1)] = np.inf
-        Dk = np.partition(D, k - 1, axis=1)[:, k - 1]
-        b = kr.band(qn[r0:r1], xn, F.shape[1])
-        got = np.take_along_axis(D, back[idx[rows[r0:r1]]], 1)
-        assert ((got < (Dk - b)[:, None]).sum(1) == (D < (Dk - b)[:, None]).sum(1)).all(), "a neighbour outside the band is missing"
-        assert (got <= (Dk + b)[:, None]).all(), "a row beyond the band was returned"
-
-
-def generic(rng, n, d, types=12):
-    M = rng.standard_normal((types, d)) * 3.0
-    t = rng.integers(0, types, n)
-    return M[t] + rng.standard_normal((n, d)), t
+        in_band(D, np.take_along_axis(D, back[idx[rows[r0:r1]]], 1), k, kr.band(qn[r0:r1], xn, F.shape[1]))
 
 
 ROWS = [
@@ -117,18 +103,15 @@ def test_lisi_table(row):
     X = X.astype(dtype)
     codes = _labels(rng, N, t, o.get("sets")).astype(np.int32)
     k = lr.neighbours_for(p)
-    tq, tn, stages, splits, smem, per, KD, threads = _geometry(d, p, N)
+    tq, tn, stages, splits, smem, per, KD, threads = geometry("hb_debug_lisi_geometry", d, p, N)
     if "splits" in o:
         assert (splits > 1) == o["splits"], (splits, o)
     if "stages" in o:
         assert stages == o["stages"]
     assert tq == o.get("tq", 128)
     dev = torch.device("cuda", 0)
-    if o.get("strided"):   # a view that ends exactly where its allocation does
-        ld = d + 3
-        buf = torch.zeros(N * ld - 3, dtype=torch.float32 if dtype == np.float32 else torch.float64, device=dev)
-        xt = torch.as_strided(buf, (N, d), (ld, 1))
-        xt.copy_(torch.as_tensor(X, device=dev))
+    if o.get("strided"):
+        xt = strided(X)
         cbuf = torch.zeros((codes.shape[0], N + 5), dtype=torch.int32, device=dev)
         ct = cbuf[:, :N]
         ct.copy_(torch.as_tensor(codes, device=dev))
@@ -167,23 +150,13 @@ def test_lisi_table(row):
           f"set-diff {share:.4%} flagged {int((flag | own_flag).sum())}")
 
 
-class _Frame:
-    """What compute_lisi needs of a pandas DataFrame."""
-
-    def __init__(self, cols):
-        self._cols, self.columns = cols, list(cols)
-
-    def __getitem__(self, name):
-        return self._cols[name]
-
-
 def test_compute_lisi_inputs_agree():
     """Host arrays, CUDA tensors, a DataFrame, CUDA integer labels and a default stream: one result."""
     import torch
     rng = np.random.default_rng(4)
     X, t = generic(rng, 6000, 30)
     batch = np.array(["b1", "b0", "b2"])[rng.integers(0, 3, len(X))]
-    meta = _Frame({"batch": batch, "type": t, "other": np.full(len(X), 1.5)})
+    meta = Frame({"batch": batch, "type": t, "other": np.full(len(X), 1.5)})
     host = compute_lisi(X, meta, ["batch", "type"])
     assert isinstance(host, np.ndarray) and host.shape == (len(X), 2) and host.dtype == np.float64
     Xd = torch.as_tensor(X, device="cuda:0")
@@ -204,35 +177,16 @@ def test_handle_state_untouched():
     """hb_lisi between cluster_cpp and moe_correct_ridge_cpp and on a mapping handle before and after hb_map: Z_corr, R
     and Y read bit for bit the same before and after the call."""
     import torch
-    from harmony_b200 import prepare_inputs
-    from helpers import make_perms, make_Y0
-    Z, meta = synthetic(20000, 50, [4], n_types=10, seed=3)
-    a = prepare_inputs(Z, meta, "cov0", nclust=50, early_stop=False)
-    Y0, perms = make_Y0(Z, 50, 1), make_perms(20000, 2 * a["max_iter_kmeans"], 2).reshape(2, a["max_iter_kmeans"], -1)
-    probe = torch.as_tensor(Z[:5000], device="cuda:0")
-    codes = torch.as_tensor(meta["cov0"][:5000].astype(np.int32), device="cuda:0")
-    state = lambda h: (h.getZcorr(), h.getR(), h.Y)  # noqa: E731
-    g = gpu_harmony()
-    g.setup(a["Z"], a["phi_i"], a["sigma"], a["theta"], a["lambda_"], a["alpha"], a["max_iter_kmeans"],
-            a["epsilon_kmeans"], a["epsilon_harmony"], 50, a["block_size"], a["B_vec"], a["batch_proportion_cutoff"])
-    g.init_cluster_cpp(Y0)
-    for it in range(2):
-        assert g.cluster_cpp(perms[it]) == 0
-        before = state(g)
-        out = g.lisi(probe, codes, 30)
-        assert not torch.isnan(out).any()
-        for u, v in zip(before, state(g)):
-            np.testing.assert_array_equal(u, v)
-        g.moe_correct_ridge_cpp()
-    ref = g.reference()
-    m = gpu_harmony()
-    m.map_setup(Z[:6000], a["phi_i"][:6000], a["B_vec"], 1.0, ref)
-    m.lisi(probe, codes, 10)
-    m.map()
-    before = state(m)
-    m.lisi(m.get_tensor("Z_corr"), np.asarray(meta["cov0"][:6000], np.int32), 30)
-    for u, v in zip(before, state(m)):
-        np.testing.assert_array_equal(u, v)
+
+    def call(h, phase, data):
+        if phase == "run":
+            assert not torch.isnan(h.lisi(data.probe, data.codes, 30)).any()
+        elif phase == "setup":
+            h.lisi(data.probe, data.codes, 10)
+        else:
+            h.lisi(h.get_tensor("Z_corr"), data.mapped_codes, 30)
+
+    handle_state_untouched(call)
 
 
 def test_refusals_launch_nothing():
@@ -246,20 +200,16 @@ def test_refusals_launch_nothing():
     lab = torch.zeros((2, N), dtype=torch.int32, device=dev)
     out = torch.zeros((N, 2), dtype=torch.float64, device=dev)
     idx, dist = torch.zeros((N, 89), dtype=torch.int32, device=dev), torch.zeros((N, 89), device=dev)
-    P = lambda t: ctypes.c_void_p(t.data_ptr())  # noqa: E731
     host = np.zeros((N, 89), np.float64)
     H = host.ctypes.data_as(ctypes.c_void_p)
-    good = dict(X=P(X), xt=0, xld=d, N=N, d=d, lab=P(lab), lld=N, sets=2, p=30.0, out=P(out), idx=P(idx), dist=P(dist))
+    good = dict(X=ptr(X), xt=0, xld=d, N=N, d=d, lab=ptr(lab), lld=N, sets=2, p=30.0, out=ptr(out), idx=ptr(idx),
+                dist=ptr(dist))
     bad = [dict(p=0.5), dict(p=float("nan")), dict(p=float("inf")), dict(p=-30.0), dict(p=43.34), dict(N=89),
            dict(N=2 ** 31), dict(d=0), dict(d=129, xld=129), dict(sets=0), dict(lld=N - 1), dict(xt=2), dict(xt=-1),
            dict(xld=d - 1), dict(X=None), dict(lab=None), dict(out=None), dict(X=H), dict(lab=H), dict(out=H),
            dict(idx=H), dict(dist=H)]
-    for change in bad:
-        a = dict(good, **change)
-        st = L.hb_lisi(g._h, a["X"], a["xt"], a["xld"], a["N"], a["d"], a["lab"], a["lld"], a["sets"], a["p"], a["out"],
-                       a["idx"], a["dist"], None)
-        assert st == 2 and L.hb_last_error(g._h), change
-        assert g.kernel_launches == 0, change
+    refusals_launch_nothing(g, lambda a: L.hb_lisi(g._h, a["X"], a["xt"], a["xld"], a["N"], a["d"], a["lab"], a["lld"],
+                                                   a["sets"], a["p"], a["out"], a["idx"], a["dist"], None), good, bad)
     a = good
     assert L.hb_lisi(g._h, a["X"], 0, d, N, d, a["lab"], N, 2, 30.0, a["out"], None, None, None) == 0   # no idx / dist
     assert g.kernel_launches > 0

@@ -8,15 +8,11 @@ import pytest
 
 import silhouette_restatement as sr
 from harmony_b200 import RunHarmony, silhouette_batch, silhouette_label, silhouette_samples
-from helpers import gpu_harmony, load_cell_lines, synthetic
+from harmony_b200._arrays import ptr
+from helpers import gpu_harmony, load_cell_lines
+from score_helpers import Frame, generic, handle_state_untouched, refusals_launch_nothing, strided
 
 pytestmark = pytest.mark.gpu
-
-
-def generic(rng, n, d, types=12):
-    M = rng.standard_normal((types, d)) * 3.0
-    t = rng.integers(0, types, n)
-    return M[t] + rng.standard_normal((n, d)), t
 
 
 ROWS = [
@@ -74,26 +70,12 @@ def _case(name, N, d, o):
     return X, t.astype(np.int32), None if g is None else g.astype(np.int32)
 
 
-def _device(X, dtype, strided):
-    import torch
-    dev = torch.device("cuda", 0)
-    tdt = torch.float32 if dtype == np.float32 else torch.float64
-    if not strided:
-        return torch.as_tensor(X.astype(dtype), device=dev)
-    N, d = X.shape
-    ld = d + 3
-    buf = torch.zeros(N * ld - 3, dtype=tdt, device=dev)   # a view that ends exactly where its allocation does
-    xt = torch.as_strided(buf, (N, d), (ld, 1))
-    xt.copy_(torch.as_tensor(X.astype(dtype), device=dev))
-    return xt
-
-
 @pytest.mark.parametrize("row", ROWS, ids=[r[0] for r in ROWS])
 def test_silhouette_table(row):
     import torch
     name, N, d, dtype, o = row
     X, t, g = _case(name, N, d, o)
-    xt = _device(X, dtype, o.get("strided"))
+    xt = strided(X.astype(dtype)) if o.get("strided") else torch.as_tensor(X.astype(dtype), device="cuda:0")
     h = gpu_harmony()
     lab = torch.as_tensor(t, device="cuda:0")
     grp = None if g is None else torch.as_tensor(g, device="cuda:0")
@@ -119,16 +101,6 @@ def test_silhouette_table(row):
           f"(ratio to bound {ratio.max() if ratio.size else 0:.3f}), median bound {np.median(finite_bound) if finite_bound.size else 0:.2e}")
 
 
-class _Frame:
-    """What the scib folds need of a pandas DataFrame."""
-
-    def __init__(self, cols):
-        self._cols, self.columns = cols, list(cols)
-
-    def __getitem__(self, name):
-        return self._cols[name]
-
-
 def test_inputs_agree_and_repeat():
     """Host arrays, CUDA tensors, a DataFrame and CUDA integer labels give one result; two calls are bit-identical."""
     import torch
@@ -146,7 +118,7 @@ def test_inputs_agree_and_repeat():
     np.testing.assert_array_equal(host, silhouette_samples(X, batch, groups=t))
     want, bound = sr.silhouette(X, bcodes, t, bound=True)
     assert (np.abs(host - want) <= bound + 1e-12).all()
-    meta = _Frame({"batch": batch, "type": t})
+    meta = Frame({"batch": batch, "type": t})
     b_host, per = silhouette_batch(X, meta, "batch", "type", return_all=True)
     b_dev = silhouette_batch(Xd, {"batch": batch, "type": torch.as_tensor(t, device="cuda:0")}, "batch", "type")
     assert b_host == b_dev and set(per) == set(range(12))
@@ -162,49 +134,32 @@ def test_handle_state_untouched():
     """hb_silhouette between cluster_cpp and moe_correct_ridge_cpp and on a mapping handle: Z_corr, R, Y and the
     covariate-tuple index read bit for bit the same before and after the call."""
     import torch
-    from harmony_b200 import _lib, prepare_inputs
-    from helpers import make_perms, make_Y0
+    from harmony_b200 import _lib
     L = _lib.lib()
-    Z, meta = synthetic(20000, 50, [4], n_types=10, seed=3)
-    a = prepare_inputs(Z, meta, "cov0", nclust=50, early_stop=False)
-    Y0, perms = make_Y0(Z, 50, 1), make_perms(20000, 2 * a["max_iter_kmeans"], 2).reshape(2, a["max_iter_kmeans"], -1)
-    probe = torch.as_tensor(Z[:5000], device="cuda:0")
-    codes = torch.as_tensor(meta["cov0"][:5000].astype(np.int32), device="cuda:0")
 
     def index(h, n):
         perm, start = np.zeros(n, np.int32), np.zeros(64, np.int64)
         J = L.hb_debug_tuple_index(h._h, perm.ctypes.data_as(ctypes.c_void_p), None, start.ctypes.data_as(ctypes.c_void_p))
         return J, perm, start[:J + 1].copy()
 
-    fields = lambda h: (h.getZcorr(), h.getR(), h.Y)  # noqa: E731
-    g = gpu_harmony()
-    g.setup(a["Z"], a["phi_i"], a["sigma"], a["theta"], a["lambda_"], a["alpha"], a["max_iter_kmeans"],
-            a["epsilon_kmeans"], a["epsilon_harmony"], 50, a["block_size"], a["B_vec"], a["batch_proportion_cutoff"])
-    g.init_cluster_cpp(Y0)
-    for it in range(2):
-        assert g.cluster_cpp(perms[it]) == 0
-        before, ib = fields(g), index(g, 20000)
-        out = g.silhouette(probe, codes)
-        assert not torch.isnan(out).any()
-        for u, v in zip(before, fields(g)):
-            np.testing.assert_array_equal(u, v)
-        ia = index(g, 20000)
-        assert ib[0] == ia[0] == 4
+    def call(h, phase, data):
+        if phase == "setup":
+            h.silhouette(data.probe, data.codes)
+            return
+        n = 20000 if phase == "run" else 6000
+        ib = index(h, n)
+        if phase == "run":
+            assert not torch.isnan(h.silhouette(data.probe, data.codes)).any()
+        else:
+            h.silhouette(h.get_tensor("Z_corr"), data.mapped_codes)
+        ia = index(h, n)
+        assert ib[0] == ia[0]
         np.testing.assert_array_equal(ib[1], ia[1])
-        np.testing.assert_array_equal(ib[2], ia[2])
-        g.moe_correct_ridge_cpp()
-    ref = g.reference()
-    m = gpu_harmony()
-    m.map_setup(Z[:6000], a["phi_i"][:6000], a["B_vec"], 1.0, ref)
-    m.silhouette(probe, codes)
-    m.map()
-    before, ib = fields(m), index(m, 6000)
-    m.silhouette(m.get_tensor("Z_corr"), np.asarray(meta["cov0"][:6000], np.int32))
-    for u, v in zip(before, fields(m)):
-        np.testing.assert_array_equal(u, v)
-    ia = index(m, 6000)
-    assert ib[0] == ia[0]
-    np.testing.assert_array_equal(ib[1], ia[1])
+        if phase == "run":
+            assert ia[0] == 4
+            np.testing.assert_array_equal(ib[2], ia[2])
+
+    handle_state_untouched(call)
 
 
 def test_refusals_launch_nothing():
@@ -218,18 +173,15 @@ def test_refusals_launch_nothing():
     lab = torch.zeros(N, dtype=torch.int32, device=dev)
     grp = torch.zeros(N, dtype=torch.int32, device=dev)
     out = torch.zeros(N, dtype=torch.float64, device=dev)
-    P = lambda t: ctypes.c_void_p(t.data_ptr())  # noqa: E731
     host = np.zeros(N, np.float64)
     H = host.ctypes.data_as(ctypes.c_void_p)
-    good = dict(X=P(X), xt=0, xld=d, N=N, d=d, lab=P(lab), nl=2, grp=P(grp), ng=1, out=P(out))
+    good = dict(X=ptr(X), xt=0, xld=d, N=N, d=d, lab=ptr(lab), nl=2, grp=ptr(grp), ng=1, out=ptr(out))
     bad = [dict(N=1), dict(N=0), dict(N=2 ** 31), dict(d=0), dict(d=129, xld=129), dict(nl=0), dict(ng=0),
            dict(nl=N + 1), dict(ng=N + 1), dict(xt=2), dict(xt=-1), dict(xld=d - 1), dict(X=None), dict(lab=None),
            dict(out=None), dict(X=H), dict(lab=H), dict(grp=H), dict(out=H)]
     call = lambda a: L.hb_silhouette(g._h, a["X"], a["xt"], a["xld"], a["N"], a["d"], a["lab"], a["nl"], a["grp"],  # noqa: E731
                                      a["ng"], a["out"], None)
-    for change in bad:
-        assert call(dict(good, **change)) == 2 and L.hb_last_error(g._h), change
-        assert g.kernel_launches == 0, change
+    refusals_launch_nothing(g, call, good, bad)
     # codes out of range: found by the index pass, status 2 naming the cell
     lab[17] = 2
     assert call(good) == 2 and b"labels of cell 17" in L.hb_last_error(g._h)

@@ -97,19 +97,30 @@ def test_python_refusals_need_no_device(monkeypatch):
     from harmony_b200 import _lib
     monkeypatch.setattr(_lib, "lib", lambda: pytest.fail("the library was loaded"))
     Q, X = _sets(5, nq=10, nx=30)
-    bad = [dict(query=Q, ref=X, k=0), dict(query=Q, ref=X, k=65), dict(query=Q, ref=X, k=31), dict(query=Q, k=10),
-           dict(query=Q, ref=X, k=2.5), dict(query=Q, ref=X[:, :5]), dict(query=Q[0], ref=X), dict(query=Q, ref=X[0]),
-           dict(query=Q, ref=X, metric="manhattan"), dict(query=np.zeros((4, 129)), ref=np.zeros((9, 129)), k=2),
-           dict(query=np.zeros((0, 3)), ref=X[:, :3], k=1)]
-    for kw in bad:
-        with pytest.raises(ValueError):
+    ref_k = "is not supported here (1 <= k <= 30: at most 64, and the rows of ref)"
+    matrices = "query and ref must be [rows, d] matrices"
+    bad = [(dict(query=Q, ref=X, k=0), f"k = 0 {ref_k}"), (dict(query=Q, ref=X, k=65), f"k = 65 {ref_k}"),
+           (dict(query=Q, ref=X, k=31), f"k = 31 {ref_k}"),
+           (dict(query=Q, k=10), "k = 10 is not supported here (1 <= k <= 9: at most 64, and the other rows)"),
+           (dict(query=Q, ref=X, k=2.5), "k must be an integer, not 2.5"),
+           (dict(query=Q, ref=X[:, :5]), "query has 7 dimensions, ref 5"), (dict(query=Q[0], ref=X), matrices),
+           (dict(query=Q, ref=X[0]), matrices),
+           (dict(query=Q, ref=X, metric="manhattan"), "metric must be one of ['cosine', 'euclidean'], not 'manhattan'"),
+           (dict(query=np.zeros((4, 129)), ref=np.zeros((9, 129)), k=2), "d = 129 is not supported (1 <= d <= 128)"),
+           (dict(query=np.zeros((0, 3)), ref=X[:, :3], k=1), "query and ref need at least one row")]
+    for kw, msg in bad:
+        with pytest.raises(ValueError) as e:
             knn(**kw)
-    for kw in (dict(ref_labels=np.zeros(29)), dict(ref_labels=np.zeros((30, 2))), dict(ref_labels=np.zeros(30), k=0),
-               dict(ref_labels=_Categorical([-1] * 30, ["a"]))):
-        with pytest.raises(ValueError):
-            TransferLabels(Q, X, **kw)
-    with pytest.raises(ValueError):
-        TransferLabels(Q, None, np.zeros(10))
+        assert e.type is ValueError and str(e.value) == msg, kw
+    for kw, msg in ((dict(ref_labels=np.zeros(29)), "ref has 30 rows, ref_labels 29 labels"),
+                    (dict(ref_labels=np.zeros((30, 2))), "ref_labels must hold one label per row of ref"),
+                    (dict(ref_labels=np.zeros(30), k=0), f"k = 0 {ref_k}"),
+                    (dict(ref_labels=_Categorical([-1] * 30, ["a"])), "ref_labels holds missing values"),
+                    (dict(ref=None, ref_labels=np.zeros(10)), "TransferLabels needs a reference embedding")):
+        kw = dict(dict(query=Q, ref=X), **kw)
+        with pytest.raises(ValueError) as e:
+            TransferLabels(**kw)
+        assert e.type is ValueError and str(e.value) == msg, kw
 
 
 def _geometry(d, k, Nq, Nx, sms):

@@ -136,18 +136,31 @@ def test_compute_lisi_refusals_need_no_device(monkeypatch):
     monkeypatch.setattr(_lib, "lib", lambda: pytest.fail("the library was loaded"))
     X, labels = _data(5, n=100)
     meta = {"batch": labels[0], "type": labels[1]}
-    bad = [dict(perplexity=0.5), dict(perplexity=float("nan")), dict(perplexity=float("inf")), dict(perplexity=43.34),
-           dict(perplexity=34), dict(perplexity=True), dict(perplexity="30"), dict(X=X[:, 0]),
-           dict(X=np.zeros((100, 129))), dict(X=np.zeros((100, 0))), dict(label_colnames=[]),
-           dict(label_colnames="nope"), dict(meta_data=labels[0]), dict(meta_data={"batch": labels[0][:99]}),
-           dict(meta_data={"batch": np.where(labels[0] == 1, np.nan, labels[0])}),
-           dict(meta_data={"batch": np.array(["a", None] * 50, dtype=object)}),
-           dict(meta_data={"batch": np.array(["a", float("nan")] * 50, dtype=object)})]
-    for change in bad:
+    missing = "column 'batch' holds missing labels"
+    bad = [(dict(perplexity=0.5), "perplexity must be finite and at least 1, not 0.5"),
+           (dict(perplexity=float("nan")), "perplexity must be finite and at least 1, not nan"),
+           (dict(perplexity=float("inf")), "perplexity must be finite and at least 1, not inf"),
+           (dict(perplexity=43.34), "perplexity 43.34 needs k = floor(3 p) - 1 = 129 neighbours; at most 128 "
+                                    "(perplexity < 43 1/3)"),
+           (dict(perplexity=34), "perplexity 34 needs k = 101 neighbours, 100 rows have 99"),
+           (dict(perplexity=True), "perplexity must be a number, not True"),
+           (dict(perplexity="30"), "perplexity must be a number, not '30'"),
+           (dict(X=X[:, 0]), "X must be an [N, d] matrix"),
+           (dict(X=np.zeros((100, 129))), "d = 129 is not supported (1 <= d <= 128)"),
+           (dict(X=np.zeros((100, 0))), "d = 0 is not supported (1 <= d <= 128)"),
+           (dict(label_colnames=[]), "label_colnames names no column"),
+           (dict(label_colnames="nope"), "meta_data has no column 'nope'"),
+           (dict(meta_data=labels[0]), "meta_data must be a DataFrame or a dict of columns"),
+           (dict(meta_data={"batch": labels[0][:99]}), "column 'batch' must hold one label per row of X (100)"),
+           (dict(meta_data={"batch": np.where(labels[0] == 1, np.nan, labels[0])}), missing),
+           (dict(meta_data={"batch": np.array(["a", None] * 50, dtype=object)}), missing),
+           (dict(meta_data={"batch": np.array(["a", float("nan")] * 50, dtype=object)}), missing)]
+    for change, msg in bad:
         kw = dict(X=X, meta_data=meta, label_colnames="batch", perplexity=10)
         kw.update(change)
-        with pytest.raises((ValueError, TypeError)):
+        with pytest.raises(ValueError) as e:
             compute_lisi(kw.pop("X"), **kw)
+        assert e.type is ValueError and str(e.value) == msg, change
 
 
 def _geometry(d, p, N, sms):

@@ -128,23 +128,30 @@ def test_refusals_need_no_device(monkeypatch):
     monkeypatch.setattr(_lib, "lib", lambda: pytest.fail("the library was loaded"))
     X, t = _data(6, n=50)
     meta = {"batch": t % 2, "type": t}
-    for kw in (dict(X=X[:, 0], labels=t), dict(X=np.zeros((50, 129)), labels=t), dict(X=np.zeros((50, 0)), labels=t),
-               dict(X=X[:1], labels=t[:1]), dict(X=X, labels=t[:49]), dict(X=X, labels=np.zeros(50)),
-               dict(X=X, labels=np.arange(50)), dict(X=X, labels=np.where(t == 1, np.nan, t)),
-               dict(X=X, labels=np.array(["a", None] * 25, dtype=object)), dict(X=X, labels=t, groups=t[:10])):
-        with pytest.raises((ValueError, TypeError)):
-            silhouette_samples(**kw)
-    for kw in (dict(meta_data=t), dict(meta_data={"type": t[:49]}), dict(label_key="nope"),
-               dict(meta_data={"type": np.zeros(50)})):
-        a = dict(X=X, meta_data=meta, label_key="type")
-        a.update(kw)
-        with pytest.raises((ValueError, TypeError)):
-            silhouette_label(a.pop("X"), **a)
-    for kw in (dict(batch_key="nope"), dict(label_key="nope"), dict(meta_data={"batch": t, "type": t[:3]})):
-        a = dict(X=X, meta_data=meta, batch_key="batch", label_key="type")
-        a.update(kw)
-        with pytest.raises((ValueError, TypeError)):
-            silhouette_batch(a.pop("X"), **a)
+    n_labels = "Number of labels is {}. Valid values are 2 to n_samples - 1 (inclusive)"
+    no_column, type_rows = "meta_data has no column 'nope'", "column 'type' must hold one label per row of X (50)"
+    calls = [(silhouette_samples, dict(X=X[:, 0], labels=t), "X must be an [N, d] matrix"),
+             (silhouette_samples, dict(X=np.zeros((50, 129)), labels=t), "d = 129 is not supported (1 <= d <= 128)"),
+             (silhouette_samples, dict(X=np.zeros((50, 0)), labels=t), "d = 0 is not supported (1 <= d <= 128)"),
+             (silhouette_samples, dict(X=X[:1], labels=t[:1]), "X has 1 rows, at least 2 are needed"),
+             (silhouette_samples, dict(X=X, labels=t[:49]), "labels must hold one label per row of X (50)"),
+             (silhouette_samples, dict(X=X, labels=np.zeros(50)), n_labels.format(1)),
+             (silhouette_samples, dict(X=X, labels=np.arange(50)), n_labels.format(50)),
+             (silhouette_samples, dict(X=X, labels=np.where(t == 1, np.nan, t)), "labels holds missing labels"),
+             (silhouette_samples, dict(X=X, labels=np.array(["a", None] * 25, dtype=object)),
+              "labels holds missing labels"),
+             (silhouette_samples, dict(X=X, labels=t, groups=t[:10]), "groups must hold one label per row of X (50)")]
+    for kw, msg in ((dict(meta_data=t), "meta_data must be a DataFrame or a dict of columns"),
+                    (dict(meta_data={"type": t[:49]}), type_rows), (dict(label_key="nope"), no_column),
+                    (dict(meta_data={"type": np.zeros(50)}), n_labels.format(1))):
+        calls.append((silhouette_label, dict(dict(X=X, meta_data=meta, label_key="type"), **kw), msg))
+    for kw, msg in ((dict(batch_key="nope"), no_column), (dict(label_key="nope"), no_column),
+                    (dict(meta_data={"batch": t, "type": t[:3]}), type_rows)):
+        calls.append((silhouette_batch, dict(dict(X=X, meta_data=meta, batch_key="batch", label_key="type"), **kw), msg))
+    for f, kw, msg in calls:
+        with pytest.raises(ValueError) as e:
+            f(**kw)
+        assert e.type is ValueError and str(e.value) == msg, (f.__name__, kw)
 
 
 def _geometry(d, N, sms):
