@@ -128,7 +128,7 @@ struct hb_handle {
   std::unique_ptr<UpdateState> upd;
   std::unique_ptr<AssignState> asg;
   std::unique_ptr<MapState> map;  // hb_map_setup only
-  std::unique_ptr<ScoreScratch> scores;  // the scratch of hb_knn, hb_lisi and hb_silhouette, from the first such call
+  std::unique_ptr<ScoreScratch> scores;  // the scratch of the score calls (knn_host.cuh), from the first such call
 
   // traces (harmony.h:55-56); values are produced on the device and pulled lazily
   DevBuf<float> trace_d;

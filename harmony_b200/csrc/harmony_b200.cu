@@ -40,6 +40,7 @@
 #include "knn.cuh"
 #include "lisi.cuh"
 #include "silhouette.cuh"
+#include "components.cuh"
 
 #include "select.cuh"
 #include "handle.cuh"
@@ -364,6 +365,7 @@ int harmony_step(hb_handle* h, const char* what, bool needs_init = true) {
 #include "knn_host.cuh"
 #include "lisi_host.cuh"
 #include "silhouette_host.cuh"
+#include "components_host.cuh"
 
 // =================================================================================================
 extern "C" {
@@ -550,6 +552,12 @@ int hb_silhouette(hb_handle* h, const void* X, int x_dtype, int64_t x_ld, int64_
                   int n_labels, const int32_t* groups, int n_groups, double* s, void* stream) {
   if (!h) return 1;
   return run_silhouette(h, DevRows{X, x_dtype, x_ld, N}, d, labels, n_labels, groups, n_groups, s, (cudaStream_t)stream);
+}
+
+int hb_graph_components(hb_handle* h, const int32_t* idx, int64_t idx_ld, int64_t N, int k, const int32_t* labels,
+                        int n_labels, int32_t* comp, int32_t* largest, void* stream) {
+  if (!h) return 1;
+  return run_components(h, idx, idx_ld, N, k, labels, n_labels, comp, largest, (cudaStream_t)stream);
 }
 
 int hb_init_cluster(hb_handle* h, const double* Y0) {

@@ -4,7 +4,7 @@
 
 namespace {
 
-// The scratch of the score calls (hb_knn, hb_lisi, hb_silhouette), shared by them: each runs on h->stream, and a buffer
+// The scratch of the score calls (hb_knn, hb_lisi, hb_silhouette, hb_graph_components), shared by them: each runs on h->stream, and a buffer
 // that grows is freed only after the device has drained.  Every buffer grows on demand and is kept for the next call.
 struct ScoreScratch {
   DevBuf<float> rows, query_rows, hx;  // prepared rows [n][KD] of X and of Q, |x - c|^2 / 2 (or |x|^2 / 2)
@@ -16,6 +16,8 @@ struct ScoreScratch {
   DevBuf<int> sort_perm, inv_sort;     // silhouette: the rows sorted by (group, label)
   DevBuf<int> pstart, count;           // silhouette: [J + 1] pair starts, [J] finite rows per pair
   DevBuf<int4> tiles;                  // silhouette: the sweep's tiles
+  DevBuf<int> sizes;                   // components: [N] rows per root
+  DevBuf<unsigned long long> bad;      // components: the range pass's smallest bad entry
 };
 ScoreScratch& score_scratch(hb_handle* h) {
   if (!h->scores) h->scores.reset(new ScoreScratch());

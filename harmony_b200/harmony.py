@@ -209,6 +209,15 @@ class harmony:
         from .silhouette import silhouette_on
         return silhouette_on(self, X, labels, groups)
 
+    def graph_components(self, idx, labels=None):
+        """Connected components of the neighbour graph ``idx`` [N, k] (int32, -1 for no neighbour; host array or CUDA
+        tensor), with edges only between rows of one label when ``labels`` (dense codes 0..n-1, [N]; numpy or int32 CUDA
+        tensor) are given, on this object's device and stream -> ``(comp, largest)``: the smallest row of each row's
+        component, and the largest component of each label.  ``harmony_b200.graph_components`` takes any label values.
+        Works in any state of the object and changes none of it."""
+        from .graph import components_on
+        return components_on(self, idx, labels)
+
     def _device_Phi(self, Phi):
         """An [N] or [N, C] int32 / int64 CUDA tensor -> contiguous [N, C] int32 on the object's device (converted, if
         need be, on the current torch stream, which hb_setup_device orders its read after)."""

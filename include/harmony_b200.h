@@ -44,7 +44,8 @@ const char* hb_last_error(const hb_handle* h);
 int hb_pop_warning(hb_handle* h, char* buf, size_t cap);
 /* Library/ABI version: major*10000 + minor*100 + patch (0.3.0: labels in device memory; 0.4.0: mapping a query onto
  * a reference, hb_reference / hb_map_setup / hb_map).  hb_knn, hb_debug_knn_geometry, hb_lisi,
- * hb_debug_lisi_geometry, hb_silhouette and hb_debug_silhouette_geometry were added without moving the number. */
+ * hb_debug_lisi_geometry, hb_silhouette, hb_debug_silhouette_geometry and hb_graph_components were added without
+ * moving the number. */
 int hb_version(void);
 
 /* ---- multi-GPU (one process per GPU; cells sharded contiguously; SURVEY §8e) ------------------- */
@@ -205,6 +206,19 @@ int hb_silhouette(hb_handle* h, const void* X, int x_dtype, int64_t x_ld, int64_
  * query tiles of N rows in one group, waves of those tiles}.  Returns 0, or 2 with out untouched for a d or N
  * hb_silhouette refuses. */
 int hb_debug_silhouette_geometry(int d, int64_t N, int num_sms, int64_t out[8]);
+/* Connected components of a neighbour graph (DESIGN.md §12).  idx [N][k] int32 with row stride idx_ld >= k: entry j of
+ * row i is the undirected edge {i, j}, -1 is no neighbour (hb_knn's fill); self and repeated entries add nothing.  With
+ * labels (int32 [N], codes 0..n_labels-1) an edge is kept only between rows of one label, so components never cross
+ * labels; labels NULL keeps every edge and ignores n_labels.  comp [N]: the smallest row of each row's component (the
+ * same whatever order the union-find runs in).  largest (NULL: not computed): [n_labels] (one entry without labels), the
+ * size of the largest component among the rows of each label, 0 for a code no row has.  All pointers in device or
+ * managed memory of the handle's device.  Limits, status 2 with a message before any launch: 1 <= N < 2^31, k >= 1,
+ * idx_ld >= k, 1 <= n_labels <= N when labels are given, a NULL (idx, comp), host or other-device pointer.  An entry
+ * outside -1..N-1 or a code outside 0..n_labels-1 is status 2 naming the row and the entry, found by a read-only pass
+ * before comp and largest are written.  Ordered on `stream` like hb_knn; needs no setup and leaves a Harmony or mapping
+ * handle's state untouched; on a sharded handle the call is local.  Region "components". */
+int hb_graph_components(hb_handle* h, const int32_t* idx, int64_t idx_ld, int64_t N, int k, const int32_t* labels,
+                        int n_labels, int32_t* comp, int32_t* largest, void* stream);
 
 /* ---- fields / getters (harmony.cpp:640-669, 675-696) ------------------------------------------- */
 enum hb_field {

@@ -1,0 +1,322 @@
+"""hb_graph_components on the GPU against the scipy restatement (components_restatement.py), bit for bit: a table of
+graphs (random, hb_knn's own lists, a deep shuffled path, stars on the first and last row, empty, self and repeated
+entries, labels that cut every edge, strided lists, 4M rows), repeatability, the handle's state, the refusals, stream
+order, and graph connectivity of an integration end to end."""
+import ctypes
+
+import numpy as np
+import pytest
+
+import components_restatement as cr
+from harmony_b200 import RunHarmony, graph_components, graph_connectivity, knn
+from harmony_b200._arrays import ptr
+from helpers import gpu_harmony
+from score_helpers import generic, handle_state_untouched, refusals_launch_nothing
+
+pytestmark = pytest.mark.gpu
+
+LAUNCHES = 6           # check, init, hook, compress, count, largest
+LAUNCHES_NO_LARGEST = 4
+
+
+def random_lists(rng, N, k, missing=0.5):
+    """Uniform random neighbours with a share of -1 entries, some self entries and repeated entries."""
+    idx = rng.integers(0, N, (N, k)).astype(np.int32)
+    idx[rng.random((N, k)) < missing] = -1
+    idx[rng.random(N) < 0.05, 0] = -1
+    selves = np.nonzero(rng.random(N) < 0.05)[0]
+    idx[selves, 0] = selves
+    if k > 1:
+        rep = rng.random(N) < 0.1
+        idx[rep, -1] = idx[rep, 0]
+    return idx
+
+
+def shuffled_path(rng, N):
+    """Rows in a random order p, each linked to the next and to the previous one: links in both directions of the row
+    order and, without compression, deep trees."""
+    p = rng.permutation(N).astype(np.int32)
+    idx = np.full((N, 2), -1, np.int32)
+    idx[p[:-1], 0] = p[1:]
+    idx[p[1:], 1] = p[:-1]
+    return idx
+
+
+def star(N, hub):
+    """Every row lists the hub (the hub itself too): one component whose links all land on one row."""
+    return np.full((N, 1), hub, np.int32)
+
+
+def graph(name, rng):
+    """-> (idx, labels or None, n_labels or None, row stride of the device copy) for a row of the table."""
+    if name == "n1_k1":
+        return np.array([[-1]], np.int32), None, None, 1
+    if name == "n1_k3_self_labelled":
+        return np.array([[0, -1, 0]], np.int32), np.array([0], np.int32), 1, 3
+    if name.startswith("random"):
+        _, N, k, nl = name.split("_")
+        N, k, nl = int(N), int(k[1:]), int(nl[1:])
+        labels = rng.integers(0, nl, N).astype(np.int32) if nl else None
+        return random_lists(rng, N, k), labels, nl or None, k
+    if name == "knn_12_labels":
+        X, t = generic(rng, 50000, 20)
+        idx, _ = knn(X.astype(np.float32), k=14)
+        return idx, t.astype(np.int32), 12, 14
+    if name == "shuffled_path_2p20":
+        return shuffled_path(rng, 1 << 20), None, None, 2
+    if name == "star_row_0":
+        return star(1 << 20, 0), None, None, 1
+    if name == "star_last_row":
+        return star(1 << 20, (1 << 20) - 1), None, None, 1
+    if name == "star_last_row_k4_labelled":
+        idx = np.concatenate([star(1 << 18, (1 << 18) - 1)] * 4, axis=1)
+        return idx, (np.arange(1 << 18) % 3 == 1).astype(np.int32), 2, 4   # the hub has label 0
+    if name == "all_missing":
+        return np.full((10000, 5), -1, np.int32), None, None, 5
+    if name == "self_only":
+        return np.repeat(np.arange(10000, dtype=np.int32)[:, None], 3, axis=1), None, None, 3
+    if name == "repeated_entries":
+        idx = np.repeat(rng.integers(0, 20000, (20000, 1)).astype(np.int32), 6, axis=1)
+        return idx, None, None, 6
+    if name == "alternating_labels_path":
+        N = 100001
+        idx = np.arange(1, N + 1, dtype=np.int32)[:, None]
+        idx[-1] = -1
+        return idx, (np.arange(N) % 2).astype(np.int32), 2, 1
+    if name == "one_label_per_row":
+        N = 30000
+        return random_lists(rng, N, 8), rng.permutation(N).astype(np.int32), N, 8
+    if name == "unused_codes":
+        N = 50000
+        return random_lists(rng, N, 6, 0.3), np.array([0, 3, 7])[rng.integers(0, 3, N)].astype(np.int32), 9, 6
+    if name == "strided_k14_ld17":
+        N = 40000
+        return random_lists(rng, N, 14, 0.8), rng.integers(0, 5, N).astype(np.int32), 5, 17
+    if name == "big_4M_k14":      # about one edge per row: a giant component and many small ones
+        return random_lists(rng, 1 << 22, 14, 0.93), None, None, 14
+    raise KeyError(name)
+
+
+ROWS = ["n1_k1", "n1_k3_self_labelled", "random_100000_k1_l0", "random_200000_k14_l0", "random_200000_k14_l20",
+        "random_50000_k64_l0", "random_50000_k64_l300", "knn_12_labels", "shuffled_path_2p20", "star_row_0",
+        "star_last_row", "star_last_row_k4_labelled", "all_missing", "self_only", "repeated_entries",
+        "alternating_labels_path", "one_label_per_row", "unused_codes", "strided_k14_ld17", "big_4M_k14"]
+
+
+def device_lists(idx, ld):
+    """idx on cuda:0 as a view of row stride ld >= k that ends exactly where its allocation does."""
+    import torch
+    N, k = idx.shape
+    buf = torch.full((N * ld - (ld - k),), -7, dtype=torch.int32, device="cuda:0")
+    view = torch.as_strided(buf, (N, k), (ld, 1))
+    view.copy_(torch.as_tensor(idx, device="cuda:0"))
+    return view
+
+
+@pytest.mark.parametrize("name", ROWS)
+def test_components_table(name):
+    import torch
+    rng = np.random.default_rng(sum(map(ord, name)))
+    idx, labels, n_labels, ld = graph(name, rng)
+    N, k = idx.shape
+    want_comp, want_largest = cr.components(idx, labels, n_labels)
+    it = device_lists(idx, ld)
+    assert ld == k or it.stride(0) == ld
+    lt = None if labels is None else torch.as_tensor(labels, device="cuda:0")
+    g = gpu_harmony()
+    comp, largest = g.graph_components(it, lt)
+    assert comp.is_cuda and comp.dtype == torch.int32 and largest.dtype == torch.int32
+    assert g.region_time("components")[1] == LAUNCHES == g.kernel_launches
+    comp, largest = comp.cpu().numpy(), largest.cpu().numpy()
+    np.testing.assert_array_equal(comp, want_comp)
+    np.testing.assert_array_equal(largest, want_largest[:len(largest)])
+    if n_labels is not None:
+        assert len(largest) == int(labels.max()) + 1 and (want_largest[len(largest):] == 0).all()
+    if name.startswith("star"):
+        assert (comp == comp.min()).all() if labels is None else largest.max() == N - N // 3
+    if name in ("all_missing", "self_only"):
+        assert (comp == np.arange(N)).all() and largest.tolist() == [1]
+    if name in ("alternating_labels_path", "one_label_per_row"):
+        assert (comp == np.arange(N)).all() and (largest == 1).all()
+    if name == "shuffled_path_2p20":
+        assert (comp == 0).all() and largest.tolist() == [N]
+    print(f"[components {name}] N={N} k={k} components {len(np.unique(comp))} largest {largest.max()}")
+
+
+@pytest.mark.parametrize("name", ["star_row_0", "star_last_row", "random_200000_k14_l0", "random_50000_k64_l300"])
+def test_two_calls_are_identical(name):
+    import torch
+    idx, labels, _, ld = graph(name, np.random.default_rng(5))
+    it = device_lists(idx, ld)
+    lt = None if labels is None else torch.as_tensor(labels, device="cuda:0")
+    g = gpu_harmony()
+    a = [t.cpu().numpy() for t in g.graph_components(it, lt)]
+    b = [t.cpu().numpy() for t in g.graph_components(it, lt)]
+    for u, v in zip(a, b):
+        np.testing.assert_array_equal(u, v)
+
+
+def test_host_and_any_labels():
+    """graph_components: host lists in -> numpy out, labels of any values folded in sorted order, as the device call."""
+    import torch
+    rng = np.random.default_rng(9)
+    idx = random_lists(rng, 20000, 5, 0.3)
+    names = np.array(["t9", "t1", "t5"])[rng.integers(0, 3, 20000)]
+    comp, largest = graph_components(idx, names)
+    assert isinstance(comp, np.ndarray) and comp.dtype == np.int32 and largest.shape == (3,)
+    codes = np.unique(names, return_inverse=True)[1]
+    want_comp, want_largest = cr.components(idx, codes, 3)
+    np.testing.assert_array_equal(comp, want_comp)
+    np.testing.assert_array_equal(largest, want_largest)
+    dcomp, dlargest = graph_components(torch.as_tensor(idx, device="cuda:0"),
+                                       torch.as_tensor(codes * 10 - 3, device="cuda:0"))
+    assert dcomp.is_cuda
+    np.testing.assert_array_equal(dcomp.cpu().numpy(), comp)
+    np.testing.assert_array_equal(dlargest.cpu().numpy(), largest)
+    comp1, largest1 = graph_components(idx)
+    np.testing.assert_array_equal(comp1, cr.components(idx)[0])
+    assert largest1.tolist() == cr.components(idx)[1].tolist()
+
+
+def _call(L, g, a):
+    return L.hb_graph_components(g._h, a["idx"], a["ld"], a["N"], a["k"], a["lab"], a["nl"], a["comp"], a["largest"],
+                                 None)
+
+
+def test_no_largest():
+    """largest NULL: comp only, four launches."""
+    import torch
+    from harmony_b200 import _lib
+    L = _lib.lib()
+    rng = np.random.default_rng(10)
+    idx = random_lists(rng, 30000, 4)
+    it = torch.as_tensor(idx, device="cuda:0")
+    comp = torch.empty(30000, dtype=torch.int32, device="cuda:0")
+    g = gpu_harmony()
+    assert L.hb_graph_components(g._h, ptr(it), 4, 30000, 4, None, 0, ptr(comp), None, None) == 0
+    assert g.region_time("components")[1] == LAUNCHES_NO_LARGEST == g.kernel_launches
+    np.testing.assert_array_equal(comp.cpu().numpy(), cr.components(idx)[0])
+
+
+def test_handle_state_untouched():
+    """knn and then components between cluster_cpp and moe_correct_ridge_cpp, and on a mapping handle before and after
+    hb_map: Z_corr, R and Y read bit for bit the same before and after the calls."""
+
+    def call(h, phase, data):
+        X = data.probe if phase != "mapped" else h.get_tensor("Z_corr")
+        codes = data.codes if phase != "mapped" else data.mapped_codes
+        idx, _ = h.knn(X, k=14)
+        comp, largest = h.graph_components(idx, codes)
+        assert comp.shape[0] == X.shape[0] and int(largest.max()) >= 1
+
+    handle_state_untouched(call)
+
+
+def test_refusals_launch_nothing():
+    import torch
+    from harmony_b200 import _lib
+    L = _lib.lib()
+    g = gpu_harmony()
+    dev = torch.device("cuda", 0)
+    N, k = 200, 4
+    idx = torch.zeros((N, k), dtype=torch.int32, device=dev)
+    lab = torch.zeros(N, dtype=torch.int32, device=dev)
+    comp = torch.zeros(N, dtype=torch.int32, device=dev)
+    largest = torch.zeros(N, dtype=torch.int32, device=dev)
+    host = np.zeros((N, k), np.int32)
+    H = host.ctypes.data_as(ctypes.c_void_p)
+    good = dict(idx=ptr(idx), ld=k, N=N, k=k, lab=ptr(lab), nl=3, comp=ptr(comp), largest=ptr(largest))
+    bad = [dict(N=0), dict(N=-1), dict(N=2 ** 31), dict(k=0), dict(k=-2), dict(ld=k - 1), dict(nl=0), dict(nl=-1),
+           dict(nl=N + 1), dict(idx=None), dict(comp=None), dict(idx=H), dict(comp=H), dict(lab=H), dict(largest=H)]
+    refusals_launch_nothing(g, lambda a: _call(L, g, a), good, bad)
+    assert _call(L, g, dict(good, lab=None, nl=0)) == 0       # n_labels is ignored without labels
+    assert g.kernel_launches == LAUNCHES
+
+
+@pytest.mark.parametrize("case", ["below_minus_1", "past_N", "label_negative", "label_past_n_labels"])
+def test_range_refusals(case):
+    """A bad entry or code: status 2 naming the row and entry, comp and largest unwritten, only the check launched."""
+    import torch
+    from harmony_b200 import _lib
+    L = _lib.lib()
+    rng = np.random.default_rng(11)
+    N, k, ld = 5000, 6, 9
+    idx = random_lists(rng, N, k)
+    labels = rng.integers(0, 4, N).astype(np.int32)
+    if case == "below_minus_1":
+        idx[4000, 5], idx[4321, 0] = -2, -5
+        msg = "hb_graph_components: idx[4000][5] = -2 is not -1 or a row in 0..4999"
+    elif case == "past_N":
+        idx[1234, 2], idx[1234, 4], idx[3000, 0] = N, N + 7, 2 ** 31 - 1
+        msg = "hb_graph_components: idx[1234][2] = 5000 is not -1 or a row in 0..4999"
+    elif case == "label_negative":
+        labels[2500], idx[2600, 1] = -1, -3
+        msg = "hb_graph_components: labels[2500] = -1 is not a code in 0..3"
+    else:
+        labels[17], labels[18] = 4, 9
+        idx[17, 5] = N     # the entry comes before the label in the row's order
+        msg = "hb_graph_components: idx[17][5] = 5000 is not -1 or a row in 0..4999"
+    it = device_lists(idx, ld)
+    lt = torch.as_tensor(labels, device="cuda:0")
+    comp = torch.full((N,), -9, dtype=torch.int32, device="cuda:0")
+    largest = torch.full((4,), -9, dtype=torch.int32, device="cuda:0")
+    g = gpu_harmony()
+    st = L.hb_graph_components(g._h, ptr(it), ld, N, k, ptr(lt), 4, ptr(comp), ptr(largest), None)
+    assert st == 2 and L.hb_last_error(g._h).decode() == msg
+    assert g.kernel_launches == 1 == g.region_time("components")[1]
+    assert (comp.cpu().numpy() == -9).all() and (largest.cpu().numpy() == -9).all()
+
+
+def test_stream_order():
+    """idx written by torch on the current stream just before the call, behind a long sleep: the call reads it after."""
+    import torch
+    rng = np.random.default_rng(12)
+    idx = shuffled_path(rng, 1 << 18)
+    src = torch.as_tensor(idx, device="cuda:0")
+    s = torch.cuda.Stream()
+    g = gpu_harmony()
+    with torch.cuda.stream(s):
+        dst = torch.full_like(src, -1)
+        torch.cuda._sleep(200_000_000)
+        dst.copy_(src)
+        comp, largest = g.graph_components(dst)
+        comp, largest = comp.cpu().numpy(), largest.cpu().numpy()
+    assert (comp == 0).all() and largest.tolist() == [1 << 18]
+
+
+def shifted_types(seed=0, n=20000, d=20):
+    """8 cell types at scale 6, 4 batch shifts at scale 2, unit noise -> (X, X without the shifts, types, batches)."""
+    rng = np.random.default_rng(seed)
+    M = rng.standard_normal((8, d)) * 6
+    S = rng.standard_normal((4, d)) * 2
+    t = rng.integers(0, 8, n)
+    b = rng.integers(0, 4, n)
+    noise = rng.standard_normal((n, d))
+    return M[t] + S[b] + noise, M[t] + noise, t, b
+
+
+def test_graph_connectivity_end_to_end():
+    """Graph connectivity of cell types in the 15-neighbour graph: 0.2597 on the input, whose 4 batch shifts split
+    every type, and 1.0 with the shifts removed (both computed in fp64 with cKDTree + scipy).  It must rise after
+    RunHarmony.  The CPU oracle's integration of the same input (default parameters, 3 and 4 rounds at two seeds),
+    scored with the restatement, gives 1.0000 at both seeds; the bar is that 1.0000 less a margin of 0.05."""
+    import torch
+    X, X0, t, b = shifted_types()
+    meta = {"type": t, "batch": b}
+    before, per = graph_connectivity(X, meta, "type", return_all=True)
+    assert set(per) == set(range(8))
+    idx, _ = knn(X, k=14)
+    _, largest = cr.components(idx, t, 8)
+    own = cr.connectivity_fold(largest, np.bincount(t))
+    assert before == own
+    assert per == {i: largest[i] / np.bincount(t)[i] for i in range(8)}
+    fp64 = cr.connectivity_fold(cr.components(cr.knn_idx(X, 15), t, 8)[1], np.bincount(t))
+    assert abs(before - fp64) < 0.01
+    Xd = torch.as_tensor(X, device="cuda:0")
+    assert graph_connectivity(Xd, {"type": torch.as_tensor(t, device="cuda:0")}, "type") == before
+    assert graph_connectivity(X0, meta, "type") == 1.0
+    Zc = RunHarmony(Xd, meta, "batch", verbose=False, seed=1)
+    after = graph_connectivity(Zc, meta, "type")
+    print(f"[components end to end] graph connectivity {before:.4f} (fp64 lists {fp64:.4f}) -> {after:.4f}")
+    assert after > before
+    assert after >= 0.95
