@@ -7,6 +7,7 @@ loudly if it is missing (there is no CPU fallback).
 """
 from .graph import graph_components, graph_connectivity  # noqa: F401
 from .harmony_option import harmony_options  # noqa: F401
+from .kbet import kbet  # noqa: F401
 from .lisi import compute_lisi  # noqa: F401
 from .mapping import HarmonyReference  # noqa: F401
 from .neighbors import TransferLabels, knn  # noqa: F401

@@ -41,6 +41,7 @@
 #include "lisi.cuh"
 #include "silhouette.cuh"
 #include "components.cuh"
+#include "kbet.cuh"
 
 #include "select.cuh"
 #include "handle.cuh"
@@ -366,6 +367,7 @@ int harmony_step(hb_handle* h, const char* what, bool needs_init = true) {
 #include "lisi_host.cuh"
 #include "silhouette_host.cuh"
 #include "components_host.cuh"
+#include "kbet_host.cuh"
 
 // =================================================================================================
 extern "C" {
@@ -558,6 +560,14 @@ int hb_graph_components(hb_handle* h, const int32_t* idx, int64_t idx_ld, int64_
                         int n_labels, int32_t* comp, int32_t* largest, void* stream) {
   if (!h) return 1;
   return run_components(h, idx, idx_ld, N, k, labels, n_labels, comp, largest, (cudaStream_t)stream);
+}
+
+int hb_kbet(hb_handle* h, const void* X, int x_dtype, int64_t x_ld, int64_t N, int d, const int32_t* batches,
+            int n_batches, const int32_t* labels, int n_labels, int k0, double* stat, double* pval, int32_t* k0_out,
+            int32_t* idx, int64_t idx_ld, void* stream) {
+  if (!h) return 1;
+  return run_kbet(h, DevRows{X, x_dtype, x_ld, N}, d, batches, n_batches, labels, n_labels, k0, stat, pval, k0_out, idx,
+                  idx_ld, (cudaStream_t)stream);
 }
 
 int hb_init_cluster(hb_handle* h, const double* Y0) {
@@ -996,6 +1006,13 @@ int hb_debug_lisi_geometry(int d, double perplexity, int64_t N, int num_sms, int
 int hb_debug_silhouette_geometry(int d, int64_t N, int num_sms, int64_t out[8]) {
   if (sil_check_shape(nullptr, N, d) != 0 || num_sms < 1) return 2;
   sil_geometry_record(d, N, num_sms, out);
+  return 0;
+}
+
+// kBET's p-value function (test hook, host only): the chi2_sf k_kbet runs.  Status 2 (out untouched) for dof < 1.
+int hb_debug_chi2_sf(double x, int dof, double* out) {
+  if (dof < 1 || !out) return 2;
+  *out = chi2_sf(x, dof);
   return 0;
 }
 

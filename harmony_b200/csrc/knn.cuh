@@ -8,11 +8,15 @@
 //                  accumulator registers: a thread compares its fragment with its rows' thresholds (the k-th best so
 //                  far); survivors go to a per-row candidate buffer which the row's warp folds into the row's sorted
 //                  list.  A query row's fragments all lie in one warp (umma::frag_row), so lists need no CTA barrier.
+//                  GROUPED (hb_kbet): a CTA takes its query rows [r0, r1) and its reference rows [g0, g1) from a tile
+//                  record, one reference split, and every row number is a position in the caller's sorted order.
 //   k_knn_merge    per query row: the direct fp32 distance of every listed candidate of every reference split, the k
 //                  smallest in ascending order.
 // Operand pipeline as in logits_tc.cuh: per-thread 16-byte cp.async into the canonical K-major layout, the raw tile is
 // the `hi` operand, the `lo` pieces are written once the copies have landed.
 #pragma once
+#include <type_traits>
+
 #include "common.cuh"
 #include "umma.cuh"
 
@@ -108,6 +112,10 @@ struct KnnArgs {
   int KD, k, stages, exclude_self;
   int64_t tiles_per_split;
 };
+// The grouped sweep's arguments: KnnArgs (Nq, Nx and tiles_per_split unused) and the tile records
+struct KnnGroupArgs : KnnArgs {
+  const int4* tiles;  // {first query row, end query row, first reference row, end reference row}
+};
 
 // (score, row) a before (score, row) b in a list: larger score, then smaller row
 __device__ __forceinline__ bool knn_before(float sa, int ia, float sb, int ib) { return sa > sb || (sa == sb && ia < ib); }
@@ -151,9 +159,9 @@ __device__ __noinline__ float knn_fold(float* ls, int* li, const float* bs, cons
 }
 
 // grid = (query tiles, reference splits), 2 TQ threads: warpgroup g multiplies query rows [64 g, 64 g + 64) of the tile.
-// E: list entries per lane, k <= 32 E (2 for hb_knn's k <= 64, 4 up to KNN_SWEEP_MAX_K)
-template <int TQ, int E>
-__global__ void __launch_bounds__(2 * TQ, 1) k_knn_tc(KnnArgs a) {
+// E: list entries per lane, k <= 32 E (2 for hb_knn's k <= 64, 4 up to KNN_SWEEP_MAX_K).  GROUPED: grid = tile records.
+template <int TQ, int E, bool GROUPED = false>
+__global__ void __launch_bounds__(2 * TQ, 1) k_knn_tc(std::conditional_t<GROUPED, KnnGroupArgs, KnnArgs> a) {
   constexpr int TN = KNN_TN;
   constexpr int THREADS = 2 * TQ, NACC = TN / 2, NG = TN / 8, NCH = TN / 16;
   extern __shared__ __align__(128) unsigned char smem_raw[];
@@ -171,23 +179,29 @@ __global__ void __launch_bounds__(2 * TQ, 1) k_knn_tc(KnnArgs a) {
   int* buf_i = reinterpret_cast<int*>(buf_s + (size_t)TQ * KNN_CAP);
   float* stage = reinterpret_cast<float*>(buf_i + (size_t)TQ * KNN_CAP);  // [warps][16][KNN_SS]  a chunk of scores
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, wg = warp >> 2, w4 = warp & 3;
-  const int64_t q0 = (int64_t)blockIdx.x * TQ;
-  const int64_t xtiles = (a.Nx + TN - 1) / TN;
-  const int64_t t_begin = (int64_t)blockIdx.y * a.tiles_per_split;
-  const int64_t t_end = t_begin + a.tiles_per_split < xtiles ? t_begin + a.tiles_per_split : xtiles;
+  int64_t q0, q_end, x0, x_end;  // query rows [q0, q_end) of this CTA (q_end: a bound, not the tile's end) and the reference's
+  if constexpr (GROUPED) {
+    const int4 tile = a.tiles[blockIdx.x];
+    q0 = tile.x, q_end = tile.y, x0 = tile.z, x_end = tile.w;
+  } else {
+    q0 = (int64_t)blockIdx.x * TQ, q_end = a.Nq, x0 = 0, x_end = a.Nx;
+  }
+  const int64_t xtiles = (x_end - x0 + TN - 1) / TN;
+  const int64_t t_begin = GROUPED ? 0 : (int64_t)blockIdx.y * a.tiles_per_split;
+  const int64_t t_end = GROUPED ? xtiles : t_begin + a.tiles_per_split < xtiles ? t_begin + a.tiles_per_split : xtiles;
 
   // reference tile t -> stage buffer (row per thread, one 16-byte piece per chunk) and its hx
   auto issue = [&](int64_t t) {
     float* dst = Braw + (size_t)(S == 2 ? (t & 1) : 0) * TN * KD;
     const int r = tid % TN;
-    const int64_t j = t * TN + r;
-    if (j < a.Nx) {
+    const int64_t j = x0 + t * TN + r;
+    if (j < x_end) {
       const float* src = a.Xp + (size_t)j * KD;
       const unsigned d0 = umma::smem_u32(dst + (size_t)r * 4);
       for (int c = tid / TN; c < KD4; c += THREADS / TN)
         asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(d0 + (unsigned)c * (TN * 16u)), "l"(src + 4 * c) : "memory");
     }
-    if (tid < TN) hxs[(t & 1) * TN + tid] = j < a.Nx ? a.hx[j] : KNN_INF;  // rows past Nx score -inf (or NaN)
+    if (tid < TN) hxs[(t & 1) * TN + tid] = j < x_end ? a.hx[j] : KNN_INF;  // rows past the end score -inf (or NaN)
     asm volatile("cp.async.commit_group;" ::: "memory");
   };
   if (t_begin < t_end) issue(t_begin);
@@ -195,7 +209,7 @@ __global__ void __launch_bounds__(2 * TQ, 1) k_knn_tc(KnnArgs a) {
   for (int i = tid; i < TQ * KD4; i += THREADS) {
     const int r = i % TQ, c = i / TQ;
     float4 z = make_float4(0.f, 0.f, 0.f, 0.f), l4;
-    if (q0 + r < a.Nq) z = *reinterpret_cast<const float4*>(a.Qp + (size_t)(q0 + r) * KD + 4 * c);
+    if (q0 + r < q_end) z = *reinterpret_cast<const float4*>(a.Qp + (size_t)(q0 + r) * KD + 4 * c);
     // the tensor core reads trunc_tf32(z); the remainder is exact in fp32 and is rounded to tf32 here
     l4.x = umma::round_tf32(z.x - __uint_as_float(__float_as_uint(z.x) & 0xffffe000u));
     l4.y = umma::round_tf32(z.y - __uint_as_float(__float_as_uint(z.y) & 0xffffe000u));
@@ -257,7 +271,7 @@ __global__ void __launch_bounds__(2 * TQ, 1) k_knn_tc(KnnArgs a) {
     }
 
     // ---- selection: score = q.x - hx against the rows' thresholds ----
-    const int64_t j0 = t * TN;
+    const int64_t j0 = x0 + t * TN;
     const float* hxt = hxs + (t & 1) * TN;
     const float t0 = thr[row0], t1 = thr[row1];
 #pragma unroll
@@ -338,7 +352,7 @@ __global__ void __launch_bounds__(2 * TQ, 1) k_knn_tc(KnnArgs a) {
     const int nb = cnt[r];
     if (nb > 0) knn_fold<E>(lst_s + (size_t)r * k, lst_i + (size_t)r * k, buf_s + r * KNN_CAP, buf_i + r * KNN_CAP, nb, k, lane);
     __syncwarp();
-    if (q0 + r < a.Nq) {
+    if (q0 + r < q_end) {
       const size_t o = ((size_t)(q0 + r) * gridDim.y + blockIdx.y) * k;
       for (int e = lane; e < k; e += 32) a.part_i[o + e] = lst_i[(size_t)r * k + e];
     }

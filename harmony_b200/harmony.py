@@ -218,6 +218,15 @@ class harmony:
         from .graph import components_on
         return components_on(self, idx, labels)
 
+    def kbet(self, X, batches, labels=None, k0=0, return_neighbors=False):
+        """kBET's per-cell test of every row of ``X`` [N, d] (host array or CUDA tensor) with the batch codes ``batches``
+        and, within each label of ``labels`` (both dense codes 0..n-1, [N]; numpy or int32 CUDA tensors; no labels: one
+        label), ``k0`` = 0 for scib's rule or a fixed 2..129, on this object's device and stream -> ``(stat, pval, k0)``,
+        with ``return_neighbors`` also ``idx``.  ``harmony_b200.kbet`` takes labels by column name and folds the score.
+        Works in any state of the object and changes none of it."""
+        from .kbet import kbet_on
+        return kbet_on(self, X, batches, labels, k0, return_neighbors)
+
     def _device_Phi(self, Phi):
         """An [N] or [N, C] int32 / int64 CUDA tensor -> contiguous [N, C] int32 on the object's device (converted, if
         need be, on the current torch stream, which hb_setup_device orders its read after)."""

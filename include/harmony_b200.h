@@ -44,8 +44,8 @@ const char* hb_last_error(const hb_handle* h);
 int hb_pop_warning(hb_handle* h, char* buf, size_t cap);
 /* Library/ABI version: major*10000 + minor*100 + patch (0.3.0: labels in device memory; 0.4.0: mapping a query onto
  * a reference, hb_reference / hb_map_setup / hb_map).  hb_knn, hb_debug_knn_geometry, hb_lisi,
- * hb_debug_lisi_geometry, hb_silhouette, hb_debug_silhouette_geometry and hb_graph_components were added without
- * moving the number. */
+ * hb_debug_lisi_geometry, hb_silhouette, hb_debug_silhouette_geometry, hb_graph_components, hb_kbet and
+ * hb_debug_chi2_sf were added without moving the number. */
 int hb_version(void);
 
 /* ---- multi-GPU (one process per GPU; cells sharded contiguously; SURVEY §8e) ------------------- */
@@ -219,6 +219,30 @@ int hb_debug_silhouette_geometry(int d, int64_t N, int num_sms, int64_t out[8]);
  * handle's state untouched; on a sharded handle the call is local.  Region "components". */
 int hb_graph_components(hb_handle* h, const int32_t* idx, int64_t idx_ld, int64_t N, int k, const int32_t* labels,
                         int n_labels, int32_t* comp, int32_t* largest, void* stream);
+/* kBET (DESIGN.md §13): for every row of X [N, d], a chi-square test of the batches among the row and its k0 - 1 nearest
+ * other rows of its label against the label's batch frequencies.  batches: int32 codes 0..n_batches-1; labels (NULL:
+ * one label): int32 codes 0..n_labels-1; both device arrays of N codes.  Only finite rows take part, as in
+ * hb_silhouette.  Per label l with n_l finite rows, n_{l,b} of them in batch b and B_l batches with n_{l,b} > 0: not
+ * tested when n_l < 10, B_l = 1 or (fixed k0) n_l < k0; else k0_l = k0, or for k0 = 0 scib's rule min(70, max(10,
+ * floor(n_l / B_l / 4))), lowered to floor((2^31 - 1) / n_l) where k0_l n_l would reach 2^31 - 1.  For a finite row i of
+ * a tested label: the row and its k0_l - 1 nearest other finite rows of its label by Euclidean distance (hb_knn's search
+ * and band), o_b their batch counts, stat[i] = sum_b (o_b - k0_l p_b)^2 / (k0_l p_b) with p_b = n_{l,b} / n_l, and
+ * pval[i] = Q((B_l - 1) / 2, stat[i] / 2), the chi-square upper tail with B_l - 1 degrees of freedom, in fp64.  Other
+ * rows get NaN.  stat and pval [N] fp64 in the caller's order; k0_out (NULL: skipped) [n_labels] (1 without labels),
+ * 0 for a label not tested; idx (NULL: skipped) [N][idx_ld] int32: a tested row's k0_l - 1 neighbours (caller's rows)
+ * by ascending distance, -1 after them and for every other row.  X of x_dtype (hb_dtype) with row stride x_ld >= d.
+ * Limits, status 2 with a message before any launch: 2 <= N < 2^31, 1 <= d <= 128, n_batches >= 1, n_labels >= 1 when
+ * labels are given, n_batches and n_labels <= N, k0 = 0 or 2 <= k0 <= 129, an unknown dtype, a row stride < d, a NULL
+ * (X, batches, stat, pval), host or other-device pointer.  Status 2 after the index pass, before any output is written:
+ * a code out of range (naming the cell), more than 1e6 (label, batch) pairs, idx_ld below the largest k0_l - 1.
+ * Ordered on `stream` like hb_knn; needs no setup and leaves a Harmony or mapping handle's state untouched; on a
+ * sharded handle the call is local; two calls give bit-identical results.  Region "kbet". */
+int hb_kbet(hb_handle* h, const void* X, int x_dtype, int64_t x_ld, int64_t N, int d, const int32_t* batches,
+            int n_batches, const int32_t* labels, int n_labels, int k0, double* stat, double* pval, int32_t* k0_out,
+            int32_t* idx, int64_t idx_ld, void* stream);
+/* Test hook (host only): the p-value function of hb_kbet, the chi-square upper tail of x with dof degrees of freedom,
+ * into *out.  Returns 0, or 2 with out untouched for dof < 1. */
+int hb_debug_chi2_sf(double x, int dof, double* out);
 
 /* ---- fields / getters (harmony.cpp:640-669, 675-696) ------------------------------------------- */
 enum hb_field {
