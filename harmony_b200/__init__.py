@@ -11,6 +11,7 @@ from .kbet import kbet  # noqa: F401
 from .lisi import compute_lisi  # noqa: F401
 from .mapping import HarmonyReference  # noqa: F401
 from .neighbors import TransferLabels, knn  # noqa: F401
+from .pcr import pcr, pcr_comparison  # noqa: F401
 from .silhouette import silhouette_batch, silhouette_label, silhouette_samples  # noqa: F401
 from .ui import MapQuery, RunHarmony, prepare_inputs  # noqa: F401
 from .utils import HarmonyConvergencePlot, harmonize  # noqa: F401

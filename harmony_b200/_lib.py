@@ -84,6 +84,8 @@ def lib():
     L.hb_graph_components.argtypes = [P, P, I64, I64, I, P, I, P, P, P]
     L.hb_kbet.argtypes = [P, P, I, I64, I64, I, P, I, P, I, I, P, P, P, P, I64, P]
     L.hb_debug_chi2_sf.argtypes = [D, I, ctypes.POINTER(D)]
+    L.hb_pcr.argtypes = [P, P, I, I64, I64, I, P, I, I, P, P, P, P, P]
+    L.hb_debug_sym_eig.argtypes = [I, P, P, P]
     L.hb_init_cluster.argtypes = [P, P]
     L.hb_cluster.argtypes = [P, P]
     L.hb_moe_correct_ridge.argtypes = [P]

@@ -42,6 +42,7 @@
 #include "silhouette.cuh"
 #include "components.cuh"
 #include "kbet.cuh"
+#include "pcr.cuh"
 
 #include "select.cuh"
 #include "handle.cuh"
@@ -368,6 +369,7 @@ int harmony_step(hb_handle* h, const char* what, bool needs_init = true) {
 #include "silhouette_host.cuh"
 #include "components_host.cuh"
 #include "kbet_host.cuh"
+#include "pcr_host.cuh"
 
 // =================================================================================================
 extern "C" {
@@ -568,6 +570,13 @@ int hb_kbet(hb_handle* h, const void* X, int x_dtype, int64_t x_ld, int64_t N, i
   if (!h) return 1;
   return run_kbet(h, DevRows{X, x_dtype, x_ld, N}, d, batches, n_batches, labels, n_labels, k0, stat, pval, k0_out, idx,
                   idx_ld, (cudaStream_t)stream);
+}
+
+int hb_pcr(hb_handle* h, const void* X, int x_dtype, int64_t x_ld, int64_t N, int d, const int32_t* batches,
+           int n_batches, int n_comps, double* var, double* r2, double* components, double* score, void* stream) {
+  if (!h) return 1;
+  return run_pcr(h, DevRows{X, x_dtype, x_ld, N}, d, batches, n_batches, n_comps, var, r2, components, score,
+                 (cudaStream_t)stream);
 }
 
 int hb_init_cluster(hb_handle* h, const double* Y0) {
@@ -1013,6 +1022,14 @@ int hb_debug_silhouette_geometry(int d, int64_t N, int num_sms, int64_t out[8]) 
 int hb_debug_chi2_sf(double x, int dof, double* out) {
   if (dof < 1 || !out) return 2;
   *out = chi2_sf(x, dof);
+  return 0;
+}
+
+// hb_pcr's eigensolver (test hook, host only) on the symmetric n x n matrix A.  Status 2 (outputs untouched) for n
+// outside 1..128 or a null pointer.
+int hb_debug_sym_eig(int n, const double* A, double* w, double* V) {
+  if (n < 1 || n > KNN_MAX_D || !A || !w || !V) return 2;
+  sym_eig(n, A, w, V);
   return 0;
 }
 

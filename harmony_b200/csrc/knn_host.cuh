@@ -4,21 +4,25 @@
 
 namespace {
 
-// The scratch of the score calls (hb_knn, hb_lisi, hb_silhouette, hb_graph_components, hb_kbet), shared by them: each runs on h->stream, and a buffer
+// The scratch of the score calls (hb_knn, hb_lisi, hb_silhouette, hb_graph_components, hb_kbet, hb_pcr), shared by them: each runs on h->stream, and a buffer
 // that grows is freed only after the device has drained.  Every buffer grows on demand and is kept for the next call.
 struct ScoreScratch {
   DevBuf<float> rows, query_rows, hx;  // prepared rows [n][KD] of X and of Q, |x - c|^2 / 2 (or |x|^2 / 2)
-  DevBuf<double> centre;               // [KNN_MAX_D] column sums of X
+  DevBuf<double> centre;               // [KNN_MAX_D] column sums of X; pcr: its column means
   DevBuf<int> part;                    // knn, kbet: [Nq][splits][k] listed candidates
   DevBuf<int32_t> idx;                 // lisi: the neighbour lists when the caller passes no idx / dist; kbet: the lists
   DevBuf<float> dist;
   DevBuf<int> phi;                     // silhouette, kbet: [N][2] (group, label) levels
-  DevBuf<int> sort_perm, inv_sort;     // silhouette, kbet: the rows sorted by (group, label)
-  DevBuf<int> pstart, count;           // silhouette, kbet: [J + 1] pair starts, [J] finite rows per pair
+  DevBuf<int> sort_perm, inv_sort;     // silhouette, kbet: the rows sorted by (group, label); pcr: by batch
+  DevBuf<int> pstart, count;           // silhouette, kbet, pcr: [J + 1] pair (batch) starts, [J] finite rows of each
   DevBuf<int4> tiles;                  // silhouette, kbet: the sweep's tiles
   DevBuf<int> sizes;                   // components: [N] rows per root
   DevBuf<unsigned long long> bad;      // components: the range pass's smallest bad entry
   DevBuf<KbetPair> kbet_pairs;         // kbet: [J] each pair's label's k0, rows, degrees of freedom and pair range
+  DevBuf<double> pcr_rows;             // pcr: [J][d] each batch's column sums, then its between-batch row
+  DevBuf<double> pcr_edge;             // pcr: [3][chunks][d] the head, tail and total piece of each chunk of rows
+  DevBuf<int> pcr_edge_n;              // pcr: [3][chunks] their finite rows
+  DevBuf<double> pcr_part, pcr_out;    // pcr: the Grams' per-CTA partials; the covariance, the scatter and n
 };
 ScoreScratch& score_scratch(hb_handle* h) {
   if (!h->scores) h->scores.reset(new ScoreScratch());

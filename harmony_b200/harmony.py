@@ -227,6 +227,14 @@ class harmony:
         from .kbet import kbet_on
         return kbet_on(self, X, batches, labels, k0, return_neighbors)
 
+    def pcr(self, X, batches, n_comps=50):
+        """Principal component regression of ``X`` [N, d] (host array or CUDA tensor) on the batch codes ``batches``
+        (dense codes 0..n-1, [N]; numpy or an int32 CUDA tensor) on this object's device and stream -> ``(var, r2,
+        components, score)`` of the min(n_comps, N, d) leading components.  ``harmony_b200.pcr`` takes the batches by
+        column name.  Works in any state of the object and changes none of it."""
+        from .pcr import pcr_on
+        return pcr_on(self, X, batches, n_comps)
+
     def _device_Phi(self, Phi):
         """An [N] or [N, C] int32 / int64 CUDA tensor -> contiguous [N, C] int32 on the object's device (converted, if
         need be, on the current torch stream, which hb_setup_device orders its read after)."""

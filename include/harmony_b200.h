@@ -44,8 +44,8 @@ const char* hb_last_error(const hb_handle* h);
 int hb_pop_warning(hb_handle* h, char* buf, size_t cap);
 /* Library/ABI version: major*10000 + minor*100 + patch (0.3.0: labels in device memory; 0.4.0: mapping a query onto
  * a reference, hb_reference / hb_map_setup / hb_map).  hb_knn, hb_debug_knn_geometry, hb_lisi,
- * hb_debug_lisi_geometry, hb_silhouette, hb_debug_silhouette_geometry, hb_graph_components, hb_kbet and
- * hb_debug_chi2_sf were added without moving the number. */
+ * hb_debug_lisi_geometry, hb_silhouette, hb_debug_silhouette_geometry, hb_graph_components, hb_kbet,
+ * hb_debug_chi2_sf, hb_pcr and hb_debug_sym_eig were added without moving the number. */
 int hb_version(void);
 
 /* ---- multi-GPU (one process per GPU; cells sharded contiguously; SURVEY §8e) ------------------- */
@@ -243,6 +243,27 @@ int hb_kbet(hb_handle* h, const void* X, int x_dtype, int64_t x_ld, int64_t N, i
 /* Test hook (host only): the p-value function of hb_kbet, the chi-square upper tail of x with dof degrees of freedom,
  * into *out.  Returns 0, or 2 with out untouched for dof < 1. */
 int hb_debug_chi2_sf(double x, int dof, double* out);
+/* Principal component regression (DESIGN.md §14): the share of X's variance that its batches explain, scib's pcr.
+ * X [N, d] of x_dtype (hb_dtype) with row stride x_ld >= d; batches: int32 device codes 0..n_batches-1, one per row.
+ * Only finite rows take part (n of them, n_b in batch b).  With m the column mean over finite rows and
+ * C = sum (x - m)(x - m)^T, the components are C's m_c = min(n_comps, N, d) leading eigenpairs (lambda_j, v_j) in
+ * descending order, v_j's entry of largest magnitude positive (the first on a tie); var[j] = lambda_j / (n - 1),
+ * components[j][.] = v_j, and r2[j] = sum_b (S_b . v_j)^2 / n_b / lambda_j clamped to [0, 1] with
+ * S_b = sum over batch b of (x - m): the R^2 of regressing PC j on the one-hot batches.  r2[j] = 0 when
+ * lambda_j <= d eps lambda_1 or fewer than two batches have finite rows.  score = sum_j r2[j] lambda_j / sum_j lambda_j.
+ * n < 2: var, r2 and score are NaN; sum_j lambda_j = 0: score is NaN.  Outputs are fp64 device arrays: var and r2
+ * [m_c], components [m_c][d] (NULL: skipped), score [1].  Limits, status 2 with a message before any launch:
+ * 2 <= N < 2^31, 1 <= d <= 128, 1 <= n_batches <= N, n_comps >= 1, an unknown dtype, a row stride < d, a NULL (X,
+ * batches, var, r2, score), host or other-device pointer.  Status 2 after the index pass, before any output is
+ * written: a batch code out of range (naming the cell).  Ordered on `stream` like hb_knn; needs no setup and leaves a
+ * Harmony or mapping handle's state untouched; on a sharded handle the call is local; two calls give bit-identical
+ * results.  Region "pcr". */
+int hb_pcr(hb_handle* h, const void* X, int x_dtype, int64_t x_ld, int64_t N, int d, const int32_t* batches,
+           int n_batches, int n_comps, double* var, double* r2, double* components, double* score, void* stream);
+/* Test hook (host only): hb_pcr's eigensolver on the symmetric n x n host matrix A (row-major, upper triangle read):
+ * the eigenvalues in descending order into w [n] and V [n][n] row-major with column j the unit eigenvector of w[j],
+ * signed as hb_pcr's components.  Returns 0, or 2 with the outputs untouched for n outside 1..128. */
+int hb_debug_sym_eig(int n, const double* A, double* w, double* V);
 
 /* ---- fields / getters (harmony.cpp:640-669, 675-696) ------------------------------------------- */
 enum hb_field {
