@@ -5,6 +5,7 @@ class); all arithmetic on cell matrices runs in hand-written CUDA behind include
 Importing this package does not load the CUDA library; constructing ``harmony`` does, and fails
 loudly if it is missing (there is no CPU fallback).
 """
+from .clustering import kmeans, nmi_ari, nmi_ari_cluster_labels_kmeans  # noqa: F401
 from .graph import graph_components, graph_connectivity  # noqa: F401
 from .harmony_option import harmony_options  # noqa: F401
 from .kbet import kbet  # noqa: F401

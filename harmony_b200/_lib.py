@@ -86,6 +86,7 @@ def lib():
     L.hb_debug_chi2_sf.argtypes = [D, I, ctypes.POINTER(D)]
     L.hb_pcr.argtypes = [P, P, I, I64, I64, I, P, I, I, P, P, P, P, P]
     L.hb_debug_sym_eig.argtypes = [I, P, P, P]
+    L.hb_kmeans.argtypes = [P, P, I, I64, I64, I, I, ctypes.c_uint64, I, I, D, P, P, P, P, P, P]
     L.hb_init_cluster.argtypes = [P, P]
     L.hb_cluster.argtypes = [P, P]
     L.hb_moe_correct_ridge.argtypes = [P]

@@ -43,6 +43,7 @@
 #include "components.cuh"
 #include "kbet.cuh"
 #include "pcr.cuh"
+#include "kmeans_score.cuh"
 
 #include "select.cuh"
 #include "handle.cuh"
@@ -370,6 +371,7 @@ int harmony_step(hb_handle* h, const char* what, bool needs_init = true) {
 #include "components_host.cuh"
 #include "kbet_host.cuh"
 #include "pcr_host.cuh"
+#include "kmeans_score_host.cuh"
 
 // =================================================================================================
 extern "C" {
@@ -577,6 +579,14 @@ int hb_pcr(hb_handle* h, const void* X, int x_dtype, int64_t x_ld, int64_t N, in
   if (!h) return 1;
   return run_pcr(h, DevRows{X, x_dtype, x_ld, N}, d, batches, n_batches, n_comps, var, r2, components, score,
                  (cudaStream_t)stream);
+}
+
+int hb_kmeans(hb_handle* h, const void* X, int x_dtype, int64_t x_ld, int64_t N, int d, int K, uint64_t seed,
+              int n_init, int max_iter, double tol, int32_t* labels, double* centres, double* inertia, int32_t* n_iter,
+              int32_t* seeds, void* stream) {
+  if (!h) return 1;
+  return run_kmeans(h, DevRows{X, x_dtype, x_ld, N}, d, K, seed, n_init, max_iter, tol, labels, centres, inertia, n_iter,
+                    seeds, (cudaStream_t)stream);
 }
 
 int hb_init_cluster(hb_handle* h, const double* Y0) {

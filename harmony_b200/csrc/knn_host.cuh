@@ -4,7 +4,7 @@
 
 namespace {
 
-// The scratch of the score calls (hb_knn, hb_lisi, hb_silhouette, hb_graph_components, hb_kbet, hb_pcr), shared by them: each runs on h->stream, and a buffer
+// The scratch of the score calls (hb_knn, hb_lisi, hb_silhouette, hb_graph_components, hb_kbet, hb_pcr, hb_kmeans), shared by them: each runs on h->stream, and a buffer
 // that grows is freed only after the device has drained.  Every buffer grows on demand and is kept for the next call.
 struct ScoreScratch {
   DevBuf<float> rows, query_rows, hx;  // prepared rows [n][KD] of X and of Q, |x - c|^2 / 2 (or |x|^2 / 2)
@@ -23,6 +23,13 @@ struct ScoreScratch {
   DevBuf<double> pcr_edge;             // pcr: [3][chunks][d] the head, tail and total piece of each chunk of rows
   DevBuf<int> pcr_edge_n;              // pcr: [3][chunks] their finite rows
   DevBuf<double> pcr_part, pcr_out;    // pcr: the Grams' per-CTA partials; the covariance, the scatter and n
+  DevBuf<unsigned char> km_fin;        // kmeans: [N] whether each row is finite
+  DevBuf<double> km_d2, km_part;       // kmeans: [N] the seeding's D^2; per-CTA partials
+  DevBuf<double> km_centres;           // kmeans: [2][K][d] the current and the next centres
+  DevBuf<int32_t> km_labels;           // kmeans: [2][N] this and the previous iteration's labels
+  DevBuf<int> km_small;                // kmeans: the winner, the changed count, [K] counts, [K] seeds
+  DevBuf<unsigned long long> km_keys;  // kmeans: [2][2 T] the race keys of two rounds
+  DevBuf<unsigned long long> km_codes; // kmeans: [J] the label of each segment of the rows sorted by label
 };
 ScoreScratch& score_scratch(hb_handle* h) {
   if (!h->scores) h->scores.reset(new ScoreScratch());
@@ -76,32 +83,20 @@ void knn_geometry_record(int d, int k, int64_t Nq, int64_t Nx, int num_sms, int6
   for (int i = 0; i < 8; ++i) out[i] = v[i];
 }
 
-// The search itself, for arguments the caller has checked, on h->stream: column sums (Euclidean), the preparation of X
-// (and of Q unless it is X), the sweep and the merge into idx / dist [Nq][k].  hb_knn and hb_lisi run it.
-int knn_search(hb_handle* h, const DevRows& Q, const DevRows& X, int d, int k, bool cosine, bool exclude_self,
-               int32_t* idx, float* dist) {
+// The sweep and the merge of prepared rows, on h->stream: the k nearest of the Nx reference rows Xp (hx their halved
+// squared norms) for each of the Nq query rows Qp, into idx / dist [Nq][k].  knn_search and hb_kmeans run it.
+int knn_sweep(hb_handle* h, const float* Qp, int64_t Nq, const float* Xp, const float* hx, int64_t Nx, int d, int k,
+              bool cosine, bool exclude_self, int32_t* idx, float* dist) {
   ScoreScratch& s = score_scratch(h);
-  const KnnGeometry g = knn_geometry(d, k, Q.n, X.n, h->num_sms);
-  const bool shared_rows = Q.p == X.p && Q.dtype == X.dtype && Q.ld == X.ld && Q.n == X.n;  // one prepared copy serves
-  CK(s.rows.reserve((size_t)X.n * g.KD));
-  if (!shared_rows) CK(s.query_rows.reserve((size_t)Q.n * g.KD));
-  CK(s.hx.reserve((size_t)X.n));
-  CK(s.part.reserve((size_t)Q.n * g.splits * k));
-  CK(s.centre.reserve((size_t)KNN_MAX_D));
-
-  TRY(prepare_centred(h, X, d, g.KD, cosine, s.centre.p, s.rows.p, s.hx.p));
-  const float* Qp = s.rows.p;
-  if (!shared_rows) {
-    TRY(knn_prepare(h, Q, d, g.KD, cosine, cosine ? nullptr : s.centre.p, (double)X.n, s.query_rows.p, nullptr));
-    Qp = s.query_rows.p;
-  }
+  const KnnGeometry g = knn_geometry(d, k, Nq, Nx, h->num_sms);
+  CK(s.part.reserve((size_t)Nq * g.splits * k));
   KnnArgs a;
   a.Qp = Qp;
-  a.Xp = s.rows.p;
-  a.hx = s.hx.p;
+  a.Xp = Xp;
+  a.hx = hx;
   a.part_i = s.part.p;
-  a.Nq = Q.n;
-  a.Nx = X.n;
+  a.Nq = Nq;
+  a.Nx = Nx;
   a.KD = g.KD;
   a.k = k;
   a.stages = g.stages;
@@ -120,8 +115,29 @@ int knn_search(hb_handle* h, const DevRows& Q, const DevRows& X, int d, int k, b
       TRY(launch(h, k_knn_tc<64, 4>, grid, dim3(128), g.smem, a));
   }
   const int nc = g.splits * k;
-  return launch(h, k_knn_merge, dim3((unsigned)((Q.n + 3) / 4)), dim3(128), (size_t)4 * 2 * nc * sizeof(float), Qp,
-                (const float*)s.rows.p, (const int*)s.part.p, Q.n, g.KD, k, nc, (int)cosine, idx, dist);
+  return launch(h, k_knn_merge, dim3((unsigned)((Nq + 3) / 4)), dim3(128), (size_t)4 * 2 * nc * sizeof(float), Qp, Xp,
+                (const int*)s.part.p, Nq, g.KD, k, nc, (int)cosine, idx, dist);
+}
+
+// The search itself, for arguments the caller has checked, on h->stream: column sums (Euclidean), the preparation of X
+// (and of Q unless it is X), the sweep and the merge into idx / dist [Nq][k].  hb_knn and hb_lisi run it.
+int knn_search(hb_handle* h, const DevRows& Q, const DevRows& X, int d, int k, bool cosine, bool exclude_self,
+               int32_t* idx, float* dist) {
+  ScoreScratch& s = score_scratch(h);
+  const int KD = (d + 7) & ~7;
+  const bool shared_rows = Q.p == X.p && Q.dtype == X.dtype && Q.ld == X.ld && Q.n == X.n;  // one prepared copy serves
+  CK(s.rows.reserve((size_t)X.n * KD));
+  if (!shared_rows) CK(s.query_rows.reserve((size_t)Q.n * KD));
+  CK(s.hx.reserve((size_t)X.n));
+  CK(s.centre.reserve((size_t)KNN_MAX_D));
+
+  TRY(prepare_centred(h, X, d, KD, cosine, s.centre.p, s.rows.p, s.hx.p));
+  const float* Qp = s.rows.p;
+  if (!shared_rows) {
+    TRY(knn_prepare(h, Q, d, KD, cosine, cosine ? nullptr : s.centre.p, (double)X.n, s.query_rows.p, nullptr));
+    Qp = s.query_rows.p;
+  }
+  return knn_sweep(h, Qp, Q.n, s.rows.p, s.hx.p, X.n, d, k, cosine, exclude_self, idx, dist);
 }
 
 int run_knn(hb_handle* h, const DevRows& Q, const DevRows& X, int d, int k, int metric, bool exclude_self, int32_t* idx,

@@ -150,16 +150,13 @@ __global__ void __launch_bounds__(256) k_pcr_mean(const double* __restrict__ tot
   }
 }
 
-// One warp per batch q: its raw sums (a batch that crossed chunk edges: the tail of its first chunk, then the heads
-// of the following ones) -> T_q = (sums - n_q m) / sqrt(n_q), 0 for a batch without finite rows, in place
-__global__ void __launch_bounds__(32 * PCR_WARPS) k_pcr_combine(PcrSumArgs a, const double* __restrict__ centre) {
-  const int lane = threadIdx.x & 31;
-  const int64_t q = (int64_t)blockIdx.x * PCR_WARPS + (threadIdx.x >> 5);
-  if (q >= a.J) return;
+// Batch q's raw column sums into s (lane's columns lane + 32 u) and its finite rows, returned: the batch's own sums,
+// or for a batch that crossed chunk edges the tail of its first chunk, then the heads of the following ones (the
+// count is then also written to a.count[q])
+__device__ __forceinline__ int pcr_batch_sum(const PcrSumArgs& a, int64_t q, int lane, double (&s)[4]) {
   const int64_t s0 = a.pstart[q], s1 = a.pstart[q + 1];
   const int64_t c0 = s0 / PCR_CHUNK, c1 = (s1 - 1) / PCR_CHUNK;
-  double* row = a.sums + q * a.d;
-  double s[4];
+  const double* row = a.sums + q * a.d;
   int n;
   if (c0 == c1) {
 #pragma unroll
@@ -178,6 +175,17 @@ __global__ void __launch_bounds__(32 * PCR_WARPS) k_pcr_combine(PcrSumArgs a, co
     }
     if (lane == 0) a.count[q] = n;
   }
+  return n;
+}
+
+// One warp per batch q: its raw sums -> T_q = (sums - n_q m) / sqrt(n_q), 0 for a batch without finite rows, in place
+__global__ void __launch_bounds__(32 * PCR_WARPS) k_pcr_combine(PcrSumArgs a, const double* __restrict__ centre) {
+  const int lane = threadIdx.x & 31;
+  const int64_t q = (int64_t)blockIdx.x * PCR_WARPS + (threadIdx.x >> 5);
+  if (q >= a.J) return;
+  double* row = a.sums + q * a.d;
+  double s[4];
+  const int n = pcr_batch_sum(a, q, lane, s);
   const double r = n > 0 ? 1.0 / sqrt((double)n) : 0.0;
 #pragma unroll
   for (int u = 0; u < 4; ++u) {

@@ -235,6 +235,13 @@ class harmony:
         from .pcr import pcr_on
         return pcr_on(self, X, batches, n_comps)
 
+    def kmeans(self, X, n_clusters, seed=0, n_init=1, max_iter=300, tol=1e-4, return_seeds=False):
+        """k-means of ``X`` [N, d] (host array or CUDA tensor) into ``n_clusters`` clusters on this object's device and
+        stream -> ``(labels, centres, inertia, n_iter)`` (and the seed rows with ``return_seeds``), as
+        ``harmony_b200.kmeans`` returns them.  Works in any state of the object and changes none of it."""
+        from .clustering import kmeans_on
+        return kmeans_on(self, X, n_clusters, seed, n_init, max_iter, tol, return_seeds)
+
     def _device_Phi(self, Phi):
         """An [N] or [N, C] int32 / int64 CUDA tensor -> contiguous [N, C] int32 on the object's device (converted, if
         need be, on the current torch stream, which hb_setup_device orders its read after)."""

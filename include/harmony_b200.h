@@ -45,7 +45,7 @@ int hb_pop_warning(hb_handle* h, char* buf, size_t cap);
 /* Library/ABI version: major*10000 + minor*100 + patch (0.3.0: labels in device memory; 0.4.0: mapping a query onto
  * a reference, hb_reference / hb_map_setup / hb_map).  hb_knn, hb_debug_knn_geometry, hb_lisi,
  * hb_debug_lisi_geometry, hb_silhouette, hb_debug_silhouette_geometry, hb_graph_components, hb_kbet,
- * hb_debug_chi2_sf, hb_pcr and hb_debug_sym_eig were added without moving the number. */
+ * hb_debug_chi2_sf, hb_pcr, hb_debug_sym_eig and hb_kmeans were added without moving the number. */
 int hb_version(void);
 
 /* ---- multi-GPU (one process per GPU; cells sharded contiguously; SURVEY §8e) ------------------- */
@@ -264,6 +264,27 @@ int hb_pcr(hb_handle* h, const void* X, int x_dtype, int64_t x_ld, int64_t N, in
  * the eigenvalues in descending order into w [n] and V [n][n] row-major with column j the unit eigenvector of w[j],
  * signed as hb_pcr's components.  Returns 0, or 2 with the outputs untouched for n outside 1..128. */
 int hb_debug_sym_eig(int n, const double* A, double* w, double* V);
+
+/* k-means of an embedding (DESIGN.md §15), the clustering behind the NMI / ARI scores: K clusters of the finite rows of
+ * X [N, d] (x_dtype, row stride x_ld >= d; a row with a NaN or an infinity takes no part and gets label -1).  n_init
+ * inits; each is seeded by greedy k-means++ (2 + floor(ln K) candidates per round, drawn with probability ~ D^2 by
+ * keyed-hash exponential races under `seed`; the candidate of the smallest potential is kept) and iterated by Lloyd's
+ * rule as sklearn's algorithm="lloyd" runs it: assign (the nearest centre by hb_knn's search, the lower index on an exact
+ * tie), means of the members in fp64 (an empty cluster keeps its centre), stop when the labels repeat or when the
+ * squared centre shift is <= tol times the mean column variance of the finite rows; after max_iter iterations without
+ * repeated labels the rows are assigned once more.  max_iter = 0: the seeds' assignment.  Of the inits, the one of the
+ * lowest inertia (sum of |x - c_label|^2 over finite rows, fp64), the earliest on a tie, gives labels [N] int32 and
+ * centres [K][d] fp64; inertia [n_init] fp64 and n_iter [n_init] int32 are per init; seeds (NULL: skipped)
+ * [n_init][K] int32 the seed rows.  All outputs in device memory.  Limits, status 2 with a message before any launch:
+ * 1 <= N < 2^31, 1 <= d <= 128, 1 <= K <= min(N, 1024), n_init >= 1, max_iter >= 0, tol finite and >= 0, an unknown
+ * dtype, a row stride < d, a NULL (X, labels, centres, inertia, n_iter), host or other-device pointer.  Status 3 with
+ * the outputs untouched: fewer than K finite rows.  Status 2 after the first passes, the outputs untouched: a finite
+ * row with |x - m|^2 > 2^124 for m the column mean (the assignment's fp32 scores would overflow).  Ordered on `stream` like hb_knn; needs no setup and leaves a
+ * Harmony or mapping handle's state untouched; on a sharded handle the call is local; two calls give bit-identical
+ * results.  Regions "kmeans" and, within it, "kmeans_seed". */
+int hb_kmeans(hb_handle* h, const void* X, int x_dtype, int64_t x_ld, int64_t N, int d, int K, uint64_t seed,
+              int n_init, int max_iter, double tol, int32_t* labels, double* centres, double* inertia, int32_t* n_iter,
+              int32_t* seeds, void* stream);
 
 /* ---- fields / getters (harmony.cpp:640-669, 675-696) ------------------------------------------- */
 enum hb_field {
