@@ -21,18 +21,31 @@ def embedding(X, what):
     return X
 
 
+def check_two_rows(X, what="X"):
+    """The refusal of the scores that compare rows with each other: ``what`` needs at least 2 rows."""
+    if X.shape[0] < 2:
+        raise ValueError(f"{what} has {X.shape[0]} rows, at least 2 are needed")
+
+
+def row_layout(t, width):
+    """A 2-D tensor of rows of ``width`` elements -> (the tensor the library reads, its row stride ``ld``).  Rows with
+    unit column stride and a row stride of at least ``width`` are read in place; any other layout is made contiguous
+    first, a single row whose column stride is not 1 included."""
+    if not (t.stride(1) == 1 and (t.shape[0] == 1 or t.stride(0) >= width)):
+        t = t.contiguous()
+    return t, int(t.stride(0) if t.shape[0] > 1 else width)
+
+
 def device_rows(obj, X, what):
     """An [n, d] float32 / float64 CUDA tensor on ``obj``'s device -> (the tensor to read, pointer, hb_dtype, row
-    stride).  Rows with unit column stride are read in place, any other layout is made contiguous first."""
+    stride), laid out by ``row_layout``."""
     import torch
     if X.dtype not in (torch.float32, torch.float64):
         raise TypeError(f"{what} must be float32 or float64, not {X.dtype}")
     if X.device.index != obj._scalar("device"):
         raise ValueError(f"{what} is on {X.device}, the harmony object on cuda:{obj._scalar('device')}")
-    if X.shape[0] > 1 and not (X.stride(1) == 1 and X.stride(0) >= X.shape[1]):
-        X = X.contiguous()
-    ld = X.stride(0) if X.shape[0] > 1 else X.shape[1]
-    return X, ctypes.c_void_p(X.data_ptr()), DTYPE[str(X.dtype)[6:]], int(ld)
+    X, ld = row_layout(X, X.shape[1])
+    return X, ctypes.c_void_p(X.data_ptr()), DTYPE[str(X.dtype)[6:]], ld
 
 
 def rows_on(obj, X, what):
@@ -45,15 +58,38 @@ def rows_on(obj, X, what):
     return host, x, args
 
 
+def device_of(obj):
+    """The torch device of a harmony object."""
+    import torch
+    return torch.device("cuda", obj._scalar("device"))
+
+
+def handle(device):
+    """A harmony object on ``device`` (None: the current one) for a call that needs no setup."""
+    from .harmony import harmony  # needs the CUDA extension; fails loudly when it is missing
+    return harmony(device=device)
+
+
+def call(obj, entry, *args):
+    """The library function ``entry`` on ``obj``'s handle with ``args`` and the current torch stream of its device, on
+    which the library orders the call; a status other than 0 raises with the library's message."""
+    obj._check(getattr(obj._L, entry)(obj._h, *args, current_stream(device_of(obj))))
+
+
 def codes_on(obj, codes):
     """Integer codes -> an int32 tensor on ``obj``'s device (a CUDA tensor must already be there)."""
     import torch
-    device = torch.device("cuda", obj._scalar("device"))
+    device = device_of(obj)
     if not is_cuda_tensor(codes):
         codes = torch.as_tensor(np.ascontiguousarray(codes, dtype=np.int32)).to(device)
     if codes.device != device:
         raise ValueError(f"codes are on {codes.device}, the harmony object on {device}")
     return codes
+
+
+def dense_on(obj, codes):
+    """Optional codes (None stays None) -> a contiguous int32 tensor on ``obj``'s device."""
+    return None if codes is None else codes_on(obj, codes).contiguous()
 
 
 def ptr(t):
@@ -64,6 +100,11 @@ def ptr(t):
 def download(host, *ts):
     """The outputs as the caller's inputs came: numpy arrays for a host caller, the tensors otherwise (None stays)."""
     return [t.cpu().numpy() if host and t is not None else t for t in ts]
+
+
+def to_host(v):
+    """A CUDA tensor -> its numpy copy; anything else -> a numpy array."""
+    return v.cpu().numpy() if is_cuda_tensor(v) else np.asarray(v)
 
 
 def to_device(obj, a):
@@ -102,6 +143,11 @@ def factorise(column, device=None):
         import torch
         codes = torch.from_numpy(codes).to(device)
     return levels, codes
+
+
+def factorise_for(column, X):
+    """``factorise`` of a label column for the rows X: the codes go to a CUDA X's device."""
+    return factorise(column, X.device if is_cuda_tensor(X) else None)
 
 
 def code_sets(codes, n):

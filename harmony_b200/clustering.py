@@ -10,7 +10,8 @@ import math
 
 import numpy as np
 
-from ._arrays import current_stream, download, embedding, factorise, label_columns, ptr, resolve_device, rows_on
+from ._arrays import (call, device_of, download, embedding, factorise, handle, label_columns, ptr, resolve_device,
+                      rows_on)
 from .utils import is_cuda_tensor
 
 MAX_CLUSTERS = 1024   # the seeding makes about K passes over the rows
@@ -56,15 +57,15 @@ def kmeans_on(obj, X, n_clusters, seed=0, n_init=1, max_iter=300, tol=1e-4, retu
     N, d = X.shape
     K, seed, n_init, max_iter, tol = check_kmeans(N, n_clusters, seed, n_init, max_iter, tol)
     import torch
-    device = torch.device("cuda", obj._scalar("device"))
+    device = device_of(obj)
     host, x, x_args = rows_on(obj, X, "X")
     labels = torch.empty(N, dtype=torch.int32, device=device)
     centres = torch.empty((K, d), dtype=torch.float64, device=device)
     inertia = torch.empty(n_init, dtype=torch.float64, device=device)
     n_iter = torch.empty(n_init, dtype=torch.int32, device=device)
     seeds = torch.empty((n_init, K), dtype=torch.int32, device=device) if return_seeds else None
-    obj._check(obj._L.hb_kmeans(obj._h, *x_args, N, int(d), K, seed, n_init, max_iter, tol, ptr(labels), ptr(centres),
-                                ptr(inertia), ptr(n_iter), ptr(seeds), current_stream(device)))
+    call(obj, "hb_kmeans", *x_args, N, int(d), K, seed, n_init, max_iter, tol, ptr(labels), ptr(centres), ptr(inertia),
+         ptr(n_iter), ptr(seeds))
     out = download(host, labels, centres, inertia, n_iter, seeds)
     return tuple(out) if return_seeds else tuple(out[:4])
 
@@ -78,9 +79,7 @@ def kmeans(X, n_clusters, seed=0, n_init=1, max_iter=300, tol=1e-4, return_seeds
     tensors; fp32 rows are assigned on 3xTF32 scores (DESIGN §9's band), means and inertia are fp64."""
     X = embedding(X, "X")
     check_kmeans(X.shape[0], n_clusters, seed, n_init, max_iter, tol)
-    device = resolve_device(device, X, "X")
-    from .harmony import harmony  # needs the CUDA extension; fails loudly when it is missing
-    return kmeans_on(harmony(device=device), X, n_clusters, seed, n_init, max_iter, tol, return_seeds)
+    return kmeans_on(handle(resolve_device(device, X, "X")), X, n_clusters, seed, n_init, max_iter, tol, return_seeds)
 
 
 def _codes(v):

@@ -12,12 +12,12 @@ int components_run(hb_handle* h, const int32_t* idx, int64_t idx_ld, int64_t N, 
   const cudaStream_t st = h->stream;
   const int cap = h->num_sms * 8;
   const int64_t k1 = (int64_t)k + 1;  // an entry's place in the bad word: row k1 + m, the label at m = k
-  CK(s.bad.reserve(1));
-  CK(cudaMemsetAsync(s.bad.p, 0xff, sizeof(unsigned long long), st));
+  CK(s.keys.reserve(1));
+  CK(cudaMemsetAsync(s.keys.p, 0xff, sizeof(unsigned long long), st));
   TRY(launch(h, k_cc_check, dim3(grid_for(N * k1, 256, cap)), dim3(256), 0, idx, idx_ld, N, k, labels, n_labels,
-             s.bad.p));
+             s.keys.p));
   unsigned long long bad = 0;
-  CK(cudaMemcpyAsync(&bad, s.bad.p, sizeof(bad), cudaMemcpyDeviceToHost, st));
+  CK(cudaMemcpyAsync(&bad, s.keys.p, sizeof(bad), cudaMemcpyDeviceToHost, st));
   CK(cudaStreamSynchronize(st));
   if (bad != ~0ull) {
     const int64_t row = (int64_t)(bad / k1);
@@ -35,11 +35,11 @@ int components_run(hb_handle* h, const int32_t* idx, int64_t idx_ld, int64_t N, 
   TRY(launch(h, k_cc_hook, dim3(grid_for(N * (int64_t)k, 256, cap)), dim3(256), 0, idx, idx_ld, N, k, labels, (int*)comp));
   TRY(launch(h, k_cc_compress, dim3(rows_grid), dim3(256), 0, N, (int*)comp));
   if (!largest) return 0;
-  CK(s.sizes.reserve((size_t)N));
-  CK(cudaMemsetAsync(s.sizes.p, 0, sizeof(int) * N, st));
+  CK(s.count.reserve((size_t)N));
+  CK(cudaMemsetAsync(s.count.p, 0, sizeof(int) * N, st));
   CK(cudaMemsetAsync(largest, 0, sizeof(int32_t) * (labels ? n_labels : 1), st));
-  TRY(launch(h, k_cc_count, dim3(rows_grid), dim3(256), 0, (const int*)comp, N, s.sizes.p));
-  return launch(h, k_cc_largest, dim3(rows_grid), dim3(256), 0, (const int*)comp, (const int*)s.sizes.p, labels, N,
+  TRY(launch(h, k_cc_count, dim3(rows_grid), dim3(256), 0, (const int*)comp, N, s.count.p));
+  return launch(h, k_cc_largest, dim3(rows_grid), dim3(256), 0, (const int*)comp, (const int*)s.count.p, labels, N,
                 (int*)largest);
 }
 
@@ -55,11 +55,8 @@ int run_components(hb_handle* h, const int32_t* idx, int64_t idx_ld, int64_t N, 
   TRY(check_device_ptr(h, comp, "comp"));
   if (labels) TRY(check_device_ptr(h, labels, "labels"));
   if (largest) TRY(check_device_ptr(h, largest, "largest"));
-  CK(cudaSetDevice(h->device));
-  return on_caller_stream(h, caller, [&] {
-    RegionScope rs(h, "components");
-    return components_run(h, idx, idx_ld, N, k, labels, n_labels, comp, largest);
-  });
+  return run_score(h, caller, "components",
+                   [&] { return components_run(h, idx, idx_ld, N, k, labels, n_labels, comp, largest); });
 }
 
 }  // namespace

@@ -72,7 +72,7 @@ struct Plan;         // plan.cuh
 struct UpdateState;  // update_host.cuh
 struct AssignState;  // assign_host.cuh
 struct MapState;     // map_host.cuh
-struct ScoreScratch;  // knn_host.cuh
+struct ScoreScratch;  // score_host.cuh
 
 }  // namespace
 
@@ -128,7 +128,7 @@ struct hb_handle {
   std::unique_ptr<UpdateState> upd;
   std::unique_ptr<AssignState> asg;
   std::unique_ptr<MapState> map;  // hb_map_setup only
-  std::unique_ptr<ScoreScratch> scores;  // the scratch of the score calls (knn_host.cuh), from the first such call
+  std::unique_ptr<ScoreScratch> scores;  // the scratch of the score calls (score_host.cuh), from the first such call
 
   // traces (harmony.h:55-56); values are produced on the device and pulled lazily
   DevBuf<float> trace_d;

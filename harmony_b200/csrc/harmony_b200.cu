@@ -365,6 +365,7 @@ int harmony_step(hb_handle* h, const char* what, bool needs_init = true) {
 }  // namespace
 
 #include "map_host.cuh"
+#include "score_host.cuh"
 #include "knn_host.cuh"
 #include "lisi_host.cuh"
 #include "silhouette_host.cuh"
@@ -798,7 +799,7 @@ int hb_get_field_device(hb_handle* h, int field, void* out, int dtype, int64_t l
     if (field == HB_Z_CORR) TRY(normalise_pending_zc(h));
     RegionScope rs(h, "download");
     with_rows(rows, [&](auto o) {  // `out` is the caller's writable array
-      using T = std::remove_const_t<std::remove_pointer_t<decltype(o)>>;
+      using T = row_t<decltype(o)>;
       copy_rows(f.buf, f.ld, const_cast<T*>(o), ld, h->inv_sort.p, 0, false, h->n, f.cols, h->num_sms, h->stream);
     });
     CKL();
@@ -1023,7 +1024,7 @@ int hb_debug_lisi_geometry(int d, double perplexity, int64_t N, int num_sms, int
 // tile, operand stages, shared-memory bytes, padded row length, threads per CTA, query tiles of N rows in one group,
 // waves of those tiles on num_sms SMs}.  Status 2 (out untouched) for a d or N hb_silhouette refuses.
 int hb_debug_silhouette_geometry(int d, int64_t N, int num_sms, int64_t out[8]) {
-  if (sil_check_shape(nullptr, N, d) != 0 || num_sms < 1) return 2;
+  if (check_score_shape(nullptr, "hb_silhouette", N, d) != 0 || num_sms < 1) return 2;
   sil_geometry_record(d, N, num_sms, out);
   return 0;
 }

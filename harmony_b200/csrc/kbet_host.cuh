@@ -1,7 +1,7 @@
 // kbet_host.cuh — hb_kbet (DESIGN §13): the checks and the launches: hb_silhouette's (label, batch) index, sorted
-// preparation and finite counts (silhouette_host.cuh), the k0 of each label on the host, k_knn_tc's grouped sweep over
-// the tested labels' tiles, k_knn_merge and k_kbet.  The call needs no setup and touches no state of a Harmony run or a
-// mapping.  Included by harmony_b200.cu.
+// preparation and finite counts (pair_index, score_host.cuh), the k0 of each label on the host, k_knn_tc's grouped sweep
+// over the tested labels' tiles, k_knn_merge and k_kbet.  The call needs no setup and touches no state of a Harmony run
+// or a mapping.  Included by harmony_b200.cu.
 #pragma once
 
 namespace {
@@ -25,26 +25,11 @@ int kbet_run(hb_handle* h, const DevRows& X, int d, const int32_t* batches, int 
   const int64_t N = X.n;
   const cudaStream_t st = h->stream;
   const int KD = (d + 7) & ~7;
-  CK(s.phi.reserve(2 * (size_t)N));
-  CK(s.rows.reserve((size_t)N * KD));
-  CK(s.hx.reserve((size_t)N));
-  CK(s.centre.reserve((size_t)KNN_MAX_D));
   // ---- the index of the (label, batch) pairs, the rows in sorted order and the finite rows per pair
-  k_silhouette_phi<<<grid_for(N, 256, h->num_sms * 8), 256, 0, st>>>(batches, labels, N, n_batches, n_labels, s.phi.p);
-  CKL();
-  TupleKeys keys;
-  TRY(tuple_keys(h, {n_labels, n_batches}, keys));
   TupleIndex ti;
   static const char* const names[2] = {"hb_kbet: labels", "hb_kbet: batches"};
-  TRY(build_tuple_index(h, s.phi.p, N, keys, false, s.sort_perm, s.inv_sort, ti, names));
+  TRY(pair_index(h, X, d, KD, labels, n_labels, batches, n_batches, names, ti));
   const int J = (int)ti.uniq.size();
-  CK(s.pstart.reserve((size_t)J + 1));
-  CK(s.count.reserve((size_t)J));
-  TRY(upload_vector(h, s.pstart, std::vector<int>(ti.tstart.begin(), ti.tstart.end())));
-  CK(cudaMemsetAsync(s.count.p, 0, sizeof(int) * J, st));
-  TRY(prepare_centred(h, X, d, KD, false, s.centre.p, s.rows.p, s.hx.p, s.sort_perm.p));
-  k_silhouette_count<<<grid_for(N, 256, h->num_sms * 8), 256, 0, st>>>(s.hx.p, N, s.pstart.p, J, s.count.p);
-  CKL();
   std::vector<int> count(J);
   CK(cudaMemcpyAsync(count.data(), s.count.p, sizeof(int) * J, cudaMemcpyDeviceToHost, st));
   CK(cudaStreamSynchronize(st));
@@ -73,8 +58,8 @@ int kbet_run(hb_handle* h, const DevRows& X, int d, const int32_t* batches, int 
     const int l = (int)(ti.uniq[q] / n_batches);
     pairs[q] = KbetPair{k0[l], (int)n[l], present[l] - 1, p0[l], p1[l]};
   }
-  CK(s.kbet_pairs.reserve((size_t)J));
-  TRY(upload_vector(h, s.kbet_pairs, pairs));
+  CK(s.pairs.reserve((size_t)J));
+  TRY(upload_vector(h, s.pairs, pairs));
 
   // ---- the grouped sweep over the tested labels' tiles, and the merge into sorted-position lists
   if (kmax > 0) {
@@ -88,34 +73,13 @@ int kbet_run(hb_handle* h, const DevRows& X, int d, const int32_t* batches, int 
     CK(s.part.reserve((size_t)N * kmax));
     CK(s.idx.reserve((size_t)N * kmax));
     CK(cudaMemsetAsync(s.part.p, 0xff, sizeof(int) * (size_t)N * kmax, st));  // rows of untested labels: no candidate
-    KnnGroupArgs a;
-    a.Qp = a.Xp = s.rows.p;
-    a.hx = s.hx.p;
-    a.part_i = s.part.p;
-    a.Nq = a.Nx = N;
-    a.KD = KD;
-    a.k = kmax;
-    a.stages = g.stages;
-    a.exclude_self = 1;
-    a.tiles_per_split = 0;
-    a.tiles = s.tiles.p;
-    const dim3 grid((unsigned)tiles.size());
-    if (kmax <= 64) {
-      if (g.tq == 128)
-        TRY(launch(h, k_knn_tc<128, 2, true>, grid, dim3(256), g.smem, a));
-      else
-        TRY(launch(h, k_knn_tc<64, 2, true>, grid, dim3(128), g.smem, a));
-    } else {
-      if (g.tq == 128)
-        TRY(launch(h, k_knn_tc<128, 4, true>, grid, dim3(256), g.smem, a));
-      else
-        TRY(launch(h, k_knn_tc<64, 4, true>, grid, dim3(128), g.smem, a));
-    }
+    const KnnGroupArgs a{{s.rows.p, s.rows.p, s.hx.p, s.part.p, N, N, KD, kmax, g.stages, 1, 0}, s.tiles.p};
+    TRY(launch_knn_tc(h, g, kmax, dim3((unsigned)tiles.size()), a));
     TRY(launch(h, k_knn_merge, dim3((unsigned)((N + 3) / 4)), dim3(128), (size_t)4 * 2 * kmax * sizeof(float),
                (const float*)s.rows.p, (const float*)s.rows.p, (const int*)s.part.p, N, KD, kmax, kmax, 0, s.idx.p,
                (float*)nullptr));
   }
-  KbetArgs k{kmax > 0 ? s.idx.p : nullptr, s.hx.p, s.pstart.p, s.count.p, s.kbet_pairs.p, s.sort_perm.p, stat, pval,
+  KbetArgs k{kmax > 0 ? s.idx.p : nullptr, s.hx.p, s.pstart.p, s.count.p, s.pairs.p, s.sort_perm.p, stat, pval,
              idx, N, idx ? idx_ld : 0, J, kmax};
   return launch(h, k_kbet, dim3((unsigned)((N + KBET_WARPS - 1) / KBET_WARPS)), dim3(32 * KBET_WARPS), 0, k);
 }
@@ -123,8 +87,7 @@ int kbet_run(hb_handle* h, const DevRows& X, int d, const int32_t* batches, int 
 int run_kbet(hb_handle* h, const DevRows& X, int d, const int32_t* batches, int n_batches, const int32_t* labels,
              int n_labels, int k0, double* stat, double* pval, int32_t* k0_out, int32_t* idx, int64_t idx_ld,
              cudaStream_t caller) {
-  if (X.n < 2) return fail(h, 2, "hb_kbet: N = %lld rows, at least 2 are needed", (long long)X.n);
-  TRY(check_search_shape(h, "hb_kbet", "N", X.n, d));
+  TRY(check_score_shape(h, "hb_kbet", X.n, d));
   if (n_batches < 1) return fail(h, 2, "hb_kbet: n_batches = %d, at least one batch is needed", n_batches);
   if (labels && n_labels < 1) return fail(h, 2, "hb_kbet: n_labels = %d, at least one label is needed", n_labels);
   if (!labels) n_labels = 1;
@@ -139,9 +102,7 @@ int run_kbet(hb_handle* h, const DevRows& X, int d, const int32_t* batches, int 
   TRY(check_device_ptr(h, pval, "pval"));
   if (k0_out) TRY(check_device_ptr(h, k0_out, "k0_out"));
   if (idx) TRY(check_device_ptr(h, idx, "idx"));
-  CK(cudaSetDevice(h->device));
-  return on_caller_stream(h, caller, [&] {
-    RegionScope rs(h, "kbet");
+  return run_score(h, caller, "kbet", [&] {
     return kbet_run(h, X, d, batches, n_batches, labels, n_labels, k0, stat, pval, k0_out, idx, idx_ld);
   });
 }

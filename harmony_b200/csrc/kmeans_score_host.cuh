@@ -35,15 +35,15 @@ struct KmeansRun {
 int kms_sqdist(KmeansRun& r, const int32_t* labels, const double* centres, double* out, int* far = nullptr) {
   hb_handle* h = r.h;
   ScoreScratch& s = score_scratch(h);
-  int* far_d = far ? s.km_small.p + 1 : nullptr;
+  int* far_d = far ? s.small.p + 1 : nullptr;
   if (far_d) CK(cudaMemsetAsync(far_d, 0, sizeof(int), h->stream));
   TRY(with_rows(r.X, [&](auto x) {
-    return launch(h, k_kms_sqdist<std::remove_const_t<std::remove_pointer_t<decltype(x)>>>, dim3((unsigned)r.ranges.ctas),
-                  dim3(32 * KMS_WARPS), 0, x, r.X.ld, r.N, r.d, r.ranges.rows, (const unsigned char*)s.km_fin.p, labels,
-                  centres, s.km_part.p, far_d);
+    return launch(h, k_kms_sqdist<row_t<decltype(x)>>, dim3((unsigned)r.ranges.ctas),
+                  dim3(32 * KMS_WARPS), 0, x, r.X.ld, r.N, r.d, r.ranges.rows, (const unsigned char*)s.finite.p, labels,
+                  centres, s.cta_part.p, far_d);
   }));
   std::vector<double> part(r.ranges.ctas);
-  CK(cudaMemcpyAsync(part.data(), s.km_part.p, sizeof(double) * part.size(), cudaMemcpyDeviceToHost, h->stream));
+  CK(cudaMemcpyAsync(part.data(), s.cta_part.p, sizeof(double) * part.size(), cudaMemcpyDeviceToHost, h->stream));
   if (far) CK(cudaMemcpyAsync(far, far_d, sizeof(int), cudaMemcpyDeviceToHost, h->stream));
   CK(cudaStreamSynchronize(h->stream));
   double t = 0.0;
@@ -58,15 +58,15 @@ int kms_prepare(KmeansRun& r, double tol) {
   hb_handle* h = r.h;
   ScoreScratch& s = score_scratch(h);
   const int ctas = r.ranges.ctas;
-  CK(s.km_part.reserve(std::max<size_t>((size_t)ctas * r.d + 1, (size_t)r.seed_grid * KMS_MAX_T)));
-  CK(s.pcr_edge_n.reserve((size_t)ctas));
+  CK(s.cta_part.reserve(std::max<size_t>((size_t)ctas * r.d + 1, (size_t)r.seed_grid * KMS_MAX_T)));
+  CK(s.chunk_n.reserve((size_t)ctas));
   CK(s.centre.reserve((size_t)KNN_MAX_D + 1));
   TRY(with_rows(r.X, [&](auto x) {
-    return launch(h, k_kms_colsum<std::remove_const_t<std::remove_pointer_t<decltype(x)>>>, dim3((unsigned)ctas),
-                  dim3(32 * KMS_WARPS), 0, x, r.X.ld, r.N, r.d, r.ranges.rows, s.km_part.p, s.pcr_edge_n.p, s.km_fin.p);
+    return launch(h, k_kms_colsum<row_t<decltype(x)>>, dim3((unsigned)ctas),
+                  dim3(32 * KMS_WARPS), 0, x, r.X.ld, r.N, r.d, r.ranges.rows, s.cta_part.p, s.chunk_n.p, s.finite.p);
   }));
   double* n_out = s.centre.p + KNN_MAX_D;
-  TRY(launch(h, k_pcr_mean, dim3((unsigned)r.d), dim3(256), 0, (const double*)s.km_part.p, (const int*)s.pcr_edge_n.p,
+  TRY(launch(h, k_pcr_mean, dim3((unsigned)r.d), dim3(256), 0, (const double*)s.cta_part.p, (const int*)s.chunk_n.p,
              (int64_t)ctas, r.d, s.centre.p, n_out));
   CK(cudaMemcpyAsync(&r.n_fin, n_out, sizeof(double), cudaMemcpyDeviceToHost, h->stream));
   CK(cudaStreamSynchronize(h->stream));
@@ -88,21 +88,21 @@ int kms_seed(KmeansRun& r, uint64_t seed, int init, int32_t* seeds, double* cent
   RegionScope rs(h, "kmeans_seed");
   ScoreScratch& s = score_scratch(h);
   const int T = r.T;
-  int* winner = s.km_small.p;
-  unsigned long long* keys[2] = {s.km_keys.p, s.km_keys.p + 2 * T};
-  const KmsSeedArgs a{s.rows.p, s.km_fin.p, s.km_d2.p, r.N, r.KD, T, kmeans_score_key(seed, (uint64_t)init)};
+  int* winner = s.small.p;
+  unsigned long long* keys[2] = {s.keys.p, s.keys.p + 2 * T};
+  const KmsSeedArgs a{s.rows.p, s.finite.p, s.d2.p, r.N, r.KD, T, kmeans_score_key(seed, (uint64_t)init)};
   const dim3 grid((unsigned)r.seed_grid), block(32 * KMS_WARPS);
-  CK(cudaMemsetAsync(s.km_keys.p, 0xff, sizeof(unsigned long long) * 4 * T, h->stream));
+  CK(cudaMemsetAsync(s.keys.p, 0xff, sizeof(unsigned long long) * 4 * T, h->stream));
   TRY(launch(h, k_kms_update, grid, block, 0, a, (const int*)nullptr, 0, keys[0]));
   for (int round = 0; round < r.K; ++round) {
     unsigned long long* cur = keys[round & 1];
-    if (round > 0) TRY(launch(h, k_kms_potential, grid, block, 0, a, (const unsigned long long*)cur, s.km_part.p));
-    TRY(launch(h, k_kms_pick, dim3(1), dim3(32), 0, (const double*)s.km_part.p, r.seed_grid, T,
+    if (round > 0) TRY(launch(h, k_kms_potential, grid, block, 0, a, (const unsigned long long*)cur, s.cta_part.p));
+    TRY(launch(h, k_kms_pick, dim3(1), dim3(32), 0, (const double*)s.cta_part.p, r.seed_grid, T,
                (const unsigned long long*)cur, round, seeds, winner, keys[(round + 1) & 1]));
     if (round + 1 < r.K) TRY(launch(h, k_kms_update, grid, block, 0, a, (const int*)winner, round + 1, keys[(round + 1) & 1]));
   }
   return with_rows(r.X, [&](auto x) {
-    return launch(h, k_kms_gather<std::remove_const_t<std::remove_pointer_t<decltype(x)>>>,
+    return launch(h, k_kms_gather<row_t<decltype(x)>>,
                   dim3((unsigned)grid_for((int64_t)r.K * r.d, 256, h->num_sms * 4)), dim3(256), 0, x, r.X.ld, r.d,
                   (const int32_t*)seeds, r.K, centres);
   });
@@ -117,36 +117,21 @@ int kms_assign(KmeansRun& r, const double* centres, int32_t* labels, const int32
   TRY(knn_prepare(h, C, r.d, r.KD, false, s.centre.p, 1.0, s.query_rows.p, s.hx.p));
   TRY(knn_sweep(h, s.rows.p, r.N, s.query_rows.p, s.hx.p, r.K, r.d, 1, false, false, labels, nullptr));
   return launch(h, k_kms_labels, dim3((unsigned)grid_for(r.N, 32 * KMS_WARPS, h->num_sms * 4)), dim3(32 * KMS_WARPS), 0,
-                labels, old, (const unsigned char*)s.km_fin.p, r.N, r.K, s.phi.p, changed);
+                labels, old, (const unsigned char*)s.finite.p, r.N, r.K, s.phi.p, changed);
 }
 
 // next <- the means of the labels' members (from a copy of cur: an empty cluster keeps its centre)
 int kms_means(KmeansRun& r, const double* cur, double* next) {
   hb_handle* h = r.h;
   ScoreScratch& s = score_scratch(h);
-  const int64_t N = r.N;
-  const int d = r.d;
-  TupleKeys keys;
-  TRY(tuple_keys(h, {r.K + 1}, keys));
   TupleIndex ti;
-  static const char* const names[1] = {"hb_kmeans: labels"};
-  TRY(build_tuple_index(h, s.phi.p, N, keys, false, s.sort_perm, s.inv_sort, ti, names));
-  const int J = (int)ti.uniq.size();
-  const int64_t chunks = (N + PCR_CHUNK - 1) / PCR_CHUNK;
-  CK(s.pstart.reserve((size_t)J + 1));
-  CK(s.count.reserve((size_t)J));
-  CK(s.pcr_rows.reserve((size_t)J * d));
-  CK(s.pcr_edge.reserve((size_t)3 * chunks * d));
-  CK(s.pcr_edge_n.reserve((size_t)3 * chunks));
-  CK(s.km_codes.reserve((size_t)J));
-  TRY(upload_vector(h, s.pstart, std::vector<int>(ti.tstart.begin(), ti.tstart.end())));
-  TRY(upload_vector(h, s.km_codes, std::vector<unsigned long long>(ti.uniq.begin(), ti.uniq.end())));
-  CK(cudaMemcpyAsync(next, cur, sizeof(double) * r.K * d, cudaMemcpyDeviceToDevice, h->stream));
-  PcrSumArgs a{r.X.ld, N, d, J, chunks, s.sort_perm.p, s.pstart.p, s.pcr_rows.p, s.count.p, s.pcr_edge.p, s.pcr_edge_n.p};
-  const dim3 gs((unsigned)((chunks + PCR_WARPS - 1) / PCR_WARPS));
-  TRY(with_rows(r.X, [&](auto x) { return launch(h, k_pcr_sums<std::remove_const_t<std::remove_pointer_t<decltype(x)>>>, gs, dim3(32 * PCR_WARPS), 0, a, x); }));
-  return launch(h, k_kms_means, dim3((unsigned)((J + PCR_WARPS - 1) / PCR_WARPS)), dim3(32 * PCR_WARPS), 0, a,
-                (const unsigned long long*)s.km_codes.p, r.K, next, s.km_small.p + 2);
+  PcrSumArgs a;
+  TRY(segment_sums(h, r.X, r.d, s.phi.p, r.K + 1, "hb_kmeans: labels", ti, a));
+  CK(s.seg_codes.reserve((size_t)a.J));
+  TRY(upload_vector(h, s.seg_codes, std::vector<unsigned long long>(ti.uniq.begin(), ti.uniq.end())));
+  CK(cudaMemcpyAsync(next, cur, sizeof(double) * r.K * r.d, cudaMemcpyDeviceToDevice, h->stream));
+  return launch(h, k_kms_means, dim3((unsigned)((a.J + PCR_WARPS - 1) / PCR_WARPS)), dim3(32 * PCR_WARPS), 0, a,
+                (const unsigned long long*)s.seg_codes.p, r.K, next, s.small.p + 2);
 }
 
 // One init: seeds, Lloyd, the final assignment; labels and centres into the scratch, inertia and n_iter out
@@ -155,10 +140,10 @@ int kms_init(KmeansRun& r, uint64_t seed, int init, int max_iter, int32_t** labe
   hb_handle* h = r.h;
   ScoreScratch& s = score_scratch(h);
   const size_t Kd = (size_t)r.K * r.d;
-  double* cen[2] = {s.km_centres.p, s.km_centres.p + Kd};
-  int32_t* lab[2] = {s.km_labels.p, s.km_labels.p + r.N};
-  int32_t* seeds = s.km_small.p + 2 + r.K;
-  int* changed = s.km_small.p + 1;
+  double* cen[2] = {s.stats.p, s.stats.p + Kd};
+  int32_t* lab[2] = {s.idx.p, s.idx.p + r.N};
+  int32_t* seeds = s.small.p + 2 + r.K;
+  int* changed = s.small.p + 1;
   TRY(kms_seed(r, seed, init, seeds, cen[0]));
   CK(cudaMemsetAsync(lab[1], 0xff, sizeof(int32_t) * r.N, h->stream));  // the previous labels of iteration 1: none
   std::vector<double> c_old(Kd), c_new(Kd);
@@ -203,15 +188,15 @@ int kmeans_run(hb_handle* h, const DevRows& X, int d, int K, uint64_t seed, int 
   KmeansRun r{h, X, d, K, (d + 7) & ~7, kmeans_trials(K), X.n};
   r.ranges = kms_ranges(X.n, h->num_sms);
   r.seed_grid = grid_for(X.n * KMS_GROUP, 32 * KMS_WARPS, h->num_sms * 8);  // KMS_GROUP lanes per row
-  CK(s.km_fin.reserve((size_t)X.n));
+  CK(s.finite.reserve((size_t)X.n));
   CK(s.rows.reserve((size_t)X.n * r.KD));
   CK(s.query_rows.reserve((size_t)K * r.KD));
   CK(s.hx.reserve((size_t)K));
-  CK(s.km_d2.reserve((size_t)X.n));
-  CK(s.km_centres.reserve((size_t)2 * K * d));
-  CK(s.km_labels.reserve((size_t)2 * X.n));
-  CK(s.km_small.reserve((size_t)2 + 2 * K));
-  CK(s.km_keys.reserve((size_t)4 * KMS_MAX_T));
+  CK(s.d2.reserve((size_t)X.n));
+  CK(s.stats.reserve((size_t)2 * K * d));
+  CK(s.idx.reserve((size_t)2 * X.n));
+  CK(s.small.reserve((size_t)2 + 2 * K));
+  CK(s.keys.reserve((size_t)4 * KMS_MAX_T));
   CK(s.phi.reserve((size_t)X.n));
   TRY(kms_prepare(r, tol));
   std::vector<double> inertia_h(n_init);
@@ -221,7 +206,7 @@ int kmeans_run(hb_handle* h, const DevRows& X, int d, int K, uint64_t seed, int 
     double* cen;
     TRY(kms_init(r, seed, init, max_iter, &lab, &cen, &inertia_h[init], &n_iter_h[init]));
     if (seeds)
-      CK(cudaMemcpyAsync(seeds + (size_t)init * K, s.km_small.p + 2 + K, sizeof(int32_t) * K, cudaMemcpyDeviceToDevice,
+      CK(cudaMemcpyAsync(seeds + (size_t)init * K, s.small.p + 2 + K, sizeof(int32_t) * K, cudaMemcpyDeviceToDevice,
                          h->stream));
     bool best = true;  // the lowest inertia, the earliest init on a tie
     for (int j = 0; j < init; ++j) best &= inertia_h[init] < inertia_h[j];
@@ -251,9 +236,7 @@ int run_kmeans(hb_handle* h, const DevRows& X, int d, int K, uint64_t seed, int 
   TRY(check_device_ptr(h, inertia, "inertia"));
   TRY(check_device_ptr(h, n_iter, "n_iter"));
   if (seeds) TRY(check_device_ptr(h, seeds, "seeds"));
-  CK(cudaSetDevice(h->device));
-  return on_caller_stream(h, caller, [&] {
-    RegionScope rs(h, "kmeans");
+  return run_score(h, caller, "kmeans", [&] {
     return kmeans_run(h, X, d, K, seed, n_init, max_iter, tol, labels, centres, inertia, n_iter, seeds);
   });
 }

@@ -35,18 +35,16 @@ int run_lisi(hb_handle* h, const DevRows& X, int d, const int32_t* labels, int64
   TRY(check_device_ptr(h, lisi, "lisi"));
   if (idx) TRY(check_device_ptr(h, idx, "idx"));
   if (dist) TRY(check_device_ptr(h, dist, "dist"));
-  CK(cudaSetDevice(h->device));
-  ScoreScratch& s = score_scratch(h);
-  if (!idx) {
-    CK(s.idx.reserve((size_t)X.n * k));
-    idx = s.idx.p;
-  }
-  if (!dist) {
-    CK(s.dist.reserve((size_t)X.n * k));
-    dist = s.dist.p;
-  }
-  return on_caller_stream(h, caller, [&] {
-    RegionScope rs(h, "lisi");
+  return run_score(h, caller, "lisi", [&] {
+    ScoreScratch& s = score_scratch(h);
+    if (!idx) {
+      CK(s.idx.reserve((size_t)X.n * k));
+      idx = s.idx.p;
+    }
+    if (!dist) {
+      CK(s.dist.reserve((size_t)X.n * k));
+      dist = s.dist.p;
+    }
     TRY(knn_search(h, X, X, d, k, false, true, idx, dist));
     return launch(h, k_lisi, dim3((unsigned)((X.n + LISI_WARPS - 1) / LISI_WARPS)), dim3(32 * LISI_WARPS), 0,
                   (const int32_t*)idx, (const float*)dist, X.n, k, labels, labels_ld, n_sets, std::log(p), lisi);

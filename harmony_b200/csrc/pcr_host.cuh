@@ -206,39 +206,27 @@ int pcr_run(hb_handle* h, const DevRows& X, int d, const int32_t* batches, int n
   const int64_t N = X.n;
   const cudaStream_t st = h->stream;
   const int KD = (d + 15) & ~15;
-  // ---- the index: the rows sorted by batch, each batch's sorted rows
-  TupleKeys keys;
-  TRY(tuple_keys(h, {n_batches}, keys));
+  // ---- the index: the rows sorted by batch, each batch's sorted rows, and the batch sums
   TupleIndex ti;
-  static const char* const names[1] = {"hb_pcr: batches"};
-  TRY(build_tuple_index(h, batches, N, keys, false, s.sort_perm, s.inv_sort, ti, names));
-  const int J = (int)ti.uniq.size();
-  const int64_t chunks = (N + PCR_CHUNK - 1) / PCR_CHUNK;
-  CK(s.pstart.reserve((size_t)J + 1));
-  CK(s.count.reserve((size_t)J));
-  CK(s.pcr_rows.reserve((size_t)J * d));
-  CK(s.pcr_edge.reserve((size_t)3 * chunks * d));
-  CK(s.pcr_edge_n.reserve((size_t)3 * chunks));
+  PcrSumArgs a;
+  TRY(segment_sums(h, X, d, batches, n_batches, "hb_pcr: batches", ti, a));
+  const int J = a.J;
   CK(s.centre.reserve((size_t)KNN_MAX_D));
-  CK(s.pcr_out.reserve((size_t)2 * KD * KD + 1));
-  TRY(upload_vector(h, s.pstart, std::vector<int>(ti.tstart.begin(), ti.tstart.end())));
-  // ---- the batch sums, the mean, the between-batch rows
-  PcrSumArgs a{X.ld, N, d, J, chunks, s.sort_perm.p, s.pstart.p, s.pcr_rows.p, s.count.p, s.pcr_edge.p, s.pcr_edge_n.p};
-  const dim3 gs((unsigned)((chunks + PCR_WARPS - 1) / PCR_WARPS));
-  TRY(with_rows(X, [&](auto x) { return launch(h, k_pcr_sums<std::remove_const_t<std::remove_pointer_t<decltype(x)>>>, gs, dim3(32 * PCR_WARPS), 0, a, x); }));
-  double* C = s.pcr_out.p;
+  CK(s.stats.reserve((size_t)2 * KD * KD + 1));
+  // ---- the mean, the between-batch rows
+  double* C = s.stats.p;
   double* M = C + (size_t)KD * KD;
   double* n_d = M + (size_t)KD * KD;
-  TRY(launch(h, k_pcr_mean, dim3((unsigned)d), dim3(256), 0, (const double*)s.pcr_edge.p + 2 * chunks * d,
-             (const int*)s.pcr_edge_n.p + 2 * chunks, chunks, d, s.centre.p, n_d));
+  TRY(launch(h, k_pcr_mean, dim3((unsigned)d), dim3(256), 0, (const double*)s.chunk_edge.p + 2 * a.chunks * d,
+             (const int*)s.chunk_n.p + 2 * a.chunks, a.chunks, d, s.centre.p, n_d));
   TRY(launch(h, k_pcr_combine, dim3((unsigned)((J + PCR_WARPS - 1) / PCR_WARPS)), dim3(32 * PCR_WARPS), 0, a,
              (const double*)s.centre.p));
   // ---- the covariance and the between-batch scatter
-  TRY(with_rows(X, [&](auto x) { return pcr_gram(h, x, X.ld, N, d, KD, s.centre.p, s.pcr_part, C); }));
-  TRY(pcr_gram(h, (const double*)s.pcr_rows.p, (int64_t)d, (int64_t)J, d, KD, (const double*)nullptr, s.pcr_part, M));
+  TRY(with_rows(X, [&](auto x) { return pcr_gram(h, x, X.ld, N, d, KD, s.centre.p, s.cta_part, C); }));
+  TRY(pcr_gram(h, (const double*)s.seg_sums.p, (int64_t)d, (int64_t)J, d, KD, (const double*)nullptr, s.cta_part, M));
   std::vector<double> out((size_t)2 * KD * KD + 1);
   std::vector<int> count(J);
-  CK(cudaMemcpyAsync(out.data(), s.pcr_out.p, sizeof(double) * out.size(), cudaMemcpyDeviceToHost, st));
+  CK(cudaMemcpyAsync(out.data(), s.stats.p, sizeof(double) * out.size(), cudaMemcpyDeviceToHost, st));
   CK(cudaMemcpyAsync(count.data(), s.count.p, sizeof(int) * J, cudaMemcpyDeviceToHost, st));
   CK(cudaStreamSynchronize(st));
 
@@ -286,8 +274,7 @@ int pcr_run(hb_handle* h, const DevRows& X, int d, const int32_t* batches, int n
 
 int run_pcr(hb_handle* h, const DevRows& X, int d, const int32_t* batches, int n_batches, int n_comps, double* var,
             double* r2, double* components, double* score, cudaStream_t caller) {
-  if (X.n < 2) return fail(h, 2, "hb_pcr: N = %lld rows, at least 2 are needed", (long long)X.n);
-  TRY(check_search_shape(h, "hb_pcr", "N", X.n, d));
+  TRY(check_score_shape(h, "hb_pcr", X.n, d));
   if (n_batches < 1) return fail(h, 2, "hb_pcr: n_batches = %d, at least one batch is needed", n_batches);
   if (n_batches > X.n) return fail(h, 2, "hb_pcr: %d batches, more codes than the N = %lld rows", n_batches, (long long)X.n);
   if (n_comps < 1) return fail(h, 2, "hb_pcr: n_comps = %d, at least one component is needed", n_comps);
@@ -297,11 +284,8 @@ int run_pcr(hb_handle* h, const DevRows& X, int d, const int32_t* batches, int n
   TRY(check_device_ptr(h, r2, "r2"));
   if (components) TRY(check_device_ptr(h, components, "components"));
   TRY(check_device_ptr(h, score, "score"));
-  CK(cudaSetDevice(h->device));
-  return on_caller_stream(h, caller, [&] {
-    RegionScope rs(h, "pcr");
-    return pcr_run(h, X, d, batches, n_batches, n_comps, var, r2, components, score);
-  });
+  return run_score(h, caller, "pcr",
+                   [&] { return pcr_run(h, X, d, batches, n_batches, n_comps, var, r2, components, score); });
 }
 
 }  // namespace

@@ -1,7 +1,6 @@
 // silhouette_host.cuh — hb_silhouette (DESIGN §11): the checks and the launches of silhouette.cuh: the (group, label)
-// index (build_tuple_index, tuples.cuh, into the score scratch), the column sums and sorted preparation of knn.cuh, the
-// finite counts, the tile list and the sweep.  The call needs no setup and
-// touches no state of a Harmony run or a mapping.  Included by harmony_b200.cu.
+// index, sorted preparation and finite counts (pair_index, score_host.cuh), the tile list and the sweep.  The call needs
+// no setup and touches no state of a Harmony run or a mapping.  Included by harmony_b200.cu.
 #pragma once
 
 namespace {
@@ -23,12 +22,6 @@ SilGeometry sil_geometry(int d) {
     }
   g.smem = sil_smem_bytes(g.tq, g.stages, g.KD);
   return g;
-}
-
-// The shape refusals hb_silhouette and hb_debug_silhouette_geometry share; h may be null (no message)
-int sil_check_shape(hb_handle* h, int64_t N, int d) {
-  if (N < 2) return refuse(h, "hb_silhouette: N = %lld rows, at least 2 are needed", (long long)N);
-  return check_search_shape(h, "hb_silhouette", "N", N, d);
 }
 
 // The eight values of hb_debug_silhouette_geometry
@@ -66,30 +59,10 @@ std::vector<int4> sil_tiles(const TupleIndex& ti, int n_labels, int tq) {
 int silhouette_run(hb_handle* h, const DevRows& X, int d, const int32_t* labels, int n_labels, const int32_t* groups,
                    int n_groups, double* s_out) {
   ScoreScratch& s = score_scratch(h);
-  const int64_t N = X.n;
   const SilGeometry g = sil_geometry(d);
-  const cudaStream_t st = h->stream;
-  CK(s.phi.reserve(2 * (size_t)N));
-  CK(s.rows.reserve((size_t)N * g.KD));
-  CK(s.hx.reserve((size_t)N));
-  CK(s.centre.reserve((size_t)KNN_MAX_D));
-  // ---- the index of the (group, label) pairs: the sorted order and the pair starts
-  k_silhouette_phi<<<grid_for(N, 256, h->num_sms * 8), 256, 0, st>>>(labels, groups, N, n_labels, n_groups, s.phi.p);
-  CKL();
-  TupleKeys keys;
-  TRY(tuple_keys(h, {n_groups, n_labels}, keys));
   TupleIndex ti;
   static const char* const names[2] = {"hb_silhouette: groups", "hb_silhouette: labels"};
-  TRY(build_tuple_index(h, s.phi.p, N, keys, false, s.sort_perm, s.inv_sort, ti, names));
-  const int J = (int)ti.uniq.size();
-  CK(s.pstart.reserve((size_t)J + 1));
-  CK(s.count.reserve((size_t)J));
-  TRY(upload_vector(h, s.pstart, std::vector<int>(ti.tstart.begin(), ti.tstart.end())));
-  CK(cudaMemsetAsync(s.count.p, 0, sizeof(int) * J, st));
-  // ---- centre, rows in sorted order, finite rows per pair
-  TRY(prepare_centred(h, X, d, g.KD, false, s.centre.p, s.rows.p, s.hx.p, s.sort_perm.p));
-  k_silhouette_count<<<grid_for(N, 256, h->num_sms * 8), 256, 0, st>>>(s.hx.p, N, s.pstart.p, J, s.count.p);
-  CKL();
+  TRY(pair_index(h, X, d, g.KD, groups, n_groups, labels, n_labels, names, ti));
   // ---- the sweep
   const std::vector<int4> tiles = sil_tiles(ti, n_labels, g.tq);
   CK(s.tiles.reserve(tiles.size()));
@@ -102,7 +75,7 @@ int silhouette_run(hb_handle* h, const DevRows& X, int d, const int32_t* labels,
 
 int run_silhouette(hb_handle* h, const DevRows& X, int d, const int32_t* labels, int n_labels, const int32_t* groups,
                    int n_groups, double* s, cudaStream_t caller) {
-  TRY(sil_check_shape(h, X.n, d));
+  TRY(check_score_shape(h, "hb_silhouette", X.n, d));
   if (n_labels < 1) return fail(h, 2, "hb_silhouette: n_labels = %d, at least one label is needed", n_labels);
   if (groups && n_groups < 1) return fail(h, 2, "hb_silhouette: n_groups = %d, at least one group is needed", n_groups);
   if (!groups) n_groups = 1;
@@ -112,11 +85,8 @@ int run_silhouette(hb_handle* h, const DevRows& X, int d, const int32_t* labels,
   TRY(check_device_ptr(h, labels, "labels"));
   if (groups) TRY(check_device_ptr(h, groups, "groups"));
   TRY(check_device_ptr(h, s, "s"));
-  CK(cudaSetDevice(h->device));
-  return on_caller_stream(h, caller, [&] {
-    RegionScope rs(h, "silhouette");
-    return silhouette_run(h, X, d, labels, n_labels, groups, n_groups, s);
-  });
+  return run_score(h, caller, "silhouette",
+                   [&] { return silhouette_run(h, X, d, labels, n_labels, groups, n_groups, s); });
 }
 
 }  // namespace

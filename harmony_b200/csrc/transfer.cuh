@@ -253,6 +253,9 @@ template <typename F>
 auto with_rows(const DevRows& r, F&& f) {
   return r.dtype == HB_FLOAT32 ? f((const float*)r.p) : f((const double*)r.p);
 }
+// The element type of the pointer with_rows passes: row_t<decltype(p)> is float or double
+template <typename P>
+using row_t = std::remove_const_t<std::remove_pointer_t<P>>;
 // `later` waits for the work queued on `earlier` so far (no host synchronisation)
 int stream_after(hb_handle* h, cudaStream_t later, cudaStream_t earlier) {
   if (later == earlier) return 0;

@@ -7,8 +7,8 @@ runs on an existing object.  Argument errors are raised before the CUDA library 
 """
 import numpy as np
 
-from ._arrays import (codes_on, current_stream, dense_codes, download, embedding, factorise, label_columns,
-                      label_vector, ptr, resolve_device, rows_on)
+from ._arrays import (call, codes_on, dense_codes, dense_on, device_of, download, embedding, factorise_for, handle,
+                      label_columns, label_vector, ptr, resolve_device, row_layout, rows_on, to_host)
 from .utils import is_cuda_tensor
 
 MAX_NEIGHBORS = 65   # hb_knn's k <= 64 other cells, plus the cell itself
@@ -47,18 +47,13 @@ def components_on(obj, idx, labels=None):
     if labels is not None:
         labels, n_labels = dense_codes(labels, N, "labels")
     import torch
-    device = torch.device("cuda", obj._scalar("device"))
+    device = device_of(obj)
     host = not is_cuda_tensor(idx)
-    idx = codes_on(obj, idx)
-    if N > 1 and not (idx.stride(1) == 1 and idx.stride(0) >= k):
-        idx = idx.contiguous()
-    ld = idx.stride(0) if N > 1 else k
-    if labels is not None:
-        labels = codes_on(obj, labels).contiguous()
+    idx, ld = row_layout(codes_on(obj, idx), k)
+    labels = dense_on(obj, labels)
     comp = torch.empty(N, dtype=torch.int32, device=device)
     largest = torch.empty(max(n_labels, 1), dtype=torch.int32, device=device)
-    obj._check(obj._L.hb_graph_components(obj._h, ptr(idx), int(ld), int(N), int(k), ptr(labels), int(n_labels),
-                                          ptr(comp), ptr(largest), current_stream(device)))
+    call(obj, "hb_graph_components", ptr(idx), ld, int(N), int(k), ptr(labels), int(n_labels), ptr(comp), ptr(largest))
     return tuple(download(host, comp, largest))
 
 
@@ -82,9 +77,8 @@ def graph_components(idx, labels=None, device=None):
             raise ValueError("labels are a CUDA tensor but idx is not: device labels go with a device idx")
         if is_cuda_tensor(labels) and labels.device != idx.device:
             raise ValueError(f"labels are on {labels.device}, idx on {idx.device}")
-        codes = factorise(labels, idx.device if on_device else None)[1]
-    from .harmony import harmony  # needs the CUDA extension; fails loudly when it is missing
-    return components_on(harmony(device=resolve_device(device, idx, "idx")), idx, codes)
+        codes = factorise_for(labels, idx)[1]
+    return components_on(handle(resolve_device(device, idx, "idx")), idx, codes)
 
 
 def connectivity_fold(largest, counts):
@@ -104,7 +98,6 @@ def graph_connectivity(X, meta_data, label_key, n_neighbors=15, device=None, ret
     ``n_neighbors - 1`` others, exact and Euclidean, 2 <= n_neighbors <= 65.  A row with a non-finite value has no
     neighbours and is nobody's neighbour: a component of its own.  ``meta_data`` as ``compute_lisi`` takes it.  A CUDA
     ``X`` (float32 / float64) stays on its device until the final fold; d <= 128."""
-    on_device = is_cuda_tensor(X)
     X = embedding(X, "X")
     N = X.shape[0]
     if isinstance(n_neighbors, bool) or int(n_neighbors) != n_neighbors:
@@ -113,11 +106,9 @@ def graph_connectivity(X, meta_data, label_key, n_neighbors=15, device=None, ret
         raise ValueError(f"n_neighbors = {n_neighbors} is not supported here (2 <= n_neighbors <= "
                          f"{min(MAX_NEIGHBORS, N)}: at most {MAX_NEIGHBORS}, and the N = {N} rows)")
     (labels,) = label_columns(meta_data, [label_key], X)
-    device = resolve_device(device, X, "X")
-    from .harmony import harmony  # needs the CUDA extension; fails loudly when it is missing
+    obj = handle(resolve_device(device, X, "X"))
     from .neighbors import knn_on
-    obj = harmony(device=device)
-    levels, codes = factorise(labels, X.device if on_device else None)
+    levels, codes = factorise_for(labels, X)
     _, x, _ = rows_on(obj, X, "X")
     idx, _ = knn_on(obj, x, None, int(n_neighbors) - 1)
     codes = codes_on(obj, codes)
@@ -128,5 +119,5 @@ def graph_connectivity(X, meta_data, label_key, n_neighbors=15, device=None, ret
     score = connectivity_fold(largest, counts)
     if not return_all:
         return score
-    levels = levels.cpu().numpy() if is_cuda_tensor(levels) else levels
+    levels = to_host(levels)
     return score, {(v.item() if hasattr(v, "item") else v): float(largest[i] / counts[i]) for i, v in enumerate(levels)}

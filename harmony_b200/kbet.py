@@ -7,9 +7,8 @@ existing object.  Argument errors are raised before the CUDA library is loaded.
 """
 import numpy as np
 
-from ._arrays import (codes_on, current_stream, dense_codes, download, embedding, factorise, label_columns, ptr,
-                      resolve_device, rows_on)
-from .utils import is_cuda_tensor
+from ._arrays import (call, check_two_rows, dense_codes, dense_on, device_of, download, embedding, factorise_for,
+                      handle, label_columns, ptr, resolve_device, rows_on, to_host)
 
 MAX_K0 = 129       # the cell and the sweep's longest list of 128 neighbours
 RULE_MAX_K0 = 70   # scib's rule: min(70, max(10, floor(mean batch size / 4)))
@@ -35,26 +34,23 @@ def kbet_on(obj, X, batches, labels=None, k0=0, return_neighbors=False):
     and for the other rows."""
     X = embedding(X, "X")
     N, d = X.shape
-    if N < 2:
-        raise ValueError(f"X has {N} rows, at least 2 are needed")
+    check_two_rows(X)
     k0 = check_k0(k0)
     batches, n_batches = dense_codes(batches, N, "batches")
     n_labels = 0
     if labels is not None:
         labels, n_labels = dense_codes(labels, N, "labels")
     import torch
-    device = torch.device("cuda", obj._scalar("device"))
+    device = device_of(obj)
     host, x, x_args = rows_on(obj, X, "X")
-    batches = codes_on(obj, batches).contiguous()
-    if labels is not None:
-        labels = codes_on(obj, labels).contiguous()
+    batches, labels = dense_on(obj, batches), dense_on(obj, labels)
     stat = torch.empty(N, dtype=torch.float64, device=device)
     pval = torch.empty(N, dtype=torch.float64, device=device)
     k0_out = torch.empty(max(n_labels, 1), dtype=torch.int32, device=device)
     width = (k0 or RULE_MAX_K0) - 1
     idx = torch.empty((N, width), dtype=torch.int32, device=device) if return_neighbors else None
-    obj._check(obj._L.hb_kbet(obj._h, *x_args, N, int(d), ptr(batches), int(n_batches), ptr(labels), int(n_labels),
-                              int(k0), ptr(stat), ptr(pval), ptr(k0_out), ptr(idx), int(width), current_stream(device)))
+    call(obj, "hb_kbet", *x_args, N, int(d), ptr(batches), int(n_batches), ptr(labels), int(n_labels), int(k0), ptr(stat),
+         ptr(pval), ptr(k0_out), ptr(idx), int(width))
     if return_neighbors:
         idx = idx[:, :max(int(k0_out.max()) - 1, 0)]
     out = download(host, stat, pval, k0_out, idx)
@@ -86,29 +82,23 @@ def kbet(X, meta_data, batch_key, label_key=None, k0=None, alpha=0.05, scaled=Tr
     The neighbours are exact and Euclidean; a cell with a non-finite value takes no part and gets NaN.  ``meta_data``
     as ``compute_lisi`` takes it.  A CUDA ``X`` (float32 / float64) stays on its device until the final fold, and
     ``(stat, pval)`` are then CUDA tensors; d <= 128."""
-    on_device = is_cuda_tensor(X)
     X = embedding(X, "X")
     N = X.shape[0]
-    if N < 2:
-        raise ValueError(f"X has {N} rows, at least 2 are needed")
+    check_two_rows(X)
     k0 = check_k0(k0)
     if isinstance(alpha, bool) or not isinstance(alpha, (int, float, np.integer, np.floating)) or not 0 < alpha < 1:
         raise ValueError(f"alpha must be a number in (0, 1), not {alpha!r}")
     names = [batch_key] + ([label_key] if label_key is not None else [])
     cols = label_columns(meta_data, names, X)
-    device = resolve_device(device, X, "X")
-    from .harmony import harmony  # needs the CUDA extension; fails loudly when it is missing
-    obj = harmony(device=device)
-    dev = X.device if on_device else None
-    bcodes = factorise(cols[0], dev)[1]
-    levels, lcodes = factorise(cols[1], dev) if label_key is not None else (None, None)
+    obj = handle(resolve_device(device, X, "X"))
+    bcodes = factorise_for(cols[0], X)[1]
+    levels, lcodes = factorise_for(cols[1], X) if label_key is not None else (None, None)
     stat, pval, k0_out = kbet_on(obj, X, bcodes, lcodes, k0)
-    host = lambda v: v.cpu().numpy() if is_cuda_tensor(v) else np.asarray(v)  # noqa: E731
-    codes = host(lcodes) if lcodes is not None else np.zeros(N, np.int32)
-    rates = kbet_fold(host(pval), codes, host(k0_out), alpha)
+    codes = to_host(lcodes) if lcodes is not None else np.zeros(N, np.int32)
+    rates = kbet_fold(to_host(pval), codes, to_host(k0_out), alpha)
     tested = rates[~np.isnan(rates)]
     score = float("nan") if not len(tested) else float(1 - tested.mean() if scaled else tested.mean())
     if not return_all:
         return score
-    keys = [None] if levels is None else [v.item() if hasattr(v, "item") else v for v in host(levels)]
+    keys = [None] if levels is None else [v.item() if hasattr(v, "item") else v for v in to_host(levels)]
     return score, dict(zip(keys, rates.tolist())), (stat, pval)

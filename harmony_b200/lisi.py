@@ -8,8 +8,8 @@ import math
 
 import numpy as np
 
-from ._arrays import (code_sets, codes_on, current_stream, download, embedding, factorise, label_columns, ptr,
-                      resolve_device, rows_on)
+from ._arrays import (call, code_sets, codes_on, device_of, download, embedding, factorise_for, handle, label_columns,
+                      ptr, resolve_device, row_layout, rows_on)
 from .utils import is_cuda_tensor
 
 MAX_K = 128   # the neighbour lists of hb_lisi's search: perplexity < 43 1/3
@@ -39,19 +39,16 @@ def lisi_on(obj, X, codes, perplexity=30, return_neighbors=False):
     k = neighbours_for(perplexity, N)
     codes = code_sets(codes, N)
     import torch
-    device = torch.device("cuda", obj._scalar("device"))
+    device = device_of(obj)
     host, x, x_args = rows_on(obj, X, "X")
-    codes = codes_on(obj, codes)
-    if not (codes.stride(1) == 1 and (codes.shape[0] == 1 or codes.stride(0) >= N)):
-        codes = codes.contiguous()
-    ld = codes.stride(0) if codes.shape[0] > 1 else N
+    codes, ld = row_layout(codes_on(obj, codes), N)
     out = torch.empty((N, codes.shape[0]), dtype=torch.float64, device=device)
     idx = dist = None
     if return_neighbors:
         idx = torch.empty((N, k), dtype=torch.int32, device=device)
         dist = torch.empty((N, k), dtype=torch.float32, device=device)
-    obj._check(obj._L.hb_lisi(obj._h, *x_args, N, int(d), ptr(codes), int(ld), int(codes.shape[0]), float(perplexity),
-                              ptr(out), ptr(idx), ptr(dist), current_stream(device)))
+    call(obj, "hb_lisi", *x_args, N, int(d), ptr(codes), ld, int(codes.shape[0]), float(perplexity), ptr(out), ptr(idx),
+         ptr(dist))
     out, idx, dist = download(host, out, idx, dist)
     return (out, idx, dist) if return_neighbors else out
 
@@ -76,10 +73,8 @@ def compute_lisi(X, meta_data, label_colnames, perplexity=30, device=None, retur
     if not names:
         raise ValueError("label_colnames names no column")
     cols = label_columns(meta_data, names, X)
-    device = resolve_device(device, X, "X")
-    from .harmony import harmony  # needs the CUDA extension; fails loudly when it is missing
-    obj = harmony(device=device)
-    codes = [factorise(c, X.device if on_device else None)[1] for c in cols]
+    obj = handle(resolve_device(device, X, "X"))
+    codes = [factorise_for(c, X)[1] for c in cols]
     if on_device:
         import torch
         codes = torch.stack(codes)

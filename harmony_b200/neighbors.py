@@ -6,7 +6,7 @@ reference cells.  Argument errors are raised before the CUDA library is loaded.
 """
 import numpy as np
 
-from ._arrays import current_stream, download, embedding, factorise, ptr, resolve_device, rows_on
+from ._arrays import call, device_of, download, embedding, factorise, handle, ptr, resolve_device, rows_on
 from .utils import is_cuda_tensor
 
 METRIC = {"euclidean": 0, "cosine": 1}   # enum hb_metric
@@ -45,13 +45,13 @@ def knn_on(obj, query, ref=None, k=15, metric="euclidean"):
     """``knn`` on an existing ``harmony`` object (any state: the search needs no setup and changes none)."""
     query, ref = _check_args(query, ref, k, metric)
     import torch
-    device = torch.device("cuda", obj._scalar("device"))
+    device = device_of(obj)
     host, q, q_args = rows_on(obj, query, "query")
     _, x, x_args = (host, q, q_args) if ref is None else rows_on(obj, ref, "ref")
     idx = torch.empty((q.shape[0], int(k)), dtype=torch.int32, device=device)
     dist = torch.empty((q.shape[0], int(k)), dtype=torch.float32, device=device)
-    obj._check(obj._L.hb_knn(obj._h, *q_args, q.shape[0], *x_args, x.shape[0], int(q.shape[1]), int(k), METRIC[metric],
-                             int(ref is None), ptr(idx), ptr(dist), current_stream(device)))
+    call(obj, "hb_knn", *q_args, q.shape[0], *x_args, x.shape[0], int(q.shape[1]), int(k), METRIC[metric],
+         int(ref is None), ptr(idx), ptr(dist))
     return tuple(download(host, idx, dist))
 
 
@@ -65,8 +65,7 @@ def knn(query, ref=None, k=15, metric="euclidean", device=None):
     Rows with non-finite values have no neighbours and are nobody's neighbour (``idx = -1``, ``dist = inf`` fill a row
     with fewer than k candidates)."""
     query, ref = _check_args(query, ref, k, metric)
-    from .harmony import harmony  # needs the CUDA extension; fails loudly when it is missing
-    return knn_on(harmony(device=resolve_device(device, query, "query")), query, ref, k, metric)
+    return knn_on(handle(resolve_device(device, query, "query")), query, ref, k, metric)
 
 
 def vote(idx, dist, codes, n_labels):

@@ -10,9 +10,8 @@ import warnings
 
 import numpy as np
 
-from ._arrays import (codes_on, current_stream, dense_codes, download, embedding, factorise, label_columns, ptr,
-                      resolve_device, rows_on)
-from .utils import is_cuda_tensor
+from ._arrays import (call, check_two_rows, dense_codes, dense_on, device_of, download, embedding, factorise_for,
+                      handle, label_columns, ptr, resolve_device, rows_on)
 
 
 def check_n_comps(n_comps):
@@ -32,21 +31,20 @@ def pcr_on(obj, X, batches, n_comps=50):
     tensor on the object's device).  The arrays come back as numpy arrays for host rows, CUDA tensors otherwise."""
     X = embedding(X, "X")
     N, d = X.shape
-    if N < 2:
-        raise ValueError(f"X has {N} rows, at least 2 are needed")
+    check_two_rows(X)
     n_comps = check_n_comps(n_comps)
     batches, n_batches = dense_codes(batches, N, "batches")
     import torch
-    device = torch.device("cuda", obj._scalar("device"))
+    device = device_of(obj)
     host, x, x_args = rows_on(obj, X, "X")
-    batches = codes_on(obj, batches).contiguous()
+    batches = dense_on(obj, batches)
     m = min(n_comps, N, d)
     var = torch.empty(m, dtype=torch.float64, device=device)
     r2 = torch.empty(m, dtype=torch.float64, device=device)
     comps = torch.empty((m, d), dtype=torch.float64, device=device)
     score = torch.empty(1, dtype=torch.float64, device=device)
-    obj._check(obj._L.hb_pcr(obj._h, *x_args, N, int(d), ptr(batches), int(n_batches), int(n_comps), ptr(var), ptr(r2),
-                             ptr(comps), ptr(score), current_stream(device)))
+    call(obj, "hb_pcr", *x_args, N, int(d), ptr(batches), int(n_batches), int(n_comps), ptr(var), ptr(r2), ptr(comps),
+         ptr(score))
     var, r2, comps = download(host, var, r2, comps)
     return var, r2, comps, float(score.item())
 
@@ -59,16 +57,12 @@ def pcr(X, meta_data, batch_key, n_comps=50, return_all=False, device=None):
 
     A row with a non-finite value takes no part.  ``meta_data`` as ``compute_lisi`` takes it.  A CUDA ``X`` (float32
     / float64) stays on its device, and the arrays are then CUDA tensors; d <= 128."""
-    on_device = is_cuda_tensor(X)
     X = embedding(X, "X")
-    if X.shape[0] < 2:
-        raise ValueError(f"X has {X.shape[0]} rows, at least 2 are needed")
+    check_two_rows(X)
     n_comps = check_n_comps(n_comps)
     col = label_columns(meta_data, [batch_key], X)[0]
-    device = resolve_device(device, X, "X")
-    from .harmony import harmony  # needs the CUDA extension; fails loudly when it is missing
-    obj = harmony(device=device)
-    codes = factorise(col, X.device if on_device else None)[1]
+    obj = handle(resolve_device(device, X, "X"))
+    codes = factorise_for(col, X)[1]
     var, r2, comps, score = pcr_on(obj, X, codes, n_comps)
     return (score, var, r2, comps) if return_all else score
 
@@ -94,9 +88,8 @@ def pcr_comparison(X_before, X_after, meta_data, batch_key, n_comps=50, scale=Tr
     batch variance is gone, 0: it did not shrink; set to 0 with a warning when it grew) or, unless ``scale``, as
     after - before.  Harmony: ``pcr_comparison(obj.getZorig().T, obj.getZcorr().T, meta, "dataset")``."""
     X_before, X_after = embedding(X_before, "X_before"), embedding(X_after, "X_after")
-    for name, Z in (("X_before", X_before), ("X_after", X_after)):
-        if Z.shape[0] < 2:
-            raise ValueError(f"{name} has {Z.shape[0]} rows, at least 2 are needed")
+    check_two_rows(X_before, "X_before")
+    check_two_rows(X_after, "X_after")
     if X_before.shape[0] != X_after.shape[0]:
         raise ValueError(f"X_before has {X_before.shape[0]} rows and X_after {X_after.shape[0]}: they must hold the "
                          f"same cells")

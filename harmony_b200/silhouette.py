@@ -9,8 +9,9 @@ library is loaded.
 """
 import numpy as np
 
-from ._arrays import (codes_on, current_stream, dense_codes, download, embedding, factorise, label_columns,
-                      label_device, label_vector, ptr, resolve_device, rows_on)
+from ._arrays import (call, check_two_rows, dense_codes, dense_on, device_of, download, embedding, factorise,
+                      factorise_for, handle, label_columns, label_device, label_vector, ptr, resolve_device, rows_on,
+                      to_host)
 from .utils import is_cuda_tensor
 
 
@@ -19,21 +20,16 @@ def silhouette_on(obj, X, labels, groups=None):
     ``labels`` / ``groups``: dense codes 0..n-1 (numpy or int32 CUDA tensors on the object's device)."""
     X = embedding(X, "X")
     N, d = X.shape
-    if N < 2:
-        raise ValueError(f"X has {N} rows, at least 2 are needed")
+    check_two_rows(X)
     labels, n_labels = dense_codes(labels, N, "labels")
     n_groups = 0
     if groups is not None:
         groups, n_groups = dense_codes(groups, N, "groups")
     import torch
-    device = torch.device("cuda", obj._scalar("device"))
     host, x, x_args = rows_on(obj, X, "X")
-    labels = codes_on(obj, labels).contiguous()
-    if groups is not None:
-        groups = codes_on(obj, groups).contiguous()
-    out = torch.empty(N, dtype=torch.float64, device=device)
-    obj._check(obj._L.hb_silhouette(obj._h, *x_args, N, int(d), ptr(labels), int(n_labels), ptr(groups),
-                                    int(n_groups), ptr(out), current_stream(device)))
+    labels, groups = dense_on(obj, labels), dense_on(obj, groups)
+    out = torch.empty(N, dtype=torch.float64, device=device_of(obj))
+    call(obj, "hb_silhouette", *x_args, N, int(d), ptr(labels), int(n_labels), ptr(groups), int(n_groups), ptr(out))
     return download(host, out)[0]
 
 
@@ -54,21 +50,18 @@ def silhouette_samples(X, labels, groups=None, device=None):
     on_device = is_cuda_tensor(X)
     X = embedding(X, "X")
     N = X.shape[0]
-    if N < 2:
-        raise ValueError(f"X has {N} rows, at least 2 are needed")
+    check_two_rows(X)
     cols = {"labels": label_vector(labels, N, "labels")}
     if groups is not None:
         cols["groups"] = label_vector(groups, N, "groups")
     label_device(cols, list(cols), X, on_device)
     device = resolve_device(device, X, "X")
-    dev = X.device if on_device else None
-    codes = factorise(cols["labels"], dev)[1]
-    gcodes = factorise(cols["groups"], dev)[1] if groups is not None else None
+    codes = factorise_for(cols["labels"], X)[1]
+    gcodes = factorise_for(cols["groups"], X)[1] if groups is not None else None
     n = _n_levels(codes)
     if groups is None and not 1 < n < N:
         raise ValueError(f"Number of labels is {n}. Valid values are 2 to n_samples - 1 (inclusive)")
-    from .harmony import harmony  # needs the CUDA extension; fails loudly when it is missing
-    return silhouette_on(harmony(device=device), X, codes, gcodes)
+    return silhouette_on(handle(device), X, codes, gcodes)
 
 
 def silhouette_label(X, meta_data, label_key, scale=True):
@@ -108,6 +101,5 @@ def silhouette_batch(X, meta_data, batch_key, label_key, scale=True, return_all=
     X = embedding(X, "X")
     batch, label = label_columns(meta_data, [batch_key, label_key], X)
     s = silhouette_samples(X, batch, groups=label)
-    host = lambda v: v.cpu().numpy() if is_cuda_tensor(v) else np.asarray(v)  # noqa: E731
-    asw, means = batch_fold(host(s), host(batch), host(label), scale)
+    asw, means = batch_fold(to_host(s), to_host(batch), to_host(label), scale)
     return (asw, means) if return_all else asw

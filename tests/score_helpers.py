@@ -1,5 +1,5 @@
-"""What the GPU tests of the embedding scores (knn, LISI, silhouette) share: their data, their input stand-ins, the
-band check of the neighbour search, the handle-state scenario and the refusal loop."""
+"""What the GPU tests of the score calls share: data, non-finite rows, input stand-ins, the band check of the neighbour
+search, the handle-state, refusal, unwritten-output and stream-order scenarios."""
 import ctypes
 from types import SimpleNamespace
 
@@ -13,6 +13,14 @@ def generic(rng, n, d, types=12):
     M = rng.standard_normal((types, d)) * 3.0
     t = rng.integers(0, types, n)
     return M[t] + rng.standard_normal((n, d)), t
+
+
+def non_finite_rows(X):
+    """The non-finite values of the table cases, written into the rows X in place: NaN rows 3, 700 and 2000, +inf in
+    column 5 of rows 11 and 2500, -inf in column 0 of row 1200."""
+    X[[3, 700, 2000]] = np.nan
+    X[[11, 2500], 5] = np.inf
+    X[1200, 0] = -np.inf
 
 
 class Frame:
@@ -118,3 +126,20 @@ def refusals_launch_nothing(g, call, good, bad):
     for change in bad:
         assert call(dict(good, **change)) == 2 and L.hb_last_error(g._h), change
         assert g.kernel_launches == 0, change
+
+
+def unwritten(fill, *outs):
+    """Every output tensor of a refused call still holds the value ``fill`` it was filled with."""
+    for t in outs:
+        assert (t.cpu().numpy() == fill).all()
+
+
+def after_late_write(src, fill, sleep, call):
+    """What ``call(dst)`` returns on a new stream right after torch fills ``dst`` with ``fill`` (None: uninitialised),
+    spins for ``sleep`` cycles and copies ``src`` into it there: a call ordered on that stream reads the copy."""
+    import torch
+    with torch.cuda.stream(torch.cuda.Stream()):
+        dst = torch.empty_like(src) if fill is None else torch.full_like(src, fill)
+        torch.cuda._sleep(sleep)
+        dst.copy_(src)
+        return call(dst)

@@ -11,7 +11,7 @@ import components_restatement as cr
 from harmony_b200 import RunHarmony, graph_components, graph_connectivity, knn
 from harmony_b200._arrays import ptr
 from helpers import gpu_harmony
-from score_helpers import generic, handle_state_untouched, refusals_launch_nothing
+from score_helpers import after_late_write, generic, handle_state_untouched, refusals_launch_nothing, unwritten
 
 pytestmark = pytest.mark.gpu
 
@@ -264,7 +264,7 @@ def test_range_refusals(case):
     st = L.hb_graph_components(g._h, ptr(it), ld, N, k, ptr(lt), 4, ptr(comp), ptr(largest), None)
     assert st == 2 and L.hb_last_error(g._h).decode() == msg
     assert g.kernel_launches == 1 == g.region_time("components")[1]
-    assert (comp.cpu().numpy() == -9).all() and (largest.cpu().numpy() == -9).all()
+    unwritten(-9, comp, largest)
 
 
 def test_stream_order():
@@ -273,14 +273,9 @@ def test_stream_order():
     rng = np.random.default_rng(12)
     idx = shuffled_path(rng, 1 << 18)
     src = torch.as_tensor(idx, device="cuda:0")
-    s = torch.cuda.Stream()
     g = gpu_harmony()
-    with torch.cuda.stream(s):
-        dst = torch.full_like(src, -1)
-        torch.cuda._sleep(200_000_000)
-        dst.copy_(src)
-        comp, largest = g.graph_components(dst)
-        comp, largest = comp.cpu().numpy(), largest.cpu().numpy()
+    comp, largest = after_late_write(src, -1, 200_000_000,
+                                     lambda dst: [v.cpu().numpy() for v in g.graph_components(dst)])
     assert (comp == 0).all() and largest.tolist() == [1 << 18]
 
 

@@ -13,7 +13,8 @@ import knn_restatement as knr
 from harmony_b200 import RunHarmony, kbet
 from harmony_b200._arrays import ptr
 from helpers import gpu_harmony, load_cell_lines
-from score_helpers import Frame, check_band, generic, handle_state_untouched, refusals_launch_nothing, strided
+from score_helpers import (Frame, after_late_write, check_band, generic, handle_state_untouched, non_finite_rows,
+                           refusals_launch_nothing, strided, unwritten)
 from silhouette_restatement import finite_rows
 
 pytestmark = pytest.mark.gpu
@@ -72,9 +73,7 @@ def _case(name, N, d, o):
     if o.get("duplicates"):
         X[N // 2:N // 2 + 1000] = X[:1000]
     if o.get("nan"):
-        X[[3, 700, 2000]] = np.nan
-        X[[11, 2500], 5] = np.inf
-        X[1200, 0] = -np.inf
+        non_finite_rows(X)
     lab = None if lab is None else lab.astype(np.int32)
     return X, b.astype(np.int32), lab, max(n_labels, 1), n_batches
 
@@ -273,8 +272,7 @@ def test_late_refusals_write_nothing(case):
         a.update(k0=30, ld=28)
         msg = "hb_kbet: idx_ld = 28 is smaller than the 29 neighbours of the largest k0"
     assert _call(L, g, a) == 2 and L.hb_last_error(g._h).decode() == msg
-    assert (stat.cpu().numpy() == -9).all() and (pval.cpu().numpy() == -9).all()
-    assert (k0o.cpu().numpy() == -9).all() and (idx.cpu().numpy() == -9).all()
+    unwritten(-9, stat, pval, k0o, idx)
 
 
 def test_launch_count_and_stream_order():
@@ -299,13 +297,8 @@ def test_launch_count_and_stream_order():
     g = gpu_harmony()
     g.kbet(xt[:40], bt[:40], small)
     assert g.kernel_launches == sil
-    s = torch.cuda.Stream()
     g = gpu_harmony()
-    with torch.cuda.stream(s):
-        dst = torch.full_like(xt, float("nan"))
-        torch.cuda._sleep(200_000_000)
-        dst.copy_(xt)
-        got = [v.cpu().numpy() for v in g.kbet(dst, bt, lt)]
+    got = after_late_write(xt, float("nan"), 200_000_000, lambda dst: [v.cpu().numpy() for v in g.kbet(dst, bt, lt)])
     for u, v in zip(want, got):
         np.testing.assert_array_equal(u, v)
 

@@ -9,9 +9,9 @@ import pytest
 import kmeans_score_restatement as kr
 import knn_restatement as knr
 from harmony_b200 import RunHarmony, kmeans, nmi_ari, nmi_ari_cluster_labels_kmeans
-from harmony_b200._arrays import ptr
+from harmony_b200._arrays import ptr, to_host
 from helpers import gpu_harmony, load_cell_lines
-from score_helpers import Frame, handle_state_untouched, refusals_launch_nothing, strided
+from score_helpers import Frame, after_late_write, handle_state_untouched, refusals_launch_nothing, strided, unwritten
 
 pytestmark = pytest.mark.gpu
 
@@ -58,7 +58,7 @@ def test_seeding_replays(row):
     name, N, d, K, dtype, o = row
     X = _case(name, N, d, K, o)
     labels, centres, inertia, n_iter, seeds = kmeans(_input(X, dtype, o), K, seed=5, max_iter=0, return_seeds=True)
-    seeds = np.asarray(seeds.cpu() if hasattr(seeds, "cpu") else seeds)[0]
+    seeds = to_host(seeds)[0]
     fin, P, _ = kr.prepare(X.astype(dtype))
     if N <= 20000:
         exact = kr.replay_seeds(P, fin, K, 5, 0, seeds)
@@ -66,8 +66,8 @@ def test_seeding_replays(row):
             np.testing.assert_array_equal(seeds, kr.seeding(P, fin, K, 5))
     assert len(set(seeds.tolist())) == K or N == K
     assert fin[seeds].all()
-    assert int(np.asarray(n_iter if not hasattr(n_iter, "cpu") else n_iter.cpu())[0]) == 0
-    C = np.asarray(centres.cpu() if hasattr(centres, "cpu") else centres)
+    assert int(to_host(n_iter)[0]) == 0
+    C = to_host(centres)
     np.testing.assert_array_equal(C, X.astype(dtype).astype(np.float64)[seeds])
 
 
@@ -88,9 +88,8 @@ def test_one_step_within_band(row):
     fp64 argmin within §9's band."""
     name, N, d, K, dtype, o = row
     X = _case(name, N, d, K, o)
-    host = lambda v: np.asarray(v.cpu() if hasattr(v, "cpu") else v)  # noqa: E731
-    lab0, C0, _, _, seeds = map(host, kmeans(_input(X, dtype, o), K, seed=1, max_iter=0, return_seeds=True))
-    labels, C, _, n_iter = map(host, kmeans(_input(X, dtype, o), K, seed=1, max_iter=1, tol=0.0))
+    lab0, C0, _, _, seeds = map(to_host, kmeans(_input(X, dtype, o), K, seed=1, max_iter=0, return_seeds=True))
+    labels, C, _, n_iter = map(to_host, kmeans(_input(X, dtype, o), K, seed=1, max_iter=1, tol=0.0))
     assert int(n_iter[0]) == 1
     Xd = X.astype(dtype).astype(np.float64)
     fin = np.isfinite(Xd).all(axis=1)
@@ -158,21 +157,25 @@ def test_duplicates_and_empty_clusters_are_deterministic():
     assert float(a[2][0]) <= 1e-20  # every row sits on its centre, the fp64 mean of identical rows
 
 
+def _sevens(K):
+    """The outputs of a 10-row, 3-column call into K clusters, filled with 7: labels, centres, inertia, n_iter."""
+    import torch
+    return [torch.full(s, 7, dtype=t, device="cuda:0")
+            for s, t in (((10,), torch.int32), ((K, 3), torch.float64), ((1,), torch.float64), ((1,), torch.int32))]
+
+
 def test_too_few_finite_rows_is_status_3_outputs_untouched():
     import torch
     from harmony_b200 import _lib
     X = torch.full((10, 3), float("nan"), device="cuda:0", dtype=torch.float64)
     X[:4] = 1.0
     g = gpu_harmony()
-    labels = torch.full((10,), 7, dtype=torch.int32, device="cuda:0")
-    C = torch.full((5, 3), 7.0, dtype=torch.float64, device="cuda:0")
-    ine = torch.full((1,), 7.0, dtype=torch.float64, device="cuda:0")
-    nit = torch.full((1,), 7, dtype=torch.int32, device="cuda:0")
+    labels, C, ine, nit = _sevens(5)
     st = _lib.lib().hb_kmeans(g._h, ptr(X), 1, 3, 10, 3, 5, 0, 1, 300, 1e-4, ptr(labels), ptr(C), ptr(ine), ptr(nit),
                               ptr(None), None)
     torch.cuda.synchronize()
     assert st == 3 and b"finite" in _lib.lib().hb_last_error(g._h)
-    assert (labels == 7).all() and (C == 7).all() and (ine == 7).all() and (nit == 7).all()
+    unwritten(7, labels, C, ine, nit)
 
 
 def test_row_beyond_fp32_range_is_status_2_outputs_untouched():
@@ -183,15 +186,12 @@ def test_row_beyond_fp32_range_is_status_2_outputs_untouched():
     X[:, 0] = torch.arange(10, device="cuda:0")
     X[4, 1] = 1e20
     g = gpu_harmony()
-    labels = torch.full((10,), 7, dtype=torch.int32, device="cuda:0")
-    C = torch.full((2, 3), 7.0, dtype=torch.float64, device="cuda:0")
-    ine = torch.full((1,), 7.0, dtype=torch.float64, device="cuda:0")
-    nit = torch.full((1,), 7, dtype=torch.int32, device="cuda:0")
+    labels, C, ine, nit = _sevens(2)
     st = _lib.lib().hb_kmeans(g._h, ptr(X), 1, 3, 10, 3, 2, 0, 1, 300, 1e-4, ptr(labels), ptr(C), ptr(ine), ptr(nit),
                               ptr(None), None)
     torch.cuda.synchronize()
     assert st == 2 and b"2^124" in _lib.lib().hb_last_error(g._h)
-    assert (labels == 7).all() and (C == 7).all() and (ine == 7).all() and (nit == 7).all()
+    unwritten(7, labels, C, ine, nit)
     X[4, 1] = 1e18  # |x - m|^2 ~ 1e36 < 2^124: runs, and every row takes part
     out = kmeans(X, 2, seed=0)
     assert (out[0] >= 0).all()
@@ -303,12 +303,7 @@ def test_launch_count_and_stream_order():
         counts.append(g.kernel_launches)
         assert g.region_time("kmeans")[1] == g.kernel_launches
     assert counts[2] - counts[1] == counts[1] - counts[0] == 14
-    s = torch.cuda.Stream()
-    with torch.cuda.stream(s):
-        Y = torch.empty_like(X)
-        torch.cuda._sleep(20_000_000)
-        Y.copy_(X)
-        lab = kmeans(Y, 10, seed=1)[0]
+    lab = after_late_write(X, None, 20_000_000, lambda Y: kmeans(Y, 10, seed=1)[0])
     torch.cuda.synchronize()
     np.testing.assert_array_equal(lab.cpu().numpy(), kmeans(X, 10, seed=1)[0].cpu().numpy())
 

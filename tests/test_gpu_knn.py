@@ -164,6 +164,19 @@ def test_numpy_and_tensor_paths_agree():
     np.testing.assert_array_equal(d0, d1.cpu().numpy())
 
 
+def test_single_strided_query_row():
+    """One query row taken as X.T[:1] of a [d, N] tensor (column stride N) is read as that row, not as the first d
+    values of its memory: the same lists as the row made contiguous."""
+    import torch
+    X = torch.as_tensor(generic(np.random.default_rng(8), 40, 3000)[0], device="cuda:0")   # [d, N]
+    q, ref = X.T[:1], X.T.contiguous()
+    i0, d0 = knn(q, ref, k=10)
+    i1, d1 = knn(q.contiguous(), ref, k=10)
+    assert q.stride(1) == 3000 and int(i0[0, 0]) == 0
+    np.testing.assert_array_equal(i0.cpu().numpy(), i1.cpu().numpy())
+    np.testing.assert_array_equal(d0.cpu().numpy(), d1.cpu().numpy())
+
+
 def test_handle_state_untouched():
     """hb_knn between cluster_cpp and moe_correct_ridge_cpp, and on a mapping handle before and after hb_map: Z_corr, R
     and Y read bit for bit the same before and after the call, and the run ends where a run without it ends (to the

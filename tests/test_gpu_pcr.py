@@ -13,7 +13,8 @@ import pcr_restatement as pr
 from harmony_b200 import RunHarmony, pcr, pcr_comparison
 from harmony_b200._arrays import ptr
 from helpers import gpu_harmony, load_cell_lines
-from score_helpers import Frame, handle_state_untouched, refusals_launch_nothing, strided
+from score_helpers import (Frame, after_late_write, handle_state_untouched, non_finite_rows, refusals_launch_nothing,
+                           strided, unwritten)
 
 pytestmark = pytest.mark.gpu
 
@@ -45,9 +46,7 @@ def _case(name, N, d, B, o):
     if o.get("offset"):
         X += o["offset"]
     if o.get("nan"):
-        X[[3, 700, 2000]] = np.nan
-        X[[11, 2500], 5] = np.inf
-        X[1200, 0] = -np.inf
+        non_finite_rows(X)
     return X, b.astype(np.int32), (N if B == 0 else B)
 
 
@@ -181,7 +180,7 @@ def test_refusals_launch_nothing():
     refusals_launch_nothing(g, lambda a: _call(L, g, a), good, bad)
     assert _call(L, g, dict(good, comp=None)) == 0     # the components are optional
     assert g.kernel_launches > 0
-    assert (comp.cpu().numpy() == -9).all()
+    unwritten(-9, comp)
 
 
 @pytest.mark.parametrize("case", ["batch_past_n_batches", "batch_negative"])
@@ -200,8 +199,7 @@ def test_range_refusal_writes_nothing(case):
     a = dict(X=ptr(X), xt=0, xld=d, N=N, d=d, bat=ptr(bat), nb=2, nc=8, var=ptr(outs[0]), r2=ptr(outs[1]),
              comp=ptr(outs[2]), score=ptr(outs[3]))
     assert _call(L, g, a) == 2 and L.hb_last_error(g._h).decode() == msg
-    for t in outs:
-        assert (t.cpu().numpy() == -9).all()
+    unwritten(-9, *outs)
 
 
 def test_launch_count_and_stream_order():
@@ -219,13 +217,8 @@ def test_launch_count_and_stream_order():
     g = gpu_harmony()
     g.pcr(xt, torch.zeros_like(bt), 20)
     assert g.kernel_launches == 6 + 7
-    s = torch.cuda.Stream()
     g = gpu_harmony()
-    with torch.cuda.stream(s):
-        dst = torch.full_like(xt, float("nan"))
-        torch.cuda._sleep(200_000_000)
-        dst.copy_(xt)
-        got = g.pcr(dst, bt, 20)
+    got = after_late_write(xt, float("nan"), 200_000_000, lambda dst: g.pcr(dst, bt, 20))
     for u, v in zip(want[:3], got[:3]):
         np.testing.assert_array_equal(u.cpu().numpy(), v.cpu().numpy())
     assert want[3] == got[3]

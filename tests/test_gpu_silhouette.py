@@ -10,7 +10,7 @@ import silhouette_restatement as sr
 from harmony_b200 import RunHarmony, silhouette_batch, silhouette_label, silhouette_samples
 from harmony_b200._arrays import ptr
 from helpers import gpu_harmony, load_cell_lines
-from score_helpers import Frame, generic, handle_state_untouched, refusals_launch_nothing, strided
+from score_helpers import Frame, generic, handle_state_untouched, non_finite_rows, refusals_launch_nothing, strided
 
 pytestmark = pytest.mark.gpu
 
@@ -64,9 +64,7 @@ def _case(name, N, d, o):
     if o.get("duplicates"):
         X[N // 2:N // 2 + 1000] = X[:1000]
     if o.get("nan"):
-        X[[3, 700, 2000]] = np.nan
-        X[[11, 2500], 5] = np.inf
-        X[1200, 0] = -np.inf
+        non_finite_rows(X)
     return X, t.astype(np.int32), None if g is None else g.astype(np.int32)
 
 

@@ -148,3 +148,21 @@ def test_geometry_hook_matches_the_rule():
     for d, k in ((129, 5), (0, 5), (50, 65), (50, 0)):
         st, g = _geometry(d, k, 1000, 1000, 132)
         assert st == 2 and g == [-7] * 8
+
+
+def test_row_layout_reads_only_unit_stride_rows_in_place():
+    """The layout rule of every caller array the scores read (_arrays.row_layout), on CPU tensors: row-strided [N, d]
+    views are read in place with their stride; a transposed view, and a single row whose column stride is not 1, are
+    made contiguous first."""
+    import torch
+    from harmony_b200._arrays import row_layout
+    A = torch.arange(20.).reshape(4, 5)
+    one = A.T[:1]                                   # [1, 4], strides (1, 5): elements 0, 5, 10, 15
+    t, ld = row_layout(one, 4)
+    assert t.stride(1) == 1 and ld == 4 and t.flatten().tolist() == [0.0, 5.0, 10.0, 15.0]
+    t, ld = row_layout(A[:1], 5)                    # one dense row: in place
+    assert t.data_ptr() == A.data_ptr() and ld == 5
+    t, ld = row_layout(A[:, :3], 3)                 # [4, 3] of row stride 5: in place
+    assert t.data_ptr() == A.data_ptr() and ld == 5
+    t, ld = row_layout(A.T, 4)                      # [5, 4] transposed: contiguous
+    assert t.is_contiguous() and ld == 4 and torch.equal(t, A.T)
