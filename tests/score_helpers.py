@@ -72,7 +72,7 @@ def handle_state_untouched(call, baseline=False):
     the two mappings use the reference of the run with the call."""
     import torch
     from harmony_b200 import prepare_inputs
-    from helpers import make_perms, make_Y0, rel_l2
+    from helpers import gpu_setup, make_perms, make_Y0, rel_l2
     Z, meta = synthetic(20000, 50, [4], n_types=10, seed=3)
     a = prepare_inputs(Z, meta, "cov0", nclust=50, early_stop=False)
     Y0, perms = make_Y0(Z, 50, 1), make_perms(20000, 2 * a["max_iter_kmeans"], 2).reshape(2, a["max_iter_kmeans"], -1)
@@ -90,9 +90,7 @@ def handle_state_untouched(call, baseline=False):
     runs = (False, True) if baseline else (True,)
     outs = []
     for with_call in runs:
-        g = gpu_harmony()
-        g.setup(a["Z"], a["phi_i"], a["sigma"], a["theta"], a["lambda_"], a["alpha"], a["max_iter_kmeans"],
-                a["epsilon_kmeans"], a["epsilon_harmony"], 50, a["block_size"], a["B_vec"], a["batch_proportion_cutoff"])
+        g = gpu_setup(a, K=50, device=0)
         g.init_cluster_cpp(Y0)
         for it in range(2):
             assert g.cluster_cpp(perms[it]) == 0

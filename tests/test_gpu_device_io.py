@@ -12,7 +12,7 @@ import numpy as np
 import pytest
 
 from harmony_b200 import RunHarmony, prepare_inputs
-from helpers import free_port, make_perms, make_Y0, rel_l2, synthetic
+from helpers import free_port, gpu_setup, make_perms, make_Y0, rel_l2, synthetic
 
 pytestmark = pytest.mark.gpu
 
@@ -20,14 +20,6 @@ torch = pytest.importorskip("torch")
 
 HB_Z_CORR, HB_Z_ORIG, HB_R, HB_Y = 0, 1, 2, 3
 HB_FLOAT32, HB_FLOAT64 = 0, 1
-
-
-def new(a, Z, T=None):
-    from harmony_b200.harmony import harmony
-    g = harmony(device=0)
-    g.setup(Z, a["phi_i"], a["sigma"], a["theta"], a["lambda_"], a["alpha"], a["max_iter_kmeans"] if T is None else T,
-            a["epsilon_kmeans"], a["epsilon_harmony"], a["K"], a["block_size"], a["B_vec"], a["batch_proportion_cutoff"])
-    return g
 
 
 def iterate(g, Y0, perms):
@@ -74,19 +66,19 @@ def c3():
 def test_setup_from_tensor_is_bit_identical(size, request):
     a = request.getfixturevalue(size)
     Z = a["Z"]
-    host = new(a, Z)
-    dev = new(a, torch.from_numpy(Z).cuda())
+    host = gpu_setup(a, Z, device=0)
+    dev = gpu_setup(a, torch.from_numpy(Z).cuda(), device=0)
     assert np.array_equal(dev.getZorig(), host.getZorig())
     assert np.array_equal(dev.getZcorr(), host.getZcorr())
     Z32 = Z.astype(np.float32)
-    g32 = new(a, torch.from_numpy(Z32).cuda())
+    g32 = gpu_setup(a, torch.from_numpy(Z32).cuda(), device=0)
     assert np.array_equal(g32.getZorig().T, Z32.astype(np.float64))
 
 
 def test_get_tensor_matches_host_getters(small):
     a = small
     N, T = a["Z"].shape[0], a["max_iter_kmeans"]
-    g = new(a, a["Z"])
+    g = gpu_setup(a, a["Z"], device=0)
 
     def check():
         for name, host in (("Z_corr", g.getZcorr), ("Z_orig", g.getZorig), ("R", g.getR)):
@@ -109,15 +101,16 @@ def test_strided_and_transposed_tensors(small):
     a = small
     Z = a["Z"]
     N, d = Z.shape
-    ref = new(a, Z).getZorig()
+    ref = gpu_setup(a, Z, device=0).getZorig()
     wide = torch.zeros((N, d + 7), dtype=torch.float64, device="cuda")
     wide[:, :d] = torch.from_numpy(Z).cuda()
     view = wide[:, :d]                                   # row stride d + 7
     assert view.stride() == (d + 7, 1)
-    assert np.array_equal(new(a, view).getZorig(), ref)
+    assert np.array_equal(gpu_setup(a, view, device=0).getZorig(), ref)
     Zt = torch.from_numpy(np.ascontiguousarray(Z.T)).cuda()   # d x N, cells as columns
-    assert np.array_equal(new(a, Zt).getZorig(), ref)
-    assert np.array_equal(new(a, torch.from_numpy(Z).cuda().T).getZorig(), ref)   # d x N view of N x d memory
+    assert np.array_equal(gpu_setup(a, Zt, device=0).getZorig(), ref)
+    dxn = torch.from_numpy(Z).cuda().T                      # d x N view of N x d memory
+    assert np.array_equal(gpu_setup(a, dxn, device=0).getZorig(), ref)
 
 
 @pytest.mark.parametrize("dtype", [torch.float32, torch.float64])
@@ -131,8 +124,8 @@ def test_unaligned_tensor_and_output(small, dtype):
     view = buf[1:].view(N, d)
     view.copy_(torch.from_numpy(Z.astype(npdt)))
     assert view.data_ptr() % 16 != 0
-    g = new(a, view)
-    aligned = new(a, torch.from_numpy(Z.astype(npdt)).cuda())
+    g = gpu_setup(a, view, device=0)
+    aligned = gpu_setup(a, torch.from_numpy(Z.astype(npdt)).cuda(), device=0)
     assert np.array_equal(g.getZorig(), aligned.getZorig())
     assert np.array_equal(g.getZcorr(), aligned.getZcorr())
     # output one element off and with row stride d + 1: the extra column must stay untouched
@@ -154,7 +147,7 @@ def test_whole_runs_match_host_runs(small):
     perms = make_perms(N, 2 * T, 4).reshape(2, T, N)
 
     def run(Zin):
-        g = new(a, Zin)
+        g = gpu_setup(a, Zin, device=0)
         iterate(g, Y0, perms)
         return g.getZcorr(), g.getR()
 
@@ -192,7 +185,7 @@ def test_side_stream_ordering(small):
     """Input written on a side stream and read by setup, result read on that stream: no explicit synchronisation."""
     a = small
     Z = a["Z"]
-    ref = new(a, Z)
+    ref = gpu_setup(a, Z, device=0)
     src = torch.from_numpy(Z).cuda()
     torch.cuda.synchronize()
     s = torch.cuda.Stream()
@@ -200,7 +193,7 @@ def test_side_stream_ordering(small):
         Zd = torch.empty_like(src)
         torch.cuda._sleep(50_000_000)      # keeps the stream busy well past the enqueue of setup's copy
         Zd.copy_(src)
-        g = new(a, Zd)
+        g = gpu_setup(a, Zd, device=0)
         assert np.array_equal(g.getZorig(), ref.getZorig())
         torch.cuda._sleep(50_000_000)      # the getter's copy must wait for this
         out = g.get_tensor("Z_orig", torch.float64)
@@ -233,10 +226,8 @@ def test_rejected_before_any_launch(small):
     assert "hb_setup_device" in g._L.hb_last_error(g._h).decode()
     assert g.kernel_launches == 0
     with pytest.raises(TypeError):
-        g.setup(Zd.half(), a["phi_i"], a["sigma"], a["theta"], a["lambda_"], a["alpha"], a["max_iter_kmeans"],
-                a["epsilon_kmeans"], a["epsilon_harmony"], a["K"], a["block_size"], a["B_vec"],
-                a["batch_proportion_cutoff"])
-    g = new(a, Zd)
+        gpu_setup(a, Zd.half(), device=0)
+    g = gpu_setup(a, Zd, device=0)
     n0 = g.kernel_launches
     for host in (False, True):   # a second setup
         assert raw_setup(g, a, Zd.data_ptr(), HB_FLOAT64, d, host=host) == 3, host
@@ -259,11 +250,9 @@ def test_rejected_before_any_launch(small):
     if torch.cuda.device_count() < 2:
         return
     other = torch.from_numpy(Z).to("cuda:1")
-    g2 = harmony(device=0)
     with pytest.raises(ValueError):
-        g2.setup(other, a["phi_i"], a["sigma"], a["theta"], a["lambda_"], a["alpha"], a["max_iter_kmeans"],
-                 a["epsilon_kmeans"], a["epsilon_harmony"], a["K"], a["block_size"], a["B_vec"],
-                 a["batch_proportion_cutoff"])
+        gpu_setup(a, other, device=0)
+    g2 = harmony(device=0)
     assert raw_setup(g2, a, other.data_ptr(), HB_FLOAT64, d) == 2
     assert "device 1" in g2._L.hb_last_error(g2._h).decode()
     assert g2.kernel_launches == 0

@@ -14,7 +14,6 @@ comparison measures that step alone:
 Every row asserts the premise it is named for (its kernel path, and re-runs, exact ties or infinite keys where named).
 """
 import ctypes
-from collections import namedtuple
 
 import numpy as np
 import pytest
@@ -23,11 +22,10 @@ from harmony_b200 import _lib
 from helpers import num_sms
 from kmeans_restatement import (LLOYD_STEPS, canonical_clusters, exact_rows, kmeans_uniform, lloyd_eps,
                                 lloyd_step_model, race_delta, race_intervals, start_cells)
-from stages import ALPHA, BLOCK, CUTOFF, SIGMA, T, TOL_ZN
+from kmeans_rows import CASES, ROWS, Row
+from stages import ALPHA, BLOCK, CUTOFF, SIGMA, T, TOL_ZN, wide_paths
 
 SEED = 77
-HB_KS_FFMA, HB_KS_WIDE = 1, 16
-M_FFMA, M_TC, M_LOGITS, M_WIDE = 1, 2, 3, 4     # hb_debug_wide_paths' k-means values
 # a Lloyd mean against the fp64 mean of its definite members, max |d|.  The fp32 sums of m unit rows (atomics on the
 # FFMA path, 3xTF32 K3 on the logits path) err by ~sqrt(m) 2^-24 on the mean for m <= 2000 members (~1e-7); one
 # member dropped or added moves the mean by ~1 / m >= 5e-4.  Measured on an H100: at most 0.24 of the bar (tc_K12).
@@ -37,59 +35,6 @@ TOL_KM_MEAN = 1e-5
 # in the fp64 restatement
 AMB_RATE = 0.02
 
-Row = namedtuple("Row", "K d N J kind launches")
-ROWS = {
-    "tc_K12": Row(12, 12, 3000, 3, "blobs", 1),
-    "tc_K64": Row(64, 50, 20000, 5, "blobs", 1),
-    "tc_K65": Row(65, 50, 20000, 5, "blobs", 2),
-    "tc_K128": Row(128, 64, 20000, 5, "blobs", 2),
-    "tc_K129": Row(129, 64, 20000, 5, "blobs", 3),
-    "tc_K256_d120": Row(256, 120, 20000, 5, "blobs", 4),
-    "ffma_K257_d120": Row(257, 120, 20000, 5, "blobs", None),
-    "ffma_d121": Row(100, 121, 20000, 5, "blobs", None),
-    "ffma_at_limit": Row(400, 128, 20000, 5, "blobs", None),
-    "wide_past_limit": Row(401, 128, 20000, 5, "blobs", None),
-    "tc_K450_d120": Row(450, 120, 20000, 5, "blobs", 8),
-    "tc_K1024_d64": Row(1024, 64, 19000, 3, "blobs", 16),      # N: enough blobs that few cells are ambiguous
-    "wide_K200_d512": Row(200, 512, 20000, 3, "blobs", None),
-    "c3like": Row(100, 50, 200000, 20, "blobs", 2),
-    "wide_forced_K705_d8": Row(705, 8, 20000, 5, "blobs", None),
-    "d1": Row(5, 1, 2000, 2, "d1", 1),
-    "antipodal": Row(64, 16, 1500, 3, "antipodal", 1),
-    "special_rows_J1": Row(100, 50, 20000, 1, "special", 2),
-    "special_rows_J100": Row(100, 50, 20000, 100, "special", 2),
-    "N_equals_K": Row(40, 16, 40, 1, "n_equals_k", 1),
-}
-# (row, kernel set, k-means path, NV of the race and pick kernels: sp_nv(KS), None on the FFMA path)
-CASES = [
-    ("tc_K12", 0, M_TC, 1),
-    ("tc_K64", 0, M_TC, 1),
-    ("tc_K65", 0, M_TC, 1),
-    ("tc_K128", 0, M_TC, 1),
-    ("tc_K129", 0, M_TC, 2),
-    ("tc_K256_d120", 0, M_TC, 2),                 # KS = 256 and d = 120: both limits of the LogitsTc choice
-    ("ffma_K257_d120", 0, M_FFMA, None),          # KS = 260 > 256
-    ("ffma_d121", 0, M_FFMA, None),               # d = 121: no k_logits_tc
-    ("ffma_at_limit", 0, M_FFMA, None),           # 4 K d = 200 KB exactly
-    ("wide_past_limit", 0, M_WIDE, 4),            # 4 K d = 200 KB + 512 B, d = 128: k_logits_wide
-    ("tc_K450_d120", 0, M_LOGITS, 4),             # past the FFMA limit, KS = 452 > 256
-    ("tc_K1024_d64", 0, M_LOGITS, 8),
-    ("wide_K200_d512", 0, M_WIDE, 2),
-    ("c3like", 0, M_TC, 1),
-    ("c3like", HB_KS_FFMA, M_FFMA, None),
-    ("c3like", HB_KS_WIDE, M_WIDE, 1),
-    ("wide_forced_K705_d8", HB_KS_WIDE, M_WIDE, 8),
-    ("d1", 0, M_TC, 1),
-    ("d1", HB_KS_FFMA, M_FFMA, None),
-    ("antipodal", 0, M_TC, 1),
-    ("antipodal", HB_KS_FFMA, M_FFMA, None),
-    ("special_rows_J1", 0, M_TC, 1),
-    ("special_rows_J1", HB_KS_FFMA, M_FFMA, None),
-    ("special_rows_J100", 0, M_TC, 1),
-    ("special_rows_J100", HB_KS_FFMA, M_FFMA, None),
-    ("N_equals_K", 0, M_TC, 1),
-    ("N_equals_K", HB_KS_FFMA, M_FFMA, None),
-]
 N_DUP = 40      # antipodal: exact copies of -e_0
 
 
@@ -124,12 +69,6 @@ def make_row(name):
         Z = np.tile(4.0 * e0, (N, 1))
         Z[rng.choice(N, 10, replace=False)] = rng.standard_normal((10, d))
     return Z, phi
-
-
-def wide_path(r, ks):
-    out = (ctypes.c_int64 * 4)()
-    _lib.lib().hb_debug_wide_paths(r.K, r.d, r.J, r.N, 20, num_sms(), ks, out)
-    return int(out[3])
 
 
 def new_model(r, Z, phi, ks, block=BLOCK):
@@ -210,7 +149,7 @@ def check_lloyd(X, means, K, d, N):
 def test_native_kmeans_init_step_by_step(name, ks, path, nv):
     r = ROWS[name]
     K, d, N = r.K, r.d, r.N
-    assert wide_path(r, ks) == path
+    assert wide_paths(r.K, r.d, r.J, r.N, num_sms(), kernel_set=ks)[3] == path
     Z, phi = make_row(name)
     g = new_model(r, Z, phi, ks)
     X32 = np.ascontiguousarray(g.getZcorr().T, dtype=np.float32)     # the library's normalised cells

@@ -20,15 +20,13 @@ import numpy as np
 import pytest
 
 from helpers import make_perms, num_sms
-from stages import (ALPHA, CUTOFF, PER_STEP, SINGLE_PASS, TOL_OBJ, TOL_OE, TOL_R, TWO_PASS, RunParams, _nested,
-                    _report, _set_zcorr, _sizes, build_case, cluster_and_compare, f32, kernel_paths, make_Y0,
-                    native_order, numpy_model, planted_zy, setup_gpu, state_errs, tables_of)
-from test_gpu_kernel_edges import EDGE_ROWS
-from test_gpu_run_parameters import sigma_vec, theta_levels
-from test_gpu_wide_shapes import A_FFMA, A_FUSED, A_LOGITS, A_WIDE, ROWS as WIDE_ROWS, wide_paths
+from stages import (A_FFMA, A_FUSED, A_LOGITS, A_WIDE, EDGE_ROWS, HB_KS_FFMA_CONTRACTIONS, HB_KS_WIDE, PER_STEP,
+                    SINGLE_PASS, TOL_OBJ, TOL_OE, TOL_R, TWO_PASS, RunParams, _nested, _report, _set_zcorr, _sizes,
+                    build_case, case_of, cluster_and_compare, f32, kernel_paths, make_Y0, native_order, numpy_model,
+                    oracle, planted_zy, prenormalised, setup_gpu, sigma_vec, state_errs, tables_of, theta_levels,
+                    wide_paths)
 
 TAG = "legacy"
-HB_KS_FFMA_CONTRACTIONS, HB_KS_WIDE = 1, 16
 # Y, the centroids of the call's last round, max |d|.  New bar: Y comes from the 3xTF32 statistics of K3 (relative
 # error of a product <= 2^-20) summed over the cells and normalised in fp32, from the R of the round before; measured
 # at most 1.0e-5 (d300_K100 after L1) and otherwise <= 7e-6 on an H100 80GB HBM3 (700 W)
@@ -73,15 +71,6 @@ LEGACY_ROWS = {
     # per-cluster sigma and per-level theta; nested covariates, fused K1 with one stage
     "sigma_theta_K113_d50": ("apply_K113_d50", 0, True, (SINGLE_PASS, 1, 0, 1, 1, 1, SINGLE_PASS, PER_STEP), A_FUSED),
 }
-
-
-def case_of(name, num_sms):
-    row = LEGACY_ROWS[name][0]
-    if row in EDGE_ROWS:
-        K, d, cov = EDGE_ROWS[row][:3]
-        return build_case(row, K, d, cov, num_sms, base=1000)
-    K, d, cov = WIDE_ROWS[row][:3]
-    return build_case(row, K, d, cov, num_sms, base=2000)
 
 
 def params_of(name, c, **kw):
@@ -131,12 +120,11 @@ def fp32_bars(c, p, Y0, perms1, Zp, Yp, perms3):
     and the call's error grows the more loosely the data pins them; the fp32 oracle measures that growth on the stage's
     own inputs.  The objective keeps stages.py's bar (the oracle sums it in fp32; its error is printed).  Returns the
     bars of L1 and of L3."""
-    from test_gpu_wide_shapes import _prenormalised
     got = {}
     for dbl in (False, True):
         got[dbl] = []
         for Z, Y, perms in ((c["Z"], Y0, perms1), (Zp, Yp, perms3)):
-            o = _oracle(c, p, dbl, _prenormalised(Z))
+            o = oracle(c, p, dbl, prenormalised(Z), legacy=True)
             o.init_cluster_cpp(Y)
             o.cluster_cpp(perms)
             got[dbl].append((o.get("R"), o.get("Y"), o.trace("objective_kmeans")[-p.T:]))
@@ -154,26 +142,15 @@ def fp32_bars(c, p, Y0, perms1, Zp, Yp, perms3):
 def test_legacy_rows_reach_their_kernels(name):
     """Each row's kernels on a 132-SM H100 with 20 update blocks; the last value of hb_debug_kernel_paths is the update
     path of a call with the legacy step (per step on every row)."""
-    c = case_of(name, 132)
+    c = case_of(LEGACY_ROWS[name][0], 132)
     _, ks, _, paths, assign = LEGACY_ROWS[name]
     J = len(c["sizes"])
     assert kernel_paths(c["K"], c["d"], J, c["N"], 132, kernel_set=ks) == paths
-    assert wide_paths(c["K"], c["d"], J, c["N"], 132, ks)[0] == assign
+    assert wide_paths(c["K"], c["d"], J, c["N"], 132, kernel_set=ks)[0] == assign
 
 
 def test_legacy_rows_cover_every_natural_order_assignment():
     assert {r[4] for r in LEGACY_ROWS.values()} == {A_FUSED, A_FFMA, A_LOGITS, A_WIDE}
-
-
-def _oracle(c, p, double=True, Z=None):
-    from oracle.oracle import OracleHarmony
-    B = sum(c["B_vec"])
-    o = OracleHarmony(double=double)
-    o.setup(Z=c["Z"] if Z is None else Z, phi_i=c["phi"], B_vec=np.asarray(c["B_vec"]), sigma=p.sigma_of(c["K"]),
-            theta=p.theta_of(B), lambda_=None, alpha=ALPHA, max_iter_kmeans=p.T, epsilon_kmeans=p.epsilon_kmeans,
-            epsilon_harmony=-np.inf, K=c["K"], block_size=p.block_size, batch_proportion_cutoff=CUTOFF)
-    o.set_legacy_centroid_step(True)
-    return o
 
 
 @pytest.mark.parametrize("name,stage", [("tiny_blocks", "L1"), ("tiny_blocks", "L2"), ("sigma_theta_K113_d50", "L2")])
@@ -181,14 +158,14 @@ def test_numpy_legacy_step_matches_oracle(name, stage):
     """The numpy legacy step and the fp64 oracle's agree on three covariates (L1, L2), on the empty and the 1e-22 mass
     clusters (L2), and under per-cluster sigma and per-level theta on nested covariates: this pins the restatement the
     GPU stages compare against, without a GPU."""
-    c = case_of(name, 132)
+    c = case_of(LEGACY_ROWS[name][0], 132)
     if name != "tiny_blocks":   # a smaller instance of the row's shape, for the oracle's plain loops
         K, d, _ = EDGE_ROWS[LEGACY_ROWS[name][0]][:3]
         c = build_case(name, K, d, lambda s: _nested(_sizes(10, 2000), 5), 132)
     p = params_of(name, c)
     rng = np.random.default_rng(11)
     Y0 = f32(make_Y0(c["Z"], c["K"], rng))
-    o = _oracle(c, p)
+    o = oracle(c, p, legacy=True)
     npy = numpy_model(c, c["Z"], None, p)
     npy.legacy_centroid_step = True
     o.init_cluster_cpp(Y0)
@@ -245,12 +222,12 @@ def test_early_stop_fixture_has_a_margin():
 @pytest.mark.parametrize("name", list(LEGACY_ROWS))
 def test_legacy_row_stages(name):
     sms = num_sms()
-    c = case_of(name, sms)
+    c = case_of(LEGACY_ROWS[name][0], sms)
     _, ks, _, paths, assign = LEGACY_ROWS[name]
     J = len(c["sizes"])
     if sms == 132:
         assert kernel_paths(c["K"], c["d"], J, c["N"], sms, kernel_set=ks) == paths
-    assert wide_paths(c["K"], c["d"], J, c["N"], sms, ks)[0] == assign
+    assert wide_paths(c["K"], c["d"], J, c["N"], sms, kernel_set=ks)[0] == assign
     p = params_of(name, c)
     rng = np.random.default_rng(11)
     Y0 = f32(make_Y0(c["Z"], c["K"], rng))

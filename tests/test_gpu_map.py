@@ -7,20 +7,11 @@ import numpy as np
 import pytest
 
 from harmony_b200 import HarmonyReference, MapQuery, RunHarmony, prepare_inputs
-from helpers import gpu_harmony, make_perms, make_Y0, num_sms, rel_l2, synthetic
+from helpers import gpu_harmony, gpu_setup, make_perms, make_Y0, num_sms, rel_l2, synthetic
 from map_restatement import assign, correct, lambda_levels, map_query, reference_stats, type_offset, weights_folded
-from stages import TOL_OE, TOL_R1, TOL_Y, TOL_Z, f32
+from stages import HB_KS_FFMA_CONTRACTIONS, HB_KS_WIDE, TOL_OE, TOL_R1, TOL_Y, TOL_Z, f32, wide_paths
 
 pytestmark = pytest.mark.gpu
-
-KS_FFMA, KS_WIDE = 1, 16
-
-
-def _wide_paths(K, d, J, n, kernel_set):
-    from harmony_b200 import _lib
-    out = (ctypes.c_int64 * 4)()
-    _lib.lib().hb_debug_wide_paths(K, d, J, n, 1, num_sms(), kernel_set, out)
-    return int(out[0]), int(out[2])
 
 
 # ---- compression ----------------------------------------------------------------------------------------------------
@@ -30,9 +21,7 @@ def test_reference_compression(d, K, N):
     d = 50 also after a further cluster_cpp, whose Z_corr the library normalises on the first read."""
     Z, meta = synthetic(N, d, [4], n_types=12, seed=d + K)
     a = prepare_inputs(Z, meta, "cov0", nclust=K, early_stop=False)
-    g = gpu_harmony()
-    g.setup(a["Z"], a["phi_i"], a["sigma"], a["theta"], a["lambda_"], a["alpha"], 5, a["epsilon_kmeans"],
-            a["epsilon_harmony"], K, a["block_size"], a["B_vec"], a["batch_proportion_cutoff"])
+    g = gpu_setup(a, T=5, device=0)
     g.init_cluster_cpp(make_Y0(Z, K, 1))
     perms = make_perms(N, 15, 2).reshape(3, 5, N)
     for it in range(2):
@@ -98,13 +87,13 @@ def planted_query(rng, N, d, B_vec, absent=(), special=False):
 ROWS = [
     # name, K, d, B_vec, kernel_set, (assign, apply) kernels, Nq, options
     ("fused_c1", 100, 50, [3], 0, (1, 1), 50000, dict(special=True, zero=5)),
-    ("ffma_c2_sigma_lam_cov", 100, 50, [3, 2], KS_FFMA, (2, 2), 5000,
+    ("ffma_c2_sigma_lam_cov", 100, 50, [3, 2], HB_KS_FFMA_CONTRACTIONS, (2, 2), 5000,
      dict(sigma="per_cluster", lam=[0.5, 2.0], special=True)),
     ("logits_c3", 300, 100, [2, 2, 2], 0, (3, 1), 129, dict(lam=0.3)),
-    ("dchunk_cols_b1", 100, 50, [1], KS_WIDE, (4, 3), 5, dict()),
+    ("dchunk_cols_b1", 100, 50, [1], HB_KS_WIDE, (4, 3), 5, dict()),
     ("ffma_cols_absent_zero", 64, 300, [4], 0, (2, 3), 2000, dict(absent=(1, 3), zero=7, sigma="per_cluster")),
     ("fused_nq1", 100, 50, [2], 0, (1, 1), 1, dict()),
-    ("wide_c2_absent", 200, 64, [3, 3], KS_WIDE, (4, 3), 3000, dict(absent=(4,), lam=[1.0, 0.2])),
+    ("wide_c2_absent", 200, 64, [3, 3], HB_KS_WIDE, (4, 3), 3000, dict(absent=(4,), lam=[1.0, 0.2])),
 ]
 
 
@@ -127,7 +116,8 @@ def test_map_stages(row):
     name, K, d, B_vec, kernel_set, paths, Nq, opts = row
     g, Z, phi, ref, lam = _map_row(K, d, B_vec, kernel_set, Nq, opts, seed=sum(map(ord, name)))
     J = len(np.unique(phi, axis=0))
-    assert _wide_paths(K, d, J, Nq, kernel_set) == paths
+    got = wide_paths(K, d, J, Nq, num_sms(), nb=1, kernel_set=kernel_set)
+    assert (got[0], got[2]) == paths          # natural-order assignment, ridge apply
     Rg = g.getR().T
     Zg = g.getZcorr().T
     np.testing.assert_array_equal(g.getZorig().T, f32(Z))

@@ -2,8 +2,8 @@
 the same inputs, with the k-means centroids and the per-round update orders injected into both
 (SURVEY.md §0.3: parity is only definable that way).
 
-Tolerances (BASELINE.json north_star): corrected embedding within 1e-4 rel-L2 of the reference-order
-fp32 oracle; hard cluster index argmax_k R identical except for cells whose top-2 gap is inside the
+Tolerances (BASELINE.json north_star; helpers.compare applies them): corrected embedding within 1e-4 rel-L2 of the
+reference-order fp32 oracle; hard cluster index argmax_k R identical except for cells whose top-2 gap is inside the
 fp32 noise band.  We additionally require the GPU to be no further from the fp64 oracle than
 2x the fp32 oracle is (+ a small floor).
 
@@ -25,102 +25,10 @@ import numpy as np
 import pytest
 
 from harmony_b200 import harmony_options, prepare_inputs
-from helpers import load_cell_lines, load_pbmc, make_perms, make_Y0, rel_l2, run_oracle, synthetic
+from helpers import (TOL_Z, assert_argmax_bounded, compare, gpu_setup, load_cell_lines, load_pbmc, make_perms, make_Y0,
+                     oracle_setup, rel_l2, run_gpu, run_oracle, synthetic)
 
 pytestmark = pytest.mark.gpu
-
-TOL_Z = 1e-4
-TIE_BAND = 1e-5
-ARGMAX_GAP_MAX = 1e-3     # a differing hard index is only tolerated on cells this close to a tie ...
-ARGMAX_FRAC_MAX = 5e-4    # ... and on at most this fraction of the cells
-
-
-def run_gpu(a, Y0, n_iter, perms, kernel_set=0):
-    from harmony_b200.harmony import harmony
-    g = harmony()
-    if kernel_set:
-        g.kernel_set = kernel_set   # test hook: force the kernels that serve out-of-limit shapes (read by setup)
-    g.setup(a["Z"], a["phi_i"], a["sigma"], a["theta"], a["lambda_"], a["alpha"], a["max_iter_kmeans"],
-            a["epsilon_kmeans"], a["epsilon_harmony"], a["K"], a["block_size"], a["B_vec"],
-            a["batch_proportion_cutoff"], False)
-    g.init_cluster_cpp(Y0)
-    iters = 0
-    for it in range(n_iter):
-        assert g.cluster_cpp(perms[it]) == 0
-        g.moe_correct_ridge_cpp()
-        iters += 1
-        if g.check_convergence(1):
-            break
-    return g, iters
-
-
-def argmax_mismatch_outside_band(Rg, Ro, band=TIE_BAND):
-    """#cells whose hard assignment differs although the oracle's top-2 gap exceeds the noise band."""
-    ag, ao = Rg.argmax(axis=1), Ro.argmax(axis=1)
-    part = np.partition(Ro, -2, axis=1)
-    gap = part[:, -1] - part[:, -2]
-    bad = (ag != ao) & (gap > band)
-    return int(bad.sum()), int((ag != ao).sum())
-
-
-def argmax_report(Rg, Ro):
-    """(#cells with a different hard index, largest top-2 gap of the oracle among them)."""
-    ag, ao = Rg.argmax(axis=1), Ro.argmax(axis=1)
-    m = ag != ao
-    if not m.any():
-        return 0, 0.0
-    part = np.partition(Ro[m], -2, axis=1)
-    return int(m.sum()), float((part[:, -1] - part[:, -2]).max())
-
-
-def assert_argmax_bounded(Rg, Ro, label, own_flips=0, own_dev=0.0):
-    """`own_flips` / `own_dev`: hard-index flips and max |dR| of the oracle instance `Ro` against the fp64 truth;
-    they widen the bounds, so that an fp32 oracle that has drifted itself (long sequential sums at several
-    100k cells per block) is not held against the GPU path."""
-    n, gap = argmax_report(Rg, Ro)
-    limit = max(1, int(np.ceil(ARGMAX_FRAC_MAX * Rg.shape[0]))) + own_flips
-    gap_max = max(ARGMAX_GAP_MAX, 2 * own_dev)
-    print(f"[{label}] hard-index mismatches: {n} of {Rg.shape[0]} (limit {limit}), largest oracle top-2 gap among them {gap:.2e} (limit {gap_max:.2e})")
-    assert n <= limit, (label, n, limit)
-    assert gap <= gap_max, (label, gap, gap_max)
-    return n
-
-
-def compare(g, o32, o64, label):
-    Zg, Z32, Z64 = g.getZcorr().T, o32.get("Z_corr"), o64.get("Z_corr")
-    Rg, R32, R64 = g.R.T, o32.get("R"), o64.get("R")
-    e_g32, e_g64, e_3264 = rel_l2(Zg, Z32), rel_l2(Zg, Z64), rel_l2(Z32, Z64)
-    dR = float(np.abs(Rg - R32).max())
-    dR64, dR3264 = float(np.abs(Rg - R64).max()), float(np.abs(R32 - R64).max())
-    # hard cluster index: identical to the fp64 truth wherever fp32 arithmetic can resolve it at all, i.e.
-    # outside a tie band of the fp32 oracle's own deviation from fp64 (>= 1e-5); the count against the
-    # fp32 oracle itself is reported as well (it flips with that oracle's sequential-sum noise)
-    bad, anydiff = argmax_mismatch_outside_band(Rg, R64, band=max(TIE_BAND, 2 * dR3264))
-    bad32, anydiff32 = argmax_mismatch_outside_band(Rg, R32)
-    dY = float(np.abs(g.Y.T - o32.get("Y")).max())
-    dO = float(np.abs(g.O.T - o32.get("O")).max() / max(1.0, np.abs(o32.get("O")).max()))
-    print(f"[{label}] relL2(Z gpu,o32)={e_g32:.2e} (gpu,o64)={e_g64:.2e} (o32,o64)={e_3264:.2e} "
-          f"max|dR|={dR:.2e} (vs o64 {dR64:.2e}; o32 vs o64 {dR3264:.2e}) max|dY|={dY:.2e} rel|dO|={dO:.2e} argmax diff={anydiff} outside band={bad}")
-    assert np.all(np.isfinite(Zg))
-    if e_3264 <= 0.5 * TOL_Z:
-        assert e_g32 <= TOL_Z
-    else:   # the reference-order fp32 arithmetic is itself outside the bar (module docstring)
-        assert e_g64 <= TOL_Z and e_g32 <= e_3264 + 1e-5, (e_g64, e_g32, e_3264)
-    assert e_g64 <= 2 * e_3264 + 2e-5
-    assert bad == 0
-    assert_argmax_bounded(Rg, R32, label + " vs oracle32", own_flips=argmax_report(R32, R64)[0], own_dev=dR3264)
-    assert_argmax_bounded(Rg, R64, label + " vs oracle64")
-    # the fp32 oracle carries the reference's own sequential-sum noise: judge R against the fp64 truth
-    assert dR64 <= 2 * dR3264 + 1e-5, (dR64, dR3264)
-    np.testing.assert_allclose(Rg.sum(axis=1), 1.0, atol=1e-5)
-    # traces: same lengths, values within fp32 summation noise of the fp64 truth
-    for name in ("objective_kmeans", "objective_harmony", "objective_kmeans_dist", "objective_kmeans_entropy",
-                 "objective_kmeans_cross"):
-        tg, t64 = getattr(g, name), o64.trace(name)
-        assert len(tg) == len(t64), name
-        np.testing.assert_allclose(tg, t64, rtol=2e-4, atol=2e-4, err_msg=name)
-    assert list(g.kmeans_rounds) == [int(x) for x in o32.trace("kmeans_rounds")]
-
 
 CASES = {
     # config 1 of BASELINE.json: cell_lines_small, 1 covariate, K=5
@@ -220,10 +128,7 @@ def test_ridge_step_against_plain_formulas(case):
     N, T = Z.shape[0], a["max_iter_kmeans"]
     Y0 = make_Y0(Z, a["K"], 17)
     perms = make_perms(N, T, 31)
-    from harmony_b200.harmony import harmony
-    g = harmony()
-    g.setup(a["Z"], a["phi_i"], a["sigma"], a["theta"], a["lambda_"], a["alpha"], T, a["epsilon_kmeans"],
-            a["epsilon_harmony"], a["K"], a["block_size"], a["B_vec"], a["batch_proportion_cutoff"], False)
+    g = gpu_setup(a)
     g.init_cluster_cpp(Y0)
     assert g.cluster_cpp(perms) == 0
     npy = NumpyHarmony(a["Z"], a["phi_i"], a["B_vec"], a["sigma"], a["theta"], a["lambda_"], a["alpha"], T, a["K"],
@@ -241,19 +146,13 @@ def test_ridge_step_against_plain_formulas(case):
 
 def test_parity_stepwise():
     """After init, after one clustering, after one correction: every exposed field against the oracle."""
-    from harmony_b200.harmony import harmony
-    from oracle.oracle import OracleHarmony
-    from helpers import setup_args
     (Z, meta) = load_cell_lines(False)
     a = prepare_inputs(Z, meta, ["cell_type", "dataset"], nclust=30)
     N, T = Z.shape[0], a["max_iter_kmeans"]
     Y0 = make_Y0(Z, a["K"], 3)
     perms = make_perms(N, T, 1)
-    o = OracleHarmony()
-    o.setup(**setup_args(a))
-    g = harmony()
-    g.setup(a["Z"], a["phi_i"], a["sigma"], a["theta"], a["lambda_"], a["alpha"], T, a["epsilon_kmeans"],
-            a["epsilon_harmony"], a["K"], a["block_size"], a["B_vec"], a["batch_proportion_cutoff"])
+    o = oracle_setup(a)
+    g = gpu_setup(a)
     assert (g.N, g.K, g.d, g.B) == (N, 30, 20, 5)
     np.testing.assert_allclose(g.getZorig().T, Z.astype(np.float32), rtol=0, atol=0)
     np.testing.assert_allclose(g.getZcorr().T, o.get("Z_corr"), atol=1e-6)

@@ -1,7 +1,7 @@
 """Stage tests of the hot-path kernels under run parameters other than the edge table's (scalar sigma = 0.1, theta = 2
 on every level, block size 0.05, 6 rounds per call, no early stop), against the fp64 numpy restatement.
 
-Each row pairs a shape of test_gpu_kernel_edges.py (or, for d127_K200, of test_gpu_wide_shapes.py) with one run
+Each row pairs a shape of stages.EDGE_ROWS (or, for d127_K200, of stages.WIDE_ROWS) with one run
 parameter, and names the code that parameter reaches:
 - sigma per cluster (fp32-distinct values in [0.1, 0.3], not monotone in k, sigma_0 not the smallest): the
   <NV, false> instances of the single-pass kernel and their objective sums, the two-pass kernel's sig_u = 0 branch,
@@ -19,51 +19,23 @@ parameter, and names the code that parameter reaches:
   rounds), and the native update orders of three such calls on each update path.
 The bars are the edge file's, except R in two places.  Where fp32 cannot hold the R bar on a row's inputs (the wide
 row; nb = 1, where round 0 removes every cell and O, E fall to fp32 noise), the bar is the wide file's: twice the fp32
-oracle's error on the same inputs, computed in the test and printed.  The wide row's R bars after S1 and S2 are 2e-5
-(measured reason at the row).
+oracle's error on the same inputs (stages.fp32_errors), computed in the test and printed.  The wide row's R bars after
+S1 and S2 are 2e-5 (measured reason at the row).
 """
 import numpy as np
 import pytest
 
 from helpers import make_perms, num_sms
-from numpy_restatement import my_ceil
-from stages import (ALPHA, CUTOFF, PER_STEP, SINGLE_PASS, TOL_OBJ, TOL_OE, TOL_R, TOL_R1, TWO_PASS, RunParams,
-                    _nested, _obj_err, _one_cov, _sizes, build_case, cluster_and_compare, f32, kernel_paths, make_Y0,
-                    native_order, numpy_model, planted_R, planted_zy, setup_gpu, stage_s1, stage_s2, stage_s3,
-                    state_errs, tables_of, _report, _table_err)
-from test_gpu_kernel_edges import EDGE_ROWS
-from test_gpu_wide_shapes import ROWS as WIDE_ROWS
+from stages import (EDGE_ROWS, HB_KS_UPDATE_PER_STEP, HB_KS_UPDATE_TWO_PASS, PER_STEP, SINGLE_PASS, TOL_OBJ, TOL_OE,
+                    TOL_R, TOL_R1, TWO_PASS, WIDE_ROWS, RunParams, _nested, _obj_err, _one_cov, _report, _sizes,
+                    block_for, case_of, cluster_and_compare, f32, fp32_errors, kernel_paths, make_Y0, native_order,
+                    numpy_model, oracle, planted_R, planted_zy, setup_gpu, sigma_vec, stage_s1, stage_s2, stage_s3,
+                    state_errs, tables_of, theta_levels)
 
-HB_KS_UPDATE_PER_STEP, HB_KS_UPDATE_TWO_PASS = 2, 4
 TAG = "runparam"
 
 
-def sigma_vec(K):
-    """0.1 (1 + 2 frac(0.618 (k + 3))): in [0.1, 0.3], not monotone, sigma_0 = 0.171 is not the smallest."""
-    k = np.arange(K)
-    return f32(0.1 * (1.0 + 2.0 * np.modf(0.618 * (k + 3))[0]))
-
-
-def theta_levels(B):
-    return np.array([(0.0, 0.5, 1.0, 2.0, 3.0)[b % 5] for b in range(B)])
-
-
-def block_for(nb):
-    """A block size that gives exactly nb blocks under the reference's my_ceil(1 / block_size)."""
-    for x in (nb, nb - 0.5):
-        bs = float(np.float32(1.0 / x))
-        if my_ceil(np.float32(1.0) / np.float32(bs)) == nb:
-            return bs
-    raise AssertionError(nb)
-
-
 # ---- rows ---------------------------------------------------------------------------------------------------------------
-def _shape(row):
-    if row in EDGE_ROWS:
-        return EDGE_ROWS[row][0], EDGE_ROWS[row][1], EDGE_ROWS[row][2]
-    return WIDE_ROWS[row][0], WIDE_ROWS[row][1], WIDE_ROWS[row][2]
-
-
 SIGMA_ROWS = {
     "k1_K33_d63": "fused K1 with per-cluster sigma, single-pass <1, false>",
     "logits_K129_d64": "k_logits_tc ranges at n_off 64 and 128, single-pass <2, false>",
@@ -109,12 +81,6 @@ EARLY_ROWS = [("k1_K33_d63", 6), ("k1_K33_d63", 8), ("two_pass_Jmax+1", 6), ("tw
               ("two_pass_Jmax+1", 40)]
 
 
-def case_of(row, num_sms, cov=None):
-    K, d, c0 = _shape(row)
-    base = 1000 if row in EDGE_ROWS else 2000
-    return build_case(row, K, d, cov or c0, num_sms, base=base)
-
-
 def update_path(c, num_sms, p, T=None, kernel_set=0):
     """The update path a call of T rounds takes (call_path: two-pass calls of more than 31 rounds run per step)."""
     path = kernel_paths(c["K"], c["d"], len(c["sizes"]), c["N"], num_sms, p.nb(), kernel_set)[0]
@@ -154,17 +120,6 @@ def test_block_rows_geometry():
             assert cpb == 1 and 1200 <= c["N"] <= 1700
 
 
-def _oracle_numpy_pair(c, p, Y0):
-    from oracle.oracle import OracleHarmony
-    B = sum(c["B_vec"])
-    o = OracleHarmony(double=True)
-    o.setup(Z=c["Z"], phi_i=c["phi"], B_vec=np.asarray(c["B_vec"]), sigma=p.sigma_of(c["K"]), theta=p.theta_of(B),
-            lambda_=None, alpha=ALPHA, max_iter_kmeans=p.T, epsilon_kmeans=p.epsilon_kmeans, epsilon_harmony=-np.inf,
-            K=c["K"], block_size=p.block_size, batch_proportion_cutoff=CUTOFF)
-    npy = numpy_model(c, c["Z"], None, p)
-    return o, npy
-
-
 def _agree(o, npy, n):
     assert np.abs(o.get("R") - npy.R).max() < 1e-9
     np.testing.assert_allclose(o.get("O").T, npy.O, rtol=1e-9, atol=1e-9)
@@ -185,7 +140,7 @@ def test_numpy_matches_oracle_on_run_parameters(what):
              early_stop=RunParams(T=8, epsilon_kmeans=np.inf))[what]
     rng = np.random.default_rng(3)
     Y0 = make_Y0(c["Z"], K, rng)
-    o, npy = _oracle_numpy_pair(c, p, Y0)
+    o, npy = oracle(c, p), numpy_model(c, c["Z"], None, p)
     o.init_cluster_cpp(Y0)
     npy.init_cluster(Y0)
     if what == "sigma_written":
@@ -205,39 +160,6 @@ def test_numpy_matches_oracle_on_run_parameters(what):
 
 
 # ---- GPU tests --------------------------------------------------------------------------------------------------------
-def _fp32_r_errors(c, p, Y0, R2, perms2, Zp, Yp, perms3, tables=False):
-    """max |R32 - R64| of the fp32 and fp64 oracles after S1, S2 and S3 on the stages' inputs (the wide file's rule);
-    tables: also the O and E errors (as _table_err measures them) after S2 and S3."""
-    from oracle.oracle import OracleHarmony
-    from test_gpu_wide_shapes import _prenormalised
-    B = sum(c["B_vec"])
-    R = {}
-    for dbl in (False, True):
-        def fresh(Z):
-            o = OracleHarmony(double=dbl)
-            o.setup(Z=Z, phi_i=c["phi"], B_vec=np.asarray(c["B_vec"]), sigma=p.sigma_of(c["K"]), theta=p.theta_of(B),
-                    lambda_=None, alpha=ALPHA, max_iter_kmeans=p.T, epsilon_kmeans=p.epsilon_kmeans,
-                    epsilon_harmony=-np.inf, K=c["K"], block_size=p.block_size, batch_proportion_cutoff=CUTOFF)
-            return o
-        o = fresh(_prenormalised(c["Z"]))
-        o.init_cluster_cpp(Y0)
-        r1 = o.get("R")
-        O2, E2 = tables_of(R2, c, o.get("Pr_b"))
-        o.set("R", R2)
-        o.set("O", O2.T)
-        o.set("E", E2.T)
-        o.cluster_cpp(perms2)
-        r2, t2 = o.get("R"), (o.get("O"), o.get("E"))
-        o = fresh(_prenormalised(Zp))
-        o.init_cluster_cpp(Yp)
-        o.cluster_cpp(perms3)
-        R[dbl] = (r1, r2, o.get("R"), t2, (o.get("O"), o.get("E")))
-    err = [float(np.abs(a - b).max()) for a, b in zip(R[False][:3], R[True][:3])]
-    if tables:
-        err += [max(_table_err(a, b) for a, b in zip(R[False][i], R[True][i])) for i in (3, 4)]
-    return err
-
-
 def _run_stages(name, c, p, stages, kernel_set=0, r_bars=None, objective=False, oe_bars=None):
     sms = num_sms()
     rng = np.random.default_rng(11)
@@ -277,7 +199,7 @@ def test_sigma_per_cluster(row):
         Y0 = f32(make_Y0(c["Z"], c["K"], rng))
         R2, _, _ = planted_R(c, rng)
         Zp, Yp = planted_zy(c, rng)
-        e32 = _fp32_r_errors(c, p, Y0, R2, make_perms(c["N"], p.T, 5), Zp, Yp, make_perms(c["N"], p.T, 6))
+        e32 = fp32_errors(c, p, Y0, R2, make_perms(c["N"], p.T, 5), Zp, Yp, make_perms(c["N"], p.T, 6), own_pr_b=True)
         # S1 and S2: 2e-5.  U from the d-chunked 3xTF32 logits over d = 127, amplified by 2 / sigma_k (up to 20), gave
         # max|dR| 1.12e-5 after S1 and 1.003e-5 after S2 on an H100 80GB HBM3 (400 W); the fp32 oracle's FFMA dot products
         # give 2.7e-6 and 2.6e-6 on the same inputs
@@ -312,7 +234,8 @@ def test_block_counts(name):
         Y0 = f32(make_Y0(c["Z"], c["K"], rng))
         R2, _, _ = planted_R(c, rng)
         Zp, Yp = planted_zy(c, rng)
-        e32 = _fp32_r_errors(c, p, Y0, R2, make_perms(c["N"], p.T, 5), Zp, Yp, make_perms(c["N"], p.T, 6), tables=True)
+        e32 = fp32_errors(c, p, Y0, R2, make_perms(c["N"], p.T, 5), Zp, Yp, make_perms(c["N"], p.T, 6), tables=True,
+                          own_pr_b=True)
         r_bars = (TOL_R1, max(TOL_R, 2 * e32[1]), max(TOL_R, 2 * e32[2]))
         oe_bars = (max(TOL_OE, 2 * e32[3]), max(TOL_OE, 2 * e32[4]))
         print(f"[{TAG} blocks {name}] fp32 oracle after S2, S3: max|dR| {e32[1]:.2e} {e32[2]:.2e}, O / E {e32[3]:.2e} "

@@ -142,15 +142,11 @@ def test_library_reproduces_the_tables_printed_by_the_reference_vignette():
     the reference printed (the closest value to a rounding boundary, 398.52, is 0.02 away — 20x the fp32 error)."""
     import os
     from harmony_b200 import prepare_inputs
-    from harmony_b200.harmony import harmony
-    from helpers import GOLDEN
+    from helpers import GOLDEN, gpu_setup
     g = np.load(os.path.join(GOLDEN, "vignette_walkthrough.npz"))
     Z, meta = load_cell_lines(small=False)
     a = prepare_inputs(Z, meta, "dataset", nclust=5, theta=1.0)
-    h = harmony(device=0)
-    h.setup(a["Z"], a["phi_i"], a["sigma"], a["theta"], a["lambda_"], a["alpha"], a["max_iter_kmeans"],
-            a["epsilon_kmeans"], a["epsilon_harmony"], a["K"], a["block_size"], a["B_vec"],
-            a["batch_proportion_cutoff"], False)
+    h = gpu_setup(a, device=0)
     h.init_cluster_cpp(g["Y"])
     assert np.array_equal(np.round(np.asarray(h.O)), g["O_init"])
     assert np.array_equal(np.round(np.asarray(h.E)), g["E_init"])
@@ -171,16 +167,11 @@ def test_library_reproduces_the_vignette_tables_after_cluster_cpp(seed, kernel_s
     assignment runs on."""
     import os
     from harmony_b200 import prepare_inputs
-    from harmony_b200.harmony import harmony
-    from helpers import GOLDEN, make_perms
+    from helpers import GOLDEN, gpu_setup, make_perms
     g = np.load(os.path.join(GOLDEN, "vignette_walkthrough.npz"))
     Z, meta = load_cell_lines(small=False)
     a = prepare_inputs(Z, meta, "dataset", nclust=5, theta=1.0)
-    h = harmony(device=0)
-    h.kernel_set = kernel_set
-    h.setup(a["Z"], a["phi_i"], a["sigma"], a["theta"], a["lambda_"], a["alpha"], 10,
-            a["epsilon_kmeans"], a["epsilon_harmony"], a["K"], a["block_size"], a["B_vec"],
-            a["batch_proportion_cutoff"], False)
+    h = gpu_setup(a, T=10, kernel_set=kernel_set, device=0)
     h.legacy_centroid_step = 1
     assert h.legacy_centroid_step == 1
     h.init_cluster_cpp(g["Y"])
@@ -198,14 +189,11 @@ def test_abort_callback_stops_cluster_cpp():
     """hb_set_abort_callback = Progress::check_abort (harmony.cpp:233): cluster_cpp returns -1 once the callback
     says so, harmonize() reports "terminated by user" like R/utils.R:27-29, and the object stays usable."""
     from harmony_b200 import prepare_inputs
-    from harmony_b200.harmony import harmony
     from harmony_b200.utils import harmonize
-    from helpers import make_Y0
+    from helpers import gpu_setup, make_Y0
     Z, meta = load_cell_lines(True)
     a = prepare_inputs(Z, meta, "dataset", nclust=5, early_stop=False)
-    g = harmony(device=0)
-    g.setup(a["Z"], a["phi_i"], a["sigma"], a["theta"], a["lambda_"], a["alpha"], a["max_iter_kmeans"],
-            a["epsilon_kmeans"], a["epsilon_harmony"], a["K"], a["block_size"], a["B_vec"], a["batch_proportion_cutoff"])
+    g = gpu_setup(a, device=0)
     g.init_cluster_cpp(make_Y0(Z, a["K"], 0))
     calls, state = [], {"abort": False}
     g.set_abort_callback(lambda: calls.append(1) or state["abort"])

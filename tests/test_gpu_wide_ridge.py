@@ -11,23 +11,20 @@ import numpy as np
 import pytest
 
 from harmony_b200 import prepare_inputs
-from helpers import make_perms, make_Y0, rel_l2, synthetic
+from helpers import gpu_setup, make_perms, make_Y0, rel_l2, synthetic
 
 pytestmark = pytest.mark.gpu
 
 
 @pytest.mark.parametrize("d,K", [(150, 20), (128, 112), (100, 50)])
 def test_ridge_step_wide_embeddings(d, K):
-    from harmony_b200.harmony import harmony
     from numpy_restatement import NumpyHarmony
     Z, meta = synthetic(6000, d, [5], n_types=12, seed=40 + d)
     a = prepare_inputs(Z, meta, "cov0", nclust=K, early_stop=False)
     N, T = Z.shape[0], a["max_iter_kmeans"]
     Y0 = make_Y0(Z, a["K"], 17)
     perms = make_perms(N, T, 31)
-    g = harmony()
-    g.setup(a["Z"], a["phi_i"], a["sigma"], a["theta"], a["lambda_"], a["alpha"], T, a["epsilon_kmeans"],
-            a["epsilon_harmony"], a["K"], a["block_size"], a["B_vec"], a["batch_proportion_cutoff"], False)
+    g = gpu_setup(a)
     g.init_cluster_cpp(Y0)
     assert g.cluster_cpp(perms) == 0
     npy = NumpyHarmony(a["Z"], a["phi_i"], a["B_vec"], a["sigma"], a["theta"], a["lambda_"], a["alpha"], T, a["K"],

@@ -4,7 +4,8 @@ passes, the column-range ridge apply and the k-means initialisation from those l
 
 The CPU tests restate today's fit tests of the FFMA kernels in Python and check, over every K in 2..1024 and d in
 1..1024, that each stage keeps its kernel where that kernel fits and takes the new one everywhere else.  The GPU tests run
-the four stages of test_gpu_kernel_edges.py on rows that straddle each new limit, against the fp64 numpy restatement.
+the four stages of stages.py on the rows of WIDE_ROWS, which straddle each new limit, against the fp64 numpy
+restatement.
 """
 import ctypes
 
@@ -12,13 +13,12 @@ import numpy as np
 import pytest
 
 from harmony_b200 import _lib
-from helpers import free_port, make_perms, num_sms, rel_l2
-from stages import (ALPHA, BLOCK, CUTOFF, NB, SIGMA, T, TOL_OBJ, TOL_OE, TOL_R, TOL_R1, TOL_Y, TOL_Y_FIXED, TOL_Z,
-                    TOL_ZN, _launches, _mix64, _nested, _obj_err, _one_cov, _set_zcorr, _sizes, _table_err, f32,
-                    kernel_paths, make_Y0, native_order, numpy_model, planted_R, tables_of)
+from helpers import compare, free_port, make_perms, num_sms, rel_l2, run_gpu
+from stages import (A_FFMA, A_FUSED, A_LOGITS, A_WIDE, C_FUSED, C_LOGITS, C_NATURAL, C_WIDE, DEFAULT, HB_KS_WIDE,
+                    M_FFMA, M_LOGITS, M_TC, M_WIDE, NB, P_COLS, P_FFMA, P_TC, SINGLE_PASS, T, TOL_R, TOL_R1, WIDE_ROWS,
+                    _mix64, case_of, f32, fp32_errors, kernel_paths, make_Y0, native_order, numpy_model, planted_R,
+                    planted_zy, setup_gpu, stage_s1, stage_s2, stage_s3, stage_s4, wide_paths)
 
-PER_STEP, TWO_PASS, SINGLE_PASS = 0, 1, 2
-HB_KS_WIDE = 16
 SMEM = 227 * 1024
 
 
@@ -46,22 +46,9 @@ def kmeans_ffma_fits(K, d):      # k_kmeans_race / k_kmeans_assign: all centroid
     return 4 * K * d <= 200 * 1024
 
 
-def wide_paths(K, d, J, n, num_sms, kernel_set=0):
-    out = (ctypes.c_int64 * 4)()
-    _lib.lib().hb_debug_wide_paths(K, d, J, n, NB, num_sms, kernel_set, out)
-    return tuple(out)
-
-
-# hb_debug_wide_paths values
-A_FUSED, A_FFMA, A_LOGITS, A_WIDE = 1, 2, 3, 4            # natural-order assignment
-C_NATURAL, C_FUSED, C_LOGITS, C_WIDE = 0, 1, 2, 3         # plan-order cold start
-P_TC, P_FFMA, P_COLS = 1, 2, 3                            # ridge apply
-M_FFMA, M_TC, M_LOGITS, M_WIDE = 1, 2, 3, 4               # k-means initialisation
-
-
 def test_every_shape_has_a_kernel_and_keeps_the_one_that_fits():
     """K in 2..1024, d in 1..1024 (20 tuples, 1M cells, 132 SMs): the old kernel wherever it fits, the new one elsewhere."""
-    L = _lib.lib()
+    L = _lib.lib()      # the hooks themselves, on reused buffers: kernel_paths / wide_paths double this loop's time
     old, new = (ctypes.c_int64 * 8)(), (ctypes.c_int64 * 4)()
     for K in range(2, 1025):
         for d in range(1, 1025):
@@ -94,7 +81,7 @@ def test_every_shape_has_a_kernel_and_keeps_the_one_that_fits():
 
 def test_wide_hook_forces_the_new_kernels():
     """HB_KS_WIDE puts every stage on the new kernels, c3 included."""
-    assert wide_paths(100, 50, 20, 1000000, 132, HB_KS_WIDE) == (A_WIDE, C_WIDE, P_COLS, M_WIDE)
+    assert wide_paths(100, 50, 20, 1000000, 132, kernel_set=HB_KS_WIDE) == (A_WIDE, C_WIDE, P_COLS, M_WIDE)
     assert kernel_paths(100, 50, 20, 1000000, 132)[1:5] == (2, 0, 1, 1)   # unchanged without the bit
 
 
@@ -119,206 +106,58 @@ def _apply_launches(K, d, wide):
     return sum(passes(min(128, DS - c)) for c in range(0, DS, 128))
 
 
-# name -> (K, d, covariate builder(num_sms), hb_debug_wide_paths, update path, kernel_set)
-ROWS = {
-    # logits past k_logits_tc (d = 127 > 120), k_assign past its shared memory at K = 200
-    "d127_K200": (200, 127, lambda s: _one_cov(_sizes(5, 6000)), (A_WIDE, C_WIDE, P_TC, M_FFMA), SINGLE_PASS, 0),
-    # k_assign one column past its limit (d = 252 runs on it)
-    "d253_K100": (100, 253, lambda s: _one_cov(_sizes(6, 6000)), (A_WIDE, C_WIDE, P_FFMA, M_FFMA), SINGLE_PASS, 0),
-    # the FFMA apply's block is 1040 threads: column ranges 128 + 128 + 4
-    "d257_K64": (64, 257, lambda s: _one_cov(_sizes(6, 6000)), (A_FFMA, C_NATURAL, P_COLS, M_FFMA), SINGLE_PASS, 0),
-    "d300_K100": (100, 300, lambda s: _nested(_sizes(8, 8000), 4), (A_WIDE, C_WIDE, P_COLS, M_FFMA), SINGLE_PASS, 0),
-    # 2 J = #SMs + 2: two-pass update, natural-order cold start from the d-chunked logits
-    "d300_K100_two_pass": (100, 300, lambda s: _nested(_sizes(s // 2 + 1, 12000), 6), (A_WIDE, C_NATURAL, P_COLS, M_FFMA),
-                           TWO_PASS, 0),
-    # two 128-cluster logits ranges, four column ranges x three cluster ranges of the apply, k-means from wide logits
-    "d512_K200": (200, 512, lambda s: _one_cov(_sizes(5, 6000)), (A_WIDE, C_WIDE, P_COLS, M_WIDE), SINGLE_PASS, 0),
-    # k_assign one cluster past its limit at d = 8 (K = 704 runs on it); per-step update
-    "K705_d8": (705, 8, lambda s: _one_cov(_sizes(4, 4000)), (A_LOGITS, C_NATURAL, P_TC, M_FFMA), PER_STEP, 0),
-    # K = 1024: softmax with 8 pieces per lane, k-means from k_logits_tc logits
-    "K1024_d64": (1024, 64, lambda s: _one_cov(_sizes(4, 4000)), (A_LOGITS, C_NATURAL, P_TC, M_LOGITS), PER_STEP, 0),
-    # config 3's shape with every new kernel forced
-    "c3_shape_wide": (100, 50, lambda s: _one_cov(_sizes(20, 20000)), (A_WIDE, C_WIDE, P_COLS, M_WIDE), SINGLE_PASS,
-                      HB_KS_WIDE),
-}
-
-
-def build_case(name, num_sms, seed=0):
-    """Inputs of a row, built like test_gpu_kernel_edges.build_case: three zero rows and three rows at 1e-25."""
-    K, d, cov, _, _, _ = ROWS[name]
-    tuples, B_vec, sizes = cov(num_sms)
-    rng = np.random.default_rng(2000 + seed + sum(map(ord, name)))
-    phi = np.concatenate([np.tile(np.asarray(t, dtype=np.int64), (s, 1)) for t, s in zip(tuples, sizes)])
-    phi = phi[rng.permutation(len(phi))]
-    N = len(phi)
-    n_types = max(4, min(K, 30))
-    centers = rng.standard_normal((n_types, d)) * 2.0
-    Z = centers[rng.integers(0, n_types, N)] + 0.7 * rng.standard_normal((N, d))
-    Z += 0.5 * rng.standard_normal((sum(B_vec), d))[phi].sum(axis=1)
-    Z *= (10.0 / np.sqrt(1.0 + np.arange(d)))[None, :]
-    special = rng.choice(N, 6, replace=False)
-    Z[special[:3]] = 0.0
-    Z[special[3:]] *= 1e-25 / np.abs(Z[special[3:]]).max(axis=1, keepdims=True)
-    return dict(Z=Z, phi=phi, B_vec=B_vec, K=K, d=d, N=N, sizes=sizes, tuples=tuples)
-
-
-@pytest.mark.parametrize("name", list(ROWS))
+@pytest.mark.parametrize("name", list(WIDE_ROWS))
 def test_wide_rows_reach_their_kernels(name):
-    c = build_case(name, 132)
-    K, d, _, want, update, ks = ROWS[name]
+    c = case_of(name, 132)
+    K, d, _, want, update, ks = WIDE_ROWS[name]
     J = len(c["sizes"])
-    assert wide_paths(K, d, J, c["N"], 132, ks) == want
+    assert wide_paths(K, d, J, c["N"], 132, kernel_set=ks) == want
     assert kernel_paths(K, d, J, c["N"], 132)[0] == update
 
 
 # ---- GPU ----------------------------------------------------------------------------------------------------------------
-def _prenormalised(Z):
-    """Z with the rows whose fp32 sum of squares under- or overflows (|v| ~ 1e-25 or 1e20) divided by their norm in fp64:
-    the reference's fp32 arithmetic does not rescale such rows, so the fp32 oracle would measure that, not the stage."""
-    Z = np.array(Z, dtype=np.float64)
-    m = np.abs(Z).max(axis=1)
-    x = (m > 0) & ((m < 1e-10) | (m > 1e10))
-    Z[x] /= np.linalg.norm(Z[x] / m[x, None], axis=1, keepdims=True) * m[x, None]
-    return Z
-
-
-def _oracle(c, Z, dbl):
-    from oracle.oracle import OracleHarmony
-    B = sum(c["B_vec"])
-    o = OracleHarmony(double=dbl)
-    o.setup(Z=Z, phi_i=c["phi"], B_vec=np.asarray(c["B_vec"]), sigma=np.full(c["K"], SIGMA), theta=np.full(B, 2.0),
-            lambda_=None, alpha=ALPHA, max_iter_kmeans=T, epsilon_kmeans=-np.inf, epsilon_harmony=-np.inf, K=c["K"],
-            block_size=BLOCK, batch_proportion_cutoff=CUTOFF)
-    return o
-
-
-def _fp32_errors(c, Y0, R2, O2, E2, perms2, Zp, Yp, perms3):
-    """max |R32 - R64| of the fp32 and fp64 oracles after each stage, each on that stage's inputs: S1 setup +
-    init_cluster_cpp(Y0); S2 R, O, E written, then cluster_cpp; S3 Z_corr = Zp and Y = Yp, then cluster_cpp.  The R
-    error of these stages comes from fp32 dot products over d columns amplified 2 / sigma = 20 times; where fp32 itself
-    cannot hold the edge file's bar (d = 512), twice this error is the stage's bar."""
-    R = {}
-    for dbl in (False, True):
-        o = _oracle(c, _prenormalised(c["Z"]), dbl)
-        o.init_cluster_cpp(Y0)
-        r1 = o.get("R")
-        o.set("R", R2)
-        o.set("O", O2.T)
-        o.set("E", E2.T)
-        o.cluster_cpp(perms2)
-        r2 = o.get("R")
-        o = _oracle(c, _prenormalised(Zp), dbl)
-        o.init_cluster_cpp(Yp)
-        o.cluster_cpp(perms3)
-        R[dbl] = (r1, r2, o.get("R"))
-    return [float(np.abs(a - b).max()) for a, b in zip(R[False], R[True])]
-
-
-def _report(name, stage, errs, bars, ratios):
-    print(f"[wide {name} {stage}] " + " ".join(f"{k}={v:.2e}(bar {bars[k]:.1e}, {v / bars[k]:.2f})" for k, v in errs.items()))
-    for k, v in errs.items():
-        ratios.append(v / bars[k])
-        assert v <= bars[k], (name, stage, k, v, bars[k])
-
-
 def _assign_launches(K, wide_logits, plan, normalise):
     lg = 1 + (K + 127) // 128 if wide_logits else (K + 63) // 64
     return lg + 2 + (1 if normalise and not plan else 0)
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("name", list(ROWS))
+@pytest.mark.parametrize("name", list(WIDE_ROWS))
 def test_wide_row_stages(name):
-    from harmony_b200.harmony import harmony
     sms = num_sms()
-    c = build_case(name, sms)
-    K, d, _, want, update, ks = ROWS[name]
-    N, B, J = c["N"], sum(c["B_vec"]), len(c["sizes"])
-    paths = wide_paths(K, d, J, N, sms, ks)
+    c = case_of(name, sms)
+    K, d, _, want, update, ks = WIDE_ROWS[name]
+    N, J = c["N"], len(c["sizes"])
+    paths = wide_paths(K, d, J, N, sms, kernel_set=ks)
     assert paths == want
     rng = np.random.default_rng(11)
     Zf = f32(c["Z"])
     Y0 = f32(make_Y0(c["Z"], K, rng))
-    # the inputs of S2 and S3 (drawn here, in the order the stages use them), then the fp32 oracle's R error per stage
+    # the inputs of S2, S4 and S3, drawn here in the order the stages use them, then the fp32 oracle's R error per stage
     R2, _, _ = planted_R(c, rng)
-    R4, kz, _ = planted_R(c, rng, special=True)
-    Zp = rng.standard_normal((N, d)) * rng.uniform(0.1, 30.0, (N, 1))
-    special = rng.choice(N, 8, replace=False)
-    Zp[special[:2]] = 0.0
-    Zp[special[2:5]] *= 1e-25 / np.abs(Zp[special[2:5]]).max(axis=1, keepdims=True)
-    Zp[special[5:]] *= 1e20 / np.abs(Zp[special[5:]]).max(axis=1, keepdims=True)
-    Zp = f32(Zp)
-    Yp = rng.standard_normal((K, d))
-    Yp = f32(Yp / np.linalg.norm(Yp, axis=1, keepdims=True))
-    perms2, perms3 = make_perms(N, T, 5), make_perms(N, T, 6)
-    npy = numpy_model(c, Zf)
-    O2, E2 = tables_of(R2, c, npy.Pr_b)
-    e32 = _fp32_errors(c, Y0, R2, O2, E2, perms2, Zp, Yp, perms3)
+    R4 = planted_R(c, rng, special=True)
+    Zp, Yp = planted_zy(c, rng)
+    e32 = fp32_errors(c, DEFAULT, Y0, R2, make_perms(N, T, 5), Zp, Yp, make_perms(N, T, 6))
     bar_R1, bar_R2, bar_R3 = max(TOL_R1, 2 * e32[0]), max(TOL_R, 2 * e32[1]), max(TOL_R, 2 * e32[2])
     print(f"[wide {name}] fp32 oracle max|dR| per stage {e32[0]:.2e} {e32[1]:.2e} {e32[2]:.2e} -> R bars "
           f"{bar_R1:.2e} {bar_R2:.2e} {bar_R3:.2e}")
     ratios = []
-
-    # ---- S1: setup + init_cluster_cpp(Y0)
-    g = harmony()
-    g.kernel_set = ks
-    g.setup(c["Z"], c["phi"], SIGMA, np.full(B, 2.0), None, ALPHA, T, -np.inf, -np.inf, K, BLOCK, c["B_vec"], CUTOFF)
-    errs = dict(Zn=float(np.abs(g.getZcorr().T - npy.Z_corr).max()))
-    as0 = _launches(g, "assign")
-    g.init_cluster_cpp(Y0)
-    npy.init_cluster(Y0)
-    if paths[0] in (A_LOGITS, A_WIDE):
-        assert _launches(g, "assign") - as0 == _assign_launches(K, paths[0] == A_WIDE, False, False)
-    errs.update(R=float(np.abs(g.R.T - npy.R).max()), O=_table_err(g.O, npy.O), E=_table_err(g.E, npy.E),
-                obj=_obj_err(g, npy, 1))
-    _report(name, "S1 assign", errs, dict(Zn=TOL_ZN, R=bar_R1, O=TOL_OE, E=TOL_OE, obj=TOL_OBJ),
-            ratios)
-
-    # ---- S2: R, O, E written through the fields, then one cluster_cpp call from them
-    g.R, g.O, g.E = R2.T, O2, E2
-    npy.R, npy.O, npy.E = R2, O2, E2
-    assert g.cluster_cpp(perms2) == 0
-    npy.cluster(perms2)
-    errs = dict(R=float(np.abs(g.R.T - npy.R).max()), O=_table_err(g.O, npy.O), E=_table_err(g.E, npy.E),
-                obj=_obj_err(g, npy, T))
-    _report(name, "S2 update from written R", errs, dict(R=bar_R2, O=TOL_OE, E=TOL_OE, obj=TOL_OBJ), ratios)
-
-    # ---- S4: ridge step from planted R, O, E, estimated then fixed lambda
-    O, E = tables_of(R4, c, npy.Pr_b)
-    g.R, g.O, g.E = R4.T, O, E
-    npy.R, npy.O, npy.E = R4, O, E
-    for lam in (None, np.concatenate([[0.0], np.linspace(0.5, 2.0, B)])):
-        if lam is not None:
-            g.lambda_ = lam
-            npy.lam = lam
-        Yb = g.Y.T.astype(np.float64)
-        npy.Y = Yb
-        ap0 = _launches(g, "ridge_apply")
-        g.moe_correct_ridge_cpp()
-        npy.moe_correct_ridge()
-        if paths[2] != P_FFMA:
-            assert _launches(g, "ridge_apply") - ap0 == _apply_launches(K, d, paths[2] == P_COLS)
-        Yg = g.Y.T
-        errs = dict(Z=rel_l2(g.getZcorr().T, npy.Z_corr), Y=float(np.abs(Yg - npy.Y).max()))
-        _report(name, f"S4 ridge {'fixed' if lam is not None else 'estimated'} lambda", errs,
-                dict(Z=TOL_Z, Y=TOL_Y if lam is None else TOL_Y_FIXED), ratios)
-        np.testing.assert_array_equal(Yg[kz], np.float32(Yb[kz]))
-
-    # ---- S3: planted Z_corr and Y, cold-start cluster_cpp
-    _set_zcorr(g, Zp)
-    g.Y = Yp.T
-    npy.Z_corr, npy.Y = Zp, Yp
-    as0 = _launches(g, "assign")
-    assert g.cluster_cpp(perms3) == 0
-    npy.cluster(perms3)
+    g = setup_gpu(c, kernel_set=ks)
+    npy = numpy_model(c, Zf)
+    logits = paths[0] in (A_LOGITS, A_WIDE)
+    stage_s1(name, g, npy, Y0, "wide", dict(R=bar_R1), ratios,
+             assign_launches=_assign_launches(K, paths[0] == A_WIDE, False, False) if logits else None)
+    assert stage_s2(name, g, npy, c, rng, tag="wide", bars=dict(R=bar_R2), ratios=ratios, R=R2) == T
+    stage_s4(name, g, npy, c, rng, tag="wide", ratios=ratios, R=R4,
+             apply_launches=_apply_launches(K, d, paths[2] == P_COLS) if paths[2] != P_FFMA else None)
     if paths[1] == C_WIDE:
-        assert _launches(g, "assign") - as0 == _assign_launches(K, True, True, True)
-    elif paths[1] == C_NATURAL and paths[0] in (A_LOGITS, A_WIDE):
-        assert _launches(g, "assign") - as0 == _assign_launches(K, paths[0] == A_WIDE, False, True)
-    errs = dict(R=float(np.abs(g.R.T - npy.R).max()), O=_table_err(g.O, npy.O), E=_table_err(g.E, npy.E),
-                obj=_obj_err(g, npy, T), Zn=float(np.abs(g.getZcorr().T - npy.Z_corr).max()))
-    _report(name, "S3 cold start", errs, dict(R=bar_R3, O=TOL_OE, E=TOL_OE, obj=TOL_OBJ, Zn=TOL_ZN), ratios)
-    assert int(g.kmeans_rounds[-1]) == T
+        cold = _assign_launches(K, True, True, True)
+    elif paths[1] == C_NATURAL and logits:
+        cold = _assign_launches(K, paths[0] == A_WIDE, False, True)
+    else:
+        cold = None
+    assert stage_s3(name, g, npy, c, rng, tag="wide", bars=dict(R=bar_R3), ratios=ratios, assign_launches=cold,
+                    Zp=Zp, Yp=Yp) == T
     print(f"[wide {name}] largest ratio to a bar: {max(ratios):.2f}")
 
 
@@ -328,7 +167,6 @@ def test_parity_d300_K100():
     test_gpu_parity.py against the fp32 and fp64 oracles."""
     from harmony_b200 import prepare_inputs
     from helpers import make_Y0 as make_Y0_h, run_oracle, synthetic
-    from test_gpu_parity import compare, run_gpu
     Z, meta = synthetic(50000, 300, [8], n_types=20, seed=41)
     a = prepare_inputs(Z, meta, "cov0", nclust=100, early_stop=False)
     N, T_ = Z.shape[0], a["max_iter_kmeans"]
@@ -364,7 +202,6 @@ def test_runharmony_cuda_tensor_d300(monkeypatch):
     import torch
     from harmony_b200 import harmony_options, prepare_inputs, ui
     from helpers import run_oracle, synthetic
-    from test_gpu_parity import compare
     SEED, ITERS = 20261015, 10
     # one cell type per cluster: with 20 types for K = 100 many clusters end up as near-duplicates after 10 iterations,
     # and their exact ties (top-2 gaps <= 3e-6) flip the hard index of ~0.2 % of the cells in any fp32 evaluation (the fp32

@@ -1,13 +1,13 @@
 """The k-means restatement (kmeans_restatement.py) against a literal one-draw-at-a-time statement of the same rule, its
-race intervals and Lloyd admissible sets on planted cases, and the kernels every row of test_gpu_kmeans_init.py
+race intervals and Lloyd admissible sets on planted cases, and the kernels every row of kmeans_rows.py
 reaches on a 132-SM H100 (host-only hooks, no GPU needed)."""
-import ctypes
-
 import numpy as np
 import pytest
 
 from kmeans_restatement import (KEY_REL, canonical_clusters, exact_rows, kmeans_centers, kmeans_centers_fast,
                                 kmeans_uniform, lloyd_admissible, lloyd_eps, race_delta, race_intervals, start_cells)
+from kmeans_rows import CASES, ROWS
+from stages import M_FFMA, M_LOGITS, M_TC, wide_paths
 
 M64 = (1 << 64) - 1
 
@@ -175,14 +175,10 @@ def _sp_nv(KS):
 def test_gpu_rows_reach_their_kernels():
     """Every row of test_gpu_kmeans_init.py on a 132-SM H100: the k-means path of hb_debug_wide_paths, NV = sp_nv(KS)
     of the race and pick kernels, and ceil(K / 64) k_logits_tc launches per logits pass."""
-    from harmony_b200 import _lib
-    from test_gpu_kmeans_init import CASES, M_FFMA, M_LOGITS, M_TC, ROWS
-    L = _lib.lib()
     for name, ks, path, nv in CASES:
         r = ROWS[name]
-        out = (ctypes.c_int64 * 4)()
-        L.hb_debug_wide_paths(r.K, r.d, r.J, r.N, 20, 132, ks, out)
-        assert out[3] == path, (name, ks, out[3], path)
+        got = wide_paths(r.K, r.d, r.J, r.N, 132, kernel_set=ks)[3]
+        assert got == path, (name, ks, got, path)
         if path != M_FFMA:
             assert _sp_nv((r.K + 3) & ~3) == nv, (name, nv)
         if path in (M_TC, M_LOGITS):              # k_logits_tc: 64 clusters per launch
