@@ -6,6 +6,7 @@ Importing this package does not load the CUDA library; constructing ``harmony`` 
 loudly if it is missing (there is no CPU fallback).
 """
 from .clustering import kmeans, nmi_ari, nmi_ari_cluster_labels_kmeans  # noqa: F401
+from .community import leiden, nmi_ari_cluster_labels_leiden, umap_connectivities  # noqa: F401
 from .graph import graph_components, graph_connectivity  # noqa: F401
 from .harmony_option import harmony_options  # noqa: F401
 from .kbet import kbet  # noqa: F401

@@ -87,6 +87,9 @@ def lib():
     L.hb_pcr.argtypes = [P, P, I, I64, I64, I, P, I, I, P, P, P, P, P]
     L.hb_debug_sym_eig.argtypes = [I, P, P, P]
     L.hb_kmeans.argtypes = [P, P, I, I64, I64, I, I, ctypes.c_uint64, I, I, D, P, P, P, P, P, P]
+    L.hb_umap_graph.argtypes = [P, P, I64, P, I64, I64, I, I, P, P, P, ctypes.POINTER(I64), P]
+    L.hb_leiden.argtypes = [P, P, P, P, I, I64, I64, D, I, P, ctypes.POINTER(I), ctypes.POINTER(D), ctypes.POINTER(I),
+                            P, P]
     L.hb_init_cluster.argtypes = [P, P]
     L.hb_cluster.argtypes = [P, P]
     L.hb_moe_correct_ridge.argtypes = [P]

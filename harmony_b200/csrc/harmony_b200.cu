@@ -44,6 +44,7 @@
 #include "kbet.cuh"
 #include "pcr.cuh"
 #include "kmeans_score.cuh"
+#include "leiden.cuh"
 
 #include "select.cuh"
 #include "handle.cuh"
@@ -373,6 +374,7 @@ int harmony_step(hb_handle* h, const char* what, bool needs_init = true) {
 #include "kbet_host.cuh"
 #include "pcr_host.cuh"
 #include "kmeans_score_host.cuh"
+#include "leiden_host.cuh"
 
 // =================================================================================================
 extern "C" {
@@ -588,6 +590,21 @@ int hb_kmeans(hb_handle* h, const void* X, int x_dtype, int64_t x_ld, int64_t N,
   if (!h) return 1;
   return run_kmeans(h, DevRows{X, x_dtype, x_ld, N}, d, K, seed, n_init, max_iter, tol, labels, centres, inertia, n_iter,
                     seeds, (cudaStream_t)stream);
+}
+
+int hb_umap_graph(hb_handle* h, const int32_t* idx, int64_t idx_ld, const float* dist, int64_t dist_ld, int64_t N, int k,
+                  int n_neighbors, int64_t* indptr, int32_t* indices, float* data, int64_t* nnz, void* stream) {
+  if (!h) return 1;
+  return run_umap_graph(h, idx, idx_ld, dist, dist_ld, N, k, n_neighbors, indptr, indices, data, nnz,
+                        (cudaStream_t)stream);
+}
+
+int hb_leiden(hb_handle* h, const int64_t* indptr, const int32_t* indices, const void* data, int dtype, int64_t N,
+              int64_t nnz, double resolution, int n_iterations, int32_t* labels, int32_t* n_communities, double* quality,
+              int32_t* iterations, int64_t* stats, void* stream) {
+  if (!h) return 1;
+  return run_leiden(h, indptr, indices, data, dtype, N, nnz, resolution, n_iterations, labels, n_communities, quality,
+                    iterations, stats, (cudaStream_t)stream);
 }
 
 int hb_init_cluster(hb_handle* h, const double* Y0) {

@@ -1,10 +1,48 @@
 // score_host.cuh — what the score calls (hb_knn, hb_lisi, hb_silhouette, hb_graph_components, hb_kbet, hb_pcr,
-// hb_kmeans; DESIGN §9-§15) share on the host: their scratch, their shape refusals, the sorted indexes and sums they
+// hb_kmeans, hb_umap_graph,
+// hb_leiden; DESIGN §9-§16) share on the host: their scratch, their shape refusals, the sorted indexes and sums they
 // build, the preparation and sweep of knn.cuh, and the way each call is ordered on the caller's stream.  Included by
 // harmony_b200.cu before the calls' own *_host.cuh.
 #pragma once
 
 namespace {
+
+// The buffers of hb_umap_graph and hb_leiden (DESIGN §16), which run alone
+// The level graph: n vertices, nnz entries, row starts, columns, fp64 weights, each entry's row, degrees
+struct LeidenGraph {
+  int n = 0, nnz = 0;
+  DevBuf<int> ip, col, row;
+  DevBuf<double> w, deg;
+  int reserve(hb_handle* h, int n_, int nnz_) {
+    n = n_;
+    nnz = nnz_;
+    CK(ip.reserve((size_t)n + 1));
+    CK(col.reserve((size_t)std::max(nnz, 1)));
+    CK(row.reserve((size_t)std::max(nnz, 1)));
+    CK(w.reserve((size_t)std::max(nnz, 1)));
+    CK(deg.reserve((size_t)std::max(n, 1)));
+    return 0;
+  }
+};
+
+template <typename T>
+void swap_bufs(DevBuf<T>& a, DevBuf<T>& b) {
+  std::swap(a.p, b.p);
+  std::swap(a.n, b.n);
+}
+struct LeidenBufs {
+  LeidenGraph g0, level[2];                    // the caller's graph, and the aggregated levels in turn
+  DevBuf<int> key, skey, sval[2], hist;         // radix sort keys, values and digit histograms
+  DevBuf<unsigned long long> scan_state;        // the chain state of the call's scans
+  DevBuf<int> eperm, eperm1;                    // entries sorted by (row, code of the column), and the first pass
+  DevBuf<int> vperm, vstart;                    // vertices sorted by a code, and the code starts [n + 1]
+  DevBuf<int> comm, next, sub, target, proposed;  // the partition, the sweep's result, sub-communities, proposals
+  DevBuf<int> newid, cmin, vmap, omap, lab;     // aggregation: ids, the next start partition, level and row maps
+  DevBuf<int> head, seg_start, size, first, small;  // pair heads and starts; community sizes and first members
+  DevBuf<double> tot, ext, win, sub_tot, sub_ext, dsmall;  // community and sub-community sums
+  DevBuf<double> rho, sigma, rsum, rcnt, uw, uwv;  // umap: per-row rho, sigma, distance sums; [N][k] and emitted weights
+  DevBuf<int> ucnt, urow, ucol;                 // umap: emitted entries per listed entry, their rows and columns
+};
 
 // The scratch of the score calls, shared by them: each runs on h->stream, and a buffer that grows is freed only after
 // the device has drained.  Every buffer grows on demand and is kept for the next call.  Buffers that no one call uses
@@ -31,6 +69,7 @@ struct ScoreScratch {
   DevBuf<double> d2;                   // kmeans: [N] the seeding's D^2
   DevBuf<int> small;                   // kmeans: the winner, the changed count, [K] counts, [K] seeds
   DevBuf<unsigned long long> seg_codes;  // kmeans: [J] the code of each segment of the sorted rows
+  LeidenBufs leiden;                   // umap_graph, leiden
 };
 ScoreScratch& score_scratch(hb_handle* h) {
   if (!h->scores) h->scores.reset(new ScoreScratch());

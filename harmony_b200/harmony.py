@@ -242,6 +242,18 @@ class harmony:
         from .clustering import kmeans_on
         return kmeans_on(self, X, n_clusters, seed, n_init, max_iter, tol, return_seeds)
 
+    def umap_connectivities(self, X, n_neighbors=15):
+        """``hb_umap_graph`` of X's exact neighbour graph on this object's device, as
+        ``harmony_b200.umap_connectivities`` returns it.  Works in any state of the object and changes none of it."""
+        from .community import umap_on
+        return umap_on(self, X, n_neighbors)
+
+    def leiden(self, X_or_graph, resolution=1.0, n_neighbors=15, n_iterations=-1, return_info=False):
+        """``hb_leiden`` on this object's device, as ``harmony_b200.leiden`` returns it.  Works in any state of the
+        object and changes none of it."""
+        from .community import leiden_on
+        return leiden_on(self, X_or_graph, resolution, n_neighbors, n_iterations, return_info)
+
     def _device_Phi(self, Phi):
         """An [N] or [N, C] int32 / int64 CUDA tensor -> contiguous [N, C] int32 on the object's device (converted, if
         need be, on the current torch stream, which hb_setup_device orders its read after)."""

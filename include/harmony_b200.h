@@ -45,7 +45,8 @@ int hb_pop_warning(hb_handle* h, char* buf, size_t cap);
 /* Library/ABI version: major*10000 + minor*100 + patch (0.3.0: labels in device memory; 0.4.0: mapping a query onto
  * a reference, hb_reference / hb_map_setup / hb_map).  hb_knn, hb_debug_knn_geometry, hb_lisi,
  * hb_debug_lisi_geometry, hb_silhouette, hb_debug_silhouette_geometry, hb_graph_components, hb_kbet,
- * hb_debug_chi2_sf, hb_pcr, hb_debug_sym_eig and hb_kmeans were added without moving the number. */
+ * hb_debug_chi2_sf, hb_pcr, hb_debug_sym_eig, hb_kmeans, hb_umap_graph and hb_leiden were added without moving the
+ * number. */
 int hb_version(void);
 
 /* ---- multi-GPU (one process per GPU; cells sharded contiguously; SURVEY §8e) ------------------- */
@@ -285,6 +286,29 @@ int hb_debug_sym_eig(int n, const double* A, double* w, double* V);
 int hb_kmeans(hb_handle* h, const void* X, int x_dtype, int64_t x_ld, int64_t N, int d, int K, uint64_t seed,
               int n_init, int max_iter, double tol, int32_t* labels, double* centres, double* inertia, int32_t* n_iter,
               int32_t* seeds, void* stream);
+
+/* scanpy's UMAP connectivities (umap-learn's fuzzy_simplicial_set, local_connectivity 1, set_op_mix_ratio 1; DESIGN
+ * §16) of neighbour lists idx / dist [N][k] (hb_knn's with exclude_self: -1 / +inf fill, rows contiguous, idx_ld =
+ * dist_ld = k <= 128) in device memory.  n_neighbors counts the cell itself (scanpy's, k + 1).  rho, sigma and the
+ * weights in fp64; the symmetric union P = W + W^T - W o W^T as a CSR in the caller's device buffers: indptr int64
+ * [N + 1], indices int32 (ascending within a row) and data fp32, each of at least 2 N k entries; *nnz (host) gets the
+ * entries written.  No diagonal and no explicit zero.  Ordered on `stream`; needs no setup and touches no handle state;
+ * two calls give bit-identical results.  Region "umap_graph". */
+int hb_umap_graph(hb_handle* h, const int32_t* idx, int64_t idx_ld, const float* dist, int64_t dist_ld, int64_t N, int k,
+                  int n_neighbors, int64_t* indptr, int32_t* indices, float* data, int64_t* nnz, void* stream);
+
+/* Deterministic Leiden (DESIGN §16) of the symmetric CSR graph indptr int64 [N + 1] / indices int32 / data (dtype
+ * HB_FLOAT32 or HB_FLOAT64, finite and > 0) in device memory, rows strictly ascending and no diagonal, for modularity
+ * with resolution gamma (RBConfigurationVertexPartition).  A graph that breaks these is refused with status 2, naming
+ * the row and entry, before any output is written.  labels int32 [N] (device): communities numbered by decreasing
+ * size, ties by the smallest member row.  Host outputs: *n_communities, *quality (Q in fp64), *iterations; stats (NULL
+ * or host int64 [3]): levels, local-moving sweeps and refinement rounds run.  n_iterations -1 repeats iterations until
+ * no label changes (at most 64), else runs that many.  A reached cap leaves a warning (hb_pop_warning).  Ordered on
+ * `stream`; needs no setup and touches no handle state; two calls give bit-identical results.  Regions "leiden" and,
+ * within it, "leiden_move", "leiden_refine" and "leiden_aggregate". */
+int hb_leiden(hb_handle* h, const int64_t* indptr, const int32_t* indices, const void* data, int dtype, int64_t N,
+              int64_t nnz, double resolution, int n_iterations, int32_t* labels, int32_t* n_communities, double* quality,
+              int32_t* iterations, int64_t* stats, void* stream);
 
 /* ---- fields / getters (harmony.cpp:640-669, 675-696) ------------------------------------------- */
 enum hb_field {
