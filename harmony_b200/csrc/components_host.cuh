@@ -12,19 +12,13 @@ int components_run(hb_handle* h, const int32_t* idx, int64_t idx_ld, int64_t N, 
   const cudaStream_t st = h->stream;
   const int cap = h->num_sms * 8;
   const int64_t k1 = (int64_t)k + 1;  // an entry's place in the bad word: row k1 + m, the label at m = k
-  CK(s.keys.reserve(1));
-  CK(cudaMemsetAsync(s.keys.p, 0xff, sizeof(unsigned long long), st));
-  TRY(launch(h, k_cc_check, dim3(grid_for(N * k1, 256, cap)), dim3(256), 0, idx, idx_ld, N, k, labels, n_labels,
-             s.keys.p));
   unsigned long long bad = 0;
-  CK(cudaMemcpyAsync(&bad, s.keys.p, sizeof(bad), cudaMemcpyDeviceToHost, st));
-  CK(cudaStreamSynchronize(st));
+  TRY(run_check(h, &bad, k_cc_check, dim3(grid_for(N * k1, 256, cap)), idx, idx_ld, N, k, labels, n_labels));
   if (bad != ~0ull) {
     const int64_t row = (int64_t)(bad / k1);
     const int m = (int)(bad % k1);
     int v = 0;
-    CK(cudaMemcpyAsync(&v, m < k ? idx + row * idx_ld + m : labels + row, sizeof(int), cudaMemcpyDeviceToHost, st));
-    CK(cudaStreamSynchronize(st));
+    TRY(read_back(h, m < k ? idx + row * idx_ld + m : labels + row, &v));
     if (m < k)
       return fail(h, 2, "hb_graph_components: idx[%lld][%d] = %d is not -1 or a row in 0..%lld", (long long)row, m, v,
                   (long long)(N - 1));

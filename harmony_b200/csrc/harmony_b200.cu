@@ -51,6 +51,7 @@
 #include "comm.cuh"
 #include "trace.cuh"
 #include "transfer.cuh"
+#include "sort.cuh"
 #include "plan.cuh"
 #include "tuples.cuh"
 #include "update_host.cuh"

@@ -1,5 +1,5 @@
-// leiden_host.cuh — hb_umap_graph and hb_leiden (DESIGN §16): the checks and launches of leiden.cuh, setup's stable
-// radix sort and chained scan for every grouping, and the loops of local moving, refinement, aggregation and
+// leiden_host.cuh — hb_umap_graph and hb_leiden (DESIGN §16): the checks and launches of leiden.cuh, sort.cuh's
+// stable radix sort and chained scan for every grouping, and the loops of local moving, refinement, aggregation and
 // iterations on the host.  The calls need no setup and touch no state of a Harmony run or a mapping.  Included by
 // harmony_b200.cu.
 #pragma once
@@ -10,63 +10,6 @@ constexpr int LEIDEN_MAX_SWEEPS = 128;      // local-moving sweeps per level
 constexpr int LEIDEN_MAX_ROUNDS = 1024;     // refinement rounds per level
 constexpr int LEIDEN_MAX_LEVELS = 1024;     // levels per iteration
 constexpr int LEIDEN_MAX_ITERATIONS = 64;   // iterations of n_iterations = -1
-
-// Exclusive scan in place of n ints (k_scan_chained) on the call's own chain state: no allocation and no wait, unlike
-// tuple_scan
-int leiden_scan(hb_handle* h, int* data, int64_t n) {
-  LeidenBufs& B = score_scratch(h).leiden;
-  const int tiles = (int)((n + SCAN_TILE - 1) / SCAN_TILE);
-  CK(B.scan_state.reserve((size_t)tiles + 1));
-  CK(cudaMemsetAsync(B.scan_state.p, 0, sizeof(unsigned long long) * ((size_t)tiles + 1), h->stream));
-  k_scan_chained<<<dim3(tiles, 1), 1024, 0, h->stream>>>(data, n, B.scan_state.p, tiles);
-  CKL();
-  return 0;
-}
-
-int bits_for(int64_t n) {
-  int b = 0;
-  while (b < 31 && (1ll << b) < n) ++b;
-  return b;
-}
-
-// Stable LSD sort of n non-negative keys below 2^bits (key is overwritten) carrying vin (null: the positions) into
-// vout; returns the buffer that holds the sorted keys
-int stable_sort(hb_handle* h, int* key, int64_t n, int bits, const int* vin, int* vout, int** sorted) {
-  LeidenBufs& B = score_scratch(h).leiden;
-  const cudaStream_t st = h->stream;
-  const int passes = (bits + 7) / 8;
-  const int nchunks = (int)std::max<int64_t>(1, (n + TI_CHUNK - 1) / TI_CHUNK);
-  const int cta = (nchunks + TI_WARPS - 1) / TI_WARPS;
-  CK(B.skey.reserve((size_t)std::max<int64_t>(n, 1)));
-  CK(B.sval[0].reserve((size_t)std::max<int64_t>(n, 1)));
-  CK(B.sval[1].reserve((size_t)std::max<int64_t>(n, 1)));
-  CK(B.hist.reserve((size_t)256 * nchunks));
-  *sorted = key;
-  if (n == 0) return 0;
-  if (passes == 0) {
-    if (vin) CK(cudaMemcpyAsync(vout, vin, sizeof(int) * n, cudaMemcpyDeviceToDevice, st));
-    else {
-      k_identity_perm<<<grid_for(n, 256, h->num_sms * 8), 256, 0, st>>>(n, vout, B.sval[0].p);
-      CKL();
-    }
-    return 0;
-  }
-  int *kin = key, *kout = B.skey.p;
-  const int* v = vin;
-  for (int p = 0; p < passes; ++p) {
-    const bool last = p == passes - 1;
-    int* vo = last ? vout : B.sval[p & 1].p;
-    k_radix_hist<<<cta, TI_WARPS * 32, 0, st>>>(kin, n, 8 * p, nchunks, B.hist.p);
-    CKL();
-    TRY(leiden_scan(h, B.hist.p, (int64_t)256 * nchunks));
-    k_radix_scatter<<<cta, TI_WARPS * 32, 0, st>>>(kin, v, n, 8 * p, nchunks, B.hist.p, kout, vo, nullptr);
-    CKL();
-    v = vo;
-    std::swap(kin, kout);
-  }
-  *sorted = kin;
-  return 0;
-}
 
 struct LeidenRun {
   hb_handle* h;
@@ -82,14 +25,9 @@ int leiden_grid(hb_handle* h, int64_t n) { return grid_for(n, 256, h->num_sms * 
 // vertices of g sorted by code (B.vperm) and the code starts (B.vstart, n + 1)
 int sort_vertices(hb_handle* h, const LeidenGraph& g, const int* code) {
   LeidenBufs& B = score_scratch(h).leiden;
-  const cudaStream_t st = h->stream;
   TRY(launch(h, k_gather_key, dim3(leiden_grid(h, g.n)), dim3(256), 0, code, (const int*)nullptr, (const int*)nullptr,
              (int64_t)g.n, B.key.p));
-  int* sorted = nullptr;
-  TRY(stable_sort(h, B.key.p, g.n, bits_for(g.n), nullptr, B.vperm.p, &sorted));
-  k_tuple_starts<<<leiden_grid(h, (int64_t)g.n + 1), 256, 0, st>>>(sorted, g.n, g.n, B.vstart.p);
-  CKL();
-  return 0;
+  return sort_by_code(h, B.sort, B.key.p, g.n, g.n, nullptr, B.vperm.p, nullptr, B.vstart.p);
 }
 // sums over the segments of sort_vertices into out
 int vertex_sums(hb_handle* h, const LeidenGraph& g, const double* vals, double* out) {
@@ -97,24 +35,22 @@ int vertex_sums(hb_handle* h, const LeidenGraph& g, const double* vals, double* 
   return launch(h, k_seg_sum, dim3(grid_for((int64_t)g.n * 32, 256, h->num_sms * 8)), dim3(256), 0, vals,
                 (const int*)B.vperm.p, (const int*)B.vstart.p, g.n, out);
 }
-// g's entries sorted by (row, code[col]) into B.eperm (codes below 2^bits_for(g.n))
-// (code_row null: by the row itself)
+// The n entries whose minor keys B.key holds, sorted stably by (major, minor) into B.eperm (by the minor key alone:
+// B.eperm1), both keys codes below n_codes.  An entry's major key is code[of[e]] (of null: code[e]); starts: the
+// majors' starts, if not null.
+int sort_pairs(hb_handle* h, int64_t n, int n_codes, const int* code, const int* of, int* starts) {
+  LeidenBufs& B = score_scratch(h).leiden;
+  TRY(sort_by_code(h, B.sort, B.key.p, n, n_codes, nullptr, B.eperm1.p, nullptr, nullptr));
+  TRY(launch(h, k_gather_key, dim3(leiden_grid(h, n)), dim3(256), 0, code, of, (const int*)B.eperm1.p, n, B.key.p));
+  return sort_by_code(h, B.sort, B.key.p, n, n_codes, B.eperm1.p, B.eperm.p, nullptr, starts);
+}
+// g's entries sorted by (row, code[col]) into B.eperm (code_row null: by the row itself, else by code_row[row])
 int sort_entries(hb_handle* h, const LeidenGraph& g, const int* code_col, const int* code_row) {
   LeidenBufs& B = score_scratch(h).leiden;
-  const int bits = bits_for(g.n);
-  const dim3 grid(leiden_grid(h, g.nnz));
-  TRY(launch(h, k_gather_key, grid, dim3(256), 0, code_col, (const int*)g.col.p, (const int*)nullptr, (int64_t)g.nnz, B.key.p));
-  int* sorted = nullptr;
-  TRY(stable_sort(h, B.key.p, g.nnz, bits, nullptr, B.eperm1.p, &sorted));
-  TRY(launch(h, k_gather_key, grid, dim3(256), 0, code_row ? code_row : (const int*)g.row.p,
-             code_row ? (const int*)g.row.p : (const int*)nullptr, (const int*)B.eperm1.p, (int64_t)g.nnz, B.key.p));
-  return stable_sort(h, B.key.p, g.nnz, bits, B.eperm1.p, B.eperm.p, &sorted);
-}
-
-int read_int(hb_handle* h, const int* p, int* out) {
-  CK(cudaMemcpyAsync(out, p, sizeof(int), cudaMemcpyDeviceToHost, h->stream));
-  CK(cudaStreamSynchronize(h->stream));
-  return 0;
+  TRY(launch(h, k_gather_key, dim3(leiden_grid(h, g.nnz)), dim3(256), 0, code_col, (const int*)g.col.p,
+             (const int*)nullptr, (int64_t)g.nnz, B.key.p));
+  return sort_pairs(h, g.nnz, g.n, code_row ? code_row : (const int*)g.row.p,
+                    code_row ? (const int*)g.row.p : (const int*)nullptr, nullptr);
 }
 
 // Local moving of g from the partition in B.comm; *moved = whether any vertex moved
@@ -138,7 +74,7 @@ int leiden_move(LeidenRun& r, const LeidenGraph& g, bool* moved) {
                            r.gamma, r.inv2m, cnt};
     TRY(launch(h, k_leiden_move, dim3(leiden_grid(h, g.n)), dim3(256), 0, a));
     int m = 0;
-    TRY(read_int(h, cnt, &m));
+    TRY(read_back(h, cnt, &m));
     ++r.sweeps;
     swap_bufs(B.comm, B.next);
     if (m) *moved = true;
@@ -180,7 +116,7 @@ int leiden_refine(LeidenRun& r, const LeidenGraph& g, bool* moved) {
     TRY(launch(h, k_leiden_propose, grid, block, 0, a));
     TRY(launch(h, k_leiden_join, grid, block, 0, (const int*)B.target.p, (const int*)B.proposed.p, g.n, B.sub.p, cnt));
     int m = 0;
-    TRY(read_int(h, cnt, &m));
+    TRY(read_back(h, cnt, &m));
     ++r.rounds;
     if (!m) break;
     *moved = true;
@@ -197,9 +133,9 @@ int leiden_aggregate(LeidenRun& r, const LeidenGraph& g, LeidenGraph& next) {
   const cudaStream_t st = h->stream;
   const dim3 grid(leiden_grid(h, g.n)), block(256);
   TRY(launch(h, k_leiden_used, dim3(leiden_grid(h, (int64_t)g.n + 1)), block, 0, (const int*)B.vstart.p, g.n, B.newid.p));
-  TRY(leiden_scan(h, B.newid.p, (int64_t)g.n + 1));
+  TRY(chained_scan(h, st, B.newid.p, (int64_t)g.n + 1, 1, B.sort.scan));
   int n2 = 0;
-  TRY(read_int(h, B.newid.p + g.n, &n2));
+  TRY(read_back(h, B.newid.p + g.n, &n2));
   CK(cudaMemsetAsync(B.cmin.p, 0x7f, sizeof(int) * g.n, st));
   TRY(launch(h, k_leiden_vmap, grid, block, 0, (const int*)B.sub.p, (const int*)B.newid.p, (const int*)B.comm.p, g.n,
              B.vmap.p, B.cmin.p));
@@ -210,9 +146,9 @@ int leiden_aggregate(LeidenRun& r, const LeidenGraph& g, LeidenGraph& next) {
   const dim3 egrid(leiden_grid(h, (int64_t)g.nnz + 1));
   TRY(launch(h, k_leiden_heads, egrid, block, 0, (const int*)B.eperm.p, (const int*)g.row.p, (const int*)g.col.p,
              (const int*)B.vmap.p, g.nnz, B.head.p));
-  TRY(leiden_scan(h, B.head.p, (int64_t)g.nnz + 1));
+  TRY(chained_scan(h, st, B.head.p, (int64_t)g.nnz + 1, 1, B.sort.scan));
   int nnz2 = 0;
-  TRY(read_int(h, B.head.p + g.nnz, &nnz2));
+  TRY(read_back(h, B.head.p + g.nnz, &nnz2));
   TRY(next.reserve(h, n2, nnz2));
   CK(B.seg_start.reserve((size_t)nnz2 + 1));
   TRY(launch(h, k_leiden_segs, egrid, block, 0, (const int*)B.eperm.p, (const int*)g.row.p, (const int*)g.col.p,
@@ -307,26 +243,16 @@ int leiden_iteration(LeidenRun& r) {
 template <typename T>
 int leiden_run(hb_handle* h, const int64_t* indptr, const int32_t* indices, const T* data, int64_t N, int64_t nnz,
                double gamma, int n_iterations, int32_t* labels, int* n_comm, double* Q, int* n_iter, int64_t* stats) {
-  ScoreScratch& s = score_scratch(h);
-  LeidenBufs& B = s.leiden;
+  LeidenBufs& B = score_scratch(h).leiden;
   const cudaStream_t st = h->stream;
   // ---- the caller's graph, read only until it passes
-  CK(s.keys.reserve(1));
-  CK(cudaMemsetAsync(s.keys.p, 0xff, sizeof(unsigned long long), st));
-  TRY(launch(h, k_leiden_check_rows, dim3(leiden_grid(h, N + 1)), dim3(256), 0, indptr, N, nnz, s.keys.p));
   unsigned long long bad = 0;
-  CK(cudaMemcpyAsync(&bad, s.keys.p, sizeof(bad), cudaMemcpyDeviceToHost, st));
-  CK(cudaStreamSynchronize(st));
+  TRY(run_check(h, &bad, k_leiden_check_rows, dim3(leiden_grid(h, N + 1)), indptr, N, nnz));
   if (bad != ~0ull) return fail(h, 2, "hb_leiden: indptr[%llu] breaks 0 = indptr[0] <= ... <= indptr[N] = nnz = %lld", bad, (long long)nnz);
   const dim3 cgrid(grid_for(N * 32, 256, h->num_sms * 8));
-  TRY(launch(h, k_leiden_check_entries<T, false>, cgrid, dim3(256), 0, indptr, indices, data, N, s.keys.p));
-  CK(cudaMemcpyAsync(&bad, s.keys.p, sizeof(bad), cudaMemcpyDeviceToHost, st));
-  CK(cudaStreamSynchronize(st));
-  if (bad == ~0ull) {  // rows in range, sorted and without diagonal: now the mirrors
-    TRY(launch(h, k_leiden_check_entries<T, true>, cgrid, dim3(256), 0, indptr, indices, data, N, s.keys.p));
-    CK(cudaMemcpyAsync(&bad, s.keys.p, sizeof(bad), cudaMemcpyDeviceToHost, st));
-    CK(cudaStreamSynchronize(st));
-  }
+  TRY(run_check(h, &bad, k_leiden_check_entries<T, false>, cgrid, indptr, indices, data, N));
+  if (bad == ~0ull)  // rows in range, sorted and without diagonal: now the mirrors
+    TRY(run_check(h, &bad, k_leiden_check_entries<T, true>, cgrid, indptr, indices, data, N));
   if (bad != ~0ull) {
     const int64_t e = (int64_t)(bad / 8);
     std::vector<int64_t> ip(N + 1);
@@ -337,8 +263,7 @@ int leiden_run(hb_handle* h, const int64_t* indptr, const int32_t* indices, cons
                                 "has a weight that is not finite and > 0", "has no mirror entry (j, i)",
                                 "has a weight that differs from its mirror (j, i)"};
     int j = 0;
-    CK(cudaMemcpyAsync(&j, indices + e, sizeof(int), cudaMemcpyDeviceToHost, st));
-    CK(cudaStreamSynchronize(st));
+    TRY(read_back(h, indices + e, &j));
     return fail(h, 2, "hb_leiden: the graph is not a symmetric CSR without diagonal: row %lld, entry %lld (column %d) %s",
                 (long long)row, (long long)e, j, why[bad % 8]);
   }
@@ -425,18 +350,12 @@ int umap_run(hb_handle* h, const int32_t* idx, const float* dist, int64_t N, int
   LeidenBufs& B = score_scratch(h).leiden;
   const cudaStream_t st = h->stream;
   const int64_t Nk = N * k;
-  ScoreScratch& s = score_scratch(h);
-  CK(s.keys.reserve(1));
-  CK(cudaMemsetAsync(s.keys.p, 0xff, sizeof(unsigned long long), st));
-  TRY(launch(h, k_umap_check, dim3(grid_for(Nk, 256, h->num_sms * 8)), dim3(256), 0, idx, N, k, s.keys.p));
   unsigned long long bad = 0;
-  CK(cudaMemcpyAsync(&bad, s.keys.p, sizeof(bad), cudaMemcpyDeviceToHost, st));
-  CK(cudaStreamSynchronize(st));
+  TRY(run_check(h, &bad, k_umap_check, dim3(grid_for(Nk, 256, h->num_sms * 8)), idx, N, k));
   if (bad != ~0ull) {
     const int64_t e = (int64_t)(bad / 2);
     int j = 0;
-    CK(cudaMemcpyAsync(&j, idx + e, sizeof(int), cudaMemcpyDeviceToHost, st));
-    CK(cudaStreamSynchronize(st));
+    TRY(read_back(h, idx + e, &j));
     if (bad % 2 == 0)
       return fail(h, 2, "hb_umap_graph: idx[%lld][%lld] = %d is not -1 or a row in 0..%lld", (long long)(e / k),
                   (long long)(e % k), j, (long long)(N - 1));
@@ -457,9 +376,9 @@ int umap_run(hb_handle* h, const int32_t* idx, const float* dist, int64_t N, int
   TRY(launch(h, k_umap_sym<false>, grid, block, 0, idx, N, k, (const double*)B.uw.p, B.ucnt.p, (const int*)nullptr,
              (int*)nullptr, (int*)nullptr, (double*)nullptr));
   CK(cudaMemsetAsync(B.ucnt.p + Nk, 0, sizeof(int), st));
-  TRY(leiden_scan(h, B.ucnt.p, Nk + 1));
+  TRY(chained_scan(h, st, B.ucnt.p, Nk + 1, 1, B.sort.scan));
   int nnz = 0;
-  TRY(read_int(h, B.ucnt.p + Nk, &nnz));
+  TRY(read_back(h, B.ucnt.p + Nk, &nnz));
   const int64_t ne = std::max(nnz, 1);
   CK(B.urow.reserve((size_t)ne));
   CK(B.ucol.reserve((size_t)ne));
@@ -470,17 +389,10 @@ int umap_run(hb_handle* h, const int32_t* idx, const float* dist, int64_t N, int
   CK(B.vstart.reserve((size_t)N + 1));
   TRY(launch(h, k_umap_sym<true>, grid, block, 0, idx, N, k, (const double*)B.uw.p, (int*)nullptr,
              (const int*)B.ucnt.p, B.urow.p, B.ucol.p, B.uwv.p));
-  // (row, col) order: by column, then stably by row
-  const int bits = bits_for(N);
-  const dim3 egrid(leiden_grid(h, ne));
-  int* sorted = nullptr;
+  // (row, col) order, and the row starts
   CK(cudaMemcpyAsync(B.key.p, B.ucol.p, sizeof(int) * nnz, cudaMemcpyDeviceToDevice, st));
-  TRY(stable_sort(h, B.key.p, nnz, bits, nullptr, B.eperm1.p, &sorted));
-  TRY(launch(h, k_gather_key, egrid, block, 0, (const int*)B.urow.p, (const int*)nullptr, (const int*)B.eperm1.p,
-             (int64_t)nnz, B.key.p));
-  TRY(stable_sort(h, B.key.p, nnz, bits, B.eperm1.p, B.eperm.p, &sorted));
-  k_tuple_starts<<<leiden_grid(h, (int64_t)nnz + 1), 256, 0, st>>>(sorted, nnz, (int)N, B.vstart.p);
-  CKL();
+  TRY(sort_pairs(h, nnz, (int)N, B.urow.p, nullptr, B.vstart.p));
+  const dim3 egrid(leiden_grid(h, ne));
   TRY(launch(h, k_indptr64, dim3(leiden_grid(h, N + 1)), block, 0, (const int*)B.vstart.p, N + 1, indptr));
   if (nnz > 0)
     TRY(launch(h, k_umap_write, egrid, block, 0, (const int*)B.eperm.p, (int64_t)nnz, (const int*)B.ucol.p,

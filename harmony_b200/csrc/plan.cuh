@@ -1,6 +1,7 @@
 // plan.cuh — the update-order plan of update_R (replaces the physical shuffles of harmony.cpp:272-291): a round's
 // cells sorted by (block, tuple, block in the next round) and the tables derived from that order.  The kernels that
-// build it and the host code that owns it; included by harmony_b200.cu once hb_handle and its helpers exist.
+// build it and the host code that owns it; its scans are sort.cuh's chained_scan.  Included by harmony_b200.cu after
+// sort.cuh.
 #pragma once
 #include "common.cuh"
 
@@ -82,73 +83,6 @@ __global__ void k_plan_hist(const int* __restrict__ blk_of, const int* __restric
   }
   __syncwarp();
   for (int j = lane; j < nb * nsub; j += 32) H[plan_hidx(j / nsub, j % nsub, c, nchunks, nsub, cq0, cnq)] = cnt[j];
-}
-// Exclusive scan of `nseg` independent int arrays of n elements (back to back in `data`, in place) by many CTAs:
-// chained scan with dynamic tile numbers.  A CTA draws the next tile (8192 elements) of its segment from a counter
-// — so a tile's predecessor has always been drawn, i.e. runs or has run: no deadlock whatever the dispatch order —,
-// scans it locally, waits for the inclusive prefix of the tile before it, publishes its own (value and flag in one
-// 64-bit word) and writes the results.  state: [nseg][1 + tiles] words, zeroed by the caller (word 0: the counter).
-constexpr int SCAN_TILE = 8192;  // 1024 threads x 8 elements
-__global__ void __launch_bounds__(1024) k_scan_chained(int* __restrict__ data, int64_t n, unsigned long long* __restrict__ state,
-                                                       int tiles_per_seg) {
-  __shared__ int wsum[32];
-  __shared__ int sh_tile, sh_carry;
-  const int seg = blockIdx.y;
-  data += (size_t)seg * (size_t)n;
-  unsigned long long* st = state + (size_t)seg * (tiles_per_seg + 1);
-  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  if (tid == 0) sh_tile = (int)atomicAdd(st, 1ull);
-  __syncthreads();
-  const int tile = sh_tile;
-  if (tile >= tiles_per_seg) return;
-  const int64_t base = (int64_t)tile * SCAN_TILE + (int64_t)tid * 8;
-  int v[8];
-  int s = 0;
-#pragma unroll
-  for (int i = 0; i < 8; ++i) {
-    v[i] = (base + i < n) ? data[base + i] : 0;
-    s += v[i];
-  }
-  // exclusive scan of the threads' sums within the CTA
-  int inc = s;
-#pragma unroll
-  for (int o = 1; o < 32; o <<= 1) {
-    const int t = __shfl_up_sync(0xffffffffu, inc, o);
-    if (lane >= o) inc += t;
-  }
-  if (lane == 31) wsum[warp] = inc;
-  __syncthreads();
-  if (warp == 0) {
-    const int w = wsum[lane];
-    int winc = w;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-      const int t = __shfl_up_sync(0xffffffffu, winc, o);
-      if (lane >= o) winc += t;
-    }
-    wsum[lane] = winc - w;  // exclusive prefix of the warps
-    if (lane == 31) {
-      // tile aggregate = winc; chain: inclusive prefix of this tile = prefix of the previous one + aggregate
-      int carry = 0;
-      if (tile > 0) {
-        unsigned long long p;
-        do {
-          asm volatile("ld.acquire.gpu.global.u64 %0, [%1];" : "=l"(p) : "l"(st + tile) : "memory");  // word 1 + (tile - 1)
-        } while ((p >> 32) == 0ull);
-        carry = (int)(unsigned)(p & 0xffffffffull);
-      }
-      const unsigned long long mine = (1ull << 32) | (unsigned)(carry + winc);
-      asm volatile("st.release.gpu.global.u64 [%0], %1;" ::"l"(st + tile + 1), "l"(mine) : "memory");
-      sh_carry = carry;
-    }
-  }
-  __syncthreads();
-  int run = sh_carry + wsum[warp] + (inc - s);
-#pragma unroll
-  for (int i = 0; i < 8; ++i) {
-    if (base + i < n) data[base + i] = run;
-    run += v[i];
-  }
 }
 // Stable scatter: order[offset(key, chunk) + rank] = cell, cells of a chunk visited in ascending order;
 // next_at[same position] = block of the cell in the next round, prev_at = its block in the previous round.
@@ -324,7 +258,7 @@ struct Plan {
   DevBuf<int> blk_of, order, next_at, prev_at, seg_start, tile_base, pt_p0, pt_len, pt_tuple, pt_blk, pt_base;
   DevBuf<int4> ranges;
   DevBuf<int> H;                          // histograms of the counting sort: [batch][nb][nsub][nchunks]
-  DevBuf<unsigned long long> scan_state;  // state of the chained scans
+  DevBuf<unsigned long long> scan_state;  // the chained scans' state, the plan's own (a prebuild scans on `stream`)
   int nchunks = 0;                        // chunks: <= CHUNK consecutive cells of one tuple, + a trailing empty one
   DevBuf<int> chunk_start, chunk_q0, chunk_nq, tuple_chunk0;
   uint64_t round_counter = 0;  // native rounds run since the seed was set, plus any prebuilt (a round's key: seed, counter)
@@ -417,14 +351,6 @@ int plan_setup(hb_handle* h, const std::vector<int64_t>& tstart, int T) {
   return 0;
 }
 
-// exclusive scan in place of nseg int arrays of len elements, back to back
-int plan_scan(hb_handle* h, int* data, int64_t len, int nseg, cudaStream_t st) {
-  const int tiles = (int)((len + SCAN_TILE - 1) / SCAN_TILE);
-  CK(cudaMemsetAsync(h->plan->scan_state.p, 0, sizeof(unsigned long long) * (size_t)nseg * (tiles + 1), st));
-  k_scan_chained<<<dim3(tiles, nseg), 1024, 0, st>>>(data, len, h->plan->scan_state.p, tiles);
-  CKL();
-  return 0;
-}
 // Counting sort of rounds [t, t + nt) of a set (nt <= batch: the histogram scratch holds that many rounds) and the
 // derived tables; round t + nt - 1 has a next round iff last_has_next.
 int plan_sort(hb_handle* h, int t, int nt, bool last_has_next, int set, cudaStream_t st) {
@@ -442,7 +368,7 @@ int plan_sort(hb_handle* h, int t, int nt, bool last_has_next, int set, cudaStre
                                                                    nb, nsub, p.H.p, h->err_flag.p, n, with_next);
   CKL();
   // offsets of the counting sort: multi-CTA scan of the nt histograms (a single CTA per round took ~145 us)
-  TRY(plan_scan(h, p.H.p, (int64_t)nb * nsub * nc, nt, st));
+  TRY(chained_scan(h, st, p.H.p, (int64_t)nb * nsub * nc, nt, p.scan_state));
   k_plan_scatter<<<dim3((nc + wpb - 1) / wpb, nt), wpb * 32, sm, st>>>(
       blk_of, p.chunk_start.p, p.chunk_q0.p, p.chunk_nq.p, nc, nb, nsub, p.H.p, p.order.p + r * n,
       p.prev_at.p ? p.prev_at.p + r * n : nullptr, p.next_at.p ? p.next_at.p + r * n : nullptr, n, with_next, t > 0);
@@ -482,7 +408,7 @@ int build_plans(hb_handle* h, int T, const int64_t* orders_d, int set, cudaStrea
   if (!step && !p.pt_p0.p) return 0;
   k_plan_tilecount<<<grid_for(S + 1, 256, 64), 256, 0, st>>>(r.seg_start, S, step ? TM : 128, base);
   CKL();
-  TRY(plan_scan(h, base, (int64_t)S + 1, 1, st));  // base[S]: the number of tiles
+  TRY(chained_scan(h, st, base, (int64_t)S + 1, 1, p.scan_state));  // base[S]: the number of tiles
   if (!step) {  // 128-row tiles, one (block, tuple) segment at a time: the cold-start assignment runs in this order
     k_plan_tilefill128<<<grid_for(S, 128, 64), 128, 0, st>>>(r.seg_start, base, S, h->J, p.pt_p0.p + set * p.pt_cap,
                                                              p.pt_len.p + set * p.pt_cap, p.pt_tuple.p + set * p.pt_cap,

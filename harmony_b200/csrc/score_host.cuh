@@ -1,8 +1,8 @@
 // score_host.cuh — what the score calls (hb_knn, hb_lisi, hb_silhouette, hb_graph_components, hb_kbet, hb_pcr,
 // hb_kmeans, hb_umap_graph,
-// hb_leiden; DESIGN §9-§16) share on the host: their scratch, their shape refusals, the sorted indexes and sums they
-// build, the preparation and sweep of knn.cuh, and the way each call is ordered on the caller's stream.  Included by
-// harmony_b200.cu before the calls' own *_host.cuh.
+// hb_leiden; DESIGN §9-§16) share on the host: their scratch, their shape refusals, the read-back of their read-only
+// checks, the sorted indexes and sums they build, the preparation and sweep of knn.cuh, and the way each call is
+// ordered on the caller's stream.  Included by harmony_b200.cu before the calls' own *_host.cuh.
 #pragma once
 
 namespace {
@@ -32,8 +32,8 @@ void swap_bufs(DevBuf<T>& a, DevBuf<T>& b) {
 }
 struct LeidenBufs {
   LeidenGraph g0, level[2];                    // the caller's graph, and the aggregated levels in turn
-  DevBuf<int> key, skey, sval[2], hist;         // radix sort keys, values and digit histograms
-  DevBuf<unsigned long long> scan_state;        // the chain state of the call's scans
+  DevBuf<int> key;                              // the sort keys
+  SortScratch sort;                             // every sort's scratch, and the chain state of the call's scans
   DevBuf<int> eperm, eperm1;                    // entries sorted by (row, code of the column), and the first pass
   DevBuf<int> vperm, vstart;                    // vertices sorted by a code, and the code starts [n + 1]
   DevBuf<int> comm, next, sub, target, proposed;  // the partition, the sweep's result, sub-communities, proposals
@@ -58,7 +58,7 @@ struct ScoreScratch {
   DevBuf<int> pstart;                  // [J + 1] each pair's or segment's first sorted row
   DevBuf<int> count;                   // [J] finite rows of each pair or segment; components: [N] rows per root
   DevBuf<int4> tiles;                  // silhouette, kbet: the sweep's tiles
-  DevBuf<unsigned long long> keys;     // components: the range pass's smallest bad entry; kmeans: [2][2 T] race keys
+  DevBuf<unsigned long long> keys;     // run_check: the smallest bad word; kmeans: [2][2 T] race keys
   DevBuf<KbetPair> pairs;              // kbet: [J] each pair's label's k0, rows, degrees of freedom and pair range
   DevBuf<double> seg_sums;             // pcr, kmeans: [J][d] each segment's column sums, then its combined row
   DevBuf<double> chunk_edge;           // pcr, kmeans: [3][chunks][d] the head, tail and total piece of each chunk
@@ -85,6 +85,24 @@ int run_score(hb_handle* h, cudaStream_t caller, const char* region, F&& work) {
     RegionScope rs(h, region);
     return work();
   });
+}
+
+// *out = *p, read once h->stream has drained
+template <typename T>
+int read_back(hb_handle* h, const T* p, T* out) {
+  CK(cudaMemcpyAsync(out, p, sizeof(T), cudaMemcpyDeviceToHost, h->stream));
+  CK(cudaStreamSynchronize(h->stream));
+  return 0;
+}
+// A read-only check on h->stream: `check` over `grid` x 256 threads with args and then s.keys, filled with ~0 first,
+// where it leaves the smallest bad word it finds.  *bad: that word (~0: none).
+template <typename... P, typename... A>
+int run_check(hb_handle* h, unsigned long long* bad, void (*check)(P...), dim3 grid, const A&... args) {
+  ScoreScratch& s = score_scratch(h);
+  CK(s.keys.reserve(1));
+  CK(cudaMemsetAsync(s.keys.p, 0xff, sizeof(unsigned long long), h->stream));
+  TRY(launch(h, check, grid, dim3(256), 0, args..., s.keys.p));
+  return read_back(h, s.keys.p, bad);
 }
 
 // Status 2, with the message when there is a handle: the geometry hooks run the shape checks without one

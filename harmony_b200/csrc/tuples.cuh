@@ -1,8 +1,8 @@
 // tuples.cuh — the covariate-tuple index of setup (and of hb_silhouette's (group, label) pairs), built on the device:
 // each cell's key (the mixed-radix number of its C levels, covariate 0 most significant), the level counts, the
 // dictionary of the distinct keys (tuple ids 0..J-1 in ascending key order), each cell's tuple id, and the stable sort
-// of the cells by tuple id (sort_perm, inv_sort, tstart).  The kernels and the host code that drives them; included by harmony_b200.cu after plan.cuh,
-// whose chained scan it reuses.
+// of the cells by tuple id (sort_perm, inv_sort, tstart).  The kernels and the host code that drives them; the scan of
+// the dictionary and the sort are sort.cuh's.  Included by harmony_b200.cu after sort.cuh.
 #pragma once
 #include "common.cuh"
 
@@ -13,8 +13,6 @@ constexpr uint32_t TI_SLOTS = 1u << TI_HASH_LOG2;
 constexpr int TI_MAX_PROBE = 512;                     // a longer probe sequence counts as a full table
 constexpr unsigned long long TI_EMPTY = ~0ull;        // no key reaches it (the level product is <= 9e18)
 constexpr int TI_SMEM_LEVELS = 8192;                  // level counts in shared memory up to this many levels
-constexpr int TI_CHUNK = 2048;                        // cells per warp in the radix passes
-constexpr int TI_WARPS = 8;                           // warps (chunks) per CTA of the radix passes
 
 __device__ __forceinline__ uint32_t ti_home(uint64_t key) { return (uint32_t)(hb_mix64(key) >> (64 - TI_HASH_LOG2)); }
 
@@ -133,74 +131,6 @@ __global__ void k_tuple_of(const unsigned long long* __restrict__ key, int64_t n
     tuple_of[i] = table ? table[key[i]] : slot_id[ti_find(slots, key[i])];
 }
 
-// ---- stable LSD radix sort of the cells by tuple id, 8-bit digits.  One warp per chunk of TI_CHUNK cells; the
-// digit histograms are laid out digit-major, H[digit * nchunks + chunk], so that one exclusive scan of H gives every
-// (digit, chunk) its first output position.
-__global__ void __launch_bounds__(TI_WARPS * 32) k_radix_hist(const int* __restrict__ key, int64_t n, int shift,
-                                                              int nchunks, int* __restrict__ H) {
-  __shared__ int cnt[TI_WARPS][256];
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int c = blockIdx.x * TI_WARPS + warp;
-  if (c >= nchunks) return;
-  for (int j = lane; j < 256; j += 32) cnt[warp][j] = 0;
-  __syncwarp();
-  const int64_t s0 = (int64_t)c * TI_CHUNK, s1 = min(n, s0 + TI_CHUNK);
-  for (int64_t s = s0 + lane; s < s1; s += 32) atomicAdd(&cnt[warp][(key[s] >> shift) & 255], 1);
-  __syncwarp();
-  for (int j = lane; j < 256; j += 32) H[(size_t)j * nchunks + c] = cnt[warp][j];
-}
-// The chunk's cells in ascending order, 32 at a time: lanes with the same digit are ranked by lane (match), so equal
-// digits keep their input order.  val_in null: the values are the positions (the first pass).  inv non-null (the
-// last pass): inv[value] = output position.
-__global__ void __launch_bounds__(TI_WARPS * 32) k_radix_scatter(const int* __restrict__ key_in, const int* __restrict__ val_in,
-                                                                 int64_t n, int shift, int nchunks, const int* __restrict__ Hoff,
-                                                                 int* __restrict__ key_out, int* __restrict__ val_out,
-                                                                 int* __restrict__ inv) {
-  __shared__ int cur[TI_WARPS][256];
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int c = blockIdx.x * TI_WARPS + warp;
-  if (c >= nchunks) return;
-  for (int j = lane; j < 256; j += 32) cur[warp][j] = Hoff[(size_t)j * nchunks + c];
-  __syncwarp();
-  const int64_t s0 = (int64_t)c * TI_CHUNK, s1 = min(n, s0 + TI_CHUNK);
-  for (int64_t base = s0; base < s1; base += 32) {
-    const int64_t s = base + lane;
-    const bool act = s < s1;
-    const int k = act ? key_in[s] : 0;
-    const int v = act ? (val_in ? val_in[s] : (int)s) : 0;
-    const int dig = act ? (k >> shift) & 255 : 256 + lane;  // inactive lanes get keys of their own
-    const unsigned m = __match_any_sync(0xffffffffu, dig);
-    const int leader = __ffs(m) - 1;
-    int start = 0;
-    if (act && lane == leader) {
-      start = cur[warp][dig];
-      cur[warp][dig] = start + __popc(m);
-    }
-    start = __shfl_sync(0xffffffffu, start, leader);
-    if (act) {
-      const int p = start + __popc(m & ((1u << lane) - 1u));
-      key_out[p] = k;
-      val_out[p] = v;
-      if (inv) inv[v] = p;
-    }
-    __syncwarp();
-  }
-}
-// J = 1: every cell keeps its place
-__global__ void k_identity_perm(int64_t n, int* __restrict__ perm, int* __restrict__ inv) {
-  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
-    perm[i] = (int)i;
-    inv[i] = (int)i;
-  }
-}
-// tstart[q] = first sorted position of tuple q, tstart[J] = n (tuples without local cells start where the next does)
-__global__ void k_tuple_starts(const int* __restrict__ sorted, int64_t n, int J, int* __restrict__ tstart) {
-  for (int64_t s = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; s <= n; s += (int64_t)gridDim.x * blockDim.x) {
-    const int prev = s > 0 ? sorted[s - 1] : -1, cur = s < n ? sorted[s] : J;
-    for (int q = prev + 1; q <= cur; ++q) tstart[q] = (int)s;
-  }
-}
-
 }  // namespace hb
 namespace {
 
@@ -214,18 +144,6 @@ struct TupleIndex {
 
 constexpr size_t TI_MAX_TUPLES = 1000000;
 int too_many_tuples(hb_handle* h) { return fail(h, 2, "more than 1e6 distinct covariate tuples are not supported"); }
-
-// exclusive scan in place of n ints (k_scan_chained, one segment) with a scratch state of its own
-int tuple_scan(hb_handle* h, int* data, int64_t n) {
-  const int tiles = (int)((n + SCAN_TILE - 1) / SCAN_TILE);
-  DevBuf<unsigned long long> state;
-  CK(state.alloc((size_t)tiles + 1));
-  CK(cudaMemsetAsync(state.p, 0, sizeof(unsigned long long) * ((size_t)tiles + 1), h->stream));
-  k_scan_chained<<<dim3(tiles, 1), 1024, 0, h->stream>>>(data, n, state.p, tiles);
-  CKL();
-  CK(cudaStreamSynchronize(h->stream));  // the state is freed on return
-  return 0;
-}
 
 // The key layout of C covariates of nlev[c] levels: covariate c's first global level (base), its weight in the key
 // (radix; covariate 0 most significant) and the number of keys.  Status 2 when the level product overflows 64 bits.
@@ -271,6 +189,7 @@ int build_tuple_index(hb_handle* h, const int* phi_d, int64_t N, const TupleKeys
   // ---- keys, validation, level counts and the dictionary in one pass
   DevBuf<unsigned long long> key, count, small, slots, uniq_d;
   DevBuf<int> geom, table, slot_id, flags;  // flags: {hash slots used, table full}
+  SortScratch srt;
   CK(key.alloc(N));
   CK(count.alloc(B));
   CK(small.alloc(1 + (size_t)C));
@@ -315,7 +234,7 @@ int build_tuple_index(hb_handle* h, const int* phi_d, int64_t N, const TupleKeys
   // ---- the local dictionary: its keys on the device (uniq_d, J_local of them, ascending on the direct path)
   int J_local = 0, hash_full = 0;
   if (direct) {
-    TRY(tuple_scan(h, table.p, (int64_t)key_space + 1));
+    TRY(chained_scan(h, st, table.p, (int64_t)key_space + 1, 1, srt.scan));
     CK(cudaMemcpyAsync(&J_local, table.p + key_space, sizeof(int), cudaMemcpyDeviceToHost, st));
     CK(cudaStreamSynchronize(st));
     CK(uniq_d.alloc(J_local));
@@ -380,7 +299,7 @@ int build_tuple_index(hb_handle* h, const int* phi_d, int64_t N, const TupleKeys
     CK(cudaStreamSynchronize(st));
   }
   uniq_d.release();
-  DevBuf<int> tid, tid2, v0, v1, H;
+  DevBuf<int> tid;
   CK(tid.alloc(N));
   k_tuple_of<<<grid, 256, 0, st>>>(key.p, N, direct ? table.p : nullptr, slots.p, slot_id.p, tid.p);
   CKL();
@@ -388,42 +307,13 @@ int build_tuple_index(hb_handle* h, const int* phi_d, int64_t N, const TupleKeys
   table.release();
   slots.release();
   slot_id.release();
-  // ---- stable sort by tuple id: ceil(log2(J) / 8) passes of 8 bits
+  srt.scan.release();
+  // ---- stable sort by tuple id, and the tuple starts
   CK(sort_perm.reserve(N));
   CK(inv_sort.reserve(N));
-  int bits = 0;
-  while (bits < 31 && (1ll << bits) < (long long)J) ++bits;
-  const int passes = (bits + 7) / 8;
-  int* kin = tid.p;
-  if (passes == 0) {
-    k_identity_perm<<<grid, 256, 0, st>>>(N, sort_perm.p, inv_sort.p);
-    CKL();
-  } else {
-    const int nchunks = (int)((N + TI_CHUNK - 1) / TI_CHUNK);
-    const int cta = (nchunks + TI_WARPS - 1) / TI_WARPS;
-    CK(tid2.alloc(N));
-    if (passes > 1) CK(v0.alloc(N));
-    if (passes > 2) CK(v1.alloc(N));
-    CK(H.alloc((size_t)256 * nchunks));
-    int* kout = tid2.p;
-    int* vbuf[2] = {v0.p, v1.p};
-    for (int p = 0; p < passes; ++p) {
-      const bool last = p == passes - 1;
-      k_radix_hist<<<cta, TI_WARPS * 32, 0, st>>>(kin, N, 8 * p, nchunks, H.p);
-      CKL();
-      TRY(tuple_scan(h, H.p, (int64_t)256 * nchunks));
-      k_radix_scatter<<<cta, TI_WARPS * 32, 0, st>>>(kin, p == 0 ? nullptr : vbuf[(p - 1) & 1], N, 8 * p, nchunks, H.p,
-                                                     kout, last ? sort_perm.p : vbuf[p & 1],
-                                                     last ? inv_sort.p : nullptr);
-      CKL();
-      std::swap(kin, kout);
-    }
-  }
-  // ---- tuple starts
   DevBuf<int> ts;
   CK(ts.alloc((size_t)J + 1));
-  k_tuple_starts<<<grid_for(N + 1, 256, h->num_sms * 8), 256, 0, st>>>(kin, N, J, ts.p);
-  CKL();
+  TRY(sort_by_code(h, srt, tid.p, N, J, nullptr, sort_perm.p, inv_sort.p, ts.p));
   std::vector<int> ts_h((size_t)J + 1);
   CK(cudaMemcpyAsync(ts_h.data(), ts.p, sizeof(int) * ts_h.size(), cudaMemcpyDeviceToHost, st));
   CK(cudaStreamSynchronize(st));
