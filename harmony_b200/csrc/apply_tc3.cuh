@@ -186,7 +186,7 @@ __device__ __forceinline__ void apply_tc_body(const ApplyTcArgs& a) {
           const int r = r0 + 8 * (j & 1), k = 8 * ks + k0 + 4 * (j >> 1);
           const float z = k < Kp ? rR[r * RS + k] : 0.f;
           ah[ks][j] = __float_as_uint(z);
-          al[ks][j] = __float_as_uint(z - __uint_as_float(__float_as_uint(z) & 0xffffe000u));
+          al[ks][j] = __float_as_uint(umma::tf32_rem(z));
         }
       }
     }

@@ -13,7 +13,8 @@
 //   k_knn_merge    per query row: the direct fp32 distance of every listed candidate of every reference split, the k
 //                  smallest in ascending order.
 // Operand pipeline as in logits_tc.cuh: per-thread 16-byte cp.async into the canonical K-major layout, the raw tile is
-// the `hi` operand, the `lo` pieces are written once the copies have landed.
+// the `hi` operand, the `lo` pieces are written once the copies have landed.  k_silhouette_tc runs the same pipeline,
+// written out in its kernel as here: taken out into a shared struct, it made ptxas serialise the wgmma (DESIGN §9).
 #pragma once
 #include <type_traits>
 
@@ -31,13 +32,14 @@ constexpr int KNN_MAX_D = 128;
 constexpr int KNN_MERGE_MAX = 1024;  // candidates per query row in k_knn_merge (splits * k)
 constexpr float KNN_INF = __builtin_huge_valf();
 
-__host__ __device__ inline size_t knn_smem_bytes(int tq, int stages, int KD, int k) {
-  const int tn = KNN_TN;
-  // Q hi / lo, reference stages + one lo tile, hx of two tiles, thresholds, counts, lists, candidate buffers, score
-  // stages of the tq / 16 warps
-  return 4 * (2 * (size_t)tq * KD + (size_t)(stages + 1) * tn * KD + 2 * (size_t)tn + 2 * (size_t)tq +
-              2 * (size_t)tq * k + 2 * (size_t)tq * KNN_CAP + (size_t)tq * KNN_SS) + 256;
+// Shared memory of the sweep's operand pipeline (k_knn_tc, k_silhouette_tc): Q hi / lo, reference stages + one lo
+// tile, hx of two tiles
+__host__ __device__ inline size_t sweep_smem_bytes(int tq, int stages, int KD) {
+  return 4 * (2 * (size_t)tq * KD + (size_t)(stages + 1) * KNN_TN * KD + 2 * (size_t)KNN_TN) + 256;
 }
+// k_knn_tc's shared memory past the pipeline, per query row: threshold, count, list, candidate buffer and the row's
+// share of its warp's score stage
+__host__ __device__ inline size_t knn_row_bytes(int k) { return 4 * (2 + 2 * (size_t)k + 2 * KNN_CAP + KNN_SS); }
 
 // ---- preparation ----------------------------------------------------------------------------------------------------
 template <typename T>
@@ -208,13 +210,9 @@ __global__ void __launch_bounds__(2 * TQ, 1) k_knn_tc(std::conditional_t<GROUPED
 
   for (int i = tid; i < TQ * KD4; i += THREADS) {
     const int r = i % TQ, c = i / TQ;
-    float4 z = make_float4(0.f, 0.f, 0.f, 0.f), l4;
+    float4 z = make_float4(0.f, 0.f, 0.f, 0.f);
     if (q0 + r < q_end) z = *reinterpret_cast<const float4*>(a.Qp + (size_t)(q0 + r) * KD + 4 * c);
-    // the tensor core reads trunc_tf32(z); the remainder is exact in fp32 and is rounded to tf32 here
-    l4.x = umma::round_tf32(z.x - __uint_as_float(__float_as_uint(z.x) & 0xffffe000u));
-    l4.y = umma::round_tf32(z.y - __uint_as_float(__float_as_uint(z.y) & 0xffffe000u));
-    l4.z = umma::round_tf32(z.z - __uint_as_float(__float_as_uint(z.z) & 0xffffe000u));
-    l4.w = umma::round_tf32(z.w - __uint_as_float(__float_as_uint(z.w) & 0xffffe000u));
+    const float4 l4 = umma::tf32_lo(z);
     *reinterpret_cast<float4*>(Qhi + ((size_t)c * TQ + r) * 4) = z;
     *reinterpret_cast<float4*>(Qlo + ((size_t)c * TQ + r) * 4) = l4;
   }
@@ -241,12 +239,7 @@ __global__ void __launch_bounds__(2 * TQ, 1) k_knn_tc(std::conditional_t<GROUPED
     if (S == 2 && t + 1 < t_end) issue(t + 1);
     for (int i = tid; i < TN * KD4; i += THREADS) {
       const float4 z = *reinterpret_cast<const float4*>(raw + (size_t)i * 4);
-      float4 l4;
-      l4.x = umma::round_tf32(z.x - __uint_as_float(__float_as_uint(z.x) & 0xffffe000u));
-      l4.y = umma::round_tf32(z.y - __uint_as_float(__float_as_uint(z.y) & 0xffffe000u));
-      l4.z = umma::round_tf32(z.z - __uint_as_float(__float_as_uint(z.z) & 0xffffe000u));
-      l4.w = umma::round_tf32(z.w - __uint_as_float(__float_as_uint(z.w) & 0xffffe000u));
-      *reinterpret_cast<float4*>(Blo + (size_t)i * 4) = l4;
+      *reinterpret_cast<float4*>(Blo + (size_t)i * 4) = umma::tf32_lo(z);
     }
     umma::fence_proxy_async();  // cp.async rows (observed above) and the `lo` writes -> tensor core
     __syncthreads();

@@ -104,11 +104,7 @@ __global__ void __launch_bounds__(LG_THREADS, 1) k_logits_tc(LogitsArgs a) {
         if (live && c < DS4) {
           z = *reinterpret_cast<const float4*>(Ahi + ((size_t)c * LG_TM + r) * 4);
           ss += (z.x * z.x + z.y * z.y) + (z.z * z.z + z.w * z.w);
-          // the tensor core reads trunc_tf32(z); the remainder is exact in fp32 and is rounded to tf32 here
-          l4.x = umma::round_tf32(z.x - __uint_as_float(__float_as_uint(z.x) & 0xffffe000u));
-          l4.y = umma::round_tf32(z.y - __uint_as_float(__float_as_uint(z.y) & 0xffffe000u));
-          l4.z = umma::round_tf32(z.z - __uint_as_float(__float_as_uint(z.z) & 0xffffe000u));
-          l4.w = umma::round_tf32(z.w - __uint_as_float(__float_as_uint(z.w) & 0xffffe000u));
+          l4 = umma::tf32_lo(z);
         }
         *reinterpret_cast<float4*>(Alo + ((size_t)c * LG_TM + r) * 4) = l4;
       }

@@ -58,9 +58,6 @@ __global__ void k_pad_rows(const float* __restrict__ Y, float* __restrict__ Ypad
 __device__ __forceinline__ void cp_async16_zfill(unsigned dst, const void* src, bool valid) {
   asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(dst), "l"(src), "r"(valid ? 16 : 0) : "memory");
 }
-__device__ __forceinline__ float tf32_rem(float z) {  // z - trunc_tf32(z), rounded to tf32
-  return umma::round_tf32(z - __uint_as_float(__float_as_uint(z) & 0xffffe000u));
-}
 
 __global__ void __launch_bounds__(LW_THREADS, 1) k_logits_wide(LogitsWideArgs a) {
   extern __shared__ __align__(128) unsigned char smem_raw[];
@@ -116,8 +113,8 @@ __global__ void __launch_bounds__(LW_THREADS, 1) k_logits_wide(LogitsWideArgs a)
       const float4 z = *reinterpret_cast<const float4*>(st + off);
       const float4 y = *reinterpret_cast<const float4*>(st + 2 * LW_PLANE + off);
       ss += (z.x * z.x + z.y * z.y) + (z.z * z.z + z.w * z.w);
-      *reinterpret_cast<float4*>(st + LW_PLANE + off) = make_float4(tf32_rem(z.x), tf32_rem(z.y), tf32_rem(z.z), tf32_rem(z.w));
-      *reinterpret_cast<float4*>(st + 3 * LW_PLANE + off) = make_float4(tf32_rem(y.x), tf32_rem(y.y), tf32_rem(y.z), tf32_rem(y.w));
+      *reinterpret_cast<float4*>(st + LW_PLANE + off) = umma::tf32_lo(z);
+      *reinterpret_cast<float4*>(st + 3 * LW_PLANE + off) = umma::tf32_lo(y);
     }
     umma::fence_proxy_async();  // this thread's cp.async pieces (observed above) and `lo` writes -> tensor core
     __syncthreads();

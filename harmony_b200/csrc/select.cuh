@@ -102,14 +102,32 @@ CallPath call_path(const KernelPaths& p, unsigned T, bool legacy_centroid) {
   return c;
 }
 
-// ---- hb_knn (knn.cuh) -------------------------------------------------------------------------------------------------
-// Launch geometry of the k-nearest-neighbour sweep: query rows per CTA (tq), operand stages of the reference tiles
-// (KNN_TN rows each) and reference splits.  The first of (128, 2), (128, 1), (64, 2), (64, 1) whose shared memory fits:
-// the query tile and the lists stay for the CTA's life, so wide rows and long lists take it from the second reference
-// stage first and from the query tile last (a 64-row tile halves the flop per reference byte and runs one warpgroup).
-// (64, 2) holds d = 128, k = 64; (64, 1), reached only by hb_lisi's k > 64, holds d = 128, k = KNN_SWEEP_MAX_K.  With
-// fewer query tiles than SMs the reference is split over grid.y so that the GPU is full, as far as k_knn_merge's
-// candidate limit and the reference's tiles allow.
+// ---- the sweep (knn.cuh): hb_knn, hb_lisi, hb_kbet, hb_silhouette -----------------------------------------------------
+// Query rows per CTA (tq) and operand stages of the reference tiles (KNN_TN rows each) of a sweep whose kernel keeps
+// row_bytes of shared memory per query row past the pipeline, and the CTA's bytes.  The first of (128, 2), (128, 1),
+// (64, 2), (64, 1) that fits: the query tile and whatever the kernel keeps per row stay for the CTA's life, so wide rows
+// and long lists take the memory from the second reference stage first and from the query tile last (a 64-row tile
+// halves the flop per reference byte and runs one warpgroup).
+struct SweepShape {
+  int tq = 0, stages = 0;
+  size_t smem = 0;
+};
+SweepShape sweep_shape(int KD, size_t row_bytes) {
+  SweepShape g;
+  static const int shapes[4][2] = {{128, 2}, {128, 1}, {64, 2}, {64, 1}};
+  for (const auto& s : shapes)
+    if (sweep_smem_bytes(s[0], s[1], KD) + s[0] * row_bytes <= SMEM_LIMIT) {
+      g.tq = s[0], g.stages = s[1];
+      break;
+    }
+  g.smem = sweep_smem_bytes(g.tq, g.stages, KD) + g.tq * row_bytes;
+  return g;
+}
+
+// Launch geometry of the k-nearest-neighbour sweep: sweep_shape for k_knn_tc's lists, and reference splits.  (64, 2)
+// holds d = 128, k = 64; (64, 1), reached only by hb_lisi's k > 64, holds d = 128, k = KNN_SWEEP_MAX_K.  With fewer
+// query tiles than SMs the reference is split over grid.y so that the GPU is full, as far as k_knn_merge's candidate
+// limit and the reference's tiles allow.
 struct KnnGeometry {
   int tq = 0, stages = 0, splits = 0, KD = 0;
   size_t smem = 0;
@@ -119,13 +137,8 @@ bool knn_fits(int d, int k) { return d >= 1 && d <= KNN_MAX_D && k >= 1 && k <= 
 KnnGeometry knn_geometry(int d, int k, int64_t Nq, int64_t Nx, int num_sms) {
   KnnGeometry g;
   g.KD = (d + 7) & ~7;
-  static const int shapes[4][2] = {{128, 2}, {128, 1}, {64, 2}, {64, 1}};
-  for (const auto& s : shapes)
-    if (knn_smem_bytes(s[0], s[1], g.KD, k) <= SMEM_LIMIT) {
-      g.tq = s[0], g.stages = s[1];
-      break;
-    }
-  g.smem = knn_smem_bytes(g.tq, g.stages, g.KD, k);
+  const SweepShape s = sweep_shape(g.KD, knn_row_bytes(k));
+  g.tq = s.tq, g.stages = s.stages, g.smem = s.smem;
   g.qtiles = (Nq + g.tq - 1) / g.tq;
   const int64_t xtiles = (Nx + KNN_TN - 1) / KNN_TN;
   int64_t splits = 1;

@@ -13,11 +13,6 @@
 
 namespace hb {
 
-// Q hi / lo, reference stages + one lo tile, hx of two tiles
-__host__ __device__ inline size_t sil_smem_bytes(int tq, int stages, int KD) {
-  return 4 * (2 * (size_t)tq * KD + (size_t)(stages + 1) * KNN_TN * KD + 2 * (size_t)KNN_TN) + 256;
-}
-
 // phi [n][2]: (group, n_groups + label), or -1 (no covariate's level) for a code outside 0..n_groups-1 / 0..n_labels-1
 __global__ void k_silhouette_phi(const int32_t* __restrict__ labels, const int32_t* __restrict__ groups, int64_t n,
                                  int n_labels, int n_groups, int* __restrict__ phi) {
@@ -101,12 +96,9 @@ __global__ void __launch_bounds__(2 * TQ, 1) k_silhouette_tc(SilArgs a) {
 
   for (int i = tid; i < TQ * KD4; i += THREADS) {
     const int r = i % TQ, c = i / TQ;
-    float4 z = make_float4(0.f, 0.f, 0.f, 0.f), l4;
+    float4 z = make_float4(0.f, 0.f, 0.f, 0.f);
     if (q0 + r < q1) z = *reinterpret_cast<const float4*>(a.Xp + (size_t)(q0 + r) * KD + 4 * c);
-    l4.x = umma::round_tf32(z.x - __uint_as_float(__float_as_uint(z.x) & 0xffffe000u));
-    l4.y = umma::round_tf32(z.y - __uint_as_float(__float_as_uint(z.y) & 0xffffe000u));
-    l4.z = umma::round_tf32(z.z - __uint_as_float(__float_as_uint(z.z) & 0xffffe000u));
-    l4.w = umma::round_tf32(z.w - __uint_as_float(__float_as_uint(z.w) & 0xffffe000u));
+    const float4 l4 = umma::tf32_lo(z);
     *reinterpret_cast<float4*>(Qhi + ((size_t)c * TQ + r) * 4) = z;
     *reinterpret_cast<float4*>(Qlo + ((size_t)c * TQ + r) * 4) = l4;
   }
@@ -144,12 +136,7 @@ __global__ void __launch_bounds__(2 * TQ, 1) k_silhouette_tc(SilArgs a) {
     if (S == 2 && t + 1 < xtiles) issue(t + 1);
     for (int i = tid; i < TN * KD4; i += THREADS) {
       const float4 z = *reinterpret_cast<const float4*>(raw + (size_t)i * 4);
-      float4 l4;
-      l4.x = umma::round_tf32(z.x - __uint_as_float(__float_as_uint(z.x) & 0xffffe000u));
-      l4.y = umma::round_tf32(z.y - __uint_as_float(__float_as_uint(z.y) & 0xffffe000u));
-      l4.z = umma::round_tf32(z.z - __uint_as_float(__float_as_uint(z.z) & 0xffffe000u));
-      l4.w = umma::round_tf32(z.w - __uint_as_float(__float_as_uint(z.w) & 0xffffe000u));
-      *reinterpret_cast<float4*>(Blo + (size_t)i * 4) = l4;
+      *reinterpret_cast<float4*>(Blo + (size_t)i * 4) = umma::tf32_lo(z);
     }
     umma::fence_proxy_async();  // cp.async rows (observed above) and the `lo` writes -> tensor core
     __syncthreads();

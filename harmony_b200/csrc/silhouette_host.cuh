@@ -5,8 +5,8 @@
 
 namespace {
 
-// Launch geometry of k_silhouette_tc: the first of (TQ, stages) = (128, 2), (128, 1), (64, 2), (64, 1) whose shared
-// memory fits (by sil_smem_bytes, (128, 2) fits every d <= 128)
+// Launch geometry of k_silhouette_tc: sweep_shape (select.cuh) of the pipeline alone, which is (128, 2) for every
+// d <= 128
 struct SilGeometry {
   int tq = 0, stages = 0, KD = 0;
   size_t smem = 0;
@@ -14,13 +14,8 @@ struct SilGeometry {
 SilGeometry sil_geometry(int d) {
   SilGeometry g;
   g.KD = (d + 7) & ~7;
-  static const int shapes[4][2] = {{128, 2}, {128, 1}, {64, 2}, {64, 1}};
-  for (const auto& s : shapes)
-    if (sil_smem_bytes(s[0], s[1], g.KD) <= SMEM_LIMIT) {
-      g.tq = s[0], g.stages = s[1];
-      break;
-    }
-  g.smem = sil_smem_bytes(g.tq, g.stages, g.KD);
+  const SweepShape s = sweep_shape(g.KD, 0);
+  g.tq = s.tq, g.stages = s.stages, g.smem = s.smem;
   return g;
 }
 

@@ -153,10 +153,7 @@ __global__ void __launch_bounds__(ST_THREADS, 1) k_stats_tc(StatsTcArgs a) {
       }
       float4 hi, lo;
       hi = make_float4(v[0], v[1], v[2], v[3]);
-      lo.x = v[0] - __uint_as_float(__float_as_uint(v[0]) & 0xffffe000u);
-      lo.y = v[1] - __uint_as_float(__float_as_uint(v[1]) & 0xffffe000u);
-      lo.z = v[2] - __uint_as_float(__float_as_uint(v[2]) & 0xffffe000u);
-      lo.w = v[3] - __uint_as_float(__float_as_uint(v[3]) & 0xffffe000u);
+      lo = make_float4(umma::tf32_rem(v[0]), umma::tf32_rem(v[1]), umma::tf32_rem(v[2]), umma::tf32_rem(v[3]));
       *reinterpret_cast<float4*>(bh_t + (ch * NB + c) * 4) = hi;
       *reinterpret_cast<float4*>(bl_t + (ch * NB + c) * 4) = lo;
     }
@@ -179,7 +176,7 @@ __global__ void __launch_bounds__(ST_THREADS, 1) k_stats_tc(StatsTcArgs a) {
           const int m = m0 + 8 * (j & 1), cell = 8 * ks + kk0 + 4 * (j >> 1);
           const float z = (cell < len && m < Kp) ? rR[cell * RK + m] : 0.f;
           ah[ks][j] = __float_as_uint(z);
-          al[ks][j] = __float_as_uint(z - __uint_as_float(__float_as_uint(z) & 0xffffe000u));
+          al[ks][j] = __float_as_uint(umma::tf32_rem(z));
         }
     }
     const uint32_t bH = umma::smem_u32(bh_t), bL = umma::smem_u32(bl_t);

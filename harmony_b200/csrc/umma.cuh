@@ -149,5 +149,10 @@ __device__ __forceinline__ void split_tf32(float x, float& hi, float& lo) {
   hi = round_tf32(x);          // nearest tf32: |x - hi| <= 2^-12 |x|
   lo = round_tf32(x - hi);     // the remainder (exact in fp32) at tf32 precision
 }
+// The same split when the raw word is the `hi` operand: the tensor core reads trunc_tf32(x), and x - trunc_tf32(x) is
+// exact in fp32.  tf32_rem leaves the remainder for the tensor core to truncate; tf32_lo rounds it to tf32.
+__device__ __forceinline__ float tf32_rem(float x) { return x - __uint_as_float(__float_as_uint(x) & 0xffffe000u); }
+__device__ __forceinline__ float tf32_lo(float x) { return round_tf32(tf32_rem(x)); }
+__device__ __forceinline__ float4 tf32_lo(float4 x) { return make_float4(tf32_lo(x.x), tf32_lo(x.y), tf32_lo(x.z), tf32_lo(x.w)); }
 
 }  // namespace umma
